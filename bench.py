@@ -1,10 +1,11 @@
 #!/usr/bin/env python
-"""bench.py -- forward throughput (M points/s) of the hot path on N B200s.
+"""bench.py -- forward throughput (M points/s) of the hot path on N H100s.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload randlanet|pointpillars|kpconv]
     python bench.py --impl reference ...        # the CPU arm (torch port of the reference forward)
+    python bench.py ... --dump-outputs DIR      # also write the last timed step's outputs as DIR/<name>.npy
 
-Launched by the driver either directly (N = 1) or through torch.distributed.run (one rank
+Launched either directly (N = 1) or through torch.distributed.run (one rank
 per GPU, NCCL).  One JSON line on rank 0.  A "step" is one forward pass of the workload's
 model over one synthetic batch:
 
@@ -43,7 +44,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
-L2_BYTES = 126e6
+L2_BYTES = 50e6          # H100 SXM
 
 
 # ----------------------------------------------------------------------------- utilities
@@ -52,7 +53,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], src="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, src="fallback (B200_PROFILING.md)")
+    return dict(hbm_gbs=3350.0, src="fallback (H100 SXM data sheet, 700 W)")
 
 
 class ClockSampler:
@@ -355,7 +356,7 @@ def run_reference(args, wl):
     emit(line)
 
 
-# ----------------------------------------------------------------------------- B200 arm
+# ----------------------------------------------------------------------------- GPU arm
 def timed_region(fn, steps, dist_on, dev):
     import torch.distributed as dist
     torch.cuda.synchronize(dev)
@@ -380,7 +381,7 @@ def timed_region(fn, steps, dist_on, dev):
 
 def pin_to_gpu_numa_node(local):
     """Binds this rank's host threads to the cores of the NUMA node its GPU hangs off (the pinned-host -> device copies
-    of the e2e region cross the inter-socket link otherwise: round-1 e2e scaling 0.90 at 8 GPUs).  Best effort."""
+    of the e2e region cross the inter-socket link otherwise).  Best effort."""
     try:
         import pynvml
         pynvml.nvmlInit()
@@ -413,18 +414,6 @@ def ev_time_ms(fn, reps=5, warm=2):
     b.record()
     torch.cuda.synchronize()
     return a.elapsed_time(b) / reps
-
-
-def measured_traffic(kind):
-    """DRAM bytes per step of the dominant kernel class from the committed ncu --set full capture of THIS
-    round's build (profiles/r02_traffic.json, written by tools/ncu_traffic.py); None when absent."""
-    path = os.path.join(ROOT, "profiles", "r02_traffic.json")
-    if not os.path.exists(path):
-        return None, None
-    d = json.load(open(path)).get(kind)
-    if not d:
-        return None, None
-    return d.get("dram_bytes_per_step"), "profiles/r02_traffic.json (%s)" % d.get("source", "ncu --set full")
 
 
 def run_b200(args, wl):
@@ -504,8 +493,12 @@ def run_b200(args, wl):
         clocks.begin()
     launches0 = L.lib().o3dml_launch_count()
     torch.cuda.cudart().cudaProfilerStart()      # ncu --profile-from-start off sees only the timed steps
-    ms = timed_region(step_resident, args.steps, dist_on, dev)
+    last = [None]
+    ms = timed_region(lambda: last.__setitem__(0, step_resident()), args.steps, dist_on, dev)
     torch.cuda.cudart().cudaProfilerStop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last[0])
+    last[0] = None
     launches = L.lib().o3dml_launch_count() - launches0
     clk = clocks.stop() if rank == 0 else None
     if hasattr(model, "backbone_neck_head"):
@@ -636,10 +629,9 @@ def run_b200(args, wl):
             e[2] += wl.roofline_bytes(d, n)
             e[3] += wl.roofline_flops(d, s, n)
         ach = tot_bytes / (tot_ms * 1e-3) / 1e9
-        traffic, tsrc = measured_traffic("lfa_pool") if (wl.B, wl.N) == (8, 45056) else (None, None)
-        roof = dict(bound="hbm", kernel="lfa_pool: tcgen05 lfa_pool_tc_kernel (d>=64) + lfa16c_kernel (d=16), all 8 launches per step",
+        roof = dict(bound="hbm", kernel="lfa_pool: wgmma lfa_pool_tc_kernel (d>=32) + lfa16c_kernel (d=16), all 8 launches per step",
                     achieved=round(ach, 2), peak=pk["hbm_gbs"], unit="GB/s", frac=round(ach / pk["hbm_gbs"], 5),
-                    algorithmic_bytes=int(tot_bytes / max(1, args.steps)), traffic=traffic, traffic_source=tsrc,
+                    algorithmic_bytes=int(tot_bytes / max(1, args.steps)), traffic=None,
                     peak_source=pk["src"], timed="CUDA events around each launch in %d eager steps run right after the "
                     "timed (graph-replayed) region" % args.steps,
                     share_of_step=round(tot_ms / lfa_ms_in_step, 4),
@@ -649,8 +641,8 @@ def run_b200(args, wl):
                                         tflops=round(e[3] / (e[0] * 1e-3) / 1e12, 2))
                                 for k, e in sorted(per.items())})
     pkj = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {}
-    peak_tf = float(pkj.get("bf16_tflops", 1590.0))
-    peak_src = "measured bf16 cuBLAS burst (MEASURED_PEAKS.json)" if pkj else "fallback (B200_PROFILING.md)"
+    peak_tf = float(pkj.get("bf16_tflops", 989.0))
+    peak_src = "measured bf16 cuBLAS burst (MEASURED_PEAKS.json)" if pkj else "fallback (H100 SXM data sheet, dense bf16, 700 W)"
     if dense_timers:
         # PointPillars: the dense BEV backbone + neck + head (SECOND/FPN/Anchor3DHead, 20 implicit-GEMM
         # launches of gemm_tc_kernel) is the dominant kernel class: tensor-core bound
@@ -658,10 +650,9 @@ def run_b200(args, wl):
         frames = sum(n for _, _, n in dense_timers)
         gflop = wl.dense_gflop_per_frame * frames
         ach = gflop / tot_ms            # GFLOP / ms = TFLOP/s
-        traffic, tsrc = measured_traffic("pp_dense")
-        roof = dict(bound="tensor", kernel="gemm_tc_kernel (tcgen05 kind::tf32, 3xTF32 split, TMA-fed): SECOND + SECONDFPN + head, 20 launches/frame",
-                    achieved=round(ach, 2), peak=peak_tf, unit="TFLOP/s", frac=round(ach / peak_tf, 5), traffic=traffic,
-                    traffic_source=tsrc, peak_source=peak_src,
+        roof = dict(bound="tensor", kernel="gemm_tc_kernel (wgmma tf32, 3xTF32 split, TMA-fed): SECOND + SECONDFPN + head, 20 launches/frame",
+                    achieved=round(ach, 2), peak=peak_tf, unit="TFLOP/s", frac=round(ach / peak_tf, 5), traffic=None,
+                    peak_source=peak_src,
                     share_of_step=round(tot_ms / ms, 4), algorithmic_gflop_per_frame=wl.dense_gflop_per_frame,
                     note="algorithmic FLOPs (SURVEY 8d); the 3xTF32 split issues 3x that at the TF32 rate (half the bf16 "
                          "rate the peak was measured at): the kernel's own ceiling is peak / 6")
@@ -692,7 +683,7 @@ def run_b200(args, wl):
             extra["gpu_eager_baseline"] = dict(value=round(wl.N / (t_g * 1e-3) / 1e6, 4), unit="Mpoints/s",
                                                what="the same torch port (oracle/models_torch.py) run eagerly on this GPU with "
                                                     "library kernels, 1 unit; informational: what the reference's own torch code "
-                                                    "gets from a B200 without this library")
+                                                    "gets from this GPU without this library")
         except Exception as e:  # noqa: BLE001
             msg = str(e)[:200]
             if "numpy" in msg:
@@ -711,14 +702,38 @@ def run_b200(args, wl):
                 config=dict(workload=wl.name, total_units=total, units_on_rank0=wl.B, points_per_unit=wl.N,
                             parallelism="frame-shard x%d (%s scaling), no data-path collective in the forward; "
                                         "post-batch all_gather of per-frame results in the e2e region" % (world, scaling),
-                            l2="inputs + activations per step (%.0f MB inputs) exceed the 126 MB L2; no flush"
-                               % (bi / 1e6),
+                            l2="inputs + activations per step (%.0f MB inputs) against the %.0f MB L2; no flush"
+                               % (bi / 1e6, L2_BYTES / 1e6),
                             launch="forward replayed from a CUDA graph" if graphed or dense_timers else "eager launches",
                             numa_node_rank0=numa),
                 clocks=clk, e2e=e2e, gpu_launches=int(launches), roofline=roof, cpu_baseline=cpu, **extra)
     emit(line)
     if dist_on:
         dist.destroy_process_group()
+
+
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(dirname, out):
+    """Writes the arrays a caller of the timed path receives as DIR/output<i>.npy: float32 (float64 for float64 and
+    integer results).  An array over its share of the 64 MB budget is reduced to a fixed, seeded sample of its rows
+    (DIR/output<i>_rows.npy holds the row indices), so that two builds can be compared output for output."""
+    os.makedirs(dirname, exist_ok=True)
+    outs = out if isinstance(out, (tuple, list)) else (out,)
+    outs = [o for o in outs if torch.is_tensor(o)]
+    share = DUMP_BYTES // max(1, len(outs))
+    for i, o in enumerate(outs):
+        a = o.detach().cpu()
+        a = a.double() if a.dtype in (torch.float64, torch.int64, torch.int32) else a.float()
+        a = a.numpy()
+        if a.nbytes > share:
+            rows = a.reshape(a.shape[0], -1) if a.ndim > 1 else a.reshape(-1, 1)
+            keep = max(1, (share - 8 * rows.shape[0]) // max(1, rows[0].nbytes + 8))
+            idx = np.sort(np.random.default_rng(0).choice(rows.shape[0], size=min(keep, rows.shape[0]), replace=False))
+            np.save(os.path.join(dirname, "output%d_rows.npy" % i), idx.astype(np.float64))
+            a = a[idx]
+        np.save(os.path.join(dirname, "output%d.npy" % i), a)
 
 
 _REAL_STDOUT = None
@@ -749,14 +764,17 @@ def main():
                     help="clouds / frames in the whole batch, sharded over the ranks: strong scaling (0 = config default)")
     ap.add_argument("--shape", default="kitti", choices=["kitti", "waymo"], help="pointpillars frame shape")
     ap.add_argument("--no-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned as DIR/<name>.npy (float32 / float64, <= 64 MB in all)")
     args = ap.parse_args()
     if args.warmup < 3 and args.impl == "b200":
         args.warmup = 3
     wl = (RandLAWorkload(args.units or 8) if args.workload == "randlanet" else
           PointPillarsWorkload(args.units or 1, shape=args.shape) if args.workload == "pointpillars" else
           KPConvWorkload(args.units or 4))
+    if args.impl == "reference" and args.steps > 50:
+        ap.error("--impl reference runs at most 50 steps (each is one full-size unit on the host cores)")
     if args.impl == "reference":
-        args.steps = min(args.steps, 50)   # bounded CPU sample: each step is one full-size unit
         run_reference(args, wl)
     else:
         run_b200(args, wl)

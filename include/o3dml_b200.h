@@ -1,5 +1,5 @@
 /*
- * o3dml_b200.h -- C ABI of libo3dml_b200.so: Blackwell (sm_100a) point-cloud operators
+ * o3dml_b200.h -- C ABI of libo3dml_b200.so: Hopper (sm_90a) point-cloud operators
  * that drop in behind the `open3d.ml.torch.{ops,layers}` / `open3d.core.nns` surface
  * consumed by isl-org/Open3D-ML's PyTorch models, plus the fused per-model hot layers.
  *
@@ -228,7 +228,7 @@ O3DML_API int o3dml_deconv_nhwc(const float* in, int batch, int H, int W, int C,
                       const float* weight_t, const float* scale, const float* shift, int act,
                       float slope, float* out, int out_ld, int out_channels, void* stream);
 
-/* Tensor-core (tcgen05, kind::tf32, 3xTF32 split: ~2^-21 relative per product) variants of the three
+/* Tensor-core (wgmma TF32, 3xTF32 split: ~2^-21 relative per product) variants of the three
  * dense entry points above.  Instead of weight_t they take the host-packed TF32 hi/lo image of the
  * weight: fp32 [2 * n_pad][k_pad] row-major, rows [0, n_pad) = tf32(w[:, n]) and rows [n_pad, 2 n_pad) =
  * tf32(w - hi) (zero padded; k_pad % 32 == 0; n_pad in {32, 64, 128*j}; 16-byte aligned;
@@ -290,9 +290,9 @@ O3DML_API int o3dml_randla_lfa16_pool(int stage, const float* coords, const void
                                       int64_t n_per_batch, const float* h_weights, float* agg,
                                       void* stream);
 
-/* Tensor-core (tcgen05, 3xFP16 split) variant of o3dml_randla_lfa_pool, same contract, d in
+/* Tensor-core (wgmma fp16, 3xFP16 split) variant of o3dml_randla_lfa_pool, same contract, d in
  * {16, 32, 64, 128, 256}.  wscore_image / wl2_image: the weight [out][in] packed by the host as
- * fp16 hi/lo operand images in the UMMA chunk-major layout ([in/8][out][8 halves] hi, then the
+ * fp16 hi/lo operand images in the chunk-major layout ([in/8][out][8 halves] hi, then the
  * same for lo; open3d_ml_b200._lib.pack_operand_image); wl2_t (fp32 [in][out]) is used instead of
  * wl2_image when d == 16.  The score bias cancels in the softmax and is not taken. */
 O3DML_API int o3dml_randla_lfa_pool_tc(int stage, int d, const float* coords, const void* neighbor_idx,
@@ -304,7 +304,7 @@ O3DML_API int o3dml_randla_lfa_pool_tc(int stage, int d, const float* coords, co
 
 /* The per-point tail of RandLA-Net in one kernel: last decoder SharedMLP on [skip | nearest_interpolation(x)]
  * (randlanet.py:284-292, 329-350) + the fc1 classifier stack (randlanet.py:110-113, 294-298), four dense layers
- * 32+32 -> 32 -> 64 -> 32 -> classes chained through tensor memory (tcgen05 kind::tf32, 3xTF32).
+ * 32+32 -> 32 -> 64 -> 32 -> classes chained through shared memory (wgmma TF32, 3xTF32).
  * weight_image: 57 344-byte device image of the four weights (open3d_ml_b200._lib.pack_tail_image: per layer and
  * 32-wide k-chunk, TF32 hi tiles then lo tiles of [N][32] floats, K-major SWIZZLE_128B); h_scale / h_shift: HOST float
  * [4][64] folded BN scale / shift (+ bias) per layer; LeakyReLU(slope) after the first three layers.

@@ -194,7 +194,7 @@ def pack_tail_image(weights_kn, n_pads):
 
 class PackedWeight:
     """A dense-layer weight in both forms: fp32 [K, Cout] for the SIMT kernel (gemm.cu) and the
-    zero-padded TF32 hi/lo image [2 * n_pad, k_pad] for the tcgen05 kernel (gemm_tc.cu)."""
+    zero-padded TF32 hi/lo image [2 * n_pad, k_pad] for the wgmma kernel (gemm_tc.cu)."""
 
     def __init__(self, w_kc):
         w = w_kc.detach().to(torch.float32).cpu().contiguous()
@@ -249,8 +249,7 @@ def _tc_ok(srcs):
 
 USE_ROW_MLP = os.environ.get("O3DML_ROW_MLP", "1") != "0"
 # one-thread-per-row layers need rows >= SMs x 256 x a few to fill the machine: below this the tensor-core kernel
-# (128 rows per CTA, K >= TC_MIN_K) has the shorter critical path (1 cloud per GPU: 11 264 rows = 44 CTAs, 25 us
-# against ~10 us; profiles/r02_launches_randlanet_1cloud.md)
+# (128 rows per CTA, K >= TC_MIN_K) has the shorter critical path
 ROW_MLP_MIN_ROWS = int(os.environ.get("O3DML_ROW_MLP_MIN_ROWS", "40000"))
 
 

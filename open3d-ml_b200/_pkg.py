@@ -1,6 +1,6 @@
 """Package body of open3d_ml_b200 (see open3d_ml_b200/__init__.py).
 
-Blackwell (sm_100a) operators behind the `open3d.ml.torch.ops` surface used by
+Hopper (sm_90a) operators behind the `open3d.ml.torch.ops` surface used by
 Open3D-ML's PyTorch models, plus fused forwards for PointPillars, RandLA-Net and
 KPFCNN.  Importing the package does not touch CUDA; calling any operator without the
 CUDA library or a CUDA device raises RuntimeError (there is no CPU fallback).

@@ -1,4 +1,4 @@
-"""Builds libo3dml_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Builds libo3dml_b200.so in-tree with nvcc for sm_90a (H100) (cross-compiles without a GPU).
 
     python open3d-ml_b200/build.py [--force]
 
@@ -16,14 +16,13 @@ CSRC = os.path.join(HERE, "csrc")
 OUT_DIR = os.path.join(HERE, "lib")
 LIB = os.path.join(OUT_DIR, "libo3dml_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-DEBUG = (["-DO3DML_DEBUG_NAN"] if os.environ.get("O3DML_DEBUG_NAN") else []) + \
-        (["-DO3DML_DEBUG_TIMING"] if os.environ.get("O3DML_DEBUG_TIMING") else [])
-FLAGS = DEBUG + ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+DEBUG = ["-DO3DML_DEBUG_NAN"] if os.environ.get("O3DML_DEBUG_NAN") else []
+FLAGS = DEBUG + ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr",
          "-ccbin", "/usr/bin/g++"]
 
 
-# development hook: extra nvcc flags (e.g. -DLTC_EAGER_INDEX) for A/B builds on the GPU box; use with --force
+# development hook: extra nvcc flags (e.g. -DO3DML_DEBUG_NAN) for A/B builds; use with --force
 FLAGS += shlex.split(os.environ.get("O3DML_NVCC_EXTRA", ""))
 
 
@@ -74,7 +73,7 @@ def _build_locked(verbose):
     with ThreadPoolExecutor(max_workers=8) as ex:
         objs = list(ex.map(cc, sources()))
     tmp = LIB + ".tmp.%d" % os.getpid()      # linked aside and renamed: a concurrent freshness check never sees a partial file
-    cmd = [NVCC, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", tmp] + objs + [
+    cmd = [NVCC, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", tmp] + objs + [
         "-cudart", "static", "-ccbin", "/usr/bin/g++",
                                                   "-Xlinker", "--no-undefined"]
     r = subprocess.run(cmd, capture_output=True, text=True)

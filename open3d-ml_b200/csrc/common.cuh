@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for the sm_100a kernels of libo3dml_b200.
+// common.cuh -- shared helpers for the sm_90a kernels of libo3dml_b200.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -36,7 +36,7 @@ extern "C" void o3dml_count_launches(int n);  // kernels enqueued (bench.py gpu_
 
 namespace o3dml {
 
-constexpr int kNumSMs = 148;  // B200 (fallback when the attribute query fails)
+constexpr int kNumSMs = 132;  // H100 SXM (fallback when the attribute query fails)
 
 // The opt-in dynamic shared-memory size is a per-device function attribute: `static bool configured` guards set it on
 // the first device only, so a process that drives two GPUs failed on the second.  One bit per device ordinal.
@@ -109,8 +109,7 @@ __device__ __forceinline__ int64_t load_index(const void* p, int64_t i, int is64
 
 // The same load with the result left untouched in two 32-bit words: a software-pipelined gather loads the index of a
 // later tile and must not compute anything from it before that tile comes up (the sign extension / select of
-// load_index is scheduled right behind the load and waits for it: 13-19 % of the stall samples of the LFA kernels
-// were on that one instruction, profiles/r02_lfa_stalls.md).  index_value() resolves it at the point of use.
+// load_index is scheduled right behind the load and waits for it).  index_value() resolves it at the point of use.
 struct RawIndex {
     int lo, hi;
 };
@@ -127,17 +126,10 @@ __device__ __forceinline__ int64_t index_value(const RawIndex& r, int is64) {
     return is64 ? (int64_t)(((uint64_t)(uint32_t)r.hi << 32) | (uint64_t)(uint32_t)r.lo) : (int64_t)r.lo;
 }
 
-// (d0, d1) += a * (b0, b1) as ONE packed instruction (sm_100 FFMA2: `FFMA2 R, R.F32, UR.F32x2, R.F32x2` -- the scalar
-// multiplicand is broadcast, the weight pair comes from a uniform-register pair loaded from the constant bank).  Two
-// independent IEEE fp32 FMAs: bit-identical to two FFMA.  lfa16c_kernel is issue bound (73-76 % of the issue slots,
-// FMA pipe 47-50 %, profiles/r02_lfa_ncu_full.md): halving the FMA instructions of its three small products is the lever.
+// (d0, d1) += a * (b0, b1): two independent IEEE fp32 FMAs (sm_90 has no packed fp32 FMA).
 __device__ __forceinline__ void ffma2(float& d0, float& d1, float a, float b0, float b1) {
-    uint64_t av, bv, cv;
-    asm("mov.b64 %0, {%1, %1};" : "=l"(av) : "f"(a));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(bv) : "f"(b0), "f"(b1));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(cv) : "f"(d0), "f"(d1));
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(cv) : "l"(av), "l"(bv));
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(d0), "=f"(d1) : "l"(cv));
+    d0 = fmaf(a, b0, d0);
+    d1 = fmaf(a, b1, d1);
 }
 
 // 2^x as ONE MUFU (ex2.approx.ftz, relative error 2^-22).  Softmax weights are taken as

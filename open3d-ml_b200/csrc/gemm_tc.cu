@@ -1,13 +1,12 @@
-// gemm_tc.cu -- the gathered GEMM / implicit-GEMM convolution of gemm.cu on the tcgen05 tensor cores,
-// round-2 design: 3xTF32 split, operands staged by the TMA engine.
+// gemm_tc.cu -- the gathered GEMM / implicit-GEMM convolution of gemm.cu on the Hopper tensor cores (wgmma):
+// 3xTF32 split, operands staged by the TMA engine.
 //
-//   D[128 x BN] = A[128 x K] * W[K x BN], fp32 in / fp32 out, accumulated in TMEM.
+//   D[128 x BN] = A[128 x K] * W[K x BN], fp32 in / fp32 out, accumulated in registers.
 //
-// Precision.  kind::tf32 keeps fp32's exponent, so -- unlike the fp16 split of round 1 -- no range
-// pass, no power-of-two scaling and no clamp are needed.  x = hi + lo with hi = x & 0xFFFFE000
-// (the 10 explicit mantissa bits TF32 keeps) and lo = x - hi (exact in fp32, <= 13 bits of which the
-// tensor core keeps 11): A*W ~= Ah*Wh + Ah*Wl + Al*Wh, relative error ~2^-21 per product, i.e. the
-// same 22 bits the fp16 split delivered (tests/test_split_numerics.py emulates it on the CPU).
+// Precision.  TF32 keeps fp32's exponent, so no range pass, no power-of-two scaling and no clamp are
+// needed.  x = hi + lo with hi = x & 0xFFFFE000 (the 10 explicit mantissa bits TF32 keeps) and lo = x - hi
+// (exact in fp32, <= 13 bits of which the tensor core keeps 11): A*W ~= Ah*Wh + Ah*Wl + Al*Wh, relative
+// error ~2^-21 per product (tests/test_split_numerics.py emulates it on the CPU).
 // The weight side is split by the host (round-to-nearest, _lib.pack_linear).
 //
 // Data movement.  The raw fp32 A slice (128 rows x 32 channels = 128 B per row) IS the hi operand:
@@ -18,21 +17,14 @@
 //   * gathered sources (index / batch-relative index / shadow rows) by 16-byte cp.async into the same
 //     128-byte-swizzled layout,
 //   * the weight slices (hi and lo image) by two more tensor copies.
-// The 8 converter warps then only run  hi = x & mask, lo = x - hi  on their row (45 instructions per
-// thread and slice against 357 + 686 in round 1) and store both parts into TENSOR MEMORY
-// (tcgen05.st): the MMAs take A from TMEM (.kind::tf32 [d], [a], b-desc) and only W from shared memory.
-// Why: an SS-mode 128x128x8 MMA reads 8 KB of shared memory in its 64 cycles, i.e. it saturates the
-// 128 B/clk shared-memory port on its own; the first round-2 version (A hi/lo rewritten in shared
-// memory) measured ~1 500 cycles per slice because the TMA fills (48 KB), the converter traffic (48 KB)
-// and the operand reads (96 KB) all queue on that port.  With A in TMEM a slice moves 48 KB of fills,
-// 16 KB of converter reads and 48 KB of W reads: 875 cycles against 768 of MMA issue.
+// The two consumer warpgroups (64 rows each) read their A fragments straight from the swizzled tile into
+// registers, split them there (hi = x & mask, lo = x - hi) and issue register-A wgmma against the W hi / lo
+// tiles in shared memory: the split never goes back to shared memory.
 // Shared-memory layout: K-major, SWIZZLE_128B (row r, 16-byte chunk c at r*128 + ((c ^ (r & 7)) << 4)),
-// UMMA descriptors with SBO = 1024, K advanced by +32 B per MMA (K = 8 TF32).
-// TMEM layout: columns [0, 2 BN) two accumulator buffers, then per stage 32 columns of A-hi and 32 of
-// A-lo (lane = row, column = k: the M = 128 A-fragment layout of the TS-mode MMA).
+// descriptors with SBO = 1024, K advanced by +32 B per wgmma (K = 8 TF32).
 //
-// TMEM accumulation truncates (measured round 1), hence every GT_FLUSH slices the accumulator is folded
-// into fp32 registers with round-to-nearest adds while the next chunk runs in the other TMEM buffer.
+// Every GT_FLUSH slices the wgmma accumulator is folded into a second fp32 register set with
+// round-to-nearest adds, so that long products do not rely on the tensor core's internal accumulation.
 #include "../../include/o3dml_b200.h"
 #include "common.cuh"
 #include "tc.cuh"
@@ -42,16 +34,12 @@
 
 namespace o3dml {
 
-#ifdef O3DML_DEBUG_TIMING
-__device__ long long g_gt_dbg[8192];
-#endif
-
 constexpr int GT_ROWS = 128;
 constexpr int GT_KS = 32;        // fp32 channels per k-slice (= one 128-byte swizzle row)
-constexpr int GT_FLUSH = 4;      // k-slices (128 channels = 48 accumulating MMAs) per TMEM accumulation chunk
+constexpr int GT_FLUSH = 4;      // k-slices (128 channels = 48 accumulating MMAs) per register accumulation chunk
 constexpr int GT_MAX_SRC = 3;
-constexpr int GT_CONV_THREADS = 256;   // warps 0-7: converters + flush + epilogue
-constexpr int GT_LOADERS = 128;        // warps 10-13 (GATHER kernels only)
+constexpr int GT_CONV_THREADS = 256;   // warps 0-7: the two consumer warpgroups
+constexpr int GT_LOADERS = 128;        // warps 8-11 (GATHER kernels only)
 constexpr int GT_A_BYTES = GT_ROWS * 128;
 
 struct GtSrc {
@@ -116,11 +104,6 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
 // TMA tiled loads (cp.async.bulk.tensor), completion counted in bytes on the mbarrier
 __device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
     asm volatile(
@@ -141,95 +124,38 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
-// K-major SWIZZLE_128B operand descriptor: rows of 128 B, 8-row groups 1024 B apart (cute::UMMA::SmemDescriptor:
-// start[0,14) lbo[16,30)=1 sbo[32,46)=64 version[46,48)=1 layout_type[61,64)=2)
-__device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t saddr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr >> 4) & 0x3fffu);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-// kind::tf32 instruction descriptor: c_format[4,6)=1 (fp32), a_format[7,10)=b_format[10,13)=2 (TF32), both K-major
-__host__ __device__ constexpr uint32_t idesc_tf32(int M, int N) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-// TS mode: A from tensor memory (lane = row, one column per TF32 element), B from shared memory
-__device__ __forceinline__ void umma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// same, W descriptor passed as its two 32-bit words (only the low word varies between MMAs)
-__device__ __forceinline__ void umma_tf32_ts2(uint32_t tmem_d, uint32_t tmem_a, uint32_t bdesc_lo, uint32_t bdesc_hi,
-                                              uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b64 d;\n\t"
-        "mov.b64 d, {%2, %3};\n\t"
-        "setp.ne.b32 p, %5, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], d, %4, p;\n\t}" ::"r"(tmem_d),
-        "r"(tmem_a), "r"(bdesc_lo), "r"(bdesc_hi), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// registers -> TMEM: 32 lanes x 32 bit, 16 consecutive columns per thread (lane = 32 * (warp % 4) + lane id)
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* r) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// LITE: two stages and 256 TMEM columns instead of 4 - 6 stages and all 512, so that TWO CTAs share an SM.  A short
-// product (K <= 512) is prologue (3.1 k cycles) + epilogue (3.5 - 6.4 k) around 0.7 k per 32-channel slice: with one CTA
-// per SM the tensor pipe and the TMA unit idle through both; a sibling CTA fills them.
+// LITE: two stages instead of 4 - 6, so that TWO CTAs share an SM.  A short product (K <= 512) is mostly
+// prologue and epilogue around a few 32-channel slices: with one CTA per SM the tensor pipe and the TMA unit
+// idle through both; a sibling CTA fills them.
 template <int BN, bool LITE = false>
 struct GtCfg {
     static constexpr int B_BYTES = BN * 128;                       // one of hi/lo per stage
     static constexpr int STAGE = GT_A_BYTES + 2 * B_BYTES;         // raw A + W hi + W lo; multiples of 1024
-    // bytes in flight = L2 bandwidth x latency: at BN = 64 a slice is consumed every ~430 cycles and takes ~2 500 to
-    // arrive, i.e. ~190 KB must be outstanding (5 x 32 KB stages measured 648 cycles per slice, TMA-latency bound)
     static constexpr int STAGES = LITE ? 2 : BN >= 128 ? 4 : 6;
-    static constexpr int A_COL0 = 2 * BN;                          // TMEM: accumulators first, then the A slots
-    static constexpr int TMEM_COLS = LITE ? 256 : 512;             // 2 * BN + STAGES * 64 <= TMEM_COLS, power of two
-    static_assert(2 * BN + STAGES * 64 <= TMEM_COLS, "TMEM budget");
     static_assert(!LITE || BN <= 64, "LITE is for the narrow tiles");
     static constexpr int TAIL = GT_MAX_SRC * GT_ROWS * 8 + GT_ROWS * 8 + 2 * BN * 4 + 256;
     static constexpr size_t SMEM = (size_t)STAGES * STAGE + TAIL + 1024;
+    static_assert(SMEM <= 227 * 1024, "shared memory budget of one H100 CTA");
     static_assert((size_t)STAGES * STAGE >= (size_t)GT_ROWS * (BN + 4) * 4, "epilogue staging lives in the stages");
 };
 
 // Pipeline (per CTA, one [128 x BN] output tile, k-slices of 32 channels through a ring of stages):
-//   warps 0-7     converters: wait full[stage], split their row of the raw A tile into (hi, lo), tcgen05.st
-//                 into the stage's TMEM slot, arrive conv[stage]; fold finished TMEM chunks into registers;
-//                 epilogue (TMEM -> BN /
-//                 residual / activation -> shared-memory staged, row-coalesced stores)
-//   warp 8        MMA issuer: waits conv[stage], one elected lane issues 12 tcgen05.mma (4 k-steps x 3
-//                 products), tcgen05.commit -> empty[stage] (+ chunk[] at chunk ends); owns the TMEM allocation
-//   warp 9        TMA producer (one elected lane): waits empty[stage], arms full[stage] with the byte count
-//                 and issues the weight-slice copies and -- for identity sources / convolution taps -- the A copy
-//   warps 10-13   (GATHER kernels) loaders: 16-byte cp.async of gathered rows into the swizzled A tile,
-//                 cp.async.mbarrier.arrive on full[stage]
+//   warps 0-7     two consumer warpgroups (rows 0-63, 64-127): wait full[stage], load and split the A
+//                 fragments of their rows, issue 12 wgmma (4 k-steps x 3 products), wait for them, arrive
+//                 empty[stage]; fold the accumulator every GT_FLUSH slices; epilogue (BN / residual /
+//                 activation through shared-memory staging, row-coalesced stores)
+//   warp 8 lane 0 TMA producer: waits empty[stage], arms full[stage] with the byte count and issues the
+//                 weight-slice copies and -- for identity sources / convolution taps -- the A copy
+//   warps 8-11    (GATHER kernels, lane 0 of warp 8 included) loaders: 16-byte cp.async of gathered rows into the
+//                 swizzled A tile, cp.async.mbarrier.arrive on full[stage].  Sharing warp 8 keeps the block at 384
+//                 threads: 168 registers per thread, which the 2 x BN / 2 accumulator and fold registers need at BN = 128
+constexpr int GT_PRODUCER_WARP = 8;
+
+template <bool GATHER>
+__host__ __device__ constexpr int gt_threads() { return GT_CONV_THREADS + (GATHER ? GT_LOADERS : 32); }
+
 template <int BN, bool GATHER, bool LITE>
-__global__ void __launch_bounds__(GATHER ? 448 : 320, LITE ? 2 : 1)
+__global__ void __launch_bounds__(gt_threads<GATHER>(), LITE ? 2 : 1)
 gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
     using C = GtCfg<BN, LITE>;
     constexpr int S = C::STAGES;
@@ -242,10 +168,7 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
     float* s_shift = s_scale + BN;                                                   // [BN]
     uint64_t* mbar = reinterpret_cast<uint64_t*>(s_shift + BN);
     uint64_t* full_bar = mbar;                // [S] operands of the slice landed
-    uint64_t* conv_bar = mbar + S;            // [S] A tile split + fenced
-    uint64_t* empty_bar = mbar + 2 * S;       // [S] MMAs that read the stage are done
-    uint64_t* chunk_bar = mbar + 3 * S;       // [2] accumulation chunk complete
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(mbar + 3 * S + 2);
+    uint64_t* empty_bar = mbar + S;           // [S] the consumers are done with the stage
 
     const int tid = threadIdx.x;
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // warp-uniform for the compiler
@@ -260,10 +183,6 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
         oy0 = (t / p.tiles_x) * p.PH;
         ox0 = (t % p.tiles_x) << p.lpw;
     }
-#ifdef O3DML_DEBUG_TIMING
-    const bool dbg = blockIdx.x == 0 && blockIdx.y == 0;
-    if (dbg && tid == 0) g_gt_dbg[4000] = clock64();
-#endif
 
     // ---- per-row bookkeeping
     for (int m = tid; m < GT_ROWS; m += blockDim.x) {
@@ -293,67 +212,20 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
 #pragma unroll
         for (int i = 0; i < S; ++i) {
             tc::mbar_init(&full_bar[i], GATHER ? 1 + GT_LOADERS : 1);
-            tc::mbar_init(&conv_bar[i], GT_CONV_THREADS);
-            tc::mbar_init(&empty_bar[i], 1);
+            tc::mbar_init(&empty_bar[i], GT_CONV_THREADS);
         }
-        tc::mbar_init(&chunk_bar[0], 1);
-        tc::mbar_init(&chunk_bar[1], 1);
         tc::fence_mbar_init();
     }
     __syncthreads();
-    if (warp == 8) tc::tmem_alloc<C::TMEM_COLS>(tmem_slot);
-    tc::tc_fence_before();
-    __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
 
     const int nsl = p.Kpad / GT_KS;
-    const int last_chunk = (nsl - 1) / GT_FLUSH;
     const uint32_t stage0 = tc::smem_u32(stages);
 
-    if (warp == 8) {
-        // ================================================================= MMA issuer
-        constexpr uint32_t idesc = idesc_tf32(GT_ROWS, BN);
-        // descriptor words (smem_desc_sw128): high = sbo 1024 B | version 1 | SWIZZLE_128B; low = start >> 4 | lbo 1
-        constexpr uint32_t DESC_HI = (1024u >> 4) | (1u << 14) | (2u << 29);
-        const uint32_t desc_lo0 = (((stage0 + GT_A_BYTES) >> 4) & 0x3fffu) | (1u << 16);
-        for (int s = 0; s < nsl; ++s) {
-            const int stage = s % S, use = s / S, chunk = s / GT_FLUSH;
-#ifdef O3DML_DEBUG_TIMING
-            const long long tm0 = clock64();
-#endif
-            tc::mbar_wait(&conv_bar[stage], use & 1);
-            tc::tc_fence_after();
-#ifdef O3DML_DEBUG_TIMING
-            const long long tm1 = clock64();
-#endif
-            if (elect_one()) {
-                // only the 14-bit start-address field of the W descriptors changes: one add per MMA
-                // (a lone thread retires ~1 dependent instruction per 4-6 cycles; rebuilding the 64-bit
-                // descriptors cost 35-45 cycles per MMA, measured: 414 / 531 cycles to issue 12 MMAs)
-                const uint32_t bh_lo = desc_lo0 + (uint32_t)stage * (C::STAGE >> 4);
-                const uint32_t bl_lo = bh_lo + (C::B_BYTES >> 4);
-                const uint32_t a_hi = tmem + (uint32_t)(C::A_COL0 + stage * 64);
-                const uint32_t acc = tmem + (uint32_t)((chunk & 1) * BN);
-                const uint32_t first_acc = (s % GT_FLUSH) != 0;
-#pragma unroll
-                for (int ks = 0; ks < GT_KS / 8; ++ks) {        // K = 8 TF32 = 8 TMEM columns / 32 bytes of W per MMA
-                    umma_tf32_ts2(acc, a_hi + ks * 8, bh_lo + ks * 2, DESC_HI, idesc, ks == 0 ? first_acc : 1u);
-                    umma_tf32_ts2(acc, a_hi + ks * 8, bl_lo + ks * 2, DESC_HI, idesc, 1u);
-                    umma_tf32_ts2(acc, a_hi + 32 + ks * 8, bh_lo + ks * 2, DESC_HI, idesc, 1u);
-                }
-                tc::umma_commit(&empty_bar[stage]);
-                if ((s % GT_FLUSH) == GT_FLUSH - 1 || s == nsl - 1) tc::umma_commit(&chunk_bar[chunk & 1]);
-#ifdef O3DML_DEBUG_TIMING
-                if (dbg && s < 300) { g_gt_dbg[2000 + 3 * s] = tm0; g_gt_dbg[2001 + 3 * s] = tm1; g_gt_dbg[2002 + 3 * s] = clock64(); }
-#endif
-            }
-            __syncwarp();
-        }
-    } else if (warp == 9) {
-        // ================================================================= TMA producer
-        if (elect_one()) {
-            tma_prefetch_desc(&p.mapB);
+    if (warp >= GT_PRODUCER_WARP) {
+        // ================================================================= TMA producer (+ gather loaders)
+        const int rt = tid - GT_CONV_THREADS;                   // loader index; 0 is also the producer
+        if (GATHER || rt == 0) {
+            if (rt == 0) tma_prefetch_desc(&p.mapB);
             const int spt = p.mode == 1 ? p.C / GT_KS : 1;      // slices per convolution tap
             int sidx = 0;
             for (int sl = 0; sl < nsl; ++sl) {
@@ -366,189 +238,102 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
                     a_tma = p.src[sidx].index == nullptr;
                 }
                 const uint32_t ah = stage0 + (uint32_t)stage * C::STAGE;
-                const uint32_t bh = ah + GT_A_BYTES;
-                mbar_arrive_expect_tx(&full_bar[stage], 2 * C::B_BYTES + (a_tma ? GT_A_BYTES : 0));
-                tma_load_2d(bh, &p.mapB, k0, col0, &full_bar[stage]);
-                tma_load_2d(bh + C::B_BYTES, &p.mapB, k0, p.Npad + col0, &full_bar[stage]);
-                if (a_tma) {
-                    if (p.mode == 0) {
-                        tma_load_2d(ah, &p.mapA[sidx], k0 - p.koff[sidx], (int)row0, &full_bar[stage]);
-                    } else {
-                        const int tap = sl / spt, cc = (sl - tap * spt) * GT_KS;
-                        const int dy = tap / 3, dx = tap - dy * 3;
-                        if (p.stride == 1) {
-                            tma_load_4d(ah, &p.mapA[0], cc, ox0 - 1 + dx, oy0 - 1 + dy, cb, &full_bar[stage]);
-                        } else {   // input pixel 2*o - 1 + d: odd parity for d = 0 (coordinate o - 1) and d = 2 (o)
-                            const int py = dy != 1, px = dx != 1;
-                            tma_load_4d(ah, &p.mapA[py * 2 + px], cc, ox0 - (dx == 0), oy0 - (dy == 0), cb,
-                                        &full_bar[stage]);
+                if (rt == 0) {
+                    const uint32_t bh = ah + GT_A_BYTES;
+                    mbar_arrive_expect_tx(&full_bar[stage], 2 * C::B_BYTES + (a_tma ? GT_A_BYTES : 0));
+                    tma_load_2d(bh, &p.mapB, k0, col0, &full_bar[stage]);
+                    tma_load_2d(bh + C::B_BYTES, &p.mapB, k0, p.Npad + col0, &full_bar[stage]);
+                    if (a_tma) {
+                        if (p.mode == 0) {
+                            tma_load_2d(ah, &p.mapA[sidx], k0 - p.koff[sidx], (int)row0, &full_bar[stage]);
+                        } else {
+                            const int tap = sl / spt, cc = (sl - tap * spt) * GT_KS;
+                            const int dy = tap / 3, dx = tap - dy * 3;
+                            if (p.stride == 1) {
+                                tma_load_4d(ah, &p.mapA[0], cc, ox0 - 1 + dx, oy0 - 1 + dy, cb, &full_bar[stage]);
+                            } else {   // input pixel 2*o - 1 + d: odd parity for d = 0 (coordinate o - 1) and d = 2 (o)
+                                const int py = dy != 1, px = dx != 1;
+                                tma_load_4d(ah, &p.mapA[py * 2 + px], cc, ox0 - (dx == 0), oy0 - (dy == 0), cb,
+                                            &full_bar[stage]);
+                            }
                         }
                     }
                 }
-            }
-        }
-    } else if (GATHER && warp >= 10) {
-        // ================================================================= gather loaders
-        const int rt = tid - 320;
-        int sidx = 0;
-        for (int sl = 0; sl < nsl; ++sl) {
-            const int stage = sl % S, use = sl / S;
-            if (use >= 1) tc::mbar_wait(&empty_bar[stage], (use - 1) & 1);
-            const int k0 = sl * GT_KS;
-            while (sidx + 1 < p.nsrc && k0 >= p.koff[sidx + 1]) ++sidx;
-            if (p.src[sidx].index != nullptr) {
-                const uint32_t ah = stage0 + (uint32_t)stage * C::STAGE;
-                const int kloc = k0 - p.koff[sidx];
-                const int cs = p.src[sidx].channels;
+                if (!GATHER) continue;
+                if (!a_tma) {
+                    const int kloc = k0 - p.koff[sidx];
+                    const int cs = p.src[sidx].channels;
 #pragma unroll
-                for (int j = 0; j < (GT_ROWS * 8) / GT_LOADERS; ++j) {     // 8 consecutive lanes = one row's 128 B
-                    const int item = rt + j * GT_LOADERS;
-                    const int m = item >> 3, c = item & 7;
-                    const float* base = rowptr[sidx * GT_ROWS + m];
-                    const int kk = kloc + c * 4;
-                    const bool ok = base != nullptr && kk < cs;
-                    cp_async16(ah + (uint32_t)m * 128u + (uint32_t)((c ^ (m & 7)) << 4),
-                               ok ? (const void*)(base + kk) : (const void*)p.src[0].data, ok ? 16 : 0);
+                    for (int j = 0; j < (GT_ROWS * 8) / GT_LOADERS; ++j) {     // 8 consecutive lanes = one row's 128 B
+                        const int item = rt + j * GT_LOADERS;
+                        const int m = item >> 3, c = item & 7;
+                        const float* base = rowptr[sidx * GT_ROWS + m];
+                        const int kk = kloc + c * 4;
+                        const bool ok = base != nullptr && kk < cs;
+                        cp_async16(ah + (uint32_t)m * 128u + (uint32_t)((c ^ (m & 7)) << 4),
+                                   ok ? (const void*)(base + kk) : (const void*)p.src[0].data, ok ? 16 : 0);
+                    }
+                    cp_async_arrive(&full_bar[stage]);
+                } else {
+                    mbar_arrive(&full_bar[stage]);
                 }
-                cp_async_arrive(&full_bar[stage]);
-            } else {
-                mbar_arrive(&full_bar[stage]);
             }
         }
-    } else if (warp < 8) {
-        // ================================================================= converters + flush + epilogue
-        const int grp = warp >> 2;                     // column half
-        const int rt = (warp & 3) * 32 + (tid & 31);   // output row = TMEM lane this thread can read
-        const uint32_t tmem_lane = tmem + ((uint32_t)((warp & 3) * 32) << 16);
-        constexpr int HB = BN / 2 < 16 ? 16 : BN / 2;  // columns owned by a group
-        constexpr int NQ = HB / 16;
-        float racc[HB];
+    } else if (warp < GT_PRODUCER_WARP) {
+        // ================================================================= consumers + fold + epilogue
+        const int lane = tid & 31, g = lane >> 2, t = lane & 3;
+        const int r0 = (warp >> 2) * 64 + (warp & 3) * 16 + g;      // fragment rows r0 and r0 + 8
+        constexpr int ND = BN / 2;                                  // accumulator registers per thread
+        float acc[ND], racc[ND];
 #pragma unroll
-        for (int i = 0; i < HB; ++i) racc[i] = 0.f;
-        const bool owns_cols = (BN >= 32) || grp == 0;
-        const int colbase = (BN >= 32) ? grp * HB : 0;
-        uint32_t ph_chunk[2] = {0, 0};
-        int next_flush = 0;                            // first chunk not folded yet
-        auto fold = [&](int chunk) {                   // racc += accumulator of `chunk` (RN adds)
-            tc::mbar_wait(&chunk_bar[chunk & 1], ph_chunk[chunk & 1]);
-            ph_chunk[chunk & 1] ^= 1;
-            tc::tc_fence_after();
-            if (owns_cols) {
-                uint32_t vr[NQ][16];       // all of this thread's columns behind one wait
-#pragma unroll
-                for (int q = 0; q < NQ; ++q) tc::tmem_ld16_issue(tmem_lane + (chunk & 1) * BN + colbase + q * 16, vr[q]);
-                tc::tmem_ld_wait();
-#pragma unroll
-                for (int q = 0; q < NQ; ++q)
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) racc[q * 16 + j] += tc::tmem_val(vr[q][j]);
-            }
-            tc::tc_fence_before();
-        };
+        for (int i = 0; i < ND; ++i) { acc[i] = 0.f; racc[i] = 0.f; }
         for (int s = 0; s < nsl; ++s) {
             const int stage = s % S, use = s / S;
-            // a chunk whose last slice is S slices behind has certainly drained (its stage was reused): fold it then,
-            // and in any case before slice (chunk + 2) * GT_FLUSH reuses its TMEM buffer (the fold waits if it must)
-            constexpr int LAG = (S - 1 < GT_FLUSH) ? S - 1 : GT_FLUSH;
-            while (next_flush < last_chunk && s >= (next_flush + 1) * GT_FLUSH + LAG) fold(next_flush++);
-#ifdef O3DML_DEBUG_TIMING
-            const long long tq0 = clock64();
-#endif
             tc::mbar_wait(&full_bar[stage], use & 1);
-            tc::tc_fence_after();       // the MMAs that read this stage's TMEM slot completed (empty -> TMA -> full)
-#ifdef O3DML_DEBUG_TIMING
-            const long long tq1 = clock64();
-#endif
-            // this thread's row, k-half `grp` (4 of the row's 8 swizzled 16-byte chunks) -> hi / lo -> TMEM
-            const uint8_t* a_row = stages + (size_t)stage * C::STAGE + (size_t)rt * 128;
-            uint32_t hi[16], lo[16];
+            // A fragments of this thread (m16n8k8 TF32: (r0, t), (r0+8, t), (r0, t+4), (r0+8, t+4) per k-step),
+            // read from the swizzled tile: the 32 lanes of a warp hit 32 different banks
+            const uint8_t* a_tile = stages + (size_t)stage * C::STAGE;
+            uint32_t ah[GT_KS / 8][4], al[GT_KS / 8][4];
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const int cch = grp * 4 + j;
-                const uint4 v = *reinterpret_cast<const uint4*>(a_row + (((cch ^ (rt & 7))) << 4));
-                const uint32_t x[4] = {v.x, v.y, v.z, v.w};
+            for (int ks = 0; ks < GT_KS / 8; ++ks)
 #pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    hi[4 * j + u] = x[u] & 0xFFFFE000u;
-                    lo[4 * j + u] = __float_as_uint(__uint_as_float(x[u]) - __uint_as_float(hi[4 * j + u]));
+                for (int e = 0; e < 4; ++e) {
+                    const int r = r0 + (e & 1) * 8, k = ks * 8 + t + (e >> 1) * 4;
+                    const uint32_t x = *reinterpret_cast<const uint32_t*>(
+                        a_tile + r * 128 + (((k >> 2) ^ (r & 7)) << 4) + (k & 3) * 4);
+                    tc::split_tf32(x, ah[ks][e], al[ks][e]);
                 }
+            const uint32_t bh = stage0 + (uint32_t)stage * C::STAGE + GT_A_BYTES, bl = bh + C::B_BYTES;
+            const uint32_t first = (s % GT_FLUSH) != 0;            // 0: this slice starts a new accumulation chunk
+            tc::wgmma_fence();
+#pragma unroll
+            for (int ks = 0; ks < GT_KS / 8; ++ks) {        // K = 8 TF32 = 32 bytes of W per wgmma
+                tc::wgmma_tf32_rs<BN>(acc, ah[ks], tc::smem_desc_sw128(bh + ks * 32), ks == 0 ? first : 1u);
+                tc::wgmma_tf32_rs<BN>(acc, ah[ks], tc::smem_desc_sw128(bl + ks * 32), 1u);
+                tc::wgmma_tf32_rs<BN>(acc, al[ks], tc::smem_desc_sw128(bh + ks * 32), 1u);
             }
-            const uint32_t a_slot = tmem_lane + (uint32_t)(C::A_COL0 + stage * 64 + grp * 16);
-            tmem_st16(a_slot, hi);
-            tmem_st16(a_slot + 32, lo);
-            tmem_st_wait();
-            tc::tc_fence_before();
-            mbar_arrive(&conv_bar[stage]);
-#ifdef O3DML_DEBUG_TIMING
-            if (dbg && tid == 0 && s < 450) {
-                g_gt_dbg[4 * s + 0] = tq0; g_gt_dbg[4 * s + 1] = tq1; g_gt_dbg[4 * s + 2] = clock64();
+            tc::wgmma_commit();
+            tc::wgmma_wait_all();
+            mbar_arrive(&empty_bar[stage]);
+            if ((s % GT_FLUSH) == GT_FLUSH - 1 || s == nsl - 1) {
+#pragma unroll
+                for (int i = 0; i < ND; ++i) racc[i] += acc[i];
             }
-#endif
         }
-        while (next_flush < last_chunk) fold(next_flush++);
-        tc::mbar_wait(&chunk_bar[last_chunk & 1], ph_chunk[last_chunk & 1]);
-        tc::tc_fence_after();
-#ifdef O3DML_DEBUG_TIMING
-        if (dbg && tid == 0) g_gt_dbg[4002] = clock64();
-#endif
-        // ---- epilogue: thread = output row, this group's column half, 16 columns at a time.
-        // Row-major and pixel-shuffle outputs are staged through the (now dead) pipeline stages so that the
-        // global stores are whole rows written by consecutive lanes.
-        const int64_t n = rown[rt];
+        // ---- epilogue: the tile goes through the (now dead) pipeline stages so that the global stores are
+        // whole rows (row-major / pixel shuffle) or whole pixel runs (NCHW) written by consecutive lanes
+        named_bar_sync(1, GT_CONV_THREADS);                          // every consumer is done with the stages
         constexpr int SLD = BN + 4;                                  // staging row stride (floats)
         float* stg = reinterpret_cast<float*>(stages);
-        const bool staged = p.out_mode == 0 || (p.out_mode == 2 && (p.dC & 3) == 0);
-        if (owns_cols) {
 #pragma unroll
-            for (int q = 0; q < NQ; ++q) {
-                const int c0 = colbase + 16 * q;
-                float v[16];
-                tc::tmem_ld16(tmem_lane + (last_chunk & 1) * BN + c0, v);   // warp-collective
-                const int cbase = col0 + c0;
-                if (n < 0 || cbase >= p.Cout) continue;
-                // staged outputs get the residual and the activation in the row-coalesced copy-out below
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    float x = fmaf(v[j] + racc[q * 16 + j], s_scale[c0 + j], s_shift[c0 + j]);
-                    if (!staged) {
-                        const int c = cbase + j;
-                        if (p.residual && c < p.Cout) x += p.residual[(size_t)n * p.res_ld + c];
-                        x = apply_act(x, p.act, p.slope);
-                    }
-                    v[j] = x;
-                }
-                if (staged) {
-#pragma unroll
-                    for (int u = 0; u < 4; ++u)
-                        *reinterpret_cast<float4*>(stg + rt * SLD + c0 + 4 * u) =
-                            make_float4(v[4 * u], v[4 * u + 1], v[4 * u + 2], v[4 * u + 3]);
-                } else if (p.out_mode == 1) {
-                    const int64_t b = n / p.plane, pix = n % p.plane;
-#pragma unroll
-                    for (int j = 0; j < 16; ++j)
-                        if (cbase + j < p.Cout) p.out[((size_t)b * p.Cout + cbase + j) * p.plane + pix] = v[j];
-                } else {
-                    const int64_t per = (int64_t)p.dIH * p.dIW;
-                    const int64_t b = n / per;
-                    const int r = (int)(n % per);
-                    const int iy = r / p.dIW, ix = r % p.dIW;
-                    const int OWd = p.dIW * p.ds;
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const int c = cbase + j;
-                        if (c < p.Cout) {
-                            const int sub = c / p.dC, co = c - sub * p.dC;
-                            const int dy = sub / p.ds, dx = sub - dy * p.ds;
-                            const size_t opix = ((size_t)b * p.dIH * p.ds + (size_t)iy * p.ds + dy) * OWd +
-                                                (size_t)ix * p.ds + dx;
-                            p.out[opix * p.out_ld + co] = v[j];
-                        }
-                    }
-                }
-            }
+        for (int i = 0; i < ND; i += 2) {
+            const int r = r0 + ((i >> 1) & 1) * 8, c = (i >> 2) * 8 + 2 * t;
+            *reinterpret_cast<float2*>(stg + r * SLD + c) =
+                make_float2(fmaf(racc[i], s_scale[c], s_shift[c]), fmaf(racc[i + 1], s_scale[c + 1], s_shift[c + 1]));
         }
+        named_bar_sync(2, GT_CONV_THREADS);
+        const bool staged = p.out_mode == 0 || (p.out_mode == 2 && (p.dC & 3) == 0);
         if (staged) {
-            named_bar_sync(2, GT_CONV_THREADS);                        // the 8 epilogue warps
             constexpr int LPR = BN / 4;                                // lanes per output row
             const int c = (tid % LPR) * 4, cg = col0 + c;
             const bool vec = (p.out_ld & 3) == 0 && (reinterpret_cast<uintptr_t>(p.out) & 15) == 0;
@@ -595,14 +380,33 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
                     }
                 }
             }
+        } else {
+            // NCHW planes and pixel shuffles with a channel count that is not a multiple of 4: one element per
+            // thread, consecutive threads on consecutive rows (= consecutive pixels of an NCHW plane)
+            for (int idx = tid; idx < GT_ROWS * BN; idx += GT_CONV_THREADS) {
+                const int r = idx % GT_ROWS, cl = idx / GT_ROWS, c = col0 + cl;
+                const int64_t n = rown[r];
+                if (n < 0 || c >= p.Cout) continue;
+                float x = stg[r * SLD + cl];
+                if (p.residual) x += p.residual[(size_t)n * p.res_ld + c];
+                x = apply_act(x, p.act, p.slope);
+                if (p.out_mode == 1) {
+                    const int64_t b = n / p.plane, pix = n % p.plane;
+                    p.out[((size_t)b * p.Cout + c) * p.plane + pix] = x;
+                } else {
+                    const int64_t per = (int64_t)p.dIH * p.dIW;
+                    const int64_t b = n / per;
+                    const int rr = (int)(n % per);
+                    const int iy = rr / p.dIW, ix = rr % p.dIW;
+                    const int sub = c / p.dC, co = c - sub * p.dC;
+                    const int dy = sub / p.ds, dx = sub - dy * p.ds;
+                    const size_t opix = ((size_t)b * p.dIH * p.ds + (size_t)iy * p.ds + dy) * (p.dIW * p.ds) +
+                                        (size_t)ix * p.ds + dx;
+                    p.out[opix * p.out_ld + co] = x;
+                }
+            }
         }
     }
-    tc::tc_fence_before();
-    __syncthreads();
-#ifdef O3DML_DEBUG_TIMING
-    if (dbg && tid == 0) g_gt_dbg[4003] = clock64();
-#endif
-    if (warp == 8) tc::tmem_dealloc<C::TMEM_COLS>(tmem);
 }
 
 // ---- host side ---------------------------------------------------------------------------------
@@ -664,7 +468,7 @@ static int gemm_tc_launch_bn(const GemmTcParams& p, unsigned grid_x, cudaStream_
         if (dev < 64) configured |= 1ull << dev;
     }
     dim3 grid(grid_x, (unsigned)(p.Npad / BN));
-    gemm_tc_kernel<BN, GATHER, LITE><<<grid, GATHER ? 448 : 320, C::SMEM, st>>>(p);
+    gemm_tc_kernel<BN, GATHER, LITE><<<grid, gt_threads<GATHER>(), C::SMEM, st>>>(p);
     O3DML_LAUNCH_CHECK();
     o3dml_count_launches(1);
     return O3DML_OK;
@@ -696,14 +500,12 @@ static int gemm_tc_launch(GemmTcParams& p, const void* wimg, cudaStream_t st) {
         row_tiles = (p.N / ((int64_t)p.OH * p.OW)) * best_tiles;
     }
     // products of plain row sources, at most 16 k-slices long, that fill the SMs more than once as 64-column tiles run on
-    // the LITE kernels, two CTAs per SM (GtCfg).  Measured (profiles/r02_gemm_lite.md): threshold 4 / 16 / 64 / none =
-    // RandLA-Net 220.0 / 220.4 / 220.3 / 220.3, PointPillars 24.4 / 24.9 / 24.9 / 24.9, KPFCNN 48.8 / 49.1 / 48.6 / 48.1
-    // M points/s against 217.1 / 24.0 / 46.5 without; LITE for the convolutions (K = 9 C) loses (PointPillars 24.5).
+    // the LITE kernels, two CTAs per SM (GtCfg); the convolutions (K = 9 C) stay on the one-CTA-per-SM kernels
     const bool lite = p.mode == 0 && !any_gather && p.Kpad / GT_KS <= gt_lite_max_slices() &&
                       row_tiles * (p.Npad / (bn == 32 ? 32 : 64)) > gt_num_sms();
     if (lite && bn == 128) bn = 64;
     // a grid that fills less than half of the SMs (PointPillars block 3: 27 x 2 CTAs; one cloud per GPU: 6 - 88)
-    // runs as 64-column tiles instead: twice the CTAs, 12 x 36 instead of 12 x 64 MMA cycles per slice each
+    // runs as 64-column tiles instead: twice the CTAs, each with half the tensor-core work per slice
     if (bn == 128 && 2 * row_tiles * (p.Npad / 128) <= gt_num_sms()) bn = 64;
     {   // weight image: fp32 [2 * Npad][Kpad] (TF32 hi rows, then lo rows)
         const uint64_t dims[2] = {(uint64_t)p.Kpad, (uint64_t)2 * p.Npad};
@@ -888,9 +690,3 @@ extern "C" int o3dml_deconv_nhwc_tc(const float* in, int batch, int H, int W, in
     p.ds = stride; p.dIH = H; p.dIW = W; p.dC = out_channels;
     return gemm_tc_launch(p, weight_image, (cudaStream_t)stream);
 }
-
-#ifdef O3DML_DEBUG_TIMING
-extern "C" __attribute__((visibility("default"))) int o3dml_gt_debug_read(long long* host, int n) {
-    return (int)cudaMemcpyFromSymbol(host, o3dml::g_gt_dbg, sizeof(long long) * n);
-}
-#endif

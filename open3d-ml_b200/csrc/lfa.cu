@@ -18,8 +18,8 @@
 //   Wsl[BK][D]     streamed weight k-slices
 // Thread (p, cg) owns the 16 neighbour rows of point p x 4 score channels, so the
 // softmax over K and the weighted sum stay in registers.
-// FP32 SIMT version (bit-level close to the reference); the tcgen05 3xTF32
-// variant plugs into the same tiles.
+// FP32 SIMT version (bit-level close to the reference); lfa_tc.cu is the
+// tensor-core (wgmma, 3xFP16) variant with the same contract.
 #include "../../include/o3dml_b200.h"
 #include "common.cuh"
 #include <stdlib.h>
@@ -431,7 +431,7 @@ lfa16_kernel(const __grid_constant__ LfaParams p, int64_t num_groups) {
 template <int STAGE>
 static int lfa16_launch(const LfaParams& p, cudaStream_t st) {
     const int64_t groups = ceil_div<int64_t>(p.total, L16_PTS);
-    int dev = 0, sms = 148;
+    int dev = 0, sms = kNumSMs;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int64_t cap = (int64_t)sms * 4;   // resident CTAs; each walks groups with a grid stride
@@ -453,8 +453,8 @@ struct alignas(16) Lfa16W {
 constexpr int W16_W10 = 0, W16_S10 = 80, W16_T10 = 88, W16_WL2 = 96, W16_S2 = 160, W16_T2 = 168,
               W16_WS = 176, W16_BS = 432;
 
-// PF = gather pipelining over the groups a CTA walks (the un-pipelined kernel spent 23 % of its stall samples on the
-// two dependent round trips index -> coordinates / features, profiles/r02_lfa_stalls.md):
+// PF = gather pipelining over the groups a CTA walks (hides the two dependent round trips index -> coordinates /
+// features):
 //   0  none            1  the neighbour index of the next group is requested one group ahead (raw word, common.cuh)
 //   2  index two groups ahead, coordinates + feature row of the next group one group ahead (14 more registers:
 //      4 CTAs per SM instead of 5)

@@ -1,22 +1,23 @@
-// lfa_tc.cu -- RandLA-Net attentive-pooling stage on the 5th-gen tensor cores (tcgen05):
-//   neighbour gather -> LocSE encoding (+ shared MLPs) -> score GEMM on tcgen05 with the
+// lfa_tc.cu -- RandLA-Net attentive-pooling stage on the Hopper tensor cores (wgmma):
+//   neighbour gather -> LocSE encoding (+ shared MLPs) -> score GEMM on the tensor cores with the
 //   3xFP16 split (tc.cuh) -> softmax over the 16 neighbours -> weighted sum  ==> agg [N, d]
 // Same contract as lfa_pool_kernel (lfa.cu); replaces randlanet.py:521-639 as used at :667-692.
 //
-// One MMA tile = 128 neighbour rows = 8 points x 16 neighbours:
+// One tile = 128 neighbour rows = 8 points x 16 neighbours, 256 threads = two warpgroups of 64 rows:
 //   A  [128 x d]  : X = [feat[nbr] | r1 or r2], built by the CTA in shared memory directly in the
-//                   UMMA chunk-major layout (one conflict-free 16-byte store per (row, 8 channels)),
+//                   chunk-major layout (one conflict-free 16-byte store per (row, 8 channels)),
 //                   as fp16 hi/lo pairs.  In stage 2 the first half of A first holds r1 (the A
 //                   operand of the lse2 GEMM) and is then overwritten by the gathered features.
 //   B  [d x d]    : score weight, host-packed hi/lo operand image; resident in shared memory for
-//                   d <= 128, streamed through a 2-slot ring of 32-channel slices for d = 256
-//   D  [128 x d]  : fp32 in TMEM, lane = neighbour row, column = score channel
-// Epilogue: thread = one neighbour row (TMEM lane); softmax over the 16 rows of a point is a
-// half-warp reduction (redux.sync max on order-preserving ints, reduce-scatter shuffles for the
-// two sums), after which lane j of the half-warp owns output channel c0+j -> coalesced stores.
-// Stage 2 chains a second MMA (r2 = lrelu(BN(Wl2 . r1)), N = d/2) through TMEM back into A
-// (d = 16: that 8x8 product stays in registers).  The score bias is not applied: it is constant
-// over the neighbours of a point and cancels in the softmax.  CTAs are persistent over tiles.
+//                   d <= 128, copied one 32-row column block at a time for d = 256
+//   D             : 32 score columns at a time, each warpgroup's [64 x 32] block in registers (wgmma), staged
+//                   through shared memory so that a thread sees one neighbour row
+// Epilogue: thread = one neighbour row; softmax over the 16 rows of a point is a half-warp reduction
+// (redux.sync max on order-preserving ints, reduce-scatter shuffles for the two sums), after which
+// lane j of the half-warp owns output channel c0+j -> coalesced stores.
+// Stage 2 chains a second GEMM (r2 = lrelu(BN(Wl2 . r1)), N = d/2) back into A (d = 16: that 8x8 product
+// stays in registers).  The score bias is not applied: it is constant over the neighbours of a point and
+// cancels in the softmax.  CTAs are persistent over tiles.
 #include "../../include/o3dml_b200.h"
 #include "common.cuh"
 #include "tc.cuh"
@@ -26,7 +27,7 @@ namespace o3dml {
 
 constexpr int LTC_ROWS = 128;  // MMA M
 constexpr int LTC_K = 16;      // neighbours
-constexpr int LTC_SLICE = 32;  // channels per streamed weight slice
+constexpr int LTC_SB_LD = 36;  // staged accumulator row stride (floats): a 32-column block + 4
 
 struct LfaTcParams {
     const float* coords;
@@ -51,185 +52,94 @@ struct LtcCfg {
     static constexpr int H = D / 2;
     static constexpr bool STREAM = D > 128;          // weights do not fit next to the A tile
     static constexpr bool MMA2 = STAGE == 2 && H >= 16;  // lse2 on the tensor core
-    // TRANS: the score GEMM runs transposed (M = score channel, N = neighbour row) and a second,
-    // identity-weight GEMM delivers X^T the same way, so that one thread sees the 16 neighbours
-    // of a (point, channel) in its own TMEM lane: the softmax needs no cross-lane traffic.
-    static constexpr bool TRANS = !STREAM && D >= 64;
-    static constexpr int NTH = (TRANS && D == 128) ? 512 : 256;   // threads per CTA
-    static constexpr int NPART = NTH / LTC_ROWS;                  // threads sharing one row
-    static constexpr int MINB = (TRANS && D == 64) ? 2 : 1;       // two CTAs per SM must fit the register file
+    static constexpr int NTH = 256;                  // threads per CTA: two warpgroups
+    static constexpr int NPART = NTH / LTC_ROWS;     // threads sharing one row
+    static constexpr int CB = D < 32 ? D : 32;       // score columns per block
+    static constexpr int CB2 = H < 32 ? H : 32;      // lse2 columns per block
     static constexpr int A_BYTES = D / 8 * LTC_ROWS * 16;  // one of hi / lo
-    static constexpr int B_BYTES = STREAM ? 0 : TRANS ? D / 8 * LTC_ROWS * 16 : D / 8 * D * 16;
-    static constexpr int I_BYTES = TRANS ? D / 8 * LTC_ROWS * 16 : 0;   // identity operand (hi only)
-    static constexpr int B2_BYTES = (MMA2 && !STREAM) ? H / 8 * H * 16 : 0;
-    static constexpr int RING_SLOT = STREAM ? 2 * (LTC_SLICE / 8) * D * 16 : 0;  // hi + lo of one slice
+    static constexpr int B_BYTES = STREAM ? D / 8 * CB * 16 : D / 8 * D * 16;
+    static constexpr int B2_BYTES = MMA2 ? (STREAM ? H / 8 * CB2 * 16 : H / 8 * H * 16) : 0;
+    static constexpr int SB_BYTES = LTC_ROWS * LTC_SB_LD * 4;
     static constexpr int W10_BYTES = 12 * H * 4;
     static constexpr int ST2_BYTES = STAGE == 2 ? (2 * H + (H < 16 ? H * H : 0)) * 4 : 0;
-    static constexpr int TMEM_NEED = TRANS ? 256 : D + (MMA2 ? H : 0);
-    static constexpr int TMEM_COLS = TMEM_NEED <= 32 ? 32 : TMEM_NEED <= 64 ? 64 : TMEM_NEED <= 128 ? 128
-                                     : TMEM_NEED <= 256 ? 256 : 512;
-    static constexpr size_t SMEM = 2 * A_BYTES + 2 * B_BYTES + I_BYTES + 2 * B2_BYTES + 2 * RING_SLOT +
-                                   W10_BYTES + ST2_BYTES + 128;
+    static constexpr size_t SMEM = 2 * A_BYTES + 2 * B_BYTES + 2 * B2_BYTES + SB_BYTES + W10_BYTES + ST2_BYTES + 128;
 };
 
-// D[tmem_d] = A[128 x K] * B[N x K]^T, all operands resident in shared memory; one thread.
-template <int N, int K>
-__device__ __forceinline__ void issue_resident(uint32_t tmem_d, const uint8_t* a_hi, const uint8_t* a_lo,
-                                               const uint8_t* b_hi, const uint8_t* b_lo) {
-    constexpr uint32_t idesc = tc::idesc_f16(LTC_ROWS, N);
-    constexpr uint32_t A_LBO = LTC_ROWS * 16, B_LBO = N * 16;
+// The warpgroup's 64 rows of A[128 x K] times a block of CBN rows of B (both hi / lo, chunk-major) -> d[CBN / 2]
+template <int CBN, int K>
+__device__ __forceinline__ void ltc_gemm(float* d, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
+                                         uint32_t b_lbo, int wg) {
+    constexpr uint32_t A_LBO = LTC_ROWS * 16;
+    a_hi += (uint32_t)wg * 64 * 16;
+    a_lo += (uint32_t)wg * 64 * 16;
+    tc::wgmma_fence();
 #pragma unroll
     for (int ks = 0; ks < K / 16; ++ks) {
-        const uint64_t ah = tc::smem_desc(tc::smem_u32(a_hi) + ks * 2 * A_LBO, A_LBO, 128);
-        const uint64_t al = tc::smem_desc(tc::smem_u32(a_lo) + ks * 2 * A_LBO, A_LBO, 128);
-        const uint64_t bh = tc::smem_desc(tc::smem_u32(b_hi) + ks * 2 * B_LBO, B_LBO, 128);
-        const uint64_t bl = tc::smem_desc(tc::smem_u32(b_lo) + ks * 2 * B_LBO, B_LBO, 128);
-        tc::umma_f16(tmem_d, ah, bh, idesc, ks > 0);
-        tc::umma_f16(tmem_d, ah, bl, idesc, 1);
-        tc::umma_f16(tmem_d, al, bh, idesc, 1);
+        const uint64_t ah = tc::smem_desc(a_hi + ks * 2 * A_LBO, A_LBO, 128);
+        const uint64_t al = tc::smem_desc(a_lo + ks * 2 * A_LBO, A_LBO, 128);
+        const uint64_t bh = tc::smem_desc(b_hi + ks * 2 * b_lbo, b_lbo, 128);
+        const uint64_t bl = tc::smem_desc(b_lo + ks * 2 * b_lbo, b_lbo, 128);
+        tc::wgmma_f16_ss<CBN>(d, ah, bh, ks > 0);
+        tc::wgmma_f16_ss<CBN>(d, ah, bl, 1u);
+        tc::wgmma_f16_ss<CBN>(d, al, bh, 1u);
     }
+    tc::wgmma_commit();
+    tc::wgmma_wait_all();
 }
 
-// D[tmem_d][c][row] = X[row][c]: A = identity (128 x K, exact in fp16), B = the X tile (hi + lo).
-template <int K>
-__device__ __forceinline__ void issue_identity(uint32_t tmem_d, const uint8_t* i_hi, const uint8_t* x_hi,
-                                               const uint8_t* x_lo) {
-    constexpr uint32_t idesc = tc::idesc_f16(LTC_ROWS, LTC_ROWS);
-    constexpr uint32_t LBO = LTC_ROWS * 16;
-#pragma unroll
-    for (int ks = 0; ks < K / 16; ++ks) {
-        const uint64_t ih = tc::smem_desc(tc::smem_u32(i_hi) + ks * 2 * LBO, LBO, 128);
-        const uint64_t xh = tc::smem_desc(tc::smem_u32(x_hi) + ks * 2 * LBO, LBO, 128);
-        const uint64_t xl = tc::smem_desc(tc::smem_u32(x_lo) + ks * 2 * LBO, LBO, 128);
-        tc::umma_f16(tmem_d, ih, xh, idesc, ks > 0);
-        tc::umma_f16(tmem_d, ih, xl, idesc, 1);
-    }
-}
-
-// Same product with B streamed from global memory (host-packed images) through a 2-slot ring of 32-channel
-// slices.  ONE thread runs the whole stream: it hands each slice (hi + lo: two contiguous blocks of the image)
-// to the bulk-copy engine (cp.async.bulk, bytes counted on full[slot]), waits for it, issues the slice's MMAs and
-// commits them to free[slot] (ring reuse) -- the copy of slice s+1 overlaps the MMAs of slice s.  Everybody else
-// only waits for `done` (the commit after the last slice).  Round 1 copied every slice with all 256 threads
-// through registers (LDG -> STS, 256 KB per tile at d = 256) with a __syncthreads per slice: 14 % tensor-pipe
-// activity, long-scoreboard stalls (profiles/r02_lfa_ncu_full.md).
-// mb[0..1] = full, mb[2..3] = free, mb[4] = done; ph[] = this thread's wait parities of the five barriers.
-template <int N, int K>
-__device__ __forceinline__ void gemm_streamed(uint32_t tmem_d, const uint8_t* a_hi, const uint8_t* a_lo,
-                                              const uint4* __restrict__ img, uint8_t* ring, int slot_bytes,
-                                              uint64_t* mb, uint32_t* ph, int tid) {
-    constexpr uint32_t idesc = tc::idesc_f16(LTC_ROWS, N);
-    constexpr uint32_t A_LBO = LTC_ROWS * 16, B_LBO = N * 16;
-    constexpr int CH = LTC_SLICE / 8;                 // 16-byte k-chunks per slice
-    constexpr int SL_U4 = CH * N;                     // uint4 per slice per image
-    constexpr int IMG_U4 = K / 8 * N;                 // uint4 per image (hi, then lo)
-    constexpr int NSL = K / LTC_SLICE;
-    constexpr uint32_t SL_BYTES = SL_U4 * 16;
-    if (tid == 0) {
-        auto copy_slice = [&](int s) {
-            const int slot = s & 1;
-            uint8_t* dst = ring + (size_t)slot * slot_bytes;
-            tc::mbar_arrive_expect_tx(&mb[slot], 2 * SL_BYTES);
-            tc::bulk_copy_g2s(dst, img + (size_t)s * SL_U4, SL_BYTES, &mb[slot]);
-            tc::bulk_copy_g2s(dst + SL_BYTES, img + IMG_U4 + (size_t)s * SL_U4, SL_BYTES, &mb[slot]);
-        };
-        copy_slice(0);
-        for (int s = 0; s < NSL; ++s) {
-            const int slot = s & 1;
-            if (s + 1 < NSL) {
-                if (s >= 1) {     // slot (s+1)&1 was read by slice s-1: wait until those MMAs are done
-                    tc::mbar_wait(&mb[2 + ((s + 1) & 1)], ph[2 + ((s + 1) & 1)]);
-                    ph[2 + ((s + 1) & 1)] ^= 1;
-                }
-                copy_slice(s + 1);
-            }
-            tc::mbar_wait(&mb[slot], ph[slot]);
-            ph[slot] ^= 1;
-            const uint8_t* b_hi = ring + (size_t)slot * slot_bytes;
-            const uint8_t* b_lo = b_hi + SL_BYTES;
-#pragma unroll
-            for (int ks = 0; ks < LTC_SLICE / 16; ++ks) {
-                const int kc = s * CH + ks * 2;  // first k-chunk of this k-step in A
-                const uint64_t ah = tc::smem_desc(tc::smem_u32(a_hi) + kc * A_LBO, A_LBO, 128);
-                const uint64_t al = tc::smem_desc(tc::smem_u32(a_lo) + kc * A_LBO, A_LBO, 128);
-                const uint64_t bh = tc::smem_desc(tc::smem_u32(b_hi) + ks * 2 * B_LBO, B_LBO, 128);
-                const uint64_t bl = tc::smem_desc(tc::smem_u32(b_lo) + ks * 2 * B_LBO, B_LBO, 128);
-                tc::umma_f16(tmem_d, ah, bh, idesc, (s | ks) > 0);
-                tc::umma_f16(tmem_d, ah, bl, idesc, 1);
-                tc::umma_f16(tmem_d, al, bh, idesc, 1);
-            }
-            tc::umma_commit(&mb[2 + slot]);
+// D[:, 32 nb + (0 .. CBN)) = A[:, 0 .. K) * W^T for the column block nb of a weight with NIMG output rows (host image
+// [K/8][NIMG][8] hi, then lo), staged into sb [128][LTC_SB_LD].  Resident weights (bsm holds the whole image) are addressed
+// in place; otherwise the block is first copied into bsm.  Ends with the staged block visible to the whole CTA.
+template <int CBN, int K, int NIMG, bool RESIDENT>
+__device__ __forceinline__ void ltc_block(const uint8_t* a_hi, const uint8_t* a_lo, uint8_t* bsm, int bsm_half_bytes,
+                                          const uint4* __restrict__ img, int nb, float* sb, int tid) {
+    if (!RESIDENT) {
+        __syncthreads();     // the previous block's MMAs are done with bsm
+        constexpr int N_U4 = K / 8 * CBN;
+        for (int i = tid; i < 2 * N_U4; i += 256) {
+            const int im = i / N_U4, rem = i % N_U4, kc = rem / CBN, r = rem % CBN;
+            reinterpret_cast<uint4*>(bsm + im * bsm_half_bytes)[rem] = img[(size_t)im * (K / 8) * NIMG + kc * NIMG + nb * CBN + r];
         }
-        tc::umma_commit(&mb[4]);
-        // the free[] commits of the last two slices are not waited for inside the loop: consume them here so
-        // that the parities are in step for the next call (they complete no later than `done`)
-        if (NSL >= 2) {
-            tc::mbar_wait(&mb[2 + ((NSL - 2) & 1)], ph[2 + ((NSL - 2) & 1)]);
-            ph[2 + ((NSL - 2) & 1)] ^= 1;
-        }
-        tc::mbar_wait(&mb[2 + ((NSL - 1) & 1)], ph[2 + ((NSL - 1) & 1)]);
-        ph[2 + ((NSL - 1) & 1)] ^= 1;
+        tc::fence_async_smem();
+        __syncthreads();
     }
-    tc::mbar_wait(&mb[4], ph[4]);
-    ph[4] ^= 1;
-    tc::tc_fence_after();
+    const uint32_t b_hi = tc::smem_u32(bsm) + (RESIDENT ? (uint32_t)nb * CBN * 16 : 0u);
+    const uint32_t b_lo = b_hi + (uint32_t)bsm_half_bytes;
+    const int wg = tid >> 7, lane = tid & 31, g = lane >> 2, t = lane & 3;
+    float d[CBN / 2];
+    ltc_gemm<CBN, K>(d, tc::smem_u32(a_hi), tc::smem_u32(a_lo), b_hi, b_lo, (RESIDENT ? NIMG : CBN) * 16, wg);
+    const int r0 = wg * 64 + ((tid >> 5) & 3) * 16 + g;
+#pragma unroll
+    for (int i = 0; i < CBN / 2; i += 2)
+        *reinterpret_cast<float2*>(sb + (r0 + ((i >> 1) & 1) * 8) * LTC_SB_LD + (i >> 2) * 8 + 2 * t) = make_float2(d[i], d[i + 1]);
+    __syncthreads();
 }
 
 template <int D, int STAGE>
-__global__ void __launch_bounds__((LtcCfg<D, STAGE>::NTH), (LtcCfg<D, STAGE>::MINB))
+__global__ void __launch_bounds__(LtcCfg<D, STAGE>::NTH, 1)
 lfa_pool_tc_kernel(const __grid_constant__ LfaTcParams p) {
     using C = LtcCfg<D, STAGE>;
-    constexpr int H = C::H, NTH = C::NTH, NPART = C::NPART;
+    constexpr int H = C::H, NTH = C::NTH, NPART = C::NPART, CB = C::CB, CB2 = C::CB2;
     extern __shared__ __align__(128) uint8_t smem[];
     uint8_t* a_hi = smem;
     uint8_t* a_lo = a_hi + C::A_BYTES;
-    uint8_t* b_hi = a_lo + C::A_BYTES;
-    uint8_t* b_lo = b_hi + C::B_BYTES;
-    uint8_t* i_hi = b_lo + C::B_BYTES;
-    uint8_t* b2_hi = i_hi + C::I_BYTES;
-    uint8_t* b2_lo = b2_hi + C::B2_BYTES;
-    uint8_t* ring = b2_lo + C::B2_BYTES;
-    float* W10 = reinterpret_cast<float*>(ring + 2 * C::RING_SLOT);  // [12][H]
+    uint8_t* b_sm = a_lo + C::A_BYTES;                                // [hi | lo] score weight (or one column block)
+    uint8_t* b2_sm = b_sm + 2 * C::B_BYTES;                           // [hi | lo] lse2 weight (or one column block)
+    float* SB = reinterpret_cast<float*>(b2_sm + 2 * C::B2_BYTES);    // [128][LTC_SB_LD] staged accumulator block
+    float* W10 = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(SB) + C::SB_BYTES);  // [12][H]
     float* ST2 = W10 + 12 * H;                                       // [2][H] (+ Wl2^T [H][H] for H < 16)
-    uint64_t* mbar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(ST2) + C::ST2_BYTES);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(mbar + 8);
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, lane = tid & 31;
     const int row = tid & (LTC_ROWS - 1);   // neighbour row of the tile this thread works on
     const int half = tid >> 7;              // which part of the channels / columns (0 .. NPART-1)
 
-    // ---- once per CTA: weights, barriers, TMEM
-    if (C::TRANS) {
-        // score weight as the M operand: 128 rows (d = 64: the 64 channels twice, so that TMEM lanes
-        // 64..127 serve the second half of the tile's points); source image is [D/8][D][8] hi, lo
-        constexpr int CH = D / 8;
-        for (int i = tid; i < 2 * CH * LTC_ROWS; i += NTH) {
-            const int im = i / (CH * LTC_ROWS), rem = i % (CH * LTC_ROWS);
-            const int kc = rem / LTC_ROWS, r = rem % LTC_ROWS;
-            reinterpret_cast<uint4*>(b_hi)[i] = p.ws_img[(size_t)im * CH * D + kc * D + (r % D)];
-        }
-        for (int i = tid; i < CH * LTC_ROWS; i += NTH) {
-            const int kc = i / LTC_ROWS, r = i % LTC_ROWS;
-            const int j = (r % D) - kc * 8;        // position of the one inside this 8-wide chunk
-            uint4 v = make_uint4(0u, 0u, 0u, 0u);
-            if (j >= 0 && j < 8) {
-                const uint32_t one = 0x3C00u << ((j & 1) * 16);
-                if ((j >> 1) == 0) v.x = one;
-                else if ((j >> 1) == 1) v.y = one;
-                else if ((j >> 1) == 2) v.z = one;
-                else v.w = one;
-            }
-            reinterpret_cast<uint4*>(i_hi)[i] = v;
-        }
-        if (C::MMA2)
-            for (int i = tid; i < 2 * C::B2_BYTES / 16; i += NTH)
-                reinterpret_cast<uint4*>(b2_hi)[i] = p.wl2_img[i];
-    } else if (!C::STREAM) {
+    // ---- once per CTA: resident weights and the small per-channel constants
+    if (!C::STREAM) {
         for (int i = tid; i < 2 * C::B_BYTES / 16; i += NTH)
-            reinterpret_cast<uint4*>(b_hi)[i] = p.ws_img[i];
+            reinterpret_cast<uint4*>(b_sm)[i] = p.ws_img[i];
         if (C::MMA2)
             for (int i = tid; i < 2 * C::B2_BYTES / 16; i += NTH)
-                reinterpret_cast<uint4*>(b2_hi)[i] = p.wl2_img[i];
+                reinterpret_cast<uint4*>(b2_sm)[i] = p.wl2_img[i];
     }
     if (STAGE == 2) {
         for (int i = tid; i < H; i += NTH) {
@@ -244,33 +154,15 @@ lfa_pool_tc_kernel(const __grid_constant__ LfaTcParams p) {
         W10[10 * H + i] = p.s10[i];
         W10[11 * H + i] = p.t10[i];
     }
-    if (tid == 0) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) tc::mbar_init(&mbar[i], 1);
-        tc::fence_mbar_init();
-    }
     tc::fence_async_smem();
     __syncthreads();
-    if (warp == 0) tc::tmem_alloc<C::TMEM_COLS>(tmem_slot);
-    tc::tc_fence_before();
-    __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    const uint32_t tmem_lane = tmem + ((uint32_t)((warp & 3) * 32) << 16);
-    // TRANS: the lse2 accumulator aliases the score columns (it is consumed before they are written)
-    constexpr int LSE2_COL = C::TRANS ? 0 : D;
-    uint32_t ph_main[2] = {0, 0};  // parities of mbar[0] (lse2) and mbar[1] (scores)
-    uint32_t ph_ring[5] = {0, 0, 0, 0, 0};  // parities of mbar[2..6]: weight ring full / free and `done` (gemm_streamed)
 
     // The gathers are software-pipelined over tiles (d >= 64): the neighbour index of tile t+2 and the
     // coordinates / feature rows of tile t+1 are requested while tile t is worked on and land behind its
     // MMAs and epilogue (two dependent global round trips leave the per-tile critical path).  d = 256 holds 64
     // feature registers per tile: there the requests for tile t+1 go out after the rows of tile t have been stored
     // (LATE) and the index stays a raw loaded word until its tile comes up (RAW_INDEX, common.cuh RawIndex).  The
-    // resident-weight kernels resolve the index of tile t+2 right behind its load: every warp of the CTA waits there
-    // for one L2 round trip, 13-19 % of the stall samples (profiles/r02_lfa_stalls.md) -- and taking that wait away
-    // made d = 64 SLOWER (2 x 188.6 / 217.3 us against 173.7 / 195.6 us per launch, same build otherwise; d = 128 equal):
-    // with two CTAs per SM the wait is where the other CTA gets the issue slots and the shared-memory port.
+    // resident-weight kernels resolve the index of tile t+2 right behind its load.
     constexpr bool PREF = D >= 64;
     constexpr bool LATE = C::STREAM;
 #ifdef LTC_RAW_INDEX_ALL
@@ -356,7 +248,7 @@ lfa_pool_tc_kernel(const __grid_constant__ LfaTcParams p) {
             for (int q = 0; q < 10; ++q) {   // warp-uniform LDS.128 of the weights
                 const float4 wa = *reinterpret_cast<const float4*>(&W10[q * H + ch * 8]);
                 const float4 wb = *reinterpret_cast<const float4*>(&W10[q * H + ch * 8 + 4]);
-                ffma2(r[0], r[1], e[q], wa.x, wa.y);   // packed FFMA2: half the FMA instructions of the LocSE MLP
+                ffma2(r[0], r[1], e[q], wa.x, wa.y);
                 ffma2(r[2], r[3], e[q], wa.z, wa.w);
                 ffma2(r[4], r[5], e[q], wb.x, wb.y);
                 ffma2(r[6], r[7], e[q], wb.z, wb.w);
@@ -454,32 +346,13 @@ lfa_pool_tc_kernel(const __grid_constant__ LfaTcParams p) {
         // ---------------- stage 2: r2 = lrelu(BN(Wl2 . r1)) on the tensor core -> channels [H, D)
         if (C::MMA2) {
             tc::fence_async_smem();
-            tc::tc_fence_before();
             __syncthreads();
-            tc::tc_fence_after();
-            if (C::STREAM) {
-                gemm_streamed<H, H>(tmem + LSE2_COL, a_hi, a_lo, p.wl2_img, ring, C::RING_SLOT, &mbar[2], ph_ring, tid);
-            } else {
-                if (tid == 0) {
-                    issue_resident<H, H>(tmem + LSE2_COL, a_hi, a_lo, b2_hi, b2_lo);
-                    tc::umma_commit(&mbar[0]);
-                }
-                tc::mbar_wait(&mbar[0], ph_main[0]);
-                ph_main[0] ^= 1;
-                tc::tc_fence_after();
-            }
-            constexpr int NR2 = H / (8 * NPART) > 0 ? H / (8 * NPART) : 1;   // 8-column groups of r2 per thread
-            constexpr int NB = NR2 > 4 ? 4 : NR2;                            // loads behind one wait
-#pragma unroll
-            for (int b0 = 0; b0 < NR2; b0 += NB) {
-                uint32_t vr[NB][8];
-#pragma unroll
-                for (int i = 0; i < NB; ++i)
-                    tc::tmem_ld8_issue(tmem_lane + LSE2_COL + (half + (b0 + i) * NPART) * 8, vr[i]);
-                tc::tmem_ld_wait();
-#pragma unroll
-                for (int i = 0; i < NB; ++i) {
-                    const int c0 = (half + (b0 + i) * NPART) * 8;
+#pragma unroll 1
+            for (int blk = 0; blk < H / CB2; ++blk) {
+                ltc_block<CB2, H, H, !C::STREAM>(a_hi, a_lo, b2_sm, C::B2_BYTES, p.wl2_img, blk, SB, tid);
+                // 8-column groups of this block: half 0 takes 0 and 16, half 1 takes 8 and 24
+                for (int cl = 8 * half; cl < CB2; cl += 16) {
+                    const int c0 = blk * CB2 + cl;
                     float v[8];
                     const float4 sa = *reinterpret_cast<const float4*>(&ST2[c0]);
                     const float4 sb = *reinterpret_cast<const float4*>(&ST2[c0 + 4]);
@@ -489,7 +362,7 @@ lfa_pool_tc_kernel(const __grid_constant__ LfaTcParams p) {
                     const float sh[8] = {ta.x, ta.y, ta.z, ta.w, tb.x, tb.y, tb.z, tb.w};
 #pragma unroll
                     for (int j = 0; j < 8; ++j) {
-                        const float a = fmaf(tc::tmem_val(vr[i][j]), sc[j], sh[j]);
+                        const float a = fmaf(SB[row * LTC_SB_LD + cl + j], sc[j], sh[j]);
                         v[j] = a >= 0.f ? a : 0.2f * a;
                     }
                     uint4 hi, lo;
@@ -497,130 +370,81 @@ lfa_pool_tc_kernel(const __grid_constant__ LfaTcParams p) {
                     *reinterpret_cast<uint4*>(a_hi + tc::op_off(LTC_ROWS, row, (H + c0) / 8)) = hi;
                     *reinterpret_cast<uint4*>(a_lo + tc::op_off(LTC_ROWS, row, (H + c0) / 8)) = lo;
                 }
+                __syncthreads();   // SB is read; after the last block every lse2 MMA has read r1
             }
         }
         // (the features overwrite r1 in stage 2: the lse2 MMAs that read it have completed)
         store_features();
         if (PREF && LATE) advance(tile);     // lands behind the score GEMM and the epilogue
         tc::fence_async_smem();
-        tc::tc_fence_before();
         __syncthreads();
-        tc::tc_fence_after();
 
-        // ---------------- scores = X . Ws^T on the tensor core
-        if (C::STREAM) {
-            gemm_streamed<D, D>(tmem, a_hi, a_lo, p.ws_img, ring, C::RING_SLOT, &mbar[2], ph_ring, tid);
-        } else {
-            if (tid == 0) {
-                if (C::TRANS) {
-                    issue_resident<LTC_ROWS, D>(tmem, b_hi, b_lo, a_hi, a_lo);   // [channel][row]
-                    issue_identity<D>(tmem + LTC_ROWS, i_hi, a_hi, a_lo);        // X^T
-                } else {
-                    issue_resident<D, D>(tmem, a_hi, a_lo, b_hi, b_lo);
-                }
-                tc::umma_commit(&mbar[1]);
-            }
-            tc::mbar_wait(&mbar[1], ph_main[1]);
-            ph_main[1] ^= 1;
-            tc::tc_fence_after();
-        }
-
-        // ---------------- softmax over the 16 rows of each point + weighted sum
-        if (C::TRANS) {
-            // thread = TMEM lane = score channel; its 2 points' 16 neighbours are 16 columns each
-            const int tl = (warp & 3) * 32 + lane;
-            const int c = tl % D;
-            const int pbase = (D == 64 ? (tl >> 6) * 4 : 0) + (warp >> 2) * 2;
-#pragma unroll
-            for (int q = 0; q < 2; ++q) {
-                const int pt = pbase + q;
-                float s[16], x[16];
-                {
-                    uint32_t sr[16], xr[16];     // scores and X^T of the point behind one wait
-                    tc::tmem_ld16_issue(tmem_lane + pt * LTC_K, sr);
-                    tc::tmem_ld16_issue(tmem_lane + LTC_ROWS + pt * LTC_K, xr);
-                    tc::tmem_ld_wait();
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        s[j] = tc::tmem_val(sr[j]);
-                        x[j] = tc::tmem_val(xr[j]);
-                    }
-                }
-                float m = s[0];
-#pragma unroll
-                for (int j = 1; j < 16; ++j) m = fmaxf(m, s[j]);
-                float num = 0.f, den = 0.f;
-                const float ml = -m * kLog2e;
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const float ev = ex2_ftz(fmaf(s[j], kLog2e, ml));
-                    den += ev;
-                    num = fmaf(ev, x[j], num);
-                }
-                const int64_t gp = tile * (LTC_ROWS / LTC_K) + pt;
-                if (gp < p.total) p.agg[(size_t)gp * D + c] = num / den;
-            }
-        }
+        // ---------------- scores = X . Ws^T on the tensor core, 32 columns at a time, then the softmax over the
+        // 16 rows of each point + weighted sum of those columns
         const bool upper = (lane & 16) != 0;
         const int j16 = lane & 15;
-        for (int c0 = half * 16; c0 < (C::TRANS ? 0 : D); c0 += 32) {
-            float s[16], x[16];
-            tc::tmem_ld16(tmem_lane + c0, s);
-#pragma unroll
-            for (int q = 0; q < 2; ++q) {
-                const uint4 hq = *reinterpret_cast<const uint4*>(a_hi + tc::op_off(LTC_ROWS, row, c0 / 8 + q));
-                const uint4 lq = *reinterpret_cast<const uint4*>(a_lo + tc::op_off(LTC_ROWS, row, c0 / 8 + q));
-                const __half2* hh = reinterpret_cast<const __half2*>(&hq);
-                const __half2* ll = reinterpret_cast<const __half2*>(&lq);
+#pragma unroll 1
+        for (int blk = 0; blk < D / CB; ++blk) {
+            ltc_block<CB, D, D, !C::STREAM>(a_hi, a_lo, b_sm, C::B_BYTES, p.ws_img, blk, SB, tid);
+            for (int cl = half * 16; cl < CB; cl += 32) {
+                const int c0 = blk * CB + cl;
+                float s[16], x[16];
 #pragma unroll
                 for (int u = 0; u < 4; ++u) {
-                    const float2 fh = __half22float2(hh[u]), fl = __half22float2(ll[u]);
-                    x[q * 8 + 2 * u] = fh.x + fl.x;
-                    x[q * 8 + 2 * u + 1] = fh.y + fl.y;
+                    const float4 v = *reinterpret_cast<const float4*>(&SB[row * LTC_SB_LD + cl + 4 * u]);
+                    s[4 * u] = v.x; s[4 * u + 1] = v.y; s[4 * u + 2] = v.z; s[4 * u + 3] = v.w;
                 }
-            }
-            float den[16], num[16];
 #pragma unroll
-            for (int i = 0; i < 16; ++i) {
-                int o = __float_as_int(s[i]);
-                o ^= (o >> 31) & 0x7fffffff;              // order-preserving float -> int
-                // per-half-warp max through two FULL-warp reductions (redux.sync with two different
-                // sub-warp masks in one instruction returned the wrong group's maximum on B200)
-                const int m_lo = __reduce_max_sync(0xffffffffu, upper ? INT_MIN : o);
-                const int m_hi = __reduce_max_sync(0xffffffffu, upper ? o : INT_MIN);
-                int m = upper ? m_hi : m_lo;
-                m ^= (m >> 31) & 0x7fffffff;
-                const float ev = ex2_ftz(fmaf(s[i], kLog2e, -__int_as_float(m) * kLog2e));
-                den[i] = ev;
-                num[i] = ev * x[i];
+                for (int q = 0; q < 2; ++q) {
+                    const uint4 hq = *reinterpret_cast<const uint4*>(a_hi + tc::op_off(LTC_ROWS, row, c0 / 8 + q));
+                    const uint4 lq = *reinterpret_cast<const uint4*>(a_lo + tc::op_off(LTC_ROWS, row, c0 / 8 + q));
+                    const __half2* hh = reinterpret_cast<const __half2*>(&hq);
+                    const __half2* ll = reinterpret_cast<const __half2*>(&lq);
+#pragma unroll
+                    for (int u = 0; u < 4; ++u) {
+                        const float2 fh = __half22float2(hh[u]), fl = __half22float2(ll[u]);
+                        x[q * 8 + 2 * u] = fh.x + fl.x;
+                        x[q * 8 + 2 * u + 1] = fh.y + fl.y;
+                    }
+                }
+                float den[16], num[16];
+#pragma unroll
+                for (int i = 0; i < 16; ++i) {
+                    int o = __float_as_int(s[i]);
+                    o ^= (o >> 31) & 0x7fffffff;              // order-preserving float -> int
+                    // per-half-warp max through two FULL-warp reductions (one redux.sync per 16-lane group)
+                    const int m_lo = __reduce_max_sync(0xffffffffu, upper ? INT_MIN : o);
+                    const int m_hi = __reduce_max_sync(0xffffffffu, upper ? o : INT_MIN);
+                    int m = upper ? m_hi : m_lo;
+                    m ^= (m >> 31) & 0x7fffffff;
+                    const float ev = ex2_ftz(fmaf(s[i], kLog2e, -__int_as_float(m) * kLog2e));
+                    den[i] = ev;
+                    num[i] = ev * x[i];
 #ifdef O3DML_DEBUG_NAN
-                if (!(ev <= 1.0f) || !(fabsf(x[i]) < 1e30f) || !(fabsf(s[i]) < 1e30f))
-                    printf("DBG tile %lld row %d c0 %d i %d s %g m %g ev %g x %g o %d mi %d\n",
-                           (long long)tile, row, c0, i, s[i], __int_as_float(m), ev, x[i], o, m);
+                    if (!(ev <= 1.0f) || !(fabsf(x[i]) < 1e30f) || !(fabsf(s[i]) < 1e30f))
+                        printf("DBG tile %lld row %d c0 %d i %d s %g m %g ev %g x %g o %d mi %d\n",
+                               (long long)tile, row, c0, i, s[i], __int_as_float(m), ev, x[i], o, m);
 #endif
-            }
-            // reduce-scatter over the 16 lanes of the group: afterwards lane j16 holds column c0+j16
-#pragma unroll
-            for (int w = 8; w >= 1; w >>= 1) {
-                const bool up = (lane & w) != 0;
-#pragma unroll
-                for (int i = 0; i < w; ++i) {
-                    const float sd = up ? den[i] : den[i + w];
-                    const float sn = up ? num[i] : num[i + w];
-                    const float rd = __shfl_xor_sync(0xffffffffu, sd, w);
-                    const float rn = __shfl_xor_sync(0xffffffffu, sn, w);
-                    den[i] = (up ? den[i + w] : den[i]) + rd;
-                    num[i] = (up ? num[i + w] : num[i]) + rn;
                 }
+                // reduce-scatter over the 16 lanes of the group: afterwards lane j16 holds column c0+j16
+#pragma unroll
+                for (int w = 8; w >= 1; w >>= 1) {
+                    const bool up = (lane & w) != 0;
+#pragma unroll
+                    for (int i = 0; i < w; ++i) {
+                        const float sd = up ? den[i] : den[i + w];
+                        const float sn = up ? num[i] : num[i + w];
+                        const float rd = __shfl_xor_sync(0xffffffffu, sd, w);
+                        const float rn = __shfl_xor_sync(0xffffffffu, sn, w);
+                        den[i] = (up ? den[i + w] : den[i]) + rd;
+                        num[i] = (up ? num[i + w] : num[i]) + rn;
+                    }
+                }
+                if (g < p.total) p.agg[(size_t)g * D + c0 + j16] = num[0] / den[0];
             }
-            if (g < p.total) p.agg[(size_t)g * D + c0 + j16] = num[0] / den[0];
+            __syncthreads();   // SB is read; after the last block the A tile is free for the next tile
         }
-        tc::tc_fence_before();
-        __syncthreads();   // TMEM accumulators and the A tile are free for the next tile
-        tc::tc_fence_after();
     }
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc<C::TMEM_COLS>(tmem);
 }
 
 template <int D, int STAGE>
@@ -634,9 +458,10 @@ static int lfa_tc_launch(const LfaTcParams& p, cudaStream_t st) {
                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
         once.done(dev);
     }
-    int per_sm = (int)(224 * 1024 / (C::SMEM + 1024));
+    // persistent CTAs: as many as are resident at once (registers and shared memory both limit it)
+    int per_sm = 0;
+    O3DML_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lfa_pool_tc_kernel<D, STAGE>, C::NTH, C::SMEM));
     if (per_sm < 1) per_sm = 1;
-    if (per_sm * C::TMEM_COLS > 512) per_sm = 512 / C::TMEM_COLS;
     if (per_sm > 4) per_sm = 4;
     int64_t grid = (int64_t)device_sm_count() * per_sm;
     if (grid > p.num_tiles) grid = p.num_tiles;

@@ -1,20 +1,20 @@
 // rl_tail.cu -- the per-point tail of RandLA-Net as ONE kernel: the last decoder layer and the classifier
 //   decoder[-1]  SharedMLP(transpose) on [skip | nearest_interpolation(x)]   (randlanet.py:284-292, 329-350)
 //   fc1          SharedMLP 32->64, SharedMLP 64->32, Dropout (eval: identity), SharedMLP 32->classes   (randlanet.py:110-113, 294-298)
-// chained through tensor memory.  Round 1 ran these four layers as four row-per-thread launches whose 8 KB weight
-// blocks miss the constant cache (230 us per 8 x 45 056-point step, 12 % of the forward, while moving < 100 MB).
+// chained through shared memory and the Hopper tensor cores.  As four row-per-thread launches these layers re-read their
+// 8 KB weight blocks for every row and write every intermediate activation to HBM.
 //
-// Per 128-row tile, thread = row = TMEM lane:
-//   load the 32 + 32 input channels of the row (skip row; coarse row through the interpolation index)
-//   for each layer:  split the fp32 activations into TF32 hi / lo and tcgen05.st them into TMEM (the A operand, TS mode),
-//                    one thread issues K/8 x 3 tcgen05.mma.kind::tf32 against the layer's resident weight image in
-//                    shared memory (3xTF32: Ah*Wh + Ah*Wl + Al*Wh, as gemm_tc.cu), commit -> mbarrier,
-//                    tcgen05.ld the fp32 result, folded BN / bias + LeakyReLU in registers
+// Per 128-row tile (one warpgroup of 128 threads):
+//   load the 32 + 32 input channels of the row (thread = row; skip row; coarse row through the interpolation index)
+//   into the activation tile in shared memory, then for each layer:
+//     the warpgroup reads the TF32 A fragments of rows 0-63 and 64-127 from the tile, splits them into hi / lo in
+//     registers and issues K/8 x 3 register-A wgmma per half against the layer's resident weight image in shared
+//     memory (3xTF32: Ah*Wh + Ah*Wl + Al*Wh, as gemm_tc.cu); folded BN / bias + LeakyReLU on the accumulators,
+//     written back into the activation tile as the next layer's input
 //   logits staged in shared memory, written as one contiguous, fully coalesced block (128 rows x classes floats).
 // Activations never touch HBM between the four layers: 256 B in, 4 x classes B out per point.
 // Weights: host-packed image (open3d_ml_b200._lib.pack_tail_image): per layer, per 32-wide k-chunk, hi then lo tiles of
 // [N rows][32 floats] in the K-major SWIZZLE_128B layout, copied once per CTA with one cp.async.bulk.
-// TMEM: columns [0, 64) accumulator, [64, 128) A-hi, [128, 192) A-lo (256 allocated: two CTAs per SM).
 #include "../../include/o3dml_b200.h"
 #include "common.cuh"
 #include "tc.cuh"
@@ -26,8 +26,8 @@ namespace o3dml {
 constexpr int RT_THREADS = 128;
 constexpr int RT_K1 = 64, RT_N1 = 32, RT_N2 = 64, RT_N3 = 32, RT_N4 = 32;   // 32+32 -> 32 -> 64 -> 32 -> classes (<= 32)
 constexpr int RT_W1 = 0, RT_W2 = 16384, RT_W3 = 32768, RT_W4 = 49152, RT_WBYTES = 57344;
-constexpr int RT_D = 0, RT_AHI = 64, RT_ALO = 128, RT_TMEM = 256;
-constexpr size_t RT_SMEM = RT_WBYTES + RT_THREADS * RT_N4 * 4 + 64 + 1024;
+constexpr int RT_LD = RT_K1 + 4;     // activation tile row stride (floats): the fragment reads hit 32 banks
+constexpr size_t RT_SMEM = RT_WBYTES + RT_THREADS * RT_LD * 4 + 64 + 1024;
 
 struct RlTailParams {
     const float* skip;
@@ -42,100 +42,67 @@ struct RlTailParams {
     float shift[4][64];
 };
 
-__device__ __forceinline__ uint64_t rt_desc(uint32_t saddr) {     // K-major SWIZZLE_128B, SBO 1024 (gemm_tc.cu)
-    return (uint64_t)((saddr >> 4) & 0x3fffu) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) |
-           ((uint64_t)2 << 61);
-}
-__host__ __device__ constexpr uint32_t rt_idesc(int N) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
-__device__ __forceinline__ void rt_mma(uint32_t d, uint32_t a, uint64_t b, uint32_t idesc, uint32_t acc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d),
-        "r"(a), "l"(b), "r"(idesc), "r"(acc)
-        : "memory");
-}
-__device__ __forceinline__ void rt_st16(uint32_t taddr, const uint32_t* r) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-        : "memory");
-}
-
-// A operand of the next layer: K activations of this thread's row -> TF32 hi / lo -> TMEM columns [AHI, AHI+K), [ALO, ALO+K)
-template <int K>
-__device__ __forceinline__ void rt_store_a(uint32_t tmem_lane, const float* a) {
-#pragma unroll
-    for (int q = 0; q < K / 16; ++q) {
-        uint32_t hi[16], lo[16];
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-            const uint32_t x = __float_as_uint(a[q * 16 + j]);
-            hi[j] = x & 0xFFFFE000u;
-            lo[j] = __float_as_uint(a[q * 16 + j] - __uint_as_float(hi[j]));
-        }
-        rt_st16(tmem_lane + RT_AHI + q * 16, hi);
-        rt_st16(tmem_lane + RT_ALO + q * 16, lo);
-    }
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-    tc::tc_fence_before();
-}
-
-// D[128 x N] = A[128 x K] (TMEM) * W[K x N] (shared image at wbase: per 32-wide k-chunk hi tiles first, then lo tiles)
+// D[128 x N] = act[128 x K] * W[K x N] as two 64-row wgmma halves (W image at wbase: per 32-wide k-chunk hi tiles
+// first, then lo tiles); the activation tile is read once per 32-channel chunk, split into TF32 hi / lo in registers
 template <int K, int N>
-__device__ __forceinline__ void rt_issue(uint32_t tmem, uint32_t wbase, uint64_t* bar) {
-    constexpr uint32_t idesc = rt_idesc(N);
+__device__ __forceinline__ void rt_layer(const float* act, uint32_t wbase, float (*d)[N / 2], int tid) {
     constexpr int CHUNKS = K / 32;
     constexpr uint32_t TILE = N * 128;                       // bytes of one [N x 32 floats] tile
+    const int lane = tid & 31, t = lane & 3;
+    const int rw = (tid >> 5) * 16 + (lane >> 2);            // fragment rows rw, rw + 8 of each half
 #pragma unroll
-    for (int c = 0; c < CHUNKS; ++c) {
+    for (int h = 0; h < 2; ++h) {
 #pragma unroll
-        for (int ks = 0; ks < 4; ++ks) {
-            const uint64_t bh = rt_desc(wbase + c * TILE + ks * 32);
-            const uint64_t bl = rt_desc(wbase + (CHUNKS + c) * TILE + ks * 32);
-            const uint32_t ah = tmem + RT_AHI + c * 32 + ks * 8, al = tmem + RT_ALO + c * 32 + ks * 8;
-            rt_mma(tmem + RT_D, ah, bh, idesc, (c | ks) != 0);
-            rt_mma(tmem + RT_D, ah, bl, idesc, 1);
-            rt_mma(tmem + RT_D, al, bh, idesc, 1);
+        for (int c = 0; c < CHUNKS; ++c) {
+            uint32_t ah[4][4], al[4][4];
+#pragma unroll
+            for (int ks = 0; ks < 4; ++ks)
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const int r = h * 64 + rw + (e & 1) * 8, k = c * 32 + ks * 8 + t + (e >> 1) * 4;
+                    tc::split_tf32(__float_as_uint(act[r * RT_LD + k]), ah[ks][e], al[ks][e]);
+                }
+            tc::wgmma_fence();
+#pragma unroll
+            for (int ks = 0; ks < 4; ++ks) {
+                const uint64_t bh = tc::smem_desc_sw128(wbase + c * TILE + ks * 32);
+                const uint64_t bl = tc::smem_desc_sw128(wbase + (CHUNKS + c) * TILE + ks * 32);
+                tc::wgmma_tf32_rs<N>(d[h], ah[ks], bh, (c | ks) != 0);
+                tc::wgmma_tf32_rs<N>(d[h], ah[ks], bl, 1u);
+                tc::wgmma_tf32_rs<N>(d[h], al[ks], bh, 1u);
+            }
+            tc::wgmma_commit();
+            tc::wgmma_wait_all();
         }
     }
-    tc::umma_commit(bar);
 }
 
-// accumulator of the layer -> folded BN / bias (+ LeakyReLU) -> registers
+// accumulators of the layer -> folded BN / bias (+ LeakyReLU) -> activation tile (row stride ld)
 template <int N, bool ACT>
-__device__ __forceinline__ void rt_load_d(uint32_t tmem_lane, const RlTailParams& p, int layer, float* a) {
-    uint32_t vr[N / 16][16];        // the whole accumulator row behind one wait (this read is on the layer chain)
+__device__ __forceinline__ void rt_store_d(const float (*d)[N / 2], const RlTailParams& p, int layer, float* act, int ld,
+                                           int ncols, int tid) {
+    const int lane = tid & 31, t = lane & 3;
+    const int rw = (tid >> 5) * 16 + (lane >> 2);
 #pragma unroll
-    for (int q = 0; q < N / 16; ++q) tc::tmem_ld16_issue(tmem_lane + RT_D + q * 16, vr[q]);
-    tc::tmem_ld_wait();
+    for (int h = 0; h < 2; ++h)
 #pragma unroll
-    for (int q = 0; q < N / 16; ++q) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-            float y = fmaf(tc::tmem_val(vr[q][j]), p.scale[layer][q * 16 + j], p.shift[layer][q * 16 + j]);
+        for (int i = 0; i < N / 2; ++i) {
+            const int r = h * 64 + rw + ((i >> 1) & 1) * 8, c = (i >> 2) * 8 + 2 * t + (i & 1);
+            float y = fmaf(d[h][i], p.scale[layer][c], p.shift[layer][c]);
             if (ACT) y = y >= 0.f ? y : y * p.slope;
-            a[q * 16 + j] = y;
+            if (c < ncols) act[r * ld + c] = y;
         }
-    }
-    tc::tc_fence_before();
 }
 
 __global__ void __launch_bounds__(RT_THREADS, 2) rl_tail_kernel(const __grid_constant__ RlTailParams p) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = tc::smem_u32(smem_raw);
     uint8_t* wsm = smem_raw + ((1024u - (raw & 1023u)) & 1023u);
-    float* stg = reinterpret_cast<float*>(wsm + RT_WBYTES);                 // [128][classes] logits of the tile
-    uint64_t* mbar = reinterpret_cast<uint64_t*>(stg + RT_THREADS * RT_N4);  // [0] weights landed, [1] MMAs of a layer done
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(mbar + 2);
-    const int tid = threadIdx.x, warp = tid >> 5;
+    float* act = reinterpret_cast<float*>(wsm + RT_WBYTES);                 // [128][RT_LD] activations / logits of the tile
+    uint64_t* mbar = reinterpret_cast<uint64_t*>(act + RT_THREADS * RT_LD);  // weights landed
+    const int tid = threadIdx.x;
     if (tid == 0) {
         tc::mbar_init(&mbar[0], 1);
-        tc::mbar_init(&mbar[1], 1);
         tc::fence_mbar_init();
     }
     __syncthreads();
@@ -143,19 +110,11 @@ __global__ void __launch_bounds__(RT_THREADS, 2) rl_tail_kernel(const __grid_con
         tc::mbar_arrive_expect_tx(&mbar[0], RT_WBYTES);
         tc::bulk_copy_g2s(wsm, p.wimg, RT_WBYTES, &mbar[0]);
     }
-    if (warp == 0) tc::tmem_alloc<RT_TMEM>(tmem_slot);
-    tc::tc_fence_before();
-    __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    const uint32_t tmem_lane = tmem + ((uint32_t)(warp * 32) << 16);
     const uint32_t wbase = tc::smem_u32(wsm);
     tc::mbar_wait(&mbar[0], 0);
-    uint32_t ph = 0;
     const int64_t tiles = ceil_div<int64_t>(p.N, RT_THREADS);
     for (int64_t tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
         const int64_t n = tile * RT_THREADS + tid;
-        float a[64];
         // ---- layer-1 operand: [skip row | interpolated coarse row]
         const float* s0 = nullptr;
         const float* s1 = nullptr;
@@ -167,54 +126,46 @@ __global__ void __launch_bounds__(RT_THREADS, 2) rl_tail_kernel(const __grid_con
                 if (r >= 0 && r < p.coarse_rows) s1 = p.coarse + (size_t)r * p.coarse_ld;
             }
         }
+        float4* arow = reinterpret_cast<float4*>(act + tid * RT_LD);
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-            const float4 v = s0 ? *reinterpret_cast<const float4*>(s0 + 4 * i) : make_float4(0.f, 0.f, 0.f, 0.f);
-            const float4 w = s1 ? *reinterpret_cast<const float4*>(s1 + 4 * i) : make_float4(0.f, 0.f, 0.f, 0.f);
-            a[4 * i] = v.x; a[4 * i + 1] = v.y; a[4 * i + 2] = v.z; a[4 * i + 3] = v.w;
-            a[32 + 4 * i] = w.x; a[32 + 4 * i + 1] = w.y; a[32 + 4 * i + 2] = w.z; a[32 + 4 * i + 3] = w.w;
+            arow[i] = s0 ? *reinterpret_cast<const float4*>(s0 + 4 * i) : make_float4(0.f, 0.f, 0.f, 0.f);
+            arow[8 + i] = s1 ? *reinterpret_cast<const float4*>(s1 + 4 * i) : make_float4(0.f, 0.f, 0.f, 0.f);
         }
-        // ---- decoder[-1]: 64 -> 32
-        rt_store_a<RT_K1>(tmem_lane, a);
         __syncthreads();
-        if (tid == 0) { tc::tc_fence_after(); rt_issue<RT_K1, RT_N1>(tmem, wbase + RT_W1, &mbar[1]); }
-        tc::mbar_wait(&mbar[1], ph); ph ^= 1;
-        tc::tc_fence_after();
-        rt_load_d<RT_N1, true>(tmem_lane, p, 0, a);
-        // ---- fc1.0: 32 -> 64
-        rt_store_a<RT_N1>(tmem_lane, a);
-        __syncthreads();
-        if (tid == 0) { tc::tc_fence_after(); rt_issue<RT_N1, RT_N2>(tmem, wbase + RT_W2, &mbar[1]); }
-        tc::mbar_wait(&mbar[1], ph); ph ^= 1;
-        tc::tc_fence_after();
-        rt_load_d<RT_N2, true>(tmem_lane, p, 1, a);
-        // ---- fc1.1: 64 -> 32
-        rt_store_a<RT_N2>(tmem_lane, a);
-        __syncthreads();
-        if (tid == 0) { tc::tc_fence_after(); rt_issue<RT_N2, RT_N3>(tmem, wbase + RT_W3, &mbar[1]); }
-        tc::mbar_wait(&mbar[1], ph); ph ^= 1;
-        tc::tc_fence_after();
-        rt_load_d<RT_N3, true>(tmem_lane, p, 2, a);
-        // ---- fc1.3: 32 -> classes (no BN, no activation)
-        rt_store_a<RT_N3>(tmem_lane, a);
-        __syncthreads();
-        if (tid == 0) { tc::tc_fence_after(); rt_issue<RT_N3, RT_N4>(tmem, wbase + RT_W4, &mbar[1]); }
-        tc::mbar_wait(&mbar[1], ph); ph ^= 1;
-        tc::tc_fence_after();
-        rt_load_d<RT_N4, false>(tmem_lane, p, 3, a);
-        // ---- logits: dense [rows x classes] block of the tile, contiguous in the output
-#pragma unroll
-        for (int c = 0; c < RT_N4; ++c)
-            if (c < p.classes) stg[tid * p.classes + c] = a[c];
-        __syncthreads();
+        {   // ---- decoder[-1]: 64 -> 32
+            float d[2][RT_N1 / 2];
+            rt_layer<RT_K1, RT_N1>(act, wbase + RT_W1, d, tid);
+            __syncthreads();
+            rt_store_d<RT_N1, true>(d, p, 0, act, RT_LD, RT_N1, tid);
+            __syncthreads();
+        }
+        {   // ---- fc1.0: 32 -> 64
+            float d[2][RT_N2 / 2];
+            rt_layer<RT_N1, RT_N2>(act, wbase + RT_W2, d, tid);
+            __syncthreads();
+            rt_store_d<RT_N2, true>(d, p, 1, act, RT_LD, RT_N2, tid);
+            __syncthreads();
+        }
+        {   // ---- fc1.1: 64 -> 32
+            float d[2][RT_N3 / 2];
+            rt_layer<RT_N2, RT_N3>(act, wbase + RT_W3, d, tid);
+            __syncthreads();
+            rt_store_d<RT_N3, true>(d, p, 2, act, RT_LD, RT_N3, tid);
+            __syncthreads();
+        }
+        {   // ---- fc1.3: 32 -> classes (no BN, no activation); logits as a dense [rows x classes] block
+            float d[2][RT_N4 / 2];
+            rt_layer<RT_N3, RT_N4>(act, wbase + RT_W4, d, tid);
+            __syncthreads();
+            rt_store_d<RT_N4, false>(d, p, 3, act, p.classes, p.classes, tid);
+            __syncthreads();
+        }
         const int64_t rows = min((int64_t)RT_THREADS, p.N - tile * RT_THREADS);
         float* o = p.out + (size_t)tile * RT_THREADS * p.classes;
-        for (int i = tid; i < (int)(rows * p.classes); i += RT_THREADS) o[i] = stg[i];
-        __syncthreads();        // staging buffer and the TMEM regions are free for the next tile
+        for (int i = tid; i < (int)(rows * p.classes); i += RT_THREADS) o[i] = act[i];
+        __syncthreads();        // the activation tile is free for the next tile
     }
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc<RT_TMEM>(tmem);
 }
 
 }  // namespace o3dml

@@ -3,8 +3,8 @@
 // These are the SharedMLPs of RandLA-Net's first level and classifier (randlanet.py:471-518 as
 // used at :110-113, :653-664, :284-292): 360 k rows per step, 8..64 channels.  Their arithmetic
 // intensity is 2*K*Cout / (4*(K + Cout)) <= 11 flop/B: HBM-bound layers.  The tiled kernels
-// (gemm.cu, gemm_tc.cu) spend their time in per-CTA set-up and barrier phases at these widths
-// (33-76 us per launch measured where 4-21 us of HBM traffic is needed).  Here a thread loads its
+// (gemm.cu, gemm_tc.cu) spend their time in per-CTA set-up and barrier phases at these widths,
+// not in moving the few bytes per row these layers need.  Here a thread loads its
 // input row (contiguous, consecutive lanes = consecutive rows), keeps it in registers, and
 // multiplies by a weight matrix that travels in the KERNEL PARAMETER block: every FFMA takes its
 // weight from the constant bank (LDCU.128 + FFMA with a uniform-register operand), so no shared

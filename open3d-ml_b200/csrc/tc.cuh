@@ -1,12 +1,15 @@
-// tc.cuh -- hand-written tcgen05 / TMEM / mbarrier primitives for sm_100a (inline PTX).
+// tc.cuh -- hand-written Hopper (sm_90a) tensor-core primitives: wgmma, mbarrier, bulk copies (inline PTX).
 //
-// Operand convention used by every tensor-core kernel in this library:
+// Operand conventions used by the tensor-core kernels of this library:
 //   * 16-bit operands (fp16), K-major, NO swizzle, "chunk-major" canonical layout
 //         element (row r, k)  ->  byte  (k / 8) * (ROWS * 16) + r * 16 + (k % 8) * 2
 //     i.e. [K/8][ROWS][8 halves]: a thread that owns 8 consecutive k of one row writes ONE
 //     16-byte shared store, consecutive rows are consecutive 16-byte words (conflict-free),
-//     and the UMMA descriptor is  LBO = ROWS*16 (next 8-wide k chunk), SBO = 128 (next 8 rows).
-//   * D = A[M x K] * B[N x K]^T accumulates in TMEM (fp32), lane = row of A, column = row of B.
+//     and the wgmma descriptor is  LBO = ROWS*16 (next 8-wide k chunk), SBO = 128 (next 8 rows).
+//   * fp32 operands (TF32), K-major, SWIZZLE_128B (row r, 16-byte chunk c at r*128 + ((c ^ (r & 7)) << 4)),
+//     SBO = 1024 (next 8 rows), K advanced by +32 B per k8 step.
+//   * wgmma: one warpgroup computes D[64 x N] (+)= A[64 x K] * B[N x K]^T into registers; warp w of the
+//     warpgroup owns rows [16w, 16w+16): d[i] is row 16w + lane/4 + 8*((i/2)%2), column 8*(i/4) + 2*(lane%4) + i%2.
 //   * 22-bit "3xFP16" precision: x = h1 + h2 with h1 = fp16(x), h2 = fp16(x - h1);
 //     A*B ~= A1*B1 + A1*B2 + A2*B1 (three MMAs into the same accumulator).  Relative error
 //     ~2^-21 per product, which keeps the 1e-4 parity bar that plain TF32/BF16 cannot
@@ -56,115 +59,77 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
 __device__ __forceinline__ void fence_async_smem() {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before() {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-
-// ---- TMEM allocation (one full warp executes these) -----------------------------------------
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst) {
-    static_assert(NCOLS == 32 || NCOLS == 64 || NCOLS == 128 || NCOLS == 256 || NCOLS == 512, "pow2 >= 32");
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-                 "n"(NCOLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-
-// ---- descriptors ----------------------------------------------------------------------------
-// shared-memory matrix descriptor, K-major, SWIZZLE_NONE (cute::UMMA::SmemDescriptor bit layout:
-// start[0,14) lbo[16,30) sbo[32,46) version[46,48)=1 layout_type[61,64)=0; all in 16-byte units)
+// ---- wgmma ------------------------------------------------------------------------------------
+// K-major shared-memory matrix descriptor (sm_90 GmmaDescriptor: start[0,14) lbo[16,30) sbo[32,46)
+// layout_type[62,64): 0 = no swizzle, 1 = 128-byte swizzle; addresses and offsets in 16-byte units)
 __device__ __forceinline__ uint64_t smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr >> 4) & 0x3fffu);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3fffu) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3fffu) << 32;
-    d |= (uint64_t)1 << 46;
     return d;
 }
-// instruction descriptor for kind::f16, fp16 x fp16 -> fp32, both operands K-major
-// (cute::UMMA::InstrDescriptor: c_format[4,6)=1 a_format[7,10)=0 b_format[10,13)=0
-//  a_major[15]=0 b_major[16]=0 n_dim[17,23)=N>>3 m_dim[24,29)=M>>4)
-__host__ __device__ constexpr uint32_t idesc_f16(int M, int N) {
-    return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// K-major SWIZZLE_128B: rows of 128 B, 8-row groups 1024 B apart
+__device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t saddr) {
+    return (uint64_t)((saddr >> 4) & 0x3fffu) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
+}
+// register writes (A fragments, accumulators) -> visible to the next wgmma of this warpgroup
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// fp32 word of a TF32 operand -> (hi, lo): hi keeps the 10 explicit mantissa bits TF32 uses,
+// lo = x - hi is exact in fp32 (the tensor core keeps 11 of its <= 13 bits)
+__device__ __forceinline__ void split_tf32(uint32_t x, uint32_t& hi, uint32_t& lo) {
+    hi = x & 0xFFFFE000u;
+    lo = __float_as_uint(__uint_as_float(x) - __uint_as_float(hi));
 }
 
-// D[tmem] (+)= A[smem] * B[smem]^T ; issued by ONE thread
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
+// wgmma_tf32_rs<N>: D[64 x N] (+)= A (registers: the m16n8k8 TF32 fragment of each warp's 16 rows) * B[smem]^T
+// wgmma_f16_ss<N>:  D[64 x N] (+)= A[smem] * B[smem]^T, fp16 operands
+// scale_d = 0 overwrites D instead of accumulating.
+// ---- generated fixed-arity wrappers (one per accumulator width) ----
+template <int N> __device__ void wgmma_tf32_rs(float* d, const uint32_t* a, uint64_t bdesc, uint32_t scale_d);
+template <> __device__ __forceinline__ void wgmma_tf32_rs<32>(float* d, const uint32_t* a, uint64_t bdesc, uint32_t scale_d) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d)
         : "memory");
 }
-// all previously issued MMAs of this thread arrive on the mbarrier when they complete
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                     smem_u32(bar))
-                 : "memory");
-}
-
-// ---- TMEM -> registers: 32 lanes x 32 bit, 16 consecutive columns per thread ----------------
-// The calling warp reads lanes [32*(warp%4), +32); thread t gets lane 32*(warp%4)+t.
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-    uint32_t r[16];
+template <> __device__ __forceinline__ void wgmma_tf32_rs<64>(float* d, const uint32_t* a, uint64_t bdesc, uint32_t scale_d) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float* v) {
-    uint32_t r[8];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// Issue-only forms: several loads in flight behind ONE tcgen05.wait::ld (tmem_ld16 / tmem_ld8 pay a TMEM round trip
-// each).  The destination registers are defined after tmem_ld_wait(); read them through tmem_val(), which pins the
-// read behind the wait in program order.
-__device__ __forceinline__ void tmem_ld16_issue(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d)
         : "memory");
 }
-__device__ __forceinline__ void tmem_ld8_issue(uint32_t taddr, uint32_t* r) {
+template <> __device__ __forceinline__ void wgmma_tf32_rs<128>(float* d, const uint32_t* a, uint64_t bdesc, uint32_t scale_d) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-        : "r"(taddr)
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d)
         : "memory");
 }
-__device__ __forceinline__ void tmem_ld_wait() {
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+template <int N> __device__ void wgmma_f16_ss(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d);
+template <> __device__ __forceinline__ void wgmma_f16_ss<16>(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(adesc), "l"(bdesc), "r"(scale_d)
+        : "memory");
 }
-__device__ __forceinline__ float tmem_val(uint32_t& r) {
-    asm volatile("" : "+r"(r));
-    return __uint_as_float(r);
+template <> __device__ __forceinline__ void wgmma_f16_ss<32>(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(adesc), "l"(bdesc), "r"(scale_d)
+        : "memory");
 }
 
 // ---- fp32 -> (h1, h2) split -----------------------------------------------------------------

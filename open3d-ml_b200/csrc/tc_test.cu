@@ -1,6 +1,6 @@
-// tc_test.cu -- bring-up / regression kernel for the tcgen05 primitives of tc.cuh:
-// D[128, N] = A[128, K] * B[N, K]^T with the 3xFP16 split, one CTA, operands converted and
-// laid out in shared memory by the CTA itself (exactly what the fused kernels do).
+// tc_test.cu -- bring-up / regression kernel for the wgmma primitives of tc.cuh:
+// D[128, N] = A[128, K] * B[N, K]^T with the 3xFP16 split, one CTA (one warpgroup), operands converted and
+// laid out in shared memory by the CTA itself in the chunk-major fp16 layout.
 // Exposed through the C ABI (o3dml_tc_gemm_test) so that tests/test_gpu_tc.py can pin the
 // descriptor encodings against torch.
 #include "../../include/o3dml_b200_bringup.h"
@@ -9,12 +9,34 @@
 
 namespace o3dml {
 
+// D rows [64 h, 64 h + 64) x columns [16 nb, 16 nb + 16) (+)= A * B^T over the whole K, three fp16 products per k16
+// step; `swap` exchanges the LBO / SBO fields (bring-up only)
+__device__ __forceinline__ void tt_block(float* d, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo, int N,
+                                         int K, int terms, bool swap, int h, int nb) {
+    const uint32_t a_lbo = 128 * 16, b_lbo = (uint32_t)N * 16;
+    const uint32_t aL = swap ? 128u : a_lbo, aS = swap ? a_lbo : 128u;
+    const uint32_t bL = swap ? 128u : b_lbo, bS = swap ? b_lbo : 128u;
+    const uint32_t aoff = (uint32_t)h * 64 * 16, boff = (uint32_t)nb * 16 * 16;
+    tc::wgmma_fence();
+    for (int ks = 0; ks < K / 16; ++ks) {
+        const uint64_t ah = tc::smem_desc(a_hi + aoff + ks * 2 * a_lbo, aL, aS);
+        const uint64_t al = tc::smem_desc(a_lo + aoff + ks * 2 * a_lbo, aL, aS);
+        const uint64_t bh = tc::smem_desc(b_hi + boff + ks * 2 * b_lbo, bL, bS);
+        const uint64_t bl = tc::smem_desc(b_lo + boff + ks * 2 * b_lbo, bL, bS);
+        tc::wgmma_f16_ss<16>(d, ah, bh, ks > 0);
+        if (terms >= 3) {
+            tc::wgmma_f16_ss<16>(d, ah, bl, 1u);
+            tc::wgmma_f16_ss<16>(d, al, bh, 1u);
+        }
+    }
+    tc::wgmma_commit();
+    tc::wgmma_wait_all();
+}
+
 __global__ void __launch_bounds__(128, 1)
 tc_gemm_test_kernel(const float* __restrict__ A, const float* __restrict__ B, float* __restrict__ D, int N,
                     int K, int terms) {
     extern __shared__ __align__(128) uint8_t smem[];
-    __shared__ uint64_t mbar;
-    __shared__ uint32_t tmem_base;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int KC = K / 8;
     uint8_t* a_hi = smem;
@@ -42,94 +64,62 @@ tc_gemm_test_kernel(const float* __restrict__ A, const float* __restrict__ B, fl
         *reinterpret_cast<uint4*>(b_lo + tc::op_off(N, r, kc)) = lo;
     }
     tc::fence_async_smem();
-    if (tid == 0) {
-        tc::mbar_init(&mbar, 1);
-        tc::fence_mbar_init();
-    }
     __syncthreads();
-    if (warp == 0) tc::tmem_alloc<256>(&tmem_base);
-    tc::tc_fence_before();
-    __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t taddr = tmem_base;
-    if (tid == 0) {
-        const uint32_t idesc = tc::idesc_f16(128, N);
-        const uint32_t a_lbo = 128 * 16, b_lbo = (uint32_t)N * 16;
-        const int variant = terms >> 8;  // bring-up only: 1 = LBO/SBO fields swapped
-        terms &= 0xff;
-        for (int ks = 0; ks < K / 16; ++ks) {
-            const uint32_t aL = variant ? 128u : a_lbo, aS = variant ? a_lbo : 128u;
-            const uint32_t bL = variant ? 128u : b_lbo, bS = variant ? b_lbo : 128u;
-            const uint64_t ah = tc::smem_desc(tc::smem_u32(a_hi) + ks * 2 * a_lbo, aL, aS);
-            const uint64_t al = tc::smem_desc(tc::smem_u32(a_lo) + ks * 2 * a_lbo, aL, aS);
-            const uint64_t bh = tc::smem_desc(tc::smem_u32(b_hi) + ks * 2 * b_lbo, bL, bS);
-            const uint64_t bl = tc::smem_desc(tc::smem_u32(b_lo) + ks * 2 * b_lbo, bL, bS);
-            tc::umma_f16(taddr, ah, bh, idesc, ks > 0);
-            if (terms >= 3) {
-                tc::umma_f16(taddr, ah, bl, idesc, 1);
-                tc::umma_f16(taddr, al, bh, idesc, 1);
+    const bool swap = (terms >> 8) != 0;  // bring-up only: 1 = LBO/SBO fields swapped
+    terms &= 0xff;
+    const int g = lane >> 2, t = lane & 3;
+    for (int h = 0; h < 2; ++h)
+        for (int nb = 0; nb < N / 16; ++nb) {
+            float d[8];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) d[i] = 0.f;
+            tt_block(d, tc::smem_u32(a_hi), tc::smem_u32(a_lo), tc::smem_u32(b_hi), tc::smem_u32(b_lo), N, K, terms,
+                     swap, h, nb);
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                const int row = h * 64 + warp * 16 + g + ((i >> 1) & 1) * 8, col = nb * 16 + (i >> 2) * 8 + 2 * t + (i & 1);
+                D[(size_t)row * N + col] = d[i];
             }
         }
-        tc::umma_commit(&mbar);
-    }
-    tc::mbar_wait(&mbar, 0);
-    tc::tc_fence_after();
-    const int row = warp * 32 + lane;
-    for (int c0 = 0; c0 < N; c0 += 16) {
-        float v[16];
-        tc::tmem_ld16(taddr + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, v);
-#pragma unroll
-        for (int i = 0; i < 16; ++i) D[(size_t)row * N + c0 + i] = v[i];
-    }
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc<256>(taddr);
 }
 
 
-// Issue-rate probe: `reps` x 6 MMAs (M=128, N, K=16 each) on resident (zeroed) operands, one commit;
+// Issue-rate probe: `reps` x 6 wgmma (M=64, N, K=16 each) per 64-row half on resident (zeroed) operands;
 // out[0] = cycles from first issue to completion, out[1] = cycles spent issuing.
 __global__ void __launch_bounds__(128, 1)
 tc_mma_rate_kernel(int N, int reps, long long* out) {
     extern __shared__ __align__(128) uint8_t smem[];
-    __shared__ uint64_t mbar;
-    __shared__ uint32_t tmem_base;
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const int tid = threadIdx.x;
     const int a_bytes = 4 * 128 * 16, b_bytes = 4 * N * 16;     // 32 channels each
     for (int i = tid; i < (2 * a_bytes + 2 * b_bytes) / 16; i += 128) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
     tc::fence_async_smem();
-    if (tid == 0) { tc::mbar_init(&mbar, 1); tc::fence_mbar_init(); }
     __syncthreads();
-    if (warp == 0) tc::tmem_alloc<256>(&tmem_base);
-    tc::tc_fence_before(); __syncthreads(); tc::tc_fence_after();
-    const uint32_t taddr = tmem_base;
-    if (tid == 0) {
-        const uint32_t idesc = tc::idesc_f16(128, N);
-        const uint32_t a_lbo = 128 * 16, b_lbo = (uint32_t)N * 16;
-        const uint32_t ah0 = tc::smem_u32(smem), al0 = ah0 + a_bytes, bh0 = al0 + a_bytes, bl0 = bh0 + b_bytes;
-        const long long t0 = clock64();
-        for (int r = 0; r < reps; ++r) {
+    const uint32_t a_lbo = 128 * 16, b_lbo = (uint32_t)N * 16;
+    const uint32_t ah0 = tc::smem_u32(smem), al0 = ah0 + a_bytes, bh0 = al0 + a_bytes, bl0 = bh0 + b_bytes;
+    float d[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    const long long t0 = clock64();
+    tc::wgmma_fence();
+    for (int r = 0; r < reps; ++r)
+        for (int nb = 0; nb < N / 16; ++nb)
 #pragma unroll
             for (int ks = 0; ks < 2; ++ks) {
                 const uint64_t ah = tc::smem_desc(ah0 + ks * 2 * a_lbo, a_lbo, 128);
                 const uint64_t al = tc::smem_desc(al0 + ks * 2 * a_lbo, a_lbo, 128);
-                const uint64_t bh = tc::smem_desc(bh0 + ks * 2 * b_lbo, b_lbo, 128);
-                const uint64_t bl = tc::smem_desc(bl0 + ks * 2 * b_lbo, b_lbo, 128);
-                tc::umma_f16(taddr, ah, bh, idesc, 1);
-                tc::umma_f16(taddr, ah, bl, idesc, 1);
-                tc::umma_f16(taddr, al, bh, idesc, 1);
+                const uint64_t bh = tc::smem_desc(bh0 + nb * 256 + ks * 2 * b_lbo, b_lbo, 128);
+                const uint64_t bl = tc::smem_desc(bl0 + nb * 256 + ks * 2 * b_lbo, b_lbo, 128);
+                tc::wgmma_f16_ss<16>(d, ah, bh, 1u);
+                tc::wgmma_f16_ss<16>(d, ah, bl, 1u);
+                tc::wgmma_f16_ss<16>(d, al, bh, 1u);
             }
-        }
-        const long long t1 = clock64();
-        tc::umma_commit(&mbar);
-        tc::mbar_wait(&mbar, 0);
-        const long long t2 = clock64();
+    tc::wgmma_commit();
+    const long long t1 = clock64();
+    tc::wgmma_wait_all();
+    const long long t2 = clock64();
+    if (tid == 0) {
         out[0] = t2 - t0;
         out[1] = t1 - t0;
     }
-    __syncthreads();
-    tc::tc_fence_before(); __syncthreads();
-    if (warp == 0) tc::tmem_dealloc<256>(taddr);
+    if (d[0] != 0.f) out[2] = 1;   // keeps the accumulator (and the MMAs) alive; never true on zeroed operands
 }
 
 }  // namespace o3dml

@@ -1,4 +1,4 @@
-"""KPFCNN forward on the sm_100a kernels: the fused replacement of ``KPFCNN.forward``
+"""KPFCNN forward on the sm_90a kernels: the fused replacement of ``KPFCNN.forward``
 (ml3d/torch/models/kpconv.py:270-291) for rigid KPConv with linear influence and sum
 aggregation (every shipped config except the deformable Paris-Lille3D one, SURVEY.md A11).
 

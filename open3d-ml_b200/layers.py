@@ -1,4 +1,4 @@
-"""``open3d.ml.torch.layers.SparseConv`` / ``SparseConvTranspose`` on the sm_100a kernels
+"""``open3d.ml.torch.layers.SparseConv`` / ``SparseConvTranspose`` on the sm_90a kernels
 (call sites: ml3d/torch/models/sparseconvnet.py:344-485 -- SubmanifoldSparseConv, Convolution, DeConvolution of
 SparseConvUnet).  Same constructor arguments and parameter names (``kernel`` [kx, ky, kz, Cin, Cout], ``bias``) as
 the upstream layers, so reference checkpoints load; inference only (no autograd through the CUDA path).

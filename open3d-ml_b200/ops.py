@@ -1,6 +1,6 @@
 """Host-side mirror of ``open3d.ml.torch.ops`` / ``open3d.ml.torch.layers`` /
 ``open3d.core.nns`` for the operators on the hot path (SURVEY.md section 2.2),
-backed by the sm_100a kernels of libo3dml_b200.so.
+backed by the sm_90a kernels of libo3dml_b200.so.
 
 Same names, argument meaning, result field names and error behaviour
 (RuntimeError) as the interface the reference's models call:

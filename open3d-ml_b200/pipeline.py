@@ -2,9 +2,9 @@
 
 The reference pipelines (ml3d/torch/pipelines/semantic_segmentation.py:141-178 run_test,
 object_detection.py:96-139 run_valid) move every batch to the device synchronously
-(`inputs['data'].to(device)`) and read the result back before touching the next batch.  On
-B200 the PCIe copy of a SemanticKITTI batch (~90 MB of neighbour indices) costs about half
-of the fused forward, so the runner overlaps them: the inputs of batch k+1 cross PCIe on a
+(`inputs['data'].to(device)`) and read the result back before touching the next batch.  The
+PCIe copy of a SemanticKITTI batch (~90 MB of neighbour indices) is comparable to the fused
+forward, so the runner overlaps them: the inputs of batch k+1 cross PCIe on a
 copy stream while batch k computes, and the result of batch k returns on a second copy
 stream.  Every batch's inputs and results still cross the bus; nothing is cached.
 """

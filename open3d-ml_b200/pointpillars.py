@@ -1,4 +1,4 @@
-"""PointPillars forward on the sm_100a kernels: the fused replacement of
+"""PointPillars forward on the sm_90a kernels: the fused replacement of
 ``PointPillars.forward`` (ml3d/torch/models/point_pillars.py:102-134):
 
     voxelize (all frames in ONE batched call, no per-frame Python loop, :112-128, :328-382)

@@ -1,4 +1,4 @@
-"""RandLA-Net forward on the sm_100a kernels: the fused replacement of
+"""RandLA-Net forward on the sm_90a kernels: the fused replacement of
 ``RandLANet.forward`` (ml3d/torch/models/randlanet.py:241-298) and of the layers it
 calls (SharedMLP :471-518, LocalSpatialEncoding :521-605, AttentivePooling :608-639,
 LocalFeatureAggregation :642-692, random_sample :300-327, nearest_interpolation
@@ -20,8 +20,8 @@ import torch
 from . import _lib as L
 
 BN_EPS = 1e-6  # randlanet.py:77,499
-# d_out values served by the tcgen05 kernel (lfa_tc.cu).  d = 16 stays on the FP32 SIMT kernel: its
-# 16x16 score product is too small to pay for the per-tile MMA round trip (0.84 vs 1.23 ms measured);
+# d_out values served by the wgmma kernel (lfa_tc.cu).  d = 16 stays on the FP32 SIMT kernel with its weights in the
+# kernel parameter block: a 16x16 score product is too small to pay for a per-tile tensor-core round trip;
 # d = 512 (fifth encoder of the 5-level configs, a few hundred points) runs on the tiled SIMT kernel (lfa.cu).
 TC_DIMS = (32, 64, 128, 256)
 SUPPORTED_DIMS = (16, 32, 64, 128, 256, 512)
@@ -89,7 +89,7 @@ class RandLANetB200:
                 raise RuntimeError("RandLANetB200: encoder %d has dim_output %d; the fused LFA kernels serve %s"
                                    % (i, d, SUPPORTED_DIMS))
             self.d_out.append(d)
-            if d in TC_DIMS:   # tcgen05 path: host-packed fp16 hi/lo operand images ([out][in])
+            if d in TC_DIMS:   # tensor-core path: host-packed fp16 hi/lo operand images ([out][in])
                 for pool in ("pool1", "pool2"):
                     self.w["%s.%s.score.img" % (p, pool)] = L.pack_operand_image(
                         sd["%s.%s.score_fn.0.weight" % (p, pool)])
@@ -123,7 +123,7 @@ class RandLANetB200:
         self.num_classes = sd["fc1.3.conv.weight"].shape[0]
         self.in_channels = sd["fc0.weight"].shape[1]
         self._buf = {}
-        # ---- fused tail (rl_tail.cu): last decoder layer + fc1 stack chained through tensor memory
+        # ---- fused tail (rl_tail.cu): last decoder layer + fc1 stack in one kernel
         self.use_tail = os.environ.get("O3DML_RL_TAIL", "1") != "0"
         self.tail = None
         pl = "decoder.%d" % (num_layers - 1)
@@ -352,7 +352,7 @@ class RandLANetB200:
         ent = self._graphs.get(key)
         if ent is None:
             import os
-            legacy = os.environ.get("O3DML_GRAPH_LEGACY") == "1"      # debugging hook: the round-2 first version
+            legacy = os.environ.get("O3DML_GRAPH_LEGACY") == "1"      # debugging hook: global capture mode
             thunk()                                        # sizes the cached buffers, sets kernel attributes
             if legacy:
                 torch.cuda.current_stream().synchronize()

@@ -9,7 +9,7 @@ README.md:313-314 / set_open3d_ml_root.sh:1-3 of the reference.  With it,
     net = ml3d.models.RandLANet(**cfg.model)
 
 runs the reference's models, dataloaders and pipelines with every native op on the
-B200 kernels.  Symbols that the reference imports at module load but that are outside
+sm_90a kernels.  Symbols that the reference imports at module load but that are outside
 the hot path (SURVEY.md Appendix B checklist) raise NotImplementedError when CALLED.
 """
 import importlib

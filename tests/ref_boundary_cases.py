@@ -2,11 +2,14 @@
 drop-in boundary open3d_ml_b200.shim.  Run as a script in a fresh process (the shim owns
 sys.modules['open3d']):
 
-    python tests/ref_boundary_cases.py <case> [--ops oracle]
+    python tests/ref_boundary_cases.py <case> [--ops oracle] [--record DIR]
 
-`--ops oracle` binds the CPU oracle instead of the CUDA library (oracle/refshim.py): a dry run of the same
-flows on a box without a GPU (used by the CPU test-suite to keep this script honest); the GPU tests in
-tests/test_gpu_reference_boundary.py run it with the product shim.  Prints one JSON line.
+`--ops oracle` binds the CPU oracle instead of the CUDA library (oracle/refshim.py): the same flows on a machine
+without a GPU.  The models get seeded weights rebuilt from a manifest (oracle/weights.py), so that
+`--record DIR` can store what a fused forward needs to be compared without the reference tree: the manifest,
+the inputs the reference's own preprocess / transform / batcher built, and a seeded sample of the reference
+outputs, as DIR/boundary_<case>.npz (tests/golden/, read by tests/test_gpu_reference_boundary.py).
+Prints one JSON line.
 """
 import json
 import os
@@ -50,6 +53,26 @@ def ref_modules():
     return m, Config
 
 
+SEED = 1234
+REC = {}          # arrays of the case for --record
+
+
+def seed_weights(net):
+    """Seeded weights with non-trivial BN statistics, rebuilt from a manifest of the class's state_dict."""
+    from oracle import weights
+    man = weights.manifest_from_state_dict(net.state_dict())
+    net.load_state_dict(weights.seeded_state_dict(man, SEED), strict=True)
+    REC.update(manifest=json.dumps(man), weight_seed=SEED)
+
+
+def record_output(name, t, m=8192):
+    """A fixed, seeded sample of a reference output: flat indices, values, shape and the scale max |t|."""
+    a = torch.as_tensor(t).detach().double().cpu().reshape(-1).numpy()
+    idx = np.sort(np.random.default_rng(len(REC)).choice(a.size, size=min(m, a.size), replace=False))
+    REC.update({name + "_idx": idx.astype(np.int64), name + "_val": a[idx], name + "_shape": np.array(list(t.shape)),
+                name + "_absmax": np.abs(a).max()})
+
+
 def rel(a, b):
     a, b = torch.as_tensor(a).double().cpu(), torch.as_tensor(b).double().cpu()
     return float((a - b).abs().max() / b.abs().max().clamp_min(1e-30))
@@ -74,11 +97,7 @@ def case_pointpillars_class(root, dev):
     torch.manual_seed(0)
     net = ml3d.models.PointPillars(**cfg.model, device=dev)
     net.eval()
-    for m in net.modules():               # non-trivial BN statistics so that folding errors would show
-        if isinstance(m, (torch.nn.BatchNorm1d, torch.nn.BatchNorm2d)):
-            m.running_mean.normal_(0, 0.1)
-            m.running_var.uniform_(0.5, 2.0)
-    net.bbox_head.conv_cls.bias.data.fill_(0.0)     # scores around 0.5: the rotated NMS has something to do
+    seed_weights(net)
     batcher = ml3d.dataloaders.ConcatBatcher(dev, model="PointPillars")
     items = []
     for s in (11, 12):
@@ -93,9 +112,14 @@ def case_pointpillars_class(root, dev):
         ref = net(data)
         boxes = net.inference_end(ref, data)
     out = dict(ref_shapes=[list(r.shape) for r in ref], boxes_per_frame=[len(b) for b in boxes])
+    from open3d_ml_b200.pointpillars import cfg_from_reference
+    REC.update(cfg=json.dumps(cfg_from_reference(cfg.model)), frames=len(data.point))
+    for i, pt in enumerate(data.point):
+        REC["point_%d" % i] = pt.detach().cpu().numpy()
+    for i, r in enumerate(ref):
+        record_output("ref_%d" % i, r)
     if dev != "cpu":
         import open3d_ml_b200 as M
-        from open3d_ml_b200.pointpillars import cfg_from_reference
         fused = M.PointPillarsB200(net.state_dict(), cfg_from_reference(cfg.model))
         got = fused(data.point)
         out["rel_err"] = [rel(g, r) for g, r in zip(got, ref)]
@@ -124,14 +148,19 @@ def case_randlanet_patch(root, dev):
     net = ml3d.models.RandLANet(**cfg.model)
     net.device = "cpu"
     net.eval()
-    for m in net.modules():
-        if isinstance(m, (torch.nn.BatchNorm1d, torch.nn.BatchNorm2d)):
-            m.running_mean.normal_(0, 0.1)
-            m.running_var.uniform_(0.5, 2.0)
+    seed_weights(net)
     inp = _randla_inputs(net, 8192, 21)
     with torch.no_grad():
         ref = net(inp)
     out = dict(ref_shape=list(ref.shape))
+    REC.update(num_layers=net.cfg.num_layers, num_neighbors=net.cfg.num_neighbors,
+               sub_sampling_ratio=np.array(list(net.cfg.sub_sampling_ratio)), features=inp["features"].numpy(),
+               ref_argmax=ref.argmax(-1).numpy().astype(np.uint8))
+    for k in ("coords", "neighbor_indices", "sub_idx", "interp_idx"):
+        for i, a in enumerate(inp[k]):
+            a = a.numpy()
+            REC["%s_%d" % (k, i)] = a.astype(np.int32) if a.dtype == np.int64 else a
+    record_output("ref", ref)
     if dev != "cpu":
         from open3d_ml_b200.randlanet import patch_reference_model
         patch_reference_model(net)
@@ -179,10 +208,7 @@ def case_kpconv_class(root, dev):
                              first_subsampling_dl=0.04, in_radius=1.5, min_in_points=3000)
     net.device = "cpu"
     net.eval()
-    for m in net.modules():
-        if isinstance(m, torch.nn.BatchNorm1d):
-            m.running_mean.normal_(0, 0.1)
-            m.running_var.uniform_(0.5, 2.0)
+    seed_weights(net)
     pts, feats = synth.room_cloud(6000, 41, room=(2.0, 1.6, 1.2))
     data = {"point": pts, "feat": feats[:, 1:4], "label": np.random.randint(0, 5, len(pts)).astype(np.int32)}
     attr = {"split": "test"}
@@ -192,6 +218,14 @@ def case_kpconv_class(root, dev):
     with torch.no_grad():
         ref = net(inputs["data"])
     out = dict(ref_shape=list(ref.shape), levels=[int(p.shape[0]) for p in inputs["data"].points])
+    b = inputs["data"]
+    REC.update(cfg=json.dumps(dict(net.cfg), default=lambda o: o.tolist() if hasattr(o, "tolist") else list(o)),
+               levels=len(b.points), features=b.features.numpy())
+    for k in ("points", "neighbors", "pools", "upsamples"):
+        for i, a in enumerate(getattr(b, k)):
+            a = a.numpy()
+            REC["%s_%d" % (k, i)] = a.astype(np.int32) if a.dtype == np.int64 else a
+    record_output("ref", ref)
     if dev != "cpu":
         import open3d_ml_b200 as M
         fused = M.KPFCNNB200(net.state_dict(), dict(net.cfg))
@@ -210,4 +244,6 @@ if __name__ == "__main__":
     root = install(ops)
     dev = "cpu" if ops == "oracle" or not torch.cuda.is_available() else "cuda"
     res = CASES[case](root, dev)
+    if "--record" in sys.argv:
+        np.savez_compressed(os.path.join(sys.argv[sys.argv.index("--record") + 1], "boundary_%s.npz" % case), **REC)
     print("RESULT " + json.dumps(dict(case=case, ops=ops, device=dev, **res)))

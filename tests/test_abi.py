@@ -31,12 +31,12 @@ def test_library_builds_loads_and_exports_everything():
     assert _lib.lib().o3dml_last_error() is not None
 
 
-def test_sass_is_sm100a_only():
+def test_sass_is_sm90a_only():
     import subprocess
     from open3d_ml_b200 import build
     out = subprocess.run(["cuobjdump", "-lelf", build.build()], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_\d+a?", out))
-    assert archs == {"sm_100a"}, archs
+    assert archs == {"sm_90a"}, archs
 
 
 def test_ops_fail_loudly_without_cuda():

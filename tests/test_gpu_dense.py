@@ -42,7 +42,7 @@ def rnd(*shape, seed=0):
                                         # short products on many row tiles: the two-CTAs-per-SM LITE kernels (gemm_tc.cu GtCfg)
                                         (30000, 64, 64), (20011, 96, 128), (40000, 128, 32)])
 def test_linear_plain(n, cin, cout, tc):
-    """tc=True: PackedWeight -> tcgen05 kernel (gemm_tc.cu) whenever cin % 8 == 0, SIMT otherwise."""
+    """tc=True: PackedWeight -> wgmma kernel (gemm_tc.cu) whenever cin % 8 == 0, SIMT otherwise."""
     x, w = rnd(n, cin, seed=1), rnd(cin, cout, seed=2) / cin ** 0.5
     s, t = rnd(cout, seed=3).abs() + 0.5, rnd(cout, seed=4)
     out = torch.full((n, cout), float("nan")).cuda()
@@ -178,7 +178,7 @@ def test_kpconv_gather_vs_torch(cin, H):
 @pytest.mark.parametrize("mag", [1e-20, 1e-6, 1e-3, 1.0, 3e4, 1e20])
 def test_linear_tc_is_magnitude_independent(mag):
     """The TF32 split keeps fp32's exponent (gemm_tc.cu): the relative error must not depend on the
-    scale of the activations (the fp16 split of round 1 needed a per-tile range normalisation for this)."""
+    scale of the activations (an fp16 split would need a per-tile range normalisation for this)."""
     n, cin, cout = 3000, 256, 64
     x, w = rnd(n, cin, seed=1) * mag, rnd(cin, cout, seed=2) * 1e-3
     out = torch.empty(n, cout).cuda()

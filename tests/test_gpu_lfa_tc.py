@@ -1,4 +1,4 @@
-"""The tcgen05 LFA kernel (lfa_tc.cu) against the FP32 SIMT kernel (lfa.cu) on identical
+"""The wgmma LFA kernel (lfa_tc.cu) against the FP32 SIMT kernel (lfa.cu) on identical
 inputs, and end-to-end through the model (the golden / port parity tests in
 test_gpu_models.py run with the tensor-core path enabled by default)."""
 import numpy as np
@@ -73,7 +73,7 @@ def lfa_reference(stage, d, coords, nidx, feat, w10, s10, t10, wl2, s2, t2, ws, 
 @pytest.mark.parametrize("d", [16, 32, 64, 128, 256])
 @pytest.mark.parametrize("stage", [1, 2])
 def test_lfa_kernels_vs_float64_reference(d, stage):
-    """Every LFA implementation (FP32 SIMT, parameter-block d = 16, tcgen05) against float64 torch;
+    """Every LFA implementation (FP32 SIMT, parameter-block d = 16, wgmma) against float64 torch;
     tolerance 1e-4 relative to the tensor scale (north_star), measured values are ~1e-6."""
     B, N = 2, 700
     args = make(d, B, N, 100 + d + stage)

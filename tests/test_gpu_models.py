@@ -269,7 +269,7 @@ def test_randlanet_five_level_config_vs_golden_reference():
 
 
 def test_randlanet_fused_tail_matches_the_layerwise_path():
-    """rl_tail.cu (last decoder layer + fc1 stack chained through tensor memory) against the four separate launches,
+    """rl_tail.cu (last decoder layer + fc1 stack in one kernel) against the four separate launches,
     on reference-shaped inputs (int64 batch-relative interp_idx, ragged last tile) and on the device pyramid."""
     sd, _ = H.state_dict("randlanet_semantickitti.manifest.json", 6)
     net = M.RandLANetB200(sd)

@@ -1,4 +1,4 @@
-"""tcgen05 bring-up: the descriptor encodings / operand layout of tc.cuh against torch."""
+"""wgmma bring-up: the descriptor encodings / operand layout of tc.cuh against torch."""
 import pytest
 import torch
 

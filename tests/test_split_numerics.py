@@ -1,4 +1,4 @@
-"""The 3xFP16 split arithmetic of the tcgen05 kernels (csrc/tc.cuh, gemm_tc.cu, lfa_tc.cu), emulated in
+"""The 3xFP16 split arithmetic of the tensor-core kernels (csrc/tc.cuh, gemm_tc.cu, lfa_tc.cu), emulated in
 numpy on the CPU: x = hi + lo with hi = fp16(x), lo = fp16(x - hi); A.B ~ A_hi.B_hi + A_hi.B_lo + A_lo.B_hi
 accumulated in fp32.  These tests pin (a) the host-side operand image layout, (b) the error level the
 kernels are designed for (~1e-6 of the result scale, 100x inside the 1e-4 parity bar), and (c) why both
@@ -41,7 +41,7 @@ def test_operand_image_layout_and_precision():
     assert torch.equal(hi, w.to(torch.float16).float())              # chunk-major [K/8][N][8]
     # hi + lo carries 22 mantissa bits of w
     assert float(((hi + lo) - w).abs().max() / w.abs().max()) < 2.0 ** -21
-    # chunk c of row r sits at uint4 index c * N + r (what the UMMA descriptor's LBO = N * 16 B assumes)
+    # chunk c of row r sits at uint4 index c * N + r (what the wgmma descriptor's LBO = N * 16 B assumes)
     u = img[: n * k].view(k // 8, n, 8)
     assert torch.equal(u[3, 5], w[5, 24:32].to(torch.float16))
 
@@ -90,7 +90,7 @@ def test_packed_weight_exponent_matches_the_kernel_contract():
     assert float((hi + lo)[40:].abs().max()) == 0.0                                # zero padding
 
 
-# ---- the 3xTF32 split of gemm_tc.cu (round 2) -------------------------------------------------------
+# ---- the 3xTF32 split of gemm_tc.cu -------------------------------------------------------------------
 def _tf32_trunc(x):
     return (x.view(np.uint32) & np.uint32(0xFFFFE000)).view(np.float32)
 
