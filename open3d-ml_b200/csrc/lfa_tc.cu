@@ -9,25 +9,28 @@
 //                   as fp16 hi/lo pairs.  In stage 2 the first half of A first holds r1 (the A
 //                   operand of the lse2 GEMM) and is then overwritten by the gathered features.
 //   B  [d x d]    : score weight, host-packed hi/lo operand image; resident in shared memory for
-//                   d <= 128, copied one 32-row column block at a time for d = 256
-//   D             : 32 score columns at a time, each warpgroup's [64 x 32] block in registers (wgmma), staged
-//                   through shared memory so that a thread sees one neighbour row
-// Epilogue: thread = one neighbour row; softmax over the 16 rows of a point is a half-warp reduction
-// (redux.sync max on order-preserving ints, reduce-scatter shuffles for the two sums), after which
-// lane j of the half-warp owns output channel c0+j -> coalesced stores.
-// Stage 2 chains a second GEMM (r2 = lrelu(BN(Wl2 . r1)), N = d/2) back into A (d = 16: that 8x8 product
-// stays in registers).  The score bias is not applied: it is constant over the neighbours of a point and
-// cancels in the softmax.  CTAs are persistent over tiles.
+//                   d <= 128, streamed for d = 256 through a ring of two 32-row column blocks filled by bulk
+//                   copies (mbarrier completion), one tile's blocks after the other's
+//   D             : CB score columns per block (64 for d = 64 / 128, 32 for d = 256, d below), each warpgroup's
+//                   [64 x CB] block in registers; block j + 1 is issued into a second accumulator set before the
+//                   epilogue of block j runs (wait_group 1)
+// Epilogue on the accumulator registers: warp w of a warpgroup holds rows [16w, 16w + 16) = the 16 neighbours of one
+// point, a thread rows g and g + 8 of its column pairs.  Column max and the sums of e and e.x over the 16 rows: the two
+// rows in registers, then the 8 lanes sharing lane % 4 (max: butterfly; sums: reduce-scatter, so that the lanes store
+// distinct columns of the point's agg row).  x = hi + lo is read from A at (row, column pair), one conflict-free 4-byte
+// load per operand.
+// Stage 2 chains a second GEMM (r2 = lrelu(BN(Wl2 . r1)), N = d/2) whose epilogue writes r2 from the registers into
+// A (d = 16: that 8x8 product stays in registers).  The score bias is not applied: it is constant over the neighbours of
+// a point and cancels in the softmax.  CTAs are persistent over tiles.  Two tiles are in flight per SM at d = 64 (two
+// CTAs) and d = 128 (two A tiles in one CTA: tile t+1 is built while tile t's score MMAs run).
 #include "../../include/o3dml_b200.h"
 #include "common.cuh"
 #include "tc.cuh"
-#include <limits.h>
 
 namespace o3dml {
 
 constexpr int LTC_ROWS = 128;  // MMA M
 constexpr int LTC_K = 16;      // neighbours
-constexpr int LTC_SB_LD = 36;  // staged accumulator row stride (floats): a 32-column block + 4
 
 struct LfaTcParams {
     const float* coords;
@@ -54,24 +57,36 @@ struct LtcCfg {
     static constexpr bool MMA2 = STAGE == 2 && H >= 16;  // lse2 on the tensor core
     static constexpr int NTH = 256;                  // threads per CTA: two warpgroups
     static constexpr int NPART = NTH / LTC_ROWS;     // threads sharing one row
-    static constexpr int CB = D < 32 ? D : 32;       // score columns per block
-    static constexpr int CB2 = H < 32 ? H : 32;      // lse2 columns per block
+    // score columns per block: 64 where the weight is resident, 32 where it streams through the ring (two 64-column
+    // slots would not fit next to the 128 KB A tile)
+    static constexpr int CB = D < 64 ? D : (STREAM ? 32 : 64);
+    static constexpr int NBLK = D / CB;
+    static constexpr int CB2 = STREAM ? 32 : (H < 64 ? H : 64);  // lse2 columns per block
     static constexpr int A_BYTES = D / 8 * LTC_ROWS * 16;  // one of hi / lo
-    static constexpr int B_BYTES = STREAM ? D / 8 * CB * 16 : D / 8 * D * 16;
+    static constexpr int SLOT_BYTES = D / 8 * CB * 16;     // one of hi / lo of one streamed column block
+    static constexpr int B_BYTES = STREAM ? 2 * SLOT_BYTES : D / 8 * D * 16;  // per hi / lo; streamed: two ring slots
     static constexpr int B2_BYTES = MMA2 ? (STREAM ? H / 8 * CB2 * 16 : H / 8 * H * 16) : 0;
-    static constexpr int SB_BYTES = LTC_ROWS * LTC_SB_LD * 4;
     static constexpr int W10_BYTES = 12 * H * 4;
     static constexpr int ST2_BYTES = STAGE == 2 ? (2 * H + (H < 16 ? H * H : 0)) * 4 : 0;
-    static constexpr size_t SMEM = 2 * A_BYTES + 2 * B_BYTES + 2 * B2_BYTES + SB_BYTES + W10_BYTES + ST2_BYTES + 128;
+    // Two tiles in flight per SM, so that the SIMT build of one tile overlaps the score MMAs of the other: d = 64 as two
+    // CTAs per SM (<= 128 registers), d = 128 as two A tiles in one CTA (the CTA builds tile t+1 into one while the
+    // tensor core works on tile t in the other).  d = 256 has room for neither.
+    static constexpr int MIN_CTAS = D == 64 ? 2 : 1;
+    static constexpr bool DBUF = D == 128;
+    static constexpr int NBUF = DBUF ? 2 : 1;
+    static constexpr size_t SMEM = NBUF * 2 * A_BYTES + 2 * B_BYTES + 2 * B2_BYTES + W10_BYTES + ST2_BYTES + 16 + 128;
 };
 
-// The warpgroup's 64 rows of A[128 x K] times a block of CBN rows of B (both hi / lo, chunk-major) -> d[CBN / 2]
+// Issues (does not wait for) the warpgroup's 64 rows of A[128 x K] times a block of CBN rows of B (both hi / lo,
+// chunk-major) -> d[CBN / 2], as one committed wgmma group
 template <int CBN, int K>
-__device__ __forceinline__ void ltc_gemm(float* d, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
-                                         uint32_t b_lbo, int wg) {
+__device__ __forceinline__ void ltc_issue(float* d, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
+                                          uint32_t b_lbo, int wg) {
     constexpr uint32_t A_LBO = LTC_ROWS * 16;
     a_hi += (uint32_t)wg * 64 * 16;
     a_lo += (uint32_t)wg * 64 * 16;
+#pragma unroll
+    for (int i = 0; i < CBN / 2; ++i) tc::fence_operand(d[i]);
     tc::wgmma_fence();
 #pragma unroll
     for (int ks = 0; ks < K / 16; ++ks) {
@@ -84,54 +99,90 @@ __device__ __forceinline__ void ltc_gemm(float* d, uint32_t a_hi, uint32_t a_lo,
         tc::wgmma_f16_ss<CBN>(d, al, bh, 1u);
     }
     tc::wgmma_commit();
-    tc::wgmma_wait_all();
+#pragma unroll
+    for (int i = 0; i < CBN / 2; ++i) tc::fence_operand(d[i]);
 }
 
-// D[:, 32 nb + (0 .. CBN)) = A[:, 0 .. K) * W^T for the column block nb of a weight with NIMG output rows (host image
-// [K/8][NIMG][8] hi, then lo), staged into sb [128][LTC_SB_LD].  Resident weights (bsm holds the whole image) are addressed
-// in place; otherwise the block is first copied into bsm.  Ends with the staged block visible to the whole CTA.
-template <int CBN, int K, int NIMG, bool RESIDENT>
-__device__ __forceinline__ void ltc_block(const uint8_t* a_hi, const uint8_t* a_lo, uint8_t* bsm, int bsm_half_bytes,
-                                          const uint4* __restrict__ img, int nb, float* sb, int tid) {
-    if (!RESIDENT) {
-        __syncthreads();     // the previous block's MMAs are done with bsm
-        constexpr int N_U4 = K / 8 * CBN;
-        for (int i = tid; i < 2 * N_U4; i += 256) {
-            const int im = i / N_U4, rem = i % N_U4, kc = rem / CBN, r = rem % CBN;
-            reinterpret_cast<uint4*>(bsm + im * bsm_half_bytes)[rem] = img[(size_t)im * (K / 8) * NIMG + kc * NIMG + nb * CBN + r];
-        }
-        tc::fence_async_smem();
-        __syncthreads();
-    }
-    const uint32_t b_hi = tc::smem_u32(bsm) + (RESIDENT ? (uint32_t)nb * CBN * 16 : 0u);
-    const uint32_t b_lo = b_hi + (uint32_t)bsm_half_bytes;
-    const int wg = tid >> 7, lane = tid & 31, g = lane >> 2, t = lane & 3;
-    float d[CBN / 2];
-    ltc_gemm<CBN, K>(d, tc::smem_u32(a_hi), tc::smem_u32(a_lo), b_hi, b_lo, (RESIDENT ? NIMG : CBN) * 16, wg);
-    const int r0 = wg * 64 + ((tid >> 5) & 3) * 16 + g;
+// Waits until at most N of this warpgroup's wgmma groups are pending; d (the oldest group's accumulators) is then final
+template <int N, int CNT>
+__device__ __forceinline__ void ltc_wait(float* d) {
+    tc::wgmma_wait<N>();
 #pragma unroll
-    for (int i = 0; i < CBN / 2; i += 2)
-        *reinterpret_cast<float2*>(sb + (r0 + ((i >> 1) & 1) * 8) * LTC_SB_LD + (i >> 2) * 8 + 2 * t) = make_float2(d[i], d[i + 1]);
-    __syncthreads();
+    for (int i = 0; i < CNT; ++i) tc::fence_operand(d[i]);
+}
+
+// One bulk copy (TMA) per (hi / lo, 8-row k chunk) of column block nb of a weight image [K/8][NIMG][8] (hi, then lo)
+// into a ring slot [hi | lo] of [K/8][CBN][8] each, completing on bar.  Every thread of the CTA runs it and the lanes of
+// the warp with `issuer` set issue the copies: the instructions are predicated rather than branched around, because a
+// divergent branch while a wgmma group is in flight makes ptxas serialize the wgmma instructions.
+template <int CBN, int K, int NIMG>
+__device__ __forceinline__ void ltc_fill(uint8_t* slot, uint64_t* bar, const uint4* __restrict__ img, int nb, int lane,
+                                         bool issuer) {
+    constexpr uint32_t ROW = CBN * 16, HALF = K / 8 * ROW;
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t"
+                 "@p mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n\t}" ::"r"(tc::smem_u32(bar)),
+                 "r"(2 * HALF), "r"((int)(issuer && lane == 0))
+                 : "memory");
+#pragma unroll
+    for (int i0 = 0; i0 < 2 * (K / 8); i0 += 32) {
+        const int i = i0 + lane, im = i / (K / 8), kc = i % (K / 8);
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
+                     "@p cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n\t}"
+                     ::"r"(tc::smem_u32(slot + im * HALF + kc * ROW)),
+                     "l"(img + ((size_t)im * (K / 8) + kc) * NIMG + nb * CBN), "r"(ROW), "r"(tc::smem_u32(bar)),
+                     "r"((int)(issuer && i < 2 * (K / 8)))
+                     : "memory");
+    }
+}
+
+// Column sums of one score block over the 16 rows (neighbours) of the warp's point, reduce-scattered over the 8 lanes
+// that share lane % 4 (lane bits 4, 3, 2).  a[i], b[i] hold column 8 (i / 2) + 2 (lane % 4) + i % 2 of the block;
+// afterwards a[0 .. CNT), b[0 .. CNT) hold columns i = base + k (same mapping) summed over all 16 rows, with
+// CNT = max(CNT0 / 8, 1).  Trip counts are template parameters so that a and b stay in registers.
+template <int CNT, int BIT>
+__device__ __forceinline__ void ltc_reduce_scatter(float* a, float* b, int lane, int& base) {
+    if constexpr (BIT >= 4) {
+        if constexpr (CNT > 1) {
+            constexpr int h = CNT / 2;
+            const bool up = (lane & BIT) != 0;
+#pragma unroll
+            for (int i = 0; i < h; ++i) {
+                const float ra = __shfl_xor_sync(0xffffffffu, up ? a[i] : a[i + h], BIT);
+                const float rb = __shfl_xor_sync(0xffffffffu, up ? b[i] : b[i + h], BIT);
+                a[i] = (up ? a[i + h] : a[i]) + ra;
+                b[i] = (up ? b[i + h] : b[i]) + rb;
+            }
+            base += up ? h : 0;
+            ltc_reduce_scatter<h, BIT / 2>(a, b, lane, base);
+        } else {
+            a[0] += __shfl_xor_sync(0xffffffffu, a[0], BIT);
+            b[0] += __shfl_xor_sync(0xffffffffu, b[0], BIT);
+            ltc_reduce_scatter<1, BIT / 2>(a, b, lane, base);
+        }
+    }
 }
 
 template <int D, int STAGE>
-__global__ void __launch_bounds__(LtcCfg<D, STAGE>::NTH, 1)
+__global__ void __launch_bounds__(LtcCfg<D, STAGE>::NTH, LtcCfg<D, STAGE>::MIN_CTAS)
 lfa_pool_tc_kernel(const __grid_constant__ LfaTcParams p) {
     using C = LtcCfg<D, STAGE>;
     constexpr int H = C::H, NTH = C::NTH, NPART = C::NPART, CB = C::CB, CB2 = C::CB2;
     extern __shared__ __align__(128) uint8_t smem[];
-    uint8_t* a_hi = smem;
-    uint8_t* a_lo = a_hi + C::A_BYTES;
-    uint8_t* b_sm = a_lo + C::A_BYTES;                                // [hi | lo] score weight (or one column block)
+    // A buffer i: hi at smem + 2 i A_BYTES, lo right behind it
+    uint8_t* b_sm = smem + C::NBUF * 2 * C::A_BYTES;  // [hi | lo] resident score weight, or two ring slots [hi | lo] each
     uint8_t* b2_sm = b_sm + 2 * C::B_BYTES;                           // [hi | lo] lse2 weight (or one column block)
-    float* SB = reinterpret_cast<float*>(b2_sm + 2 * C::B2_BYTES);    // [128][LTC_SB_LD] staged accumulator block
-    float* W10 = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(SB) + C::SB_BYTES);  // [12][H]
+    float* W10 = reinterpret_cast<float*>(b2_sm + 2 * C::B2_BYTES);  // [12][H]
     float* ST2 = W10 + 12 * H;                                       // [2][H] (+ Wl2^T [H][H] for H < 16)
+    uint64_t* ring_full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(W10) + C::W10_BYTES + C::ST2_BYTES);
 
     const int tid = threadIdx.x, lane = tid & 31;
     const int row = tid & (LTC_ROWS - 1);   // neighbour row of the tile this thread works on
     const int half = tid >> 7;              // which part of the channels / columns (0 .. NPART-1)
+    // accumulator fragment of this thread (tc.cuh): rows r0 and r0 + 8 of the tile, i.e. neighbours g and g + 8 of point
+    // wg * 4 + warp of the tile
+    const int wg = tid >> 7, g = lane >> 2, t = lane & 3;
+    const int r0 = wg * 64 + ((tid >> 5) & 3) * 16 + g;
+    const int pt = r0 >> 4;
 
     // ---- once per CTA: resident weights and the small per-channel constants
     if (!C::STREAM) {
@@ -154,8 +205,20 @@ lfa_pool_tc_kernel(const __grid_constant__ LfaTcParams p) {
         W10[10 * H + i] = p.s10[i];
         W10[11 * H + i] = p.t10[i];
     }
+    // streamed score weight: a ring of two column blocks, filled by bulk copies.  The ring runs over the block sequence
+    // 0 .. NBLK-1 of every tile in turn, so blocks 0 and 1 of the next tile are in flight during this tile's last blocks.
+    uint32_t ring_phase = 0;                // bit s: parity of the next completion of slot s
+    if (C::STREAM && tid == 0) {
+        tc::mbar_init(&ring_full[0], 1);
+        tc::mbar_init(&ring_full[1], 1);
+        tc::fence_mbar_init();
+    }
     tc::fence_async_smem();
     __syncthreads();
+    if (C::STREAM) {
+        ltc_fill<CB, D, D>(b_sm, &ring_full[0], p.ws_img, 0, lane, tid < 32);
+        ltc_fill<CB, D, D>(b_sm + 2 * C::SLOT_BYTES, &ring_full[1], p.ws_img, 1, lane, tid < 32);
+    }
 
     // The gathers are software-pipelined over tiles (d >= 64): the neighbour index of tile t+2 and the
     // coordinates / feature rows of tile t+1 are requested while tile t is worked on and land behind its
@@ -289,7 +352,9 @@ lfa_pool_tc_kernel(const __grid_constant__ LfaTcParams p) {
     // register path) to channels [H, D)
     constexpr uint32_t R1_OFF = (STAGE == 2 && C::MMA2) ? 0u : (uint32_t)(H / 8) * LTC_ROWS * 16;
 
-    for (int64_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+    // Builds the A tile of `tile` (tiles in the CTA's order) into (a_hi, a_lo); ends with the writes fenced for the
+    // tensor core, not with a barrier.  A tile past the end is built from zeros and never used.
+    auto build = [&](int64_t tile, uint8_t* a_hi, uint8_t* a_lo) {
         // ---------------- neighbour id + encoding + LocSE MLP of this thread's row
         int64_t g = tile * (LTC_ROWS / LTC_K) + (row >> 4);
         int64_t nb = -1;
@@ -321,7 +386,9 @@ lfa_pool_tc_kernel(const __grid_constant__ LfaTcParams p) {
         // gathered neighbour features -> channels [0, H) of A
         auto store_features = [&]() {
 #pragma unroll
-            for (int ch = half, fi = 0; ch < H / 8; ch += NPART, ++fi) {
+            for (int fi = 0; fi < (H / 8 + NPART - 1) / NPART; ++fi) {   // compile-time trip count: f_cur stays in registers
+                const int ch = half + fi * NPART;
+                if (ch >= H / 8) break;
                 float x[8];
                 if (PREF) {
                     const float4 v0 = f_cur[fi < FCH ? fi : 0][0], v1 = f_cur[fi < FCH ? fi : 0][1];
@@ -349,101 +416,153 @@ lfa_pool_tc_kernel(const __grid_constant__ LfaTcParams p) {
             __syncthreads();
 #pragma unroll 1
             for (int blk = 0; blk < H / CB2; ++blk) {
-                ltc_block<CB2, H, H, !C::STREAM>(a_hi, a_lo, b2_sm, C::B2_BYTES, p.wl2_img, blk, SB, tid);
-                // 8-column groups of this block: half 0 takes 0 and 16, half 1 takes 8 and 24
-                for (int cl = 8 * half; cl < CB2; cl += 16) {
-                    const int c0 = blk * CB2 + cl;
-                    float v[8];
-                    const float4 sa = *reinterpret_cast<const float4*>(&ST2[c0]);
-                    const float4 sb = *reinterpret_cast<const float4*>(&ST2[c0 + 4]);
-                    const float4 ta = *reinterpret_cast<const float4*>(&ST2[H + c0]);
-                    const float4 tb = *reinterpret_cast<const float4*>(&ST2[H + c0 + 4]);
-                    const float sc[8] = {sa.x, sa.y, sa.z, sa.w, sb.x, sb.y, sb.z, sb.w};
-                    const float sh[8] = {ta.x, ta.y, ta.z, ta.w, tb.x, tb.y, tb.z, tb.w};
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const float a = fmaf(SB[row * LTC_SB_LD + cl + j], sc[j], sh[j]);
-                        v[j] = a >= 0.f ? a : 0.2f * a;
+                if (C::STREAM) {   // one column block at a time through b2_sm
+                    if (blk > 0) __syncthreads();    // both warpgroups' MMAs of the previous block are done with b2_sm
+                    constexpr int N_U4 = H / 8 * CB2;
+                    for (int i = tid; i < 2 * N_U4; i += NTH) {
+                        const int im = i / N_U4, rem = i % N_U4, kc = rem / CB2, r = rem % CB2;
+                        reinterpret_cast<uint4*>(b2_sm + im * C::B2_BYTES)[rem] =
+                            p.wl2_img[(size_t)im * (H / 8) * H + kc * H + blk * CB2 + r];
                     }
-                    uint4 hi, lo;
-                    tc::split8(v, hi, lo);
-                    *reinterpret_cast<uint4*>(a_hi + tc::op_off(LTC_ROWS, row, (H + c0) / 8)) = hi;
-                    *reinterpret_cast<uint4*>(a_lo + tc::op_off(LTC_ROWS, row, (H + c0) / 8)) = lo;
+                    tc::fence_async_smem();
+                    __syncthreads();
                 }
-                __syncthreads();   // SB is read; after the last block every lse2 MMA has read r1
+                const uint32_t bh = tc::smem_u32(b2_sm) + (C::STREAM ? 0u : (uint32_t)blk * CB2 * 16);
+                float d2[CB2 / 2];
+                ltc_issue<CB2, H>(d2, tc::smem_u32(a_hi), tc::smem_u32(a_lo), bh, bh + C::B2_BYTES,
+                                  (C::STREAM ? CB2 : H) * 16, wg);
+                ltc_wait<0, CB2 / 2>(d2);
+                // r2 = lrelu(BN(.)) of the fragment, split, straight from the registers into channels [H, D) of A
+#pragma unroll
+                for (int q = 0; q < CB2 / 8; ++q) {
+                    const int c = blk * CB2 + 8 * q + 2 * t;
+                    const float2 sc = *reinterpret_cast<const float2*>(&ST2[c]);
+                    const float2 sh = *reinterpret_cast<const float2*>(&ST2[H + c]);
+#pragma unroll
+                    for (int hh = 0; hh < 2; ++hh) {
+                        float v0 = fmaf(d2[4 * q + 2 * hh], sc.x, sh.x), v1 = fmaf(d2[4 * q + 2 * hh + 1], sc.y, sh.y);
+                        v0 = v0 >= 0.f ? v0 : 0.2f * v0;
+                        v1 = v1 >= 0.f ? v1 : 0.2f * v1;
+                        const uint32_t hi = tc::cvt_f16x2_sat(v0, v1);
+                        const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+                        const uint32_t off = tc::op_off(LTC_ROWS, r0 + 8 * hh, (H + blk * CB2) / 8 + q) + 4 * t;
+                        *reinterpret_cast<uint32_t*>(a_hi + off) = hi;
+                        *reinterpret_cast<uint32_t*>(a_lo + off) = tc::cvt_f16x2_sat(v0 - f.x, v1 - f.y);
+                    }
+                }
             }
+            __syncthreads();   // every lse2 MMA has read r1
         }
-        // (the features overwrite r1 in stage 2: the lse2 MMAs that read it have completed)
-        store_features();
+        store_features();      // (overwrites r1 in stage 2)
         if (PREF && LATE) advance(tile);     // lands behind the score GEMM and the epilogue
         tc::fence_async_smem();
-        __syncthreads();
+    };
 
-        // ---------------- scores = X . Ws^T on the tensor core, 32 columns at a time, then the softmax over the
-        // 16 rows of each point + weighted sum of those columns
-        const bool upper = (lane & 16) != 0;
-        const int j16 = lane & 15;
-#pragma unroll 1
-        for (int blk = 0; blk < D / CB; ++blk) {
-            ltc_block<CB, D, D, !C::STREAM>(a_hi, a_lo, b_sm, C::B_BYTES, p.ws_img, blk, SB, tid);
-            for (int cl = half * 16; cl < CB; cl += 32) {
-                const int c0 = blk * CB + cl;
-                float s[16], x[16];
+    // ---------------- scores = X . Ws^T on the tensor core, CB columns per block; block j + 1 is issued before the
+    // softmax over the 16 rows of the point + weighted sum of block j runs on the accumulator registers.
+    // A NaN score still yields NaN: fmaxf skips it in the max, but its own exponential is NaN and enters both sums.
+    auto softmax = [&](int64_t tile, const float* s, int c0, const uint8_t* a_hi, const uint8_t* a_lo) {
+            const int64_t gp = tile * (LTC_ROWS / LTC_K) + pt;   // this warp's point
+            constexpr int M = CB / 4;   // columns of the block in this thread's fragment
+            float den[M], num[M];
 #pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const float4 v = *reinterpret_cast<const float4*>(&SB[row * LTC_SB_LD + cl + 4 * u]);
-                    s[4 * u] = v.x; s[4 * u + 1] = v.y; s[4 * u + 2] = v.z; s[4 * u + 3] = v.w;
+            for (int q = 0; q < CB / 8; ++q) {
+                // x = hi + lo of this thread's (row, column pair), rows r0 and r0 + 8
+                const uint32_t off = tc::op_off(LTC_ROWS, r0, c0 / 8 + q) + 4 * t;
+                const float2 h0 = __half22float2(*reinterpret_cast<const __half2*>(a_hi + off));
+                const float2 l0 = __half22float2(*reinterpret_cast<const __half2*>(a_lo + off));
+                const float2 h1 = __half22float2(*reinterpret_cast<const __half2*>(a_hi + off + 8 * 16));
+                const float2 l1 = __half22float2(*reinterpret_cast<const __half2*>(a_lo + off + 8 * 16));
+                const float x0[2] = {h0.x + l0.x, h0.y + l0.y}, x1[2] = {h1.x + l1.x, h1.y + l1.y};
+#pragma unroll
+                for (int u = 0; u < 2; ++u) {
+                    const float v0 = s[4 * q + u], v1 = s[4 * q + 2 + u];
+                    float m = fmaxf(v0, v1);
+                    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
+                    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 8));
+                    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 16));
+                    const float ml = -m * kLog2e;
+                    const float e0 = ex2_ftz(fmaf(v0, kLog2e, ml)), e1 = ex2_ftz(fmaf(v1, kLog2e, ml));
+                    den[2 * q + u] = e0 + e1;
+                    num[2 * q + u] = e0 * x0[u] + e1 * x1[u];
                 }
-#pragma unroll
-                for (int q = 0; q < 2; ++q) {
-                    const uint4 hq = *reinterpret_cast<const uint4*>(a_hi + tc::op_off(LTC_ROWS, row, c0 / 8 + q));
-                    const uint4 lq = *reinterpret_cast<const uint4*>(a_lo + tc::op_off(LTC_ROWS, row, c0 / 8 + q));
-                    const __half2* hh = reinterpret_cast<const __half2*>(&hq);
-                    const __half2* ll = reinterpret_cast<const __half2*>(&lq);
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) {
-                        const float2 fh = __half22float2(hh[u]), fl = __half22float2(ll[u]);
-                        x[q * 8 + 2 * u] = fh.x + fl.x;
-                        x[q * 8 + 2 * u + 1] = fh.y + fl.y;
-                    }
-                }
-                float den[16], num[16];
-#pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                    int o = __float_as_int(s[i]);
-                    o ^= (o >> 31) & 0x7fffffff;              // order-preserving float -> int
-                    // per-half-warp max through two FULL-warp reductions (one redux.sync per 16-lane group)
-                    const int m_lo = __reduce_max_sync(0xffffffffu, upper ? INT_MIN : o);
-                    const int m_hi = __reduce_max_sync(0xffffffffu, upper ? o : INT_MIN);
-                    int m = upper ? m_hi : m_lo;
-                    m ^= (m >> 31) & 0x7fffffff;
-                    const float ev = ex2_ftz(fmaf(s[i], kLog2e, -__int_as_float(m) * kLog2e));
-                    den[i] = ev;
-                    num[i] = ev * x[i];
-#ifdef O3DML_DEBUG_NAN
-                    if (!(ev <= 1.0f) || !(fabsf(x[i]) < 1e30f) || !(fabsf(s[i]) < 1e30f))
-                        printf("DBG tile %lld row %d c0 %d i %d s %g m %g ev %g x %g o %d mi %d\n",
-                               (long long)tile, row, c0, i, s[i], __int_as_float(m), ev, x[i], o, m);
-#endif
-                }
-                // reduce-scatter over the 16 lanes of the group: afterwards lane j16 holds column c0+j16
-#pragma unroll
-                for (int w = 8; w >= 1; w >>= 1) {
-                    const bool up = (lane & w) != 0;
-#pragma unroll
-                    for (int i = 0; i < w; ++i) {
-                        const float sd = up ? den[i] : den[i + w];
-                        const float sn = up ? num[i] : num[i + w];
-                        const float rd = __shfl_xor_sync(0xffffffffu, sd, w);
-                        const float rn = __shfl_xor_sync(0xffffffffu, sn, w);
-                        den[i] = (up ? den[i + w] : den[i]) + rd;
-                        num[i] = (up ? num[i + w] : num[i]) + rn;
-                    }
-                }
-                if (g < p.total) p.agg[(size_t)g * D + c0 + j16] = num[0] / den[0];
             }
-            __syncthreads();   // SB is read; after the last block the A tile is free for the next tile
+            int base = 0;
+            ltc_reduce_scatter<M, 16>(den, num, lane, base);
+            if (gp < p.total) {
+                float* dst = p.agg + (size_t)gp * D + c0 + 8 * (base >> 1) + 2 * t;
+                if (M == 16) *reinterpret_cast<float2*>(dst) = make_float2(num[0] / den[0], num[1] / den[1]);
+                else if (M > 4 || !(lane & 4)) dst[base & 1] = num[0] / den[0];   // M = 4: lane bit 2 holds a copy
+            }
+        };
+    auto issue = [&](float* d, int j, uint32_t ah, uint32_t al) {   // block j: resident weight in place, streamed weight from ring slot j % 2
+            if (C::STREAM) {
+                const int s = j & 1;
+                tc::mbar_wait(&ring_full[s], (ring_phase >> s) & 1u);
+                ring_phase ^= 1u << s;
+                const uint32_t bh = tc::smem_u32(b_sm) + (uint32_t)s * 2 * C::SLOT_BYTES;
+                ltc_issue<CB, D>(d, ah, al, bh, bh + C::SLOT_BYTES, CB * 16, wg);
+            } else {
+                const uint32_t bh = tc::smem_u32(b_sm) + (uint32_t)j * CB * 16;
+                ltc_issue<CB, D>(d, ah, al, bh, bh + C::B_BYTES, D * 16, wg);
+            }
+        };
+    float acc0[CB / 2], acc1[CB / 2];
+    if (C::DBUF) {
+        // tile t's two score blocks are issued, then tile t+1 is built in the other A buffer, then tile t's softmax runs
+        static_assert(!C::DBUF || (C::NBLK == 2 && !C::STREAM), "double-buffered A: two resident score blocks");
+        build(blockIdx.x, smem, smem + C::A_BYTES);
+        __syncthreads();
+        int buf = 0;
+#pragma unroll 1
+        for (int64_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+            uint8_t* a_hi = smem + buf * 2 * C::A_BYTES;
+            uint8_t* nx_hi = smem + (buf ^ 1) * 2 * C::A_BYTES;
+            const uint32_t ah = tc::smem_u32(a_hi), al = ah + C::A_BYTES;
+            issue(acc0, 0, ah, al);
+            issue(acc1, 1, ah, al);
+            build(tile + gridDim.x, nx_hi, nx_hi + C::A_BYTES);
+            ltc_wait<1, CB / 2>(acc0);
+            softmax(tile, acc0, 0, a_hi, a_hi + C::A_BYTES);
+            ltc_wait<0, CB / 2>(acc1);
+            softmax(tile, acc1, CB, a_hi, a_hi + C::A_BYTES);
+            __syncthreads();   // tile t's buffer is read, tile t+1's is built
+            buf ^= 1;
         }
+        return;
+    }
+    uint8_t* a_hi = smem;
+    uint8_t* a_lo = smem + C::A_BYTES;
+    const uint32_t ah = tc::smem_u32(a_hi), al = tc::smem_u32(a_lo);
+    for (int64_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        build(tile, a_hi, a_lo);
+        __syncthreads();
+        const bool more = tile + gridDim.x < p.num_tiles;
+        auto step = [&](int j, float* cur, float* nxt) {   // block j lands in cur; block j + 1 goes to nxt
+            if (j + 1 < C::NBLK) {
+                issue(nxt, j + 1, ah, al);
+                ltc_wait<1, CB / 2>(cur);
+            } else {
+                ltc_wait<0, CB / 2>(cur);
+            }
+            if (C::STREAM) {
+                __syncthreads();      // both warpgroups are done with slot j % 2: refill it with the block two ahead
+                ltc_fill<CB, D, D>(b_sm + (j & 1) * 2 * C::SLOT_BYTES, &ring_full[j & 1], p.ws_img,
+                                   j + 2 < C::NBLK ? j + 2 : j + 2 - C::NBLK, lane, tid < 32 && (j + 2 < C::NBLK || more));
+            }
+            softmax(tile, cur, j * CB, a_hi, a_lo);
+        };
+        issue(acc0, 0, ah, al);
+        if (C::NBLK == 1) {
+            step(0, acc0, acc1);
+        } else {
+#pragma unroll 1
+            for (int j = 0; j < C::NBLK; j += 2) {
+                step(j, acc0, acc1);
+                step(j + 1, acc1, acc0);
+            }
+        }
+        __syncthreads();   // MMAs and softmax have read the A tile: free for the next tile
     }
 }
 
