@@ -308,7 +308,12 @@ O3DML_API int o3dml_randla_lfa_pool_tc(int stage, int d, const float* coords, co
  * weight_image: 57 344-byte device image of the four weights (open3d_ml_b200._lib.pack_tail_image: per layer and
  * 32-wide k-chunk, TF32 hi tiles then lo tiles of [N][32] floats, K-major SWIZZLE_128B); h_scale / h_shift: HOST float
  * [4][64] folded BN scale / shift (+ bias) per layer; LeakyReLU(slope) after the first three layers.
- * interp_index [num_rows] (int32 / int64, batch-relative when out_rows_per_batch > 0).  out [num_rows, classes]. */
+ * interp_index [num_rows] (int32 / int64).  Row n reads coarse row r = interp_index[n] when out_rows_per_batch == 0
+ * (global), r = interp_index[n] + (n / out_rows_per_batch) * src_rows_per_batch when out_rows_per_batch > 0
+ * (batch-relative).  The coarse half of row n is zero when interp_index[n] < 0, when interp_index[n] >=
+ * src_rows_per_batch (batch-relative), or when r >= coarse_rows.  skip_ld / coarse_ld: row strides in floats, multiples
+ * of 4 with 16-byte aligned rows.  classes 1..32.  out [num_rows, classes], exactly num_rows rows written; num_rows
+ * <= 0 returns without a launch. */
 O3DML_API int o3dml_randla_tail_supported(int skip_channels, int coarse_channels, int c1, int c2, int c3, int classes);
 O3DML_API int o3dml_randla_tail(const float* skip, int skip_ld, const float* coarse, int coarse_ld,
                                 int64_t coarse_rows, const void* interp_index, int index_is64,

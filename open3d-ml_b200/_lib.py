@@ -294,8 +294,9 @@ def linear(srcs, weight, out, scale=None, shift=None, residual=None, act=None, s
 def pack_operand_image_host(w_nk):
     """fp32 [N, K] (K contiguous, i.e. nn.Linear's [out, in]) -> uint8 CPU tensor holding the
     3xFP16 operand images of csrc/tc.cuh: [K/8][N][8 halves] of hi = fp16(w), then the same
-    layout of lo = fp16(w - hi)."""
-    w = w_nk.detach().to(torch.float32).cpu().clamp(-65504.0, 65504.0)
+    layout of lo = fp16(w - hi).  Like the kernels' split (tc.cuh split8), nothing is clamped: a weight of magnitude
+    >= 65520, Inf or NaN gives a non-finite hi or lo, so the product it enters is non-finite rather than silently wrong."""
+    w = w_nk.detach().to(torch.float32).cpu()
     n, k = w.shape
     assert k % 8 == 0 and n % 8 == 0
     hi = w.to(torch.float16)

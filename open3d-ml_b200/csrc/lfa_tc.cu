@@ -443,11 +443,11 @@ lfa_pool_tc_kernel(const __grid_constant__ LfaTcParams p) {
                         float v0 = fmaf(d2[4 * q + 2 * hh], sc.x, sh.x), v1 = fmaf(d2[4 * q + 2 * hh + 1], sc.y, sh.y);
                         v0 = v0 >= 0.f ? v0 : 0.2f * v0;
                         v1 = v1 >= 0.f ? v1 : 0.2f * v1;
-                        const uint32_t hi = tc::cvt_f16x2_sat(v0, v1);
+                        const uint32_t hi = tc::cvt_f16x2(v0, v1);
                         const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hi));
                         const uint32_t off = tc::op_off(LTC_ROWS, r0 + 8 * hh, (H + blk * CB2) / 8 + q) + 4 * t;
                         *reinterpret_cast<uint32_t*>(a_hi + off) = hi;
-                        *reinterpret_cast<uint32_t*>(a_lo + off) = tc::cvt_f16x2_sat(v0 - f.x, v1 - f.y);
+                        *reinterpret_cast<uint32_t*>(a_lo + off) = tc::cvt_f16x2(v0 - f.x, v1 - f.y);
                     }
                 }
             }

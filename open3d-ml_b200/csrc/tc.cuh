@@ -13,7 +13,12 @@
 //   * 22-bit "3xFP16" precision: x = h1 + h2 with h1 = fp16(x), h2 = fp16(x - h1);
 //     A*B ~= A1*B1 + A1*B2 + A2*B1 (three MMAs into the same accumulator).  Relative error
 //     ~2^-21 per product, which keeps the 1e-4 parity bar that plain TF32/BF16 cannot
-//     (SURVEY.md section 7).  Valid for |x| < 65504 (post-BN activations and weights are O(1)).
+//     (SURVEY.md section 7).  hi + lo represents x to max(|x| 2^-22, 2^-25): lo falls to fp16 subnormals below
+//     2^-14 of |x|.  Without range normalisation (lfa_tc.cu) a tensor of scale s keeps 1e-4 of s for s >= ~2^-11.7;
+//     from |x| >= 65520 hi is Inf and, like +-Inf and NaN, the split is non-finite (the conversion does not saturate).
+//     Measured through lfa_tc on an H100 (tests/test_gpu_lfa_tc.py): agg stays within 1e-4 of float64 for features of
+//     scale 2^-12 .. 2^8 with coordinates within 1e2 of the origin (the reference's crop centres the clouds,
+//     ml3d/datasets/utils/transforms.py:123); coordinates near 1e3 cost 1.5e-4 at any feature scale.
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -147,31 +152,28 @@ template <int N> __device__ __forceinline__ void wgmma_wait() {
 __device__ __forceinline__ void fence_operand(float& r) { asm volatile("" : "+f"(r)::"memory"); }
 
 // ---- fp32 -> (h1, h2) split -----------------------------------------------------------------
-__device__ __forceinline__ void split_f16(float x, __half& h1, __half& h2) {
-    x = fminf(fmaxf(x, -65504.f), 65504.f);
-    h1 = __float2half_rn(x);
-    h2 = __float2half_rn(x - __half2float(h1));
-}
 // 8 consecutive-k floats of one row -> two 16-byte words (hi parts, lo parts)
 __device__ __forceinline__ uint32_t pack_h2(__half a, __half b) {
     __half2 t = __halves2half2(a, b);  // a -> low 16 bits (lower k)
     return *reinterpret_cast<uint32_t*>(&t);
 }
-// packed, saturating fp32 pair -> fp16 pair (F2FP.SATFINITE.F16.F32.PACK_AB): `lo` lands in the low half (lower k)
-__device__ __forceinline__ uint32_t cvt_f16x2_sat(float lo, float hi) {
+// packed fp32 pair -> fp16 pair (F2FP.F16.F32.PACK_AB): `lo` lands in the low half (lower k).  Not saturating: +-Inf and
+// |x| >= 65520 become +-Inf, so that the split of such a value (hi = Inf, lo = x - hi = -Inf or NaN) is non-finite
+// instead of a silently clamped +-65504.
+__device__ __forceinline__ uint32_t cvt_f16x2(float lo, float hi) {
     uint32_t r;
-    asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+    asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
     return r;
 }
-// 3 instructions per element (F2FP, HADD2.F32, FADD, F2FP over pairs) against ~7 of the scalar clamp + convert
-// sequence: the split is ~15 % of the SIMT instructions of an LFA tile
+// 3 instructions per element (F2FP, HADD2.F32, FADD, F2FP over pairs) against ~7 of the scalar convert sequence: the
+// split is ~15 % of the SIMT instructions of an LFA tile
 __device__ __forceinline__ void split8(const float* x, uint4& hi, uint4& lo) {
     uint32_t h[4], l[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-        h[i] = cvt_f16x2_sat(x[2 * i], x[2 * i + 1]);
+        h[i] = cvt_f16x2(x[2 * i], x[2 * i + 1]);
         const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&h[i]));
-        l[i] = cvt_f16x2_sat(x[2 * i] - f.x, x[2 * i + 1] - f.y);
+        l[i] = cvt_f16x2(x[2 * i] - f.x, x[2 * i + 1] - f.y);
     }
     hi = make_uint4(h[0], h[1], h[2], h[3]);
     lo = make_uint4(l[0], l[1], l[2], l[3]);

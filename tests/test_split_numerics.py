@@ -90,6 +90,43 @@ def test_packed_weight_exponent_matches_the_kernel_contract():
     assert float((hi + lo)[40:].abs().max()) == 0.0                                # zero padding
 
 
+def test_lfa_operand_split_error_and_range():
+    """The A operand of lfa_tc.cu (features, LocSE activations) is split without range normalisation: hi + lo
+    represents x to max(|x| 2^-22, 2^-25), the 2^-25 being half of fp16's smallest subnormal that lo falls to.  So a
+    tensor of scale s keeps 1e-4 of s for s >= about 2^-11.7; 2^-10 is the bound with margin, 2^-13 misses it."""
+    rng = np.random.default_rng(4)
+    base = rng.standard_normal(1 << 16)
+    base = (base / np.abs(base).max()).astype(np.float32)                   # scale 2^e exactly below
+    for e in range(-30, 16):
+        x = base * np.float32(2.0 ** e)
+        x = x[np.abs(x) < 65504]
+        hi, lo = split(x)
+        err = np.abs((hi.astype(np.float64) + lo) - x.astype(np.float64))
+        assert (err <= np.maximum(np.abs(x.astype(np.float64)) * 2.0 ** -22, 2.0 ** -25)).all(), e
+    for e, holds in ((-10, True), (-13, False)):
+        x = base * np.float32(2.0 ** e)
+        hi, lo = split(x)
+        assert (float(np.abs((hi.astype(np.float64) + lo) - x).max() / np.abs(x).max()) < 1e-4) == holds, e
+
+
+def test_lfa_operand_split_is_not_finite_out_of_range():
+    """fp16 ends at 65504: x up to 65519 still splits exactly (hi = 65504), from 65520 on hi is Inf and the split is
+    non-finite, as are +-Inf and NaN (cvt.rn.f16x2.f32 in tc.cuh, no .satfinite).  The host image of a weight
+    (pack_operand_image_host) follows the same rule: no clamp to +-65504."""
+    x = np.array([65504.0, 65519.0, -65519.0, 65520.0, -70000.0, np.inf, -np.inf, np.nan], np.float32)
+    with np.errstate(invalid="ignore", over="ignore"):
+        hi, lo = split(x)
+    ok = np.isfinite(hi) & np.isfinite(lo)
+    assert ok.tolist() == [True, True, True, False, False, False, False, False]
+    assert np.array_equal(hi[:3] + lo[:3], x[:3])
+    w = torch.from_numpy(np.tile(x, (8, 1)).T.copy())                        # [N = 8 values, K = 8]
+    img = L.pack_operand_image_host(w).view(torch.float16).float()
+    n = w.numel()
+    hi_img = img[:n].view(1, 8, 8).permute(1, 0, 2).reshape(8, 8)
+    lo_img = img[n:].view(1, 8, 8).permute(1, 0, 2).reshape(8, 8)
+    assert (torch.isfinite(hi_img) & torch.isfinite(lo_img)).all(1).tolist() == ok.tolist()
+
+
 # ---- the 3xTF32 split of gemm_tc.cu -------------------------------------------------------------------
 def _tf32_trunc(x):
     return (x.view(np.uint32) & np.uint32(0xFFFFE000)).view(np.float32)
