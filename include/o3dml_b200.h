@@ -186,6 +186,21 @@ O3DML_API int o3dml_nms(const float* boxes, const float* scores, int64_t num_box
 O3DML_API int o3dml_iou_matrix(const float* boxes_a, int64_t num_a, const float* boxes_b, int64_t num_b,
                                int mode, float* out, void* stream);
 
+/* PointPillars box decoding (Anchor3DHead.get_bboxes, ml3d/torch/models/point_pillars.py:945-1025) for a batch of
+ *   frames, contract in DESIGN.md section 2.  cls [B, A*C, H, W], reg [B, A*7, H, W], dir [B, A*2, H, W]: NCHW with
+ *   contiguous H x W planes, frame b at map + b * <map>_batch_stride floats.  anchors [H*W*A, 7] float32 are the
+ *   reference's grid_anchors for this (H, W) (row (y * W + x) * A + a).  With K = min(nms_pre, H*W*A) the outputs
+ *   are boxes [B, C*K, 7], scores [B, C*K], labels int64 [B, C*K] (rows at or past d_counts[b] are zero, label -1)
+ *   and d_counts int64 [B].  nms_pre is at most 4096.  No host synchronisation; capturable into a CUDA graph. */
+O3DML_API size_t o3dml_pp_detect_workspace_bytes(int64_t batch, int64_t height, int64_t width, int num_anchors,
+                                                 int num_classes, int64_t nms_pre);
+O3DML_API int o3dml_pp_detect(const float* cls, int64_t cls_batch_stride, const float* reg, int64_t reg_batch_stride,
+                              const float* dir, int64_t dir_batch_stride, int64_t batch, int64_t height,
+                              int64_t width, int num_anchors, int num_classes, const float* anchors, int64_t nms_pre,
+                              float score_thr, float dir_offset, float* out_boxes, float* out_scores,
+                              int64_t* out_labels, int64_t* d_counts, void* workspace, size_t workspace_bytes,
+                              void* stream);
+
 /* ------------------------------------------------------ dense layers ---- */
 
 /* One operand of the gathered GEMM: rows of `channels` floats (row stride ld); when `index`

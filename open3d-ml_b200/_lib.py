@@ -48,6 +48,8 @@ _SIGNATURES = {
     "o3dml_nms_workspace_bytes": (Z, [L]),
     "o3dml_nms": (I, [P, P, L, F, P, P, P, Z, P]),
     "o3dml_iou_matrix": (I, [P, L, P, L, I, P, P]),
+    "o3dml_pp_detect_workspace_bytes": (Z, [L, L, L, I, I, L]),
+    "o3dml_pp_detect": (I, [P, L, P, L, P, L, L, L, L, I, I, P, L, F, F, P, P, P, P, P, Z, P]),
     "o3dml_pp_pfn_scatter": (I, [P, I, I, P, P, P, P, P, L, P, P, P, I, F, F, F, F, I, I, I, P, P,
                                  I, P]),
     "o3dml_linear": (I, [L, ctypes.POINTER(Src), I, P, P, P, P, I, I, F, P, I, I, I, P]),

@@ -13,6 +13,10 @@ Python, so it is captured once per canvas shape into a CUDA graph and replayed
 (`use_graph=False` or O3DML_PP_GRAPH=0 keeps the eager launches).
 Built from a reference ``state_dict``; returns (cls, reg, dir) in NCHW like the
 reference head.
+
+Box decoding (``Anchor3DHead.get_bboxes``, :945-1025) runs on the device too: get_bboxes_padded() is one batched
+call into detect.cu (top-k, decode, per-class rotated NMS) that reads nothing back to the host, and get_bboxes()
+adds the one read of the per-frame counts that splitting the result into per-frame lists needs.
 """
 import numpy as np
 import torch
@@ -31,7 +35,8 @@ def _fold_bn(sd, prefix, eps=BN_EPS):
 
 class PointPillarsB200:
     """cfg keys: point_cloud_range, voxel_size, max_num_points, max_voxels (eval value),
-    output_shape [ny, nx], layer_nums, layer_strides, upsample_strides."""
+    output_shape [ny, nx], layer_nums, layer_strides, upsample_strides; for the box decoding also
+    num_classes and head = {nms_pre, score_thr, dir_offset, ranges, sizes, rotations} (cfg_from_reference)."""
 
     def __init__(self, state_dict, cfg, device=None, use_graph=None):
         L.require_cuda()
@@ -95,6 +100,7 @@ class PointPillarsB200:
         self.y_off = float(self.vy / 2 + r[1])
         self.ny, self.nx = cfg["output_shape"]
         self._buf = {}
+        self._anchors = {}
 
     def _get(self, name, shape, dtype=torch.float32):
         key = (name, tuple(shape), dtype)
@@ -212,9 +218,110 @@ class PointPillarsB200:
 
     __call__ = forward
 
+    # ---------------------------------------------------------- box decoding
+    def _head_cfg(self):
+        head, nc = self.cfg.get("head"), self.cfg.get("num_classes")
+        if head is None or nc is None:
+            raise RuntimeError("PointPillarsB200: box decoding needs cfg['head'] and cfg['num_classes'] "
+                               "(cfg_from_reference builds both)")
+        A = len(head["sizes"]) * len(head["rotations"])
+        if self.head_split != [A * nc, A * 7, A * 2]:
+            raise RuntimeError("PointPillarsB200: head channels %s do not match %d anchors x %d classes"
+                               % (self.head_split, A, nc))
+        return head, int(nc), A
+
+    def anchors(self, H, W, device):
+        """Anchor3DRangeGenerator.grid_anchors (objdet_helper.py:164-245) as [H * W * A, 7], row (y * W + x) * A + a,
+        a = size * R + rotation; built once per (H, W, device) with torch.linspace on that device, as the reference
+        builds it (torch's CPU and CUDA linspace round differently, so it is not recomputed in a kernel)."""
+        head, _, _ = self._head_cfg()
+        key = (int(H), int(W), str(device))
+        t = self._anchors.get(key)
+        if t is None:
+            t = self._anchors[key] = grid_anchors(head, H, W, device)
+        return t
+
+    def get_bboxes_padded(self, cls, reg, dir):
+        """Head maps of B frames (NCHW, any batch stride) -> (boxes [B, C*K, 7], scores [B, C*K], labels int64 [B, C*K],
+        counts int64 [B]) with K = min(nms_pre, H * W * A).  Frame b's boxes are rows [0, counts[b]): class 0's in
+        NMS visiting order, then class 1's, ...; the rows after them are zero with label -1.  No host synchronisation;
+        capturable into a CUDA graph (DESIGN.md section 2, "PointPillars box decoding")."""
+        head, C, A = self._head_cfg()
+        B, _, H, W = cls.shape
+        maps = []
+        for t, ch in ((cls, A * C), (reg, A * 7), (dir, A * 2)):
+            if t.dim() != 4 or tuple(t.shape) != (B, ch, H, W):
+                raise RuntimeError("PointPillarsB200.get_bboxes: map of shape %s, expected %s"
+                                   % (tuple(t.shape), (B, ch, H, W)))
+            if t.dtype != torch.float32 or not t.is_cuda:
+                raise RuntimeError("PointPillarsB200.get_bboxes: maps must be float32 CUDA tensors")
+            if t.stride(3) != 1 or t.stride(2) != W or t.stride(1) != H * W:
+                t = t.contiguous()
+            maps.append(t)
+        nms_pre = int(head["nms_pre"])
+        lib = L.lib()
+        ws_bytes = lib.o3dml_pp_detect_workspace_bytes(B, H, W, A, C, nms_pre)
+        if ws_bytes == 0:
+            L.check(lib.o3dml_pp_detect(None, 0, None, 0, None, 0, B, H, W, A, C, None, nms_pre, 0.0, 0.0,
+                                        None, None, None, None, None, 0, L.stream()))
+        K = min(nms_pre, H * W * A)
+        dev = cls.device
+        boxes = torch.empty((B, C * K, 7), dtype=torch.float32, device=dev)
+        scores = torch.empty((B, C * K), dtype=torch.float32, device=dev)
+        labels = torch.empty((B, C * K), dtype=torch.int64, device=dev)
+        counts = torch.empty((B,), dtype=torch.int64, device=dev)
+        ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+        anchors = self.anchors(H, W, dev)
+        c, r, d = maps
+        L.check(lib.o3dml_pp_detect(L.ptr(c), c.stride(0), L.ptr(r), r.stride(0), L.ptr(d), d.stride(0), B, H, W, A, C,
+                                    L.ptr(anchors), nms_pre, float(head["score_thr"]), float(head["dir_offset"]),
+                                    L.ptr(boxes), L.ptr(scores), L.ptr(labels), L.ptr(counts), L.ptr(ws), ws_bytes,
+                                    L.stream()))
+        return boxes, scores, labels, counts
+
+    def get_bboxes(self, cls, reg, dir):
+        """Anchor3DHead.get_bboxes: (list of boxes [n_b, 7], list of scores [n_b], list of labels int64 [n_b]) per
+        frame, all on the device.  One device-to-host read (the per-frame counts)."""
+        boxes, scores, labels, counts = self.get_bboxes_padded(cls, reg, dir)
+        n = counts.tolist()
+        return ([boxes[b, :k] for b, k in enumerate(n)], [scores[b, :k] for b, k in enumerate(n)],
+                [labels[b, :k] for b, k in enumerate(n)])
+
+
+def grid_anchors(head, H, W, device):
+    """The anchors of a head cfg for an H x W map as [H * W * A, 7] (see PointPillarsB200.anchors)."""
+    sizes = torch.tensor(head["sizes"], device=device).reshape(-1, 3)
+    ranges = list(head["ranges"])
+    if len(ranges) != len(sizes):
+        ranges = ranges * len(sizes)
+    rots = torch.tensor(head["rotations"], device=device)
+    S, R = sizes.shape[0], rots.shape[0]
+    t = torch.empty((H, W, S, R, 7), dtype=torch.float32, device=device)
+    for s in range(S):
+        # the float32 range values, as the reference's torch.tensor(anchor_range); host floats, so that building
+        # the anchors reads nothing back from the device
+        r = torch.tensor(ranges[s], dtype=torch.float32).tolist()
+        t[:, :, s, :, 0] = torch.linspace(r[0], r[3], W, device=device).view(1, W, 1)
+        t[:, :, s, :, 1] = torch.linspace(r[1], r[4], H, device=device).view(H, 1, 1)
+        t[:, :, s, :, 2] = torch.linspace(r[2], r[5], 1, device=device)
+        t[:, :, s, :, 3:6] = sizes[s]
+        t[:, :, s, :, 6] = rots
+    return t.view(H * W * S * R, 7)
+
+
+def _head_from_reference(head, classes):
+    """Anchor3DHead's decoding parameters with its constructor defaults (point_pillars.py:760-770)."""
+    head = head or {}
+    return dict(nms_pre=int(head.get("nms_pre", 100)), score_thr=float(head.get("score_thr", 0.1)),
+                dir_offset=float(head.get("dir_offset", 0)),
+                ranges=[list(map(float, r)) for r in head.get("ranges", [[0, -40.0, -3, 70.0, 40.0, 1]])],
+                sizes=[list(map(float, s)) for s in head.get("sizes", [[0.6, 1.0, 1.5]])],
+                rotations=[float(r) for r in head.get("rotations", [0, 1.57])]), len(classes)
+
 
 def cfg_from_reference(model_cfg):
     """Builds the cfg dict from a reference yml `model:` section (pointpillars_kitti.yml:7-66)."""
+    head, num_classes = _head_from_reference(model_cfg.get("head"), model_cfg.get("classes", ["car"]))
     return dict(point_cloud_range=list(model_cfg["point_cloud_range"]),
                 voxel_size=list(model_cfg["voxelize"]["voxel_size"]),
                 max_num_points=model_cfg["voxelize"]["max_num_points"],
@@ -222,4 +329,34 @@ def cfg_from_reference(model_cfg):
                 output_shape=list(model_cfg["scatter"]["output_shape"]),
                 layer_nums=list(model_cfg["backbone"]["layer_nums"]),
                 layer_strides=list(model_cfg["backbone"]["layer_strides"]),
-                upsample_strides=list(model_cfg["neck"]["upsample_strides"]))
+                upsample_strides=list(model_cfg["neck"]["upsample_strides"]),
+                head=head, num_classes=num_classes)
+
+
+def patch_reference_model(model):
+    """Drop-in: make an (unmodified) reference ``PointPillars`` instance run its forward and its
+    ``bbox_head.get_bboxes`` on the fused CUDA path, so that its own ``inference_end`` and
+    ``ObjectDetection.run_inference`` return the fused boxes.  Built from ``model.state_dict()`` and the
+    modules' own attributes; BN must be in eval mode."""
+    vl, hd = model.voxel_layer, model.bbox_head
+    gen = hd.anchor_generator
+    cfg = dict(point_cloud_range=list(model.point_cloud_range), voxel_size=[float(v) for v in vl.voxel_size],
+               max_num_points=int(vl.max_num_points), max_voxels=int(vl.max_voxels[1]),
+               output_shape=[int(model.middle_encoder.ny), int(model.middle_encoder.nx)],
+               layer_nums=[(len(blk) - 3) // 3 for blk in model.backbone.blocks],
+               layer_strides=[int(blk[0].stride[0]) for blk in model.backbone.blocks],
+               upsample_strides=[int(d[0].stride[0]) for d in model.neck.deblocks],
+               head=dict(nms_pre=int(hd.nms_pre), score_thr=float(hd.score_thr), dir_offset=float(hd.dir_offset),
+                         ranges=[[float(v) for v in r] for r in gen.ranges],
+                         sizes=[[float(v) for v in s] for s in gen.sizes],
+                         rotations=[float(r) for r in gen.rotations]),
+               num_classes=int(hd.num_classes))
+    fused = PointPillarsB200(model.state_dict(), cfg)
+
+    def forward(inputs):
+        if model.training:
+            raise RuntimeError("open3d_ml_b200: the fused PointPillars path is inference-only")
+        return fused.forward(inputs)
+    model.forward = forward
+    model.bbox_head.get_bboxes = fused.get_bboxes
+    return model
