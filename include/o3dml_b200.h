@@ -286,7 +286,8 @@ O3DML_API int o3dml_linear_rows_small(int64_t num_rows, const o3dml_src_t* srcs,
 /* LocalSpatialEncoding + AttentivePooling score/softmax/sum fused (randlanet.py:521-639, as
  * used by LocalFeatureAggregation.forward :667-692).  stage 1: X = [feat[nbr] | r1];
  * stage 2: X = [feat[nbr] | lrelu(BN(wl2 r1))].  feat [B*N, d/2]; agg out [B*N, d].
- * w10_t [10, d/2], wl2_t [d/2, d/2], wscore_t [d, d] are [in, out]; s, t = folded BN(+bias). */
+ * w10_t [10, d/2], wl2_t [d/2, d/2], wscore_t [d, d] are [in, out]; s, t = folded BN(+bias).
+ * d in {16, 32, 64, 128, 256, 512}, all on the tiled FP32 SIMT kernel. */
 O3DML_API int o3dml_randla_lfa_pool(int stage, int d, const float* coords, const void* neighbor_idx,
                           int idx_is64, int num_neighbors, const float* feat, int64_t batch,
                           int64_t n_per_batch, const float* w10_t, const float* s10,

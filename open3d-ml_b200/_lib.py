@@ -144,9 +144,6 @@ def make_src(data, index=None, index_ld=1, out_rows_per_batch=0, src_rows_per_ba
     return s
 
 
-USE_TC_GEMM = os.environ.get("O3DML_GEMM_TC", "1") != "0"
-
-
 def tf32_round(x):
     """fp32 -> nearest TF32 (10 explicit mantissa bits, ties to even), returned as fp32."""
     u = x.contiguous().view(torch.int32).to(torch.int64) & 0xFFFFFFFF
@@ -235,24 +232,24 @@ def pack_linear(w_kc):
     return PackedWeight(w_kc)
 
 
-TC_MIN_K = int(os.environ.get("O3DML_GEMM_TC_MIN_K", "64"))
+TC_MIN_K = 64
 
 
 def _tc_ok(srcs):
     """Tensor-core kernel only where it pays (K >= TC_MIN_K) and where the operand contract of gemm_tc.cu
     holds: every source 4-channel aligned with 16-byte aligned rows, and every source but the last a
     multiple of 32 channels (a 32-channel k-slice never straddles two sources)."""
-    if not USE_TC_GEMM or sum(s.channels for s in srcs) < TC_MIN_K:
+    if sum(s.channels for s in srcs) < TC_MIN_K:
         return False
     if any(s.channels % 32 for s in srcs[:-1]):
         return False
     return all((s.channels % 4 == 0) and (s.ld % 4 == 0) and (s.data % 16 == 0) for s in srcs)
 
 
-USE_ROW_MLP = os.environ.get("O3DML_ROW_MLP", "1") != "0"
+USE_ROW_MLP = True
 # one-thread-per-row layers need rows >= SMs x 256 x a few to fill the machine: below this the tensor-core kernel
 # (128 rows per CTA, K >= TC_MIN_K) has the shorter critical path
-ROW_MLP_MIN_ROWS = int(os.environ.get("O3DML_ROW_MLP_MIN_ROWS", "40000"))
+ROW_MLP_MIN_ROWS = 40000
 
 
 def _rows_small_ok(srcs, out, ld, co):
@@ -312,3 +309,12 @@ def pack_operand_image_host(w_nk):
 def pack_operand_image(w_nk):
     """pack_operand_image_host, moved to the device."""
     return pack_operand_image_host(w_nk).cuda()
+
+
+def pack_lfa16_weights(w10_t, s10, t10, wl2_t, s2, t2, wscore_t, bscore):
+    """The host weight block of o3dml_randla_lfa16_pool (O3DML_LFA16_WEIGHT_FLOATS = 448 floats): w10_t [10, 8], s10,
+    t10 [8], wl2_t [8, 8], s2, t2 [8], wscore_t [16, 16], bscore [16], matrices [in, out], concatenated in that order.
+    Returns a float32 CPU tensor."""
+    parts = [t.detach().to("cpu", torch.float32).reshape(-1) for t in (w10_t, s10, t10, wl2_t, s2, t2, wscore_t, bscore)]
+    assert [p.numel() for p in parts] == [80, 8, 8, 64, 8, 8, 256, 16], [p.numel() for p in parts]
+    return torch.cat(parts).contiguous()

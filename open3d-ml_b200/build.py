@@ -6,7 +6,6 @@ The library has no torch dependency: it is a plain C ABI (include/o3dml_b200.h)
 over CUDA kernels, statically linked against cudart.
 """
 import os
-import shlex
 import subprocess
 import sys
 from concurrent.futures import ThreadPoolExecutor
@@ -16,14 +15,9 @@ CSRC = os.path.join(HERE, "csrc")
 OUT_DIR = os.path.join(HERE, "lib")
 LIB = os.path.join(OUT_DIR, "libo3dml_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-DEBUG = ["-DO3DML_DEBUG_NAN"] if os.environ.get("O3DML_DEBUG_NAN") else []
-FLAGS = DEBUG + ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr",
          "-ccbin", "/usr/bin/g++"]
-
-
-# development hook: extra nvcc flags (e.g. -DO3DML_DEBUG_NAN) for A/B builds; use with --force
-FLAGS += shlex.split(os.environ.get("O3DML_NVCC_EXTRA", ""))
 
 
 def sources():

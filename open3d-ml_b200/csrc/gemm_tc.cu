@@ -28,7 +28,6 @@
 #include "../../include/o3dml_b200.h"
 #include "common.cuh"
 #include "tc.cuh"
-#include <stdlib.h>
 #include <cuda.h>
 #include <algorithm>
 
@@ -458,14 +457,12 @@ int gt_num_sms() {
 template <int BN, bool GATHER, bool LITE = false>
 static int gemm_tc_launch_bn(const GemmTcParams& p, unsigned grid_x, cudaStream_t st) {
     using C = GtCfg<BN, LITE>;
-    // the opt-in shared-memory size is a per-device function attribute: set it once per device ordinal
-    static unsigned long long configured = 0;
-    int dev = 0;
-    O3DML_CUDA(cudaGetDevice(&dev));
-    if (dev >= 64 || !((configured >> dev) & 1ull)) {
+    static PerDeviceOnce once;
+    const int dev = current_device();
+    if (once.need(dev)) {
         O3DML_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, GATHER, LITE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                         (int)C::SMEM));
-        if (dev < 64) configured |= 1ull << dev;
+        once.done(dev);
     }
     dim3 grid(grid_x, (unsigned)(p.Npad / BN));
     gemm_tc_kernel<BN, GATHER, LITE><<<grid, gt_threads<GATHER>(), C::SMEM, st>>>(p);
@@ -474,15 +471,7 @@ static int gemm_tc_launch_bn(const GemmTcParams& p, unsigned grid_x, cudaStream_
     return O3DML_OK;
 }
 
-// development hook: O3DML_GEMM_LITE = the longest product (in 32-channel k-slices) that runs on the LITE kernels;
-// 0 keeps everything on the one-CTA-per-SM kernels
-static int gt_lite_max_slices() {
-    static const int n = [] {
-        const char* e = getenv("O3DML_GEMM_LITE");
-        return e ? atoi(e) : 16;
-    }();
-    return n;
-}
+constexpr int GT_LITE_MAX_SLICES = 16;   // longest product, in 32-channel k-slices, that runs on the LITE kernels
 
 static int gemm_tc_launch(GemmTcParams& p, const void* wimg, cudaStream_t st) {
     if (p.N <= 0 || p.Cout <= 0) return O3DML_OK;
@@ -501,7 +490,7 @@ static int gemm_tc_launch(GemmTcParams& p, const void* wimg, cudaStream_t st) {
     }
     // products of plain row sources, at most 16 k-slices long, that fill the SMs more than once as 64-column tiles run on
     // the LITE kernels, two CTAs per SM (GtCfg); the convolutions (K = 9 C) stay on the one-CTA-per-SM kernels
-    const bool lite = p.mode == 0 && !any_gather && p.Kpad / GT_KS <= gt_lite_max_slices() &&
+    const bool lite = p.mode == 0 && !any_gather && p.Kpad / GT_KS <= GT_LITE_MAX_SLICES &&
                       row_tiles * (p.Npad / (bn == 32 ? 32 : 64)) > gt_num_sms();
     if (lite && bn == 128) bn = 64;
     // a grid that fills less than half of the SMs (PointPillars block 3: 27 x 2 CTAs; one cloud per GPU: 6 - 88)

@@ -7,8 +7,36 @@ PCIe copy of a SemanticKITTI batch (~90 MB of neighbour indices) is comparable t
 forward, so the runner overlaps them: the inputs of batch k+1 cross PCIe on a
 copy stream while batch k computes, and the result of batch k returns on a second copy
 stream.  Every batch's inputs and results still cross the bus; nothing is cached.
+
+graph_replay() is the CUDA-graph capture and replay the models use for their launch-bound parts.
 """
 import torch
+
+from . import _lib as L
+
+GRAPH_CACHE_ENTRIES = 8
+
+
+def graph_replay(cache, key, thunk, device):
+    """Replays thunk() from a CUDA graph captured at its first call under `key` and returns a clone of its result (a
+    tensor or a tuple of tensors; the graph's own outputs are overwritten by the next replay).  thunk must be free of
+    host synchronisation and allocation-stable (cached buffers), and the key must name every address it reads.
+    `cache` is the caller's dict; it is cleared when it would exceed GRAPH_CACHE_ENTRIES graphs."""
+    ent = cache.get(key)
+    if ent is None:
+        thunk()                          # sizes the cached buffers and sets kernel attributes, neither capturable
+        torch.cuda.synchronize(device)   # nothing of this device in flight while capturing
+        graph = torch.cuda.CUDAGraph()
+        n0 = L.lib().o3dml_launch_count()
+        with torch.cuda.graph(graph, capture_error_mode="thread_local"):
+            out = thunk()
+        if len(cache) >= GRAPH_CACHE_ENTRIES:
+            cache.clear()
+        ent = cache[key] = (graph, out, L.lib().o3dml_launch_count() - n0)
+    graph, out, launches = ent
+    graph.replay()
+    L.lib().o3dml_launch_count_add(launches)
+    return out.clone() if _is_t(out) else tuple(o.clone() for o in out)
 
 
 def _is_t(x):

@@ -10,7 +10,7 @@ No device->host synchronisation happens inside forward(): the voxel count stays 
 the device (the reference syncs at :106 and once per frame inside the op).
 The dense part (20 launches of 20-60 us each at one KITTI frame) is launch-bound from
 Python, so it is captured once per canvas shape into a CUDA graph and replayed
-(`use_graph=False` or O3DML_PP_GRAPH=0 keeps the eager launches).
+(`use_graph=False` keeps the eager launches).
 Built from a reference ``state_dict``; returns (cls, reg, dir) in NCHW like the
 reference head.
 
@@ -23,6 +23,7 @@ import torch
 
 from . import _lib as L
 from . import ops
+from .pipeline import graph_replay
 
 BN_EPS = 1e-3  # point_pillars.py:409,648,724
 
@@ -38,10 +39,9 @@ class PointPillarsB200:
     output_shape [ny, nx], layer_nums, layer_strides, upsample_strides; for the box decoding also
     num_classes and head = {nms_pre, score_thr, dir_offset, ranges, sizes, rotations} (cfg_from_reference)."""
 
-    def __init__(self, state_dict, cfg, device=None, use_graph=None):
+    def __init__(self, state_dict, cfg, device=None, use_graph=True):
         L.require_cuda()
-        import os
-        self.use_graph = (os.environ.get("O3DML_PP_GRAPH", "1") != "0") if use_graph is None else bool(use_graph)
+        self.use_graph = bool(use_graph)
         self._graphs = {}
         self.device = dev = torch.device(device or "cuda")
         self.cfg = cfg
@@ -143,7 +143,7 @@ class PointPillarsB200:
         OH, OW = (H - 1) // stride + 1, (W - 1) // stride + 1
         out = self._get(name, (B, OH, OW, cout))
         pw = self.w[name + ".wt"]
-        if L.USE_TC_GEMM and cin % 32 == 0:
+        if cin % 32 == 0:
             L.check(L.lib().o3dml_conv3x3_nhwc_tc(L.ptr(x), B, H, W, cin, stride, L.ptr(pw.img), pw.k_pad,
                                                   pw.n_pad, L.ptr(self.w[name + ".s"]),
                                                   L.ptr(self.w[name + ".t"]), 1, 0.0, L.ptr(out), cout,
@@ -159,21 +159,7 @@ class PointPillarsB200:
         if not self.use_graph:
             return self._bnh_eager(canvas)
         key = (canvas.data_ptr(), tuple(canvas.shape))
-        ent = self._graphs.get(key)
-        if ent is None:
-            # eager pass first: sizes the cached buffers and runs the one-time cudaFuncSetAttribute
-            # calls, neither of which may happen under stream capture
-            self._bnh_eager(canvas)
-            torch.cuda.current_stream().synchronize()
-            graph = torch.cuda.CUDAGraph()
-            n0 = L.lib().o3dml_launch_count()
-            with torch.cuda.graph(graph):
-                outs = self._bnh_eager(canvas)
-            ent = self._graphs[key] = (graph, outs, L.lib().o3dml_launch_count() - n0)
-        graph, outs, launches = ent
-        graph.replay()
-        L.lib().o3dml_launch_count_add(launches)
-        return tuple(o.clone() for o in outs)   # the graph's own outputs are overwritten by the next replay
+        return graph_replay(self._graphs, key, lambda: self._bnh_eager(canvas), self.device)
 
     def _bnh_eager(self, canvas):
         B, H, W = canvas.shape[0], canvas.shape[1], canvas.shape[2]
@@ -191,7 +177,7 @@ class PointPillarsB200:
             if h * us != OH or w_ * us != OW:
                 raise RuntimeError("PointPillarsB200: neck scales do not line up")
             pw = self.w[p + ".wt"]
-            if L.USE_TC_GEMM and cin % 4 == 0:
+            if cin % 4 == 0:
                 L.check(L.lib().o3dml_deconv_nhwc_tc(L.ptr(f), B, h, w_, cin, us, L.ptr(pw.img), pw.k_pad,
                                                      pw.n_pad, L.ptr(self.w[p + ".s"]), L.ptr(self.w[p + ".t"]),
                                                      1, 0.0, neck.data_ptr() + 4 * off, self.neck_channels,

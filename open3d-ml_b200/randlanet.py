@@ -18,6 +18,7 @@ indices); the output is ``[B, N, num_classes]`` like the reference.
 import torch
 
 from . import _lib as L
+from .pipeline import graph_replay
 
 BN_EPS = 1e-6  # randlanet.py:77,499
 # d_out values served by the wgmma kernel (lfa_tc.cu).  d = 16 stays on the FP32 SIMT kernel with its weights in the
@@ -36,15 +37,13 @@ def _fold_bn(sd, prefix, bias=None, eps=BN_EPS):
 
 
 class RandLANetB200:
-    def __init__(self, state_dict, num_layers=4, num_neighbors=16, device=None, use_tc=None,
-                 sub_sampling_ratio=None, use_graph=None):
+    def __init__(self, state_dict, num_layers=4, num_neighbors=16, device=None, sub_sampling_ratio=None,
+                 use_graph=True):
         L.require_cuda()
-        import os
         self.sub_sampling_ratio = list(sub_sampling_ratio or [4] * num_layers)
-        self.use_graph = (os.environ.get("O3DML_RL_GRAPH", "1") != "0") if use_graph is None else bool(use_graph)
+        self.use_graph = bool(use_graph)
         self._graphs = {}
         self._splits = {}
-        self.use_tc = (os.environ.get("O3DML_LFA_TC", "1") != "0") if use_tc is None else bool(use_tc)
         self.device = torch.device(device or "cuda")
         self.num_layers = num_layers
         self.k = num_neighbors
@@ -97,16 +96,10 @@ class RandLANetB200:
                     self.w[p + ".lse2.mlp.img"] = L.pack_operand_image(sd[p + ".lse2.mlp.conv.weight"][:, :, 0, 0])
             if d == 16:   # lfa16c_kernel: weights travel in the kernel parameter block (HOST memory)
                 for stage, pool in ((1, "pool1"), (2, "pool2")):
-                    hw = torch.zeros(448, dtype=torch.float32)
-                    hw[0:80] = self.w[p + ".lse1.mlp.wt"].cpu().reshape(-1)
-                    hw[80:88] = self.w[p + ".lse1.mlp.s"].cpu()
-                    hw[88:96] = self.w[p + ".lse1.mlp.t"].cpu()
-                    hw[96:160] = self.w[p + ".lse2.mlp.wt"].cpu().reshape(-1)
-                    hw[160:168] = self.w[p + ".lse2.mlp.s"].cpu()
-                    hw[168:176] = self.w[p + ".lse2.mlp.t"].cpu()
-                    hw[176:432] = self.w["%s.%s.score.wt" % (p, pool)].cpu().reshape(-1)
-                    hw[432:448] = self.w["%s.%s.score.b" % (p, pool)].cpu()
-                    self.w["%s.lfa16.%d" % (p, stage)] = hw.contiguous()
+                    self.w["%s.lfa16.%d" % (p, stage)] = L.pack_lfa16_weights(
+                        *(self.w[p + n] for n in (".lse1.mlp.wt", ".lse1.mlp.s", ".lse1.mlp.t", ".lse2.mlp.wt",
+                                                  ".lse2.mlp.s", ".lse2.mlp.t")),
+                        self.w["%s.%s.score.wt" % (p, pool)], self.w["%s.%s.score.b" % (p, pool)])
             # mlp2 + shortcut as ONE gemm over [p2 | feat] with the BN scales folded into the rows
             s2, t2 = _fold_bn(sd, p + ".mlp2.batch_norm", sd[p + ".mlp2.conv.bias"])
             ss, ts = _fold_bn(sd, p + ".shortcut.batch_norm", sd[p + ".shortcut.conv.bias"])
@@ -124,14 +117,13 @@ class RandLANetB200:
         self.in_channels = sd["fc0.weight"].shape[1]
         self._buf = {}
         # ---- fused tail (rl_tail.cu): last decoder layer + fc1 stack in one kernel
-        self.use_tail = os.environ.get("O3DML_RL_TAIL", "1") != "0"
         self.tail = None
         pl = "decoder.%d" % (num_layers - 1)
         wd = sd[pl + ".conv.weight"][:, :, 0, 0]                          # ConvTranspose2d [in, out]
         w0, w1, w3 = (sd["fc1.%d.conv.weight" % j][:, :, 0, 0].t() for j in (0, 1, 3))
         skip_c = 2 * self.d_out[0]
-        if self.use_tail and L.lib().o3dml_randla_tail_supported(skip_c, wd.shape[0] - skip_c, wd.shape[1], w0.shape[1],
-                                                                 w1.shape[1], self.num_classes):
+        if L.lib().o3dml_randla_tail_supported(skip_c, wd.shape[0] - skip_c, wd.shape[1], w0.shape[1],
+                                               w1.shape[1], self.num_classes):
             img = L.pack_tail_image([wd, w0, w1, w3], [32, 64, 32, 32]).to(dev)
             sc, sh = torch.ones(4, 64), torch.zeros(4, 64)
             for li, name in enumerate((pl, "fc1.0", "fc1.1")):
@@ -156,7 +148,7 @@ class RandLANetB200:
     def _lfa_pool(self, stage, d, coords, nidx, feat, B, N, p, agg):
         w = self.w
         pool = "pool1" if stage == 1 else "pool2"
-        if self.use_tc and d in TC_DIMS:
+        if d in TC_DIMS:
             L.check(L.lib().o3dml_randla_lfa_pool_tc(
                 stage, d, L.ptr(coords), L.ptr(nidx), 1 if nidx.dtype == torch.int64 else 0, self.k,
                 L.ptr(feat), B, N, L.ptr(w[p + ".lse1.mlp.wt"]), L.ptr(w[p + ".lse1.mlp.s"]),
@@ -167,7 +159,7 @@ class RandLANetB200:
                 L.ptr(w[p + ".lse2.mlp.t"]) if stage == 2 else None,
                 L.ptr(w["%s.%s.score.img" % (p, pool)]), L.ptr(agg), L.stream()))
             return
-        if d == 16 and self.use_tc:
+        if d == 16:
             L.check(L.lib().o3dml_randla_lfa16_pool(
                 stage, L.ptr(coords), L.ptr(nidx), 1 if nidx.dtype == torch.int64 else 0, self.k,
                 L.ptr(feat), B, N, w["%s.lfa16.%d" % (p, stage)].data_ptr(), L.ptr(agg), L.stream()))
@@ -344,31 +336,11 @@ class RandLANetB200:
     # ------------------------------------------------------------- CUDA graph
     def _graphed(self, name, tensors, thunk):
         """Replays thunk() from a CUDA graph captured at first use for these tensor addresses (the
-        forward is ~40 launches of 5-60 us: launch-bound from Python at one cloud per GPU).  thunk must
-        be sync-free and allocation-stable (cached buffers); the result is cloned."""
+        forward is ~40 launches of 5-60 us: launch-bound from Python at one cloud per GPU)."""
         if not self.use_graph:
             return thunk()
         key = (name,) + tuple((t.data_ptr(), tuple(t.shape), t.dtype) for t in tensors)
-        ent = self._graphs.get(key)
-        if ent is None:
-            import os
-            legacy = os.environ.get("O3DML_GRAPH_LEGACY") == "1"      # debugging hook: global capture mode
-            thunk()                                        # sizes the cached buffers, sets kernel attributes
-            if legacy:
-                torch.cuda.current_stream().synchronize()
-            else:
-                torch.cuda.synchronize(self.device)        # nothing of this device in flight while capturing
-            graph = torch.cuda.CUDAGraph()
-            n0 = L.lib().o3dml_launch_count()
-            with torch.cuda.graph(graph, capture_error_mode="global" if legacy else "thread_local"):
-                out = thunk()
-            if len(self._graphs) > 8:
-                self._graphs.clear()
-            ent = self._graphs[key] = (graph, out, L.lib().o3dml_launch_count() - n0)
-        graph, out, launches = ent
-        graph.replay()
-        L.lib().o3dml_launch_count_add(launches)
-        return out.clone()
+        return graph_replay(self._graphs, key, thunk, self.device)
 
     def forward_graphed(self, inputs):
         """forward() for DEVICE-resident inputs, replayed from a CUDA graph keyed by their addresses."""
