@@ -357,6 +357,20 @@ O3DML_API int o3dml_kpconv_gather(const float* query_points, int64_t num_queries
                         int num_kernel_points, float kp_extent, float* weighted_features,
                         void* stream);
 
+/* The same operand for a deformable KPConv (kpconv.py:1011-1106, modulated = False): query n uses the
+ * kernel points kp_k + kp_extent * offsets[n * offset_ld + 3k .. 3k+2] (product, then sum, each rounded
+ * in fp32).  A neighbour is kept when |nb_h - q - kp_k|^2 < kp_extent^2 for some k; dropped neighbours
+ * contribute nothing (their features are never read, so a non-finite one does not propagate), kept
+ * neighbours contribute for every k and are summed in ascending h.  offsets is [num_queries, offset_ld]
+ * with offset_ld >= 3K.  Supports in_channels % 4 == 0 with 16-byte aligned features / output, or
+ * in_channels <= 8; anything else is rejected. */
+O3DML_API int o3dml_kpconv_gather_deformable(const float* query_points, int64_t num_queries,
+                        const float* support_points, int64_t num_support,
+                        const void* neighbor_index, int index_is64, int max_neighbors,
+                        const float* features, int in_channels, const float* kernel_points,
+                        int num_kernel_points, float kp_extent, const float* offsets, int offset_ld,
+                        float* weighted_features, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

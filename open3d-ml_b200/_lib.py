@@ -68,6 +68,7 @@ _SIGNATURES = {
     "o3dml_randla_tail": (I, [P, I, P, I, L, P, I, L, L, L, P, P, P, F, I, P, P]),
     "o3dml_gather_max": (I, [P, L, I, I, P, I, L, I, L, L, I, P, I, P]),
     "o3dml_kpconv_gather": (I, [P, L, P, L, P, I, I, P, I, P, I, F, P, P]),
+    "o3dml_kpconv_gather_deformable": (I, [P, L, P, L, P, I, I, P, I, P, I, F, P, I, P, P]),
 }
 EXPORTS = tuple(_SIGNATURES)           # the product ABI: exactly what include/o3dml_b200.h declares
 # bring-up / profiling hooks (include/o3dml_b200_bringup.h): exported by the library, not part of the product ABI

@@ -138,23 +138,32 @@ kpconv_gather_kernel(const float* __restrict__ q_pts, const float* __restrict__ 
 // current chunk of LPQ neighbours and parks them in shared memory; the accumulate loop then
 // fetches 16 weights with 4 LDS.128 per neighbour and feeds 60 FMAs per lane from them, and the
 // neighbour's feature row arrives as one float4 per lane (LPQ x 16 B contiguous).
-template <int LPQ, int NE>   // NE channels per lane: 4 (float4 rows) or 1 (unaligned Cin <= 8, the first layer)
+//
+// DEFORM (deformable KPConv, kpconv.py:1011-1106, modulated = False): every query has its own kernel
+// points kp_k + extent * offsets[q, 3k .. 3k+2] (product and sum rounded separately, as the reference),
+// parked per query in shared memory.  A neighbour is kept when d2 < extent^2 for at least one of
+// them; the group compacts its kept neighbours in ascending row position (ballot + popc) into the
+// w_s / nb_s slots, so a dropped neighbour costs neither a feature load nor an FMA.
+template <int LPQ, int NE, bool DEFORM = false>   // NE channels per lane: 4 (float4 rows) or 1 (unaligned Cin <= 8)
 __global__ void __launch_bounds__(256)
 kpconv_gather_grouped_kernel(const float* __restrict__ q_pts, const float* __restrict__ s_pts,
                              int64_t n_support, const void* __restrict__ nidx, int idx_is64, int H,
                              const float* __restrict__ x, int Cin, const float* __restrict__ kpts, int K,
-                             float extent, int64_t nq, float* __restrict__ out) {
+                             float extent, int64_t nq, float* __restrict__ out,
+                             const float* __restrict__ offsets = nullptr, int offset_ld = 0) {
     constexpr int QPW = 32 / LPQ;                       // queries per warp
-    __shared__ float4 kp4[KP_MAXK];
+    __shared__ float4 kp4[(DEFORM ? 8 * QPW : 1) * KP_MAXK];   // DEFORM: [warp][query][kernel point]
     // [warp][4 kernel points][slot]: slot = row ^ (row / LPQ) spreads the QPW rows that are read
     // together (same neighbour position of the QPW queries) over different banks
     __shared__ float4 w_s[8][KP_MAXK / 4][32];
     __shared__ int nb_s[8][32];
-    if (threadIdx.x < KP_MAXK)
-        kp4[threadIdx.x] = threadIdx.x < K ? make_float4(kpts[3 * threadIdx.x], kpts[3 * threadIdx.x + 1],
-                                                         kpts[3 * threadIdx.x + 2], 0.f)
-                                           : make_float4(1e18f, 1e18f, 1e18f, 0.f);   // unused slot: weight 0
-    __syncthreads();
+    if constexpr (!DEFORM) {
+        if (threadIdx.x < KP_MAXK)
+            kp4[threadIdx.x] = threadIdx.x < K ? make_float4(kpts[3 * threadIdx.x], kpts[3 * threadIdx.x + 1],
+                                                             kpts[3 * threadIdx.x + 2], 0.f)
+                                               : make_float4(1e18f, 1e18f, 1e18f, 0.f);   // unused slot: weight 0
+        __syncthreads();
+    }
     const float inv_ext = 1.f / extent;
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const int qg = lane / LPQ, lq = lane % LPQ;          // query of this lane within the warp, lane within group
@@ -164,6 +173,22 @@ kpconv_gather_grouped_kernel(const float* __restrict__ q_pts, const float* __res
     const bool qok = q < nq;
     float qx = 0.f, qy = 0.f, qz = 0.f;
     if (qok) { qx = q_pts[3 * q]; qy = q_pts[3 * q + 1]; qz = q_pts[3 * q + 2]; }
+    float4* const kpw = kp4 + (DEFORM ? (wib * QPW + qg) * KP_MAXK : 0);   // this lane's kernel points
+    float ext2 = 0.f;
+    if constexpr (DEFORM) {
+        ext2 = extent * extent;
+        for (int k = lq; k < KP_MAXK; k += LPQ) {
+            float4 d = make_float4(1e18f, 1e18f, 1e18f, 0.f);                  // unused slot: never in range
+            if (qok && k < K) {
+                const float* o = offsets + (size_t)q * offset_ld + 3 * k;
+                d = make_float4(__fadd_rn(__fmul_rn(o[0], extent), kpts[3 * k]),
+                                __fadd_rn(__fmul_rn(o[1], extent), kpts[3 * k + 1]),
+                                __fadd_rn(__fmul_rn(o[2], extent), kpts[3 * k + 2]), 0.f);
+            }
+            kpw[k] = d;
+        }
+        __syncwarp();
+    }
     const int KK = K * Cin;
     for (int c0 = 0; c0 < Cin; c0 += LPQ * NE) {
         const int c = c0 + NE * lq;
@@ -181,38 +206,53 @@ kpconv_gather_grouped_kernel(const float* __restrict__ q_pts, const float* __res
             }
             // trailing all-shadow positions (the padded tail of the neighbour rows) are skipped for the
             // whole warp; hc = one past the last position that is valid for any of the QPW queries
-            const unsigned valid = __ballot_sync(0xffffffffu, nb >= 0);
-            if (valid == 0u) continue;
             int hc = 0;
+            if constexpr (!DEFORM) {
+                const unsigned valid = __ballot_sync(0xffffffffu, nb >= 0);
+                if (valid == 0u) continue;
 #pragma unroll
-            for (int g = 0; g < QPW; ++g) {
-                const unsigned mg = (LPQ == 32) ? valid : ((valid >> (g * LPQ)) & ((1u << (LPQ & 31)) - 1u));
-                hc = max(hc, 32 - __clz(mg));
+                for (int g = 0; g < QPW; ++g) {
+                    const unsigned mg = (LPQ == 32) ? valid : ((valid >> (g * LPQ)) & ((1u << (LPQ & 31)) - 1u));
+                    hc = max(hc, 32 - __clz(mg));
+                }
             }
             float w[KP_MAXK];
 #pragma unroll
             for (int k = 0; k < KP_MAXK; ++k) w[k] = 0.f;
+            bool keep = false;
             if (nb >= 0) {
                 const float nx = s_pts[3 * (size_t)nb] - qx, ny = s_pts[3 * (size_t)nb + 1] - qy,
                             nz = s_pts[3 * (size_t)nb + 2] - qz;
 #pragma unroll
                 for (int k = 0; k < KP_MAXK; ++k) {      // linear influence max(0, 1 - |y - kp_k| / extent)
-                    const float4 kk = kp4[k];
+                    const float4 kk = DEFORM ? kpw[k] : kp4[k];
                     const float dx = nx - kk.x, dy = ny - kk.y, dz = nz - kk.z;
                     const float d2 = fmaf(dz, dz, fmaf(dy, dy, dx * dx));
+                    if constexpr (DEFORM) keep |= d2 < ext2;
                     float dist;                          // 2-ulp sqrt: far inside the 1e-4 feature tolerance
                     asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(dist) : "f"(d2));
                     w[k] = fmaxf(fmaf(-dist, inv_ext, 1.f), 0.f);
                 }
             }
+            // DEFORM: slot row of this lane's neighbour after compaction, and the group's kept count
+            int row = lane, kept = 0;
+            if constexpr (DEFORM) {
+                const unsigned valid = __ballot_sync(0xffffffffu, keep);
+                if (valid == 0u) continue;
+                const unsigned mg = (LPQ == 32) ? valid : ((valid >> (qg * LPQ)) & ((1u << (LPQ & 31)) - 1u));
+                kept = __popc(mg);
+                row = qg * LPQ + __popc(mg & ((1u << lq) - 1u));
+            }
             __syncwarp();                                   // previous chunk fully consumed
+            if (!DEFORM || keep) {
 #pragma unroll
-            for (int k4 = 0; k4 < KP_MAXK / 4; ++k4)
-                w_s[wib][k4][lane ^ qg] = make_float4(w[4 * k4], w[4 * k4 + 1], w[4 * k4 + 2], w[4 * k4 + 3]);
-            nb_s[wib][lane] = nb;
+                for (int k4 = 0; k4 < KP_MAXK / 4; ++k4)
+                    w_s[wib][k4][row ^ qg] = make_float4(w[4 * k4], w[4 * k4 + 1], w[4 * k4 + 2], w[4 * k4 + 3]);
+                nb_s[wib][row] = nb;
+            }
             __syncwarp();
-            // ---- accumulate the chunk: 4 channels per lane
-            for (int hh = 0; hh < hc; ++hh) {
+            // ---- accumulate the chunk: 4 channels per lane (DEFORM: the group's kept neighbours only)
+            for (int hh = 0; hh < (DEFORM ? kept : hc); ++hh) {
                 const int nbh = nb_s[wib][qg * LPQ + hh];
                 float xv[NE];
 #pragma unroll
@@ -314,6 +354,38 @@ extern "C" int o3dml_kpconv_gather(const float* query_points, int64_t num_querie
     else if (in_channels <= 64) KP_LAUNCH(2);
     else KP_LAUNCH(4);
 #undef KP_LAUNCH
+    O3DML_LAUNCH_CHECK();
+    o3dml_count_launches(1);
+    return O3DML_OK;
+}
+
+extern "C" int o3dml_kpconv_gather_deformable(const float* query_points, int64_t num_queries,
+                                              const float* support_points, int64_t num_support,
+                                              const void* neighbor_index, int index_is64, int max_neighbors,
+                                              const float* features, int in_channels,
+                                              const float* kernel_points, int num_kernel_points,
+                                              float kp_extent, const float* offsets, int offset_ld,
+                                              float* weighted_features, void* stream) {
+    O3DML_CHECK(num_kernel_points >= 1 && num_kernel_points <= KP_MAXK,
+                "kpconv_deformable: at most %d kernel points", KP_MAXK);
+    O3DML_CHECK(max_neighbors >= 0 && in_channels >= 1 && kp_extent > 0.f, "kpconv_deformable: bad sizes");
+    O3DML_CHECK(offsets != nullptr && offset_ld >= 3 * num_kernel_points,
+                "kpconv_deformable: offsets [num_queries, >= 3K] required");
+    const bool aligned = (in_channels & 3) == 0 &&
+                         ((reinterpret_cast<uintptr_t>(features) | reinterpret_cast<uintptr_t>(weighted_features)) & 15) == 0;
+    O3DML_CHECK(num_support < ((int64_t)1 << 31) && (aligned || in_channels <= 8),
+                "kpconv_deformable: Cin % 4 == 0 with 16-byte aligned rows, or Cin <= 8; fewer than 2^31 supports");
+    if (num_queries <= 0) return O3DML_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+#define KPD_LAUNCH(LPQ, NE)                                                                                             \
+    kpconv_gather_grouped_kernel<LPQ, NE, true><<<(unsigned)ceil_div<int64_t>(num_queries, 8 * (32 / LPQ)), 256, 0, st>>>( \
+        query_points, support_points, num_support, neighbor_index, index_is64, max_neighbors, features, in_channels,     \
+        kernel_points, num_kernel_points, kp_extent, num_queries, weighted_features, offsets, offset_ld)
+    if (!aligned) KPD_LAUNCH(8, 1);
+    else if (in_channels <= 32) KPD_LAUNCH(8, 4);
+    else if (in_channels <= 64) KPD_LAUNCH(16, 4);
+    else KPD_LAUNCH(32, 4);
+#undef KPD_LAUNCH
     O3DML_LAUNCH_CHECK();
     o3dml_count_launches(1);
     return O3DML_OK;

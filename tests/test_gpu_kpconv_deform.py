@@ -1,0 +1,224 @@
+"""o3dml_kpconv_gather_deformable against a float64 torch restatement of the offsets and the neighbour
+re-selection (tests/kpconv_deform_support.py), and KPFCNNB200 on the deformable Paris-Lille3D config against the
+unmodified reference (tests/golden/boundary_kpconv_deform_class.npz) and the torch port."""
+import ctypes
+import json
+
+import numpy as np
+import pytest
+import torch
+
+import kpconv_deform_support as KD
+from conftest import rel_err
+from test_oracle_kpconv_deform import fixture, sampled_rel_err
+
+pytestmark = pytest.mark.gpu
+
+K = 15
+EXT = 0.3
+# H100 80GB HBM3: largest gather error 1.3e-6 of max(1, row scale) over the Cin x H grid; fixture model error 2.5e-5
+GATHER_TOL = 7e-6
+MODEL_TOL = 1e-4
+# the 18 k-point batch against the float64 port: 1.9e-4 at the logits.  The error grows through depth (2e-7 after
+# block 0, 4.7e-6 after block 4, 2.4e-4 after block 9): with seeded weights the offsets reach ~2.5 extents and a
+# deformable conv turns a feature error into a kernel-point shift with a 1 / extent slope
+BATCH_TOL = 1e-3
+
+
+def lib():
+    from open3d_ml_b200 import _lib as L
+    return L
+
+
+def gather_deform(q, s, nidx, x, kp, off, extent=EXT, out=None, nq=None):
+    L = lib()
+    nq = q.shape[0] if nq is None else nq
+    if out is None:
+        out = torch.full((q.shape[0], K * x.shape[1]), 7.0, device="cuda")
+    L.check(L.lib().o3dml_kpconv_gather_deformable(
+        L.ptr(q), nq, L.ptr(s), s.shape[0], L.ptr(nidx), 1 if nidx.dtype == torch.int64 else 0, nidx.shape[1],
+        L.ptr(x), x.shape[1], L.ptr(kp), kp.shape[0], float(extent), L.ptr(off), off.stride(0), L.ptr(out),
+        L.stream()))
+    return out
+
+
+def case(cin, H, seed, strided=False, is64=True, nq=300, ns=400, off_scale=0.5):
+    g = torch.Generator().manual_seed(seed)
+    s = torch.rand((ns, 3), generator=g) * 1.2
+    q = s[:nq].clone() if not strided else torch.rand((nq // 3 + 1, 3), generator=g) * 1.2
+    nidx = torch.randint(0, ns, (q.shape[0], H), generator=g)
+    if H:
+        nidx[torch.rand((q.shape[0], H), generator=g) < 0.1] = ns        # shadow ids >= n_support
+        nidx[torch.rand((q.shape[0], H), generator=g) < 0.05] = -1      # and < 0
+        nidx[3] = ns                                                      # an all-shadow row
+    x = torch.randn((ns, cin), generator=g)
+    kp = torch.randn((K, 3), generator=g) * 0.2 * EXT
+    kp[0] = 0
+    off = torch.zeros((q.shape[0], 48))
+    off[:, :3 * K] = torch.randn((q.shape[0], 3 * K), generator=g) * off_scale
+    nidx = nidx if is64 else nidx.int()
+    return [t.cuda().contiguous() for t in (q, s, nidx, x, kp)] + [off.cuda()]
+
+
+def want_deform(q, s, nidx, x, kp, off, extent=EXT):
+    d = lambda t: t.double().cpu()  # noqa: E731
+    dkp = d(off[:, :3 * K]).view(-1, K, 3) * extent + d(kp)
+    n = d(nidx.long())
+    return KD.deform_gather(d(q), d(s), n.long(), d(x), dkp, extent).reshape(q.shape[0], -1)
+
+
+def row_err(got, want):
+    return float(((got.double().cpu() - want).abs().amax(1) / want.abs().amax(1).clamp_min(1.0)).max())
+
+
+@pytest.mark.parametrize("cin", [1, 5, 32, 64, 128, 512])
+@pytest.mark.parametrize("H", [0, 1, 31, 32, 33, 400])
+def test_deformable_gather_matches_float64(cin, H):
+    seed = cin * 1000 + H
+    args = case(cin, H, seed, strided=(H % 2 == 1), is64=(cin % 2 == 0))
+    got = gather_deform(*args)
+    want = want_deform(*args)
+    assert torch.isfinite(got).all()
+    err = row_err(got, want)
+    print("gather err cin=%d H=%d %.3g" % (cin, H, err))
+    assert err < GATHER_TOL
+
+
+def test_offsets_away_from_every_neighbour_give_zero_rows():
+    q, s, nidx, x, kp, off = case(64, 40, 5)
+    off[:, :3 * K] = 100.0
+    assert torch.equal(gather_deform(q, s, nidx, x, kp, off), torch.zeros((q.shape[0], K * 64), device="cuda"))
+
+
+def test_inf_feature_propagates_only_from_kept_neighbours():
+    q, s, nidx, x, kp, off = case(32, 40, 6)
+    _, kept = KD.deform_influence(q.double().cpu(), s.double().cpu(), nidx.cpu(),
+                                  off[:, :3 * K].double().cpu().view(-1, K, 3) * EXT + kp.double().cpu(), EXT)
+    valid = (nidx.cpu() >= 0) & (nidx.cpu() < s.shape[0])
+    r = 10
+    nk = int(nidx[r, int(torch.nonzero(kept[r])[0])])
+    nd = int(nidx[r, int(torch.nonzero(valid[r] & ~kept[r])[0])])
+    for n in (nk, nd):
+        x2 = x.clone()
+        x2[n, 0] = float("inf")
+        out = gather_deform(q, s, nidx, x2, kp, off)
+        keeps = ((nidx.cpu() == n) & kept).any(1)
+        assert torch.equal(torch.isfinite(out).all(1).cpu(), ~keeps), n
+        assert bool(keeps[r]) == (n == nk)       # row r: non-finite through its kept neighbour only
+
+
+def test_zero_offsets_agree_with_the_rigid_kernel():
+    L = lib()
+    q, s, nidx, x, kp, off = case(128, 48, 7, off_scale=0.0)
+    got = gather_deform(q, s, nidx, x, kp, off)
+    rigid = torch.empty_like(got)
+    L.check(L.lib().o3dml_kpconv_gather(
+        L.ptr(q), q.shape[0], L.ptr(s), s.shape[0], L.ptr(nidx), 1, nidx.shape[1], L.ptr(x), 128, L.ptr(kp), K,
+        EXT, L.ptr(rigid), L.stream()))
+    assert float((got - rigid).abs().max() / rigid.abs().max()) < 1e-6
+
+
+@pytest.mark.parametrize("cin", [5, 64])
+def test_rows_do_not_depend_on_nq_and_sentinels_stay(cin):
+    q, s, nidx, x, kp, off = case(cin, 70, 8)
+    full = gather_deform(q, s, nidx, x, kp, off)
+    for nq in (1, 37, 150):
+        part = gather_deform(q, s, nidx, x, kp, off, nq=nq)
+        assert torch.equal(part[:nq], full[:nq])
+        assert bool((part[nq:] == 7.0).all())
+
+
+def test_argument_rejections_and_export():
+    L = lib()
+    assert hasattr(ctypes.CDLL(L.LIB_PATH), "o3dml_kpconv_gather_deformable")
+    q, s, nidx, x, kp, off = case(32, 8, 9)
+    out = torch.empty((q.shape[0], K * 32), device="cuda")
+
+    def call(x=x, kpn=K, extent=EXT, off_ptr=None, ld=48, out_ptr=None, cin=None):
+        return L.lib().o3dml_kpconv_gather_deformable(
+            L.ptr(q), q.shape[0], L.ptr(s), s.shape[0], L.ptr(nidx), 1, nidx.shape[1], L.ptr(x) if cin is None
+            else x, x.shape[1] if cin is None else cin, L.ptr(kp), kpn, float(extent),
+            L.ptr(off) if off_ptr is None else off_ptr, ld, L.ptr(out) if out_ptr is None else out_ptr, L.stream())
+    assert call() == 0
+    for bad in (dict(off_ptr=0), dict(ld=3 * K - 1), dict(kpn=17), dict(extent=0.0), dict(extent=-1.0),
+                dict(out_ptr=out.data_ptr() + 4)):
+        assert call(**bad) != 0, bad
+    x12 = torch.zeros((400 * 12 + 1,), device="cuda")
+    assert call(x=x12.data_ptr() + 4, cin=12) != 0          # Cin > 8 without 16-byte rows
+    torch.cuda.synchronize()
+
+
+# ------------------------------------------------------------------------------------------------- model level
+def test_kpfcnn_b200_matches_the_unmodified_reference_on_paris_lille3d():
+    import open3d_ml_b200 as M
+    g, sd, batch, cfg = fixture()
+    net = M.KPFCNNB200(sd, cfg)
+    taps = {}
+    got = net(batch, taps=taps)
+    errs = {"ref": sampled_rel_err(got, g, "ref")}
+    for i in g["deform_blocks"].tolist():
+        errs[i] = sampled_rel_err(taps["encoder_blocks.%d" % i], g, "enc_%d" % i)
+    print("fixture errors", json.dumps(errs))
+    assert max(errs.values()) < MODEL_TOL, errs
+
+
+def paris_cfg():
+    _, _, _, cfg = fixture()
+    return cfg
+
+
+def test_build_batch_paris_lille3d_matches_the_oracle_pyramid_at_deform_radii():
+    from open3d_ml_b200.kpconv import build_batch, layer_radii
+    from oracle import ops as O, models_torch as MT
+    cfg = paris_cfg()
+    clouds = KD.paris_clouds(300, batch_limit=8000)
+    b = build_batch(clouds, cfg)
+    P = np.concatenate([c[0] for c in clouds])
+    lens = [len(c[0]) for c in clouds]
+    r = cfg["first_subsampling_dl"] * cfg["conv_radius"]
+    for lvl, (rc, rp, ru) in enumerate(layer_radii(cfg)[:cfg["num_layers"]]):
+        assert np.array_equal(b["points"][lvl].cpu().numpy(), P)
+        assert np.array_equal(b["neighbors"][lvl].cpu().numpy(), MT.kp_batch_neighbors(P, P, lens, lens, rc))
+        if lvl < cfg["num_layers"] - 1:
+            Q, ql = O.c_subsample_batch(P, lens, None, None, 2 * r / cfg["conv_radius"])
+            assert np.array_equal(b["pools"][lvl].cpu().numpy(), MT.kp_batch_neighbors(Q, P, ql, lens, rp))
+            assert np.array_equal(b["upsamples"][lvl].cpu().numpy(), MT.kp_batch_neighbors(P, Q, lens, ql, ru))
+            P, lens, r = Q, list(ql), 2 * r
+
+
+def test_kpfcnn_b200_paris_lille3d_batch_matches_the_port():
+    import open3d_ml_b200 as M
+    from open3d_ml_b200.kpconv import build_batch
+    _, sd, _, cfg = fixture()
+    b = build_batch(KD.paris_clouds(400), cfg)
+    got = M.KPFCNNB200(sd, cfg)(b)
+    sdc = {k: v.cuda().double() if v.is_floating_point() else v.cuda() for k, v in sd.items()}
+    b64 = dict(b, features=b["features"].double(), points=[p.double() for p in b["points"]])
+    with torch.no_grad():
+        want = KD.kpfcnn_forward(sdc, b64, cfg)
+    err = rel_err(got, want)
+    print("paris batch rel err %.3g over %d points" % (err, b["points"][0].shape[0]))
+    assert err < BATCH_TOL
+
+
+def test_forward_does_not_sync_the_host():
+    import open3d_ml_b200 as M
+    from open3d_ml_b200.kpconv import build_batch
+    _, sd, _, cfg = fixture()
+    b = build_batch(KD.paris_clouds(500, batch_limit=8000), cfg)
+    net = M.KPFCNNB200(sd, cfg)
+    want = net(b).clone()                    # first call caches what the GEMMs keep on the host
+    torch.cuda.synchronize()
+    torch.cuda.set_sync_debug_mode("error")
+    try:
+        got = net(b)
+    finally:
+        torch.cuda.set_sync_debug_mode(0)
+    assert torch.equal(got, want)
+
+
+def test_modulated_is_rejected():
+    import open3d_ml_b200 as M
+    _, sd, _, cfg = fixture()
+    with pytest.raises(RuntimeError, match="modulated"):
+        M.KPFCNNB200(sd, dict(cfg, modulated=True))
