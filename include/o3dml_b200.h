@@ -204,7 +204,7 @@ O3DML_API int o3dml_pp_detect(const float* cls, int64_t cls_batch_stride, const 
 /* ------------------------------------------------------ dense layers ---- */
 
 /* One operand of the gathered GEMM: rows of `channels` floats (row stride ld); when `index`
- * is given, output row n reads row index[n * index_ld] (ids outside [0, rows) read zeros:
+ * is given, output row n reads row index[n * index_ld], index_ld <= 0 reading as 1 (ids outside [0, rows) read zeros:
  * the "shadow" neighbours of kpconv.py:821-858); with out_rows_per_batch > 0 the ids are
  * relative to the batch item n / out_rows_per_batch (RandLA-Net's [B,N,1] interp_idx). */
 typedef struct o3dml_src_t {

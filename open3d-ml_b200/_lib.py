@@ -291,6 +291,42 @@ def linear(srcs, weight, out, scale=None, shift=None, residual=None, act=None, s
     return out
 
 
+def conv3x3(x, weight, out, scale=None, shift=None, stride=1, act=None, slope=0.0):
+    """out = act(scale * conv3x3(x) + shift): padding 1, stride 1 or 2, x [B, H, W, C] and out [B, OH, OW, Cout]
+    contiguous NHWC.  `weight` [9 C, Cout] (row (ky * 3 + kx) * C + c) is either an fp32 tensor (SIMT kernel) or a
+    PackedWeight (tensor-core kernel when C % 32 == 0, SIMT otherwise)."""
+    B, H, W, C = x.shape
+    co = out.shape[3]
+    if isinstance(weight, PackedWeight) and C % 32 == 0:
+        check(lib().o3dml_conv3x3_nhwc_tc(ptr(x), B, H, W, C, stride, ptr(weight.img), weight.k_pad, weight.n_pad,
+                                          ptr(scale), ptr(shift), act_code(act), float(slope), ptr(out), co, stream()))
+    else:
+        wt = weight.wt if isinstance(weight, PackedWeight) else weight
+        check(lib().o3dml_conv3x3_nhwc(ptr(x), B, H, W, C, stride, ptr(wt), ptr(scale), ptr(shift), act_code(act),
+                                       float(slope), ptr(out), co, stream()))
+    return out
+
+
+def deconv(x, weight, out, scale=None, shift=None, stride=1, act=None, slope=0.0):
+    """ConvTranspose2d with kernel == stride: out = act(scale * deconv(x) + shift), x [B, H, W, C] contiguous NHWC,
+    out [B, H * stride, W * stride, Cout] NHWC with unit channel stride, possibly a channel slice of a wider buffer.
+    `weight` [C, stride^2 * Cout] (column (ky * stride + kx) * Cout + co); scale / shift tiled to [stride^2 * Cout].
+    An fp32 tensor runs the SIMT kernel; a PackedWeight the tensor-core kernel when C % 4 == 0, SIMT otherwise."""
+    B, H, W, C = x.shape
+    co, ld = out.shape[3], out.stride(2)
+    if out.stride(3) != 1 or out.stride(1) != out.shape[2] * ld or out.stride(0) != out.shape[1] * out.stride(1):
+        raise ValueError("deconv: out must be NHWC rows of a uniform stride")
+    if isinstance(weight, PackedWeight) and C % 4 == 0:
+        check(lib().o3dml_deconv_nhwc_tc(ptr(x), B, H, W, C, stride, ptr(weight.img), weight.k_pad, weight.n_pad,
+                                         ptr(scale), ptr(shift), act_code(act), float(slope), ptr(out), ld, co,
+                                         stream()))
+    else:
+        wt = weight.wt if isinstance(weight, PackedWeight) else weight
+        check(lib().o3dml_deconv_nhwc(ptr(x), B, H, W, C, stride, ptr(wt), ptr(scale), ptr(shift), act_code(act),
+                                      float(slope), ptr(out), ld, co, stream()))
+    return out
+
+
 def pack_operand_image_host(w_nk):
     """fp32 [N, K] (K contiguous, i.e. nn.Linear's [out, in]) -> uint8 CPU tensor holding the
     3xFP16 operand images of csrc/tc.cuh: [K/8][N][8 halves] of hi = fp16(w), then the same

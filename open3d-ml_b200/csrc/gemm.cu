@@ -16,7 +16,7 @@
 // This file is the FP32 SIMT implementation (exact to ~1e-6 of the reference);
 // register-tiled 8x4 per thread, BK = 16, register prefetch of the next k-tile.
 #include "../../include/o3dml_b200.h"
-#include "common.cuh"
+#include "dense.cuh"
 
 namespace o3dml {
 
@@ -26,54 +26,19 @@ constexpr int GEMM_TM = 8;
 constexpr int GEMM_TN = 4;
 constexpr int MAX_SRC = 3;
 
-struct GemmSrc {
-    const float* data;
-    const void* index;        // null = identity
-    int64_t rows;             // rows in data (index outside [0, rows) -> zero row)
-    int64_t out_rows_per_batch;  // 0 = global indices
-    int64_t src_rows_per_batch;
-    int32_t channels, ld, index_is64, index_ld;
-};
-
 struct GemmParams {
     int64_t N;
     int K, Cout;
     int mode;  // 0 rows, 1 conv3x3
     int nsrc;
-    GemmSrc src[MAX_SRC];
+    o3dml_src_t src[MAX_SRC];
     int koff[MAX_SRC + 1];
     int vec_a;  // all sources float4-loadable
     // conv3x3 (src[0].data = NHWC input)
     int H, W, OH, OW, stride, C;
     const float* Wt;  // [K, Cout]
-    const float* scale;
-    const float* shift;
-    const float* residual;
-    int res_ld;
-    int act;
-    float slope;
-    float* out;
-    int out_ld;
-    int out_mode;   // 0 rows, 1 NCHW, 2 deconv pixel shuffle
-    int64_t plane;  // NCHW: rows per image
-    int ds, dIH, dIW, dC;
+    DenseEpilogue ep;
 };
-
-// Resolves the address of A[n, k..k+3] (vector path) -- returns nullptr for zero rows.
-__device__ __forceinline__ const float* rows_src_ptr(const GemmParams& p, int s, int64_t n) {
-    const GemmSrc& S = p.src[s];
-    int64_t r = n;
-    if (S.index) {
-        r = load_index(S.index, n * S.index_ld, S.index_is64);
-        if (r < 0) return nullptr;
-        if (S.out_rows_per_batch > 0) {
-            if (r >= S.src_rows_per_batch) return nullptr;
-            r += (n / S.out_rows_per_batch) * S.src_rows_per_batch;
-        }
-        if (r >= S.rows) return nullptr;
-    }
-    return S.data + (size_t)r * S.ld;
-}
 
 template <int BN>
 __global__ void __launch_bounds__(GEMM_THREADS)
@@ -88,6 +53,7 @@ gemm_gather_kernel(const __grid_constant__ GemmParams p) {
     __shared__ const float* rowptr[MAX_SRC][BM];  // rows mode: per-source row base
     __shared__ int rowinfo[BM][3];                // conv mode: image base pixel, iy0, ix0
 
+    const DenseEpilogue& ep = p.ep;
     const int tid = threadIdx.x;
     const int tx = tid % TX, ty = tid / TX;
     const int64_t row0 = (int64_t)blockIdx.x * BM;
@@ -98,7 +64,7 @@ gemm_gather_kernel(const __grid_constant__ GemmParams p) {
         for (int i = tid; i < p.nsrc * BM; i += GEMM_THREADS) {
             int s = i / BM, m = i % BM;
             int64_t n = row0 + m;
-            rowptr[s][m] = (n < p.N) ? rows_src_ptr(p, s, n) : nullptr;
+            rowptr[s][m] = (n < p.N) ? src_row(p.src[s], n) : nullptr;
         }
     } else {
         for (int m = tid; m < BM; m += GEMM_THREADS) {
@@ -239,8 +205,8 @@ gemm_gather_kernel(const __grid_constant__ GemmParams p) {
 #pragma unroll
     for (int j = 0; j < GEMM_TN; ++j) {
         int c = cbase + j;
-        sc[j] = (p.scale && c < p.Cout) ? p.scale[c] : 1.f;
-        sh[j] = (p.shift && c < p.Cout) ? p.shift[c] : 0.f;
+        sc[j] = (ep.scale && c < p.Cout) ? ep.scale[c] : 1.f;
+        sh[j] = (ep.shift && c < p.Cout) ? ep.shift[c] : 0.f;
     }
 #pragma unroll
     for (int i = 0; i < GEMM_TM; ++i) {
@@ -251,48 +217,51 @@ gemm_gather_kernel(const __grid_constant__ GemmParams p) {
         for (int j = 0; j < GEMM_TN; ++j) {
             int c = cbase + j;
             float x = fmaf(acc[i][j], sc[j], sh[j]);
-            if (p.residual && c < p.Cout) x += p.residual[(size_t)n * p.res_ld + c];
-            v[j] = apply_act(x, p.act, p.slope);
+            if (ep.residual && c < p.Cout) x += ep.residual[(size_t)n * ep.res_ld + c];
+            v[j] = apply_act(x, ep.act, ep.slope);
         }
-        if (p.out_mode == 0) {
-            float* o = p.out + (size_t)n * p.out_ld + cbase;
-            if (cbase + 3 < p.Cout && (p.out_ld & 3) == 0 &&
-                ((reinterpret_cast<uintptr_t>(p.out) & 15) == 0)) {
+        if (ep.mode == 0) {
+            float* o = ep.out + (size_t)n * ep.out_ld + cbase;
+            if (cbase + 3 < p.Cout && (ep.out_ld & 3) == 0 &&
+                ((reinterpret_cast<uintptr_t>(ep.out) & 15) == 0)) {
                 *reinterpret_cast<float4*>(o) = make_float4(v[0], v[1], v[2], v[3]);
             } else {
 #pragma unroll
                 for (int j = 0; j < GEMM_TN; ++j)
                     if (cbase + j < p.Cout) o[j] = v[j];
             }
-        } else if (p.out_mode == 1) {
-            const int64_t b = n / p.plane, pix = n % p.plane;
+        } else if (ep.mode == 1) {
+            const int64_t b = n / ep.plane, pix = n % ep.plane;
 #pragma unroll
             for (int j = 0; j < GEMM_TN; ++j)
                 if (cbase + j < p.Cout)
-                    p.out[((size_t)b * p.Cout + cbase + j) * p.plane + pix] = v[j];
+                    ep.out[((size_t)b * p.Cout + cbase + j) * ep.plane + pix] = v[j];
         } else {
-            const int64_t per = (int64_t)p.dIH * p.dIW;
+            const int64_t per = (int64_t)ep.dIH * ep.dIW;
             const int64_t b = n / per;
             const int r = (int)(n % per);
-            const int iy = r / p.dIW, ix = r % p.dIW;
-            const int OWd = p.dIW * p.ds;
+            const int iy = r / ep.dIW, ix = r % ep.dIW;
+            const int OWd = ep.dIW * ep.ds;
 #pragma unroll
             for (int j = 0; j < GEMM_TN; ++j) {
                 int c = cbase + j;
                 if (c < p.Cout) {
-                    int sub = c / p.dC, co = c - sub * p.dC;
-                    int dy = sub / p.ds, dx = sub - dy * p.ds;
-                    size_t opix = ((size_t)b * p.dIH * p.ds + (size_t)iy * p.ds + dy) * OWd +
-                                  (size_t)ix * p.ds + dx;
-                    p.out[opix * p.out_ld + co] = v[j];
+                    int sub = c / ep.dC, co = c - sub * ep.dC;
+                    int dy = sub / ep.ds, dx = sub - dy * ep.ds;
+                    size_t opix = ((size_t)b * ep.dIH * ep.ds + (size_t)iy * ep.ds + dy) * OWd +
+                                  (size_t)ix * ep.ds + dx;
+                    ep.out[opix * ep.out_ld + co] = v[j];
                 }
             }
         }
     }
 }
 
-static int gemm_launch(const GemmParams& p, cudaStream_t st) {
+static int gemm_launch(GemmParams& p, cudaStream_t st) {
     if (p.N <= 0 || p.Cout <= 0) return O3DML_OK;
+    p.vec_a = 1;
+    for (int s = 0; s < p.nsrc; ++s)
+        if ((p.src[s].channels & 3) || (p.src[s].ld & 3) || (reinterpret_cast<uintptr_t>(p.src[s].data) & 15)) p.vec_a = 0;
     // widest column tile that the output fills; narrow outputs get the tall tile
     if (p.Cout <= 32) {
         dim3 grid((unsigned)ceil_div<int64_t>(p.N, 256), (unsigned)ceil_div(p.Cout, 32));
@@ -313,86 +282,32 @@ static int gemm_launch(const GemmParams& p, cudaStream_t st) {
 
 using namespace o3dml;
 
-static int fill_common(GemmParams& p, const float* weight_t, const float* scale, const float* shift,
-                       const float* residual, int residual_ld, int act, float slope, float* out,
-                       int out_ld, int out_channels) {
-    p.Wt = weight_t;
-    p.scale = scale;
-    p.shift = shift;
-    p.residual = residual;
-    p.res_ld = residual_ld;
-    p.act = act;
-    p.slope = slope;
-    p.out = out;
-    p.out_ld = out_ld;
-    p.Cout = out_channels;
-    O3DML_CHECK(act >= 0 && act <= 2, "linear: unknown activation %d", act);
-    O3DML_CHECK(weight_t && out, "linear: null weight/out");
-    O3DML_CHECK((reinterpret_cast<uintptr_t>(weight_t) & 15) == 0, "linear: weight must be 16-byte aligned");
-    return O3DML_OK;
-}
-
 extern "C" int o3dml_linear(int64_t num_rows, const o3dml_src_t* srcs, int num_srcs,
                             const float* weight_t, const float* scale, const float* shift,
                             const float* residual, int residual_ld, int act, float slope,
                             float* out, int out_ld, int out_channels, int out_nchw_plane,
                             void* stream) {
-    O3DML_CHECK(num_srcs >= 1 && num_srcs <= MAX_SRC, "linear: 1..3 sources");
     GemmParams p = {};
     p.N = num_rows;
     p.mode = 0;
     p.nsrc = num_srcs;
-    int k = 0, vec = 1;
-    for (int s = 0; s < num_srcs; ++s) {
-        const o3dml_src_t& S = srcs[s];
-        O3DML_CHECK(S.data && S.channels > 0 && S.ld >= S.channels, "linear: bad source %d", s);
-        p.src[s].data = S.data;
-        p.src[s].index = S.index;
-        p.src[s].rows = S.rows;
-        p.src[s].out_rows_per_batch = S.out_rows_per_batch;
-        p.src[s].src_rows_per_batch = S.src_rows_per_batch;
-        p.src[s].channels = S.channels;
-        p.src[s].ld = S.ld;
-        p.src[s].index_is64 = S.index_is64;
-        p.src[s].index_ld = S.index ? (S.index_ld > 0 ? S.index_ld : 1) : 0;
-        p.koff[s] = k;
-        k += S.channels;
-        if ((S.channels & 3) || (S.ld & 3) || (reinterpret_cast<uintptr_t>(S.data) & 15)) vec = 0;
-    }
-    for (int s = num_srcs; s <= MAX_SRC; ++s) p.koff[s] = k;
-    p.K = k;
-    p.vec_a = vec;
-    int rc = fill_common(p, weight_t, scale, shift, residual, residual_ld, act, slope, out, out_ld,
-                         out_channels);
+    p.Wt = weight_t;
+    int rc = set_srcs("linear", srcs, num_srcs, p.src, p.koff);
+    if (!rc) rc = set_epilogue("linear", p, weight_t, scale, shift, residual, residual_ld, act, slope, out, out_ld,
+                               out_channels, out_nchw_plane);
     if (rc) return rc;
-    if (out_nchw_plane > 0) {
-        p.out_mode = 1;
-        p.plane = out_nchw_plane;
-    }
+    p.K = p.koff[MAX_SRC];
     return gemm_launch(p, (cudaStream_t)stream);
 }
 
 extern "C" int o3dml_conv3x3_nhwc(const float* in, int batch, int H, int W, int C, int stride,
                                   const float* weight_t, const float* scale, const float* shift,
                                   int act, float slope, float* out, int out_channels, void* stream) {
-    O3DML_CHECK(in && batch > 0 && H > 0 && W > 0, "conv3x3: bad input");
-    O3DML_CHECK((C % 16) == 0, "conv3x3: input channels must be a multiple of 16");
-    O3DML_CHECK(stride == 1 || stride == 2, "conv3x3: stride 1 or 2");
-    O3DML_CHECK((reinterpret_cast<uintptr_t>(in) & 15) == 0, "conv3x3: input must be 16-byte aligned");
     GemmParams p = {};
-    p.mode = 1;
-    p.nsrc = 1;
-    p.src[0].data = in;
-    p.H = H;
-    p.W = W;
-    p.C = C;
-    p.stride = stride;
-    p.OH = (H + 2 - 3) / stride + 1;
-    p.OW = (W + 2 - 3) / stride + 1;
-    p.N = (int64_t)batch * p.OH * p.OW;
-    p.K = 9 * C;
-    int rc = fill_common(p, weight_t, scale, shift, nullptr, 0, act, slope, out, out_channels,
-                         out_channels);
+    p.Wt = weight_t;
+    int rc = set_conv3x3("conv3x3", p, in, batch, H, W, C, stride, 16);
+    if (!rc) rc = set_epilogue("conv3x3", p, weight_t, scale, shift, nullptr, 0, act, slope, out, out_channels,
+                               out_channels, 0);
     if (rc) return rc;
     return gemm_launch(p, (cudaStream_t)stream);
 }
@@ -401,37 +316,10 @@ extern "C" int o3dml_deconv_nhwc(const float* in, int batch, int H, int W, int C
                                  const float* weight_t, const float* scale, const float* shift,
                                  int act, float slope, float* out, int out_ld, int out_channels,
                                  void* stream) {
-    O3DML_CHECK(in && batch > 0 && H > 0 && W > 0 && stride >= 1, "deconv: bad input");
-    o3dml_src_t s = {};
-    s.data = in;
-    s.rows = (int64_t)batch * H * W;
-    s.channels = C;
-    s.ld = C;
     GemmParams p = {};
-    p.N = s.rows;
-    p.mode = 0;
-    p.nsrc = 1;
-    p.src[0].data = in;
-    p.src[0].rows = s.rows;
-    p.src[0].channels = C;
-    p.src[0].ld = C;
-    p.koff[0] = 0;
-    for (int i = 1; i <= MAX_SRC; ++i) p.koff[i] = C;
-    p.K = C;
-    p.vec_a = ((C & 3) == 0) && ((reinterpret_cast<uintptr_t>(in) & 15) == 0);
-    int rc = fill_common(p, weight_t, nullptr, nullptr, nullptr, 0, act, slope, out, out_ld,
-                         stride * stride * out_channels);
+    p.Wt = weight_t;
+    int rc = set_deconv("deconv", p, weight_t, in, batch, H, W, C, stride, scale, shift, act, slope, out, out_ld,
+                        out_channels);
     if (rc) return rc;
-    (void)scale;
-    (void)shift;
-    p.out_mode = 2;
-    p.ds = stride;
-    p.dIH = H;
-    p.dIW = W;
-    p.dC = out_channels;
-    // per-channel affine repeats over the stride*stride sub-pixels: the caller passes
-    // scale/shift already tiled to [stride*stride*out_channels]
-    p.scale = scale;
-    p.shift = shift;
     return gemm_launch(p, (cudaStream_t)stream);
 }

@@ -26,7 +26,7 @@
 // Every GT_FLUSH slices the wgmma accumulator is folded into a second fp32 register set with
 // round-to-nearest adds, so that long products do not rely on the tensor core's internal accumulation.
 #include "../../include/o3dml_b200.h"
-#include "common.cuh"
+#include "dense.cuh"
 #include "tc.cuh"
 #include <cuda.h>
 #include <algorithm>
@@ -41,13 +41,6 @@ constexpr int GT_CONV_THREADS = 256;   // warps 0-7: the two consumer warpgroups
 constexpr int GT_LOADERS = 128;        // warps 8-11 (GATHER kernels only)
 constexpr int GT_A_BYTES = GT_ROWS * 128;
 
-struct GtSrc {
-    const float* data;
-    const void* index;
-    int64_t rows, out_rows_per_batch, src_rows_per_batch;
-    int32_t channels, ld, index_is64, index_ld;
-};
-
 struct alignas(64) GemmTcParams {
     CUtensorMap mapA[4];   // rows mode: one per identity source; conv: stride 1 -> [0], stride 2 -> parity (py*2+px)
     CUtensorMap mapB;      // {Kpad, 2*Npad}: hi rows [0, Npad), lo rows [Npad, 2*Npad)
@@ -55,37 +48,12 @@ struct alignas(64) GemmTcParams {
     int K, Kpad, Cout, Npad;
     int mode;  // 0 rows, 1 conv3x3
     int nsrc;
-    GtSrc src[GT_MAX_SRC];
+    o3dml_src_t src[GT_MAX_SRC];
     int koff[GT_MAX_SRC + 1];
     int H, W, OH, OW, stride, C;
     int lpw, PH, tiles_x, tiles_y;   // conv: patch = (1 << lpw) x PH output pixels per CTA
-    const float* scale;
-    const float* shift;
-    const float* residual;
-    int res_ld;
-    int act;
-    float slope;
-    float* out;
-    int out_ld;
-    int out_mode;   // 0 rows, 1 NCHW, 2 deconv pixel shuffle
-    int64_t plane;
-    int ds, dIH, dIW, dC;
+    DenseEpilogue ep;
 };
-
-__device__ __forceinline__ const float* gt_src_ptr(const GemmTcParams& p, int s, int64_t n) {
-    const GtSrc& S = p.src[s];
-    int64_t r = n;
-    if (S.index) {
-        r = load_index(S.index, n * S.index_ld, S.index_is64);
-        if (r < 0) return nullptr;
-        if (S.out_rows_per_batch > 0) {
-            if (r >= S.src_rows_per_batch) return nullptr;
-            r += (n / S.out_rows_per_batch) * S.src_rows_per_batch;
-        }
-        if (r >= S.rows) return nullptr;
-    }
-    return S.data + (size_t)r * S.ld;
-}
 
 // ---- async-copy primitives ---------------------------------------------------------------------
 __device__ __forceinline__ void cp_async16(uint32_t smem_dst, const void* gsrc, int src_bytes) {
@@ -169,6 +137,7 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
     uint64_t* full_bar = mbar;                // [S] operands of the slice landed
     uint64_t* empty_bar = mbar + S;           // [S] the consumers are done with the stage
 
+    const DenseEpilogue& ep = p.ep;
     const int tid = threadIdx.x;
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // warp-uniform for the compiler
     const int col0 = blockIdx.y * BN;
@@ -197,14 +166,14 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
     }
     for (int i = tid; i < BN; i += blockDim.x) {      // per-column epilogue constants: read once, not per element
         const int c = col0 + i;
-        s_scale[i] = (p.scale && c < p.Cout) ? p.scale[c] : 1.f;
-        s_shift[i] = (p.shift && c < p.Cout) ? p.shift[c] : 0.f;
+        s_scale[i] = (ep.scale && c < p.Cout) ? ep.scale[c] : 1.f;
+        s_shift[i] = (ep.shift && c < p.Cout) ? ep.shift[c] : 0.f;
     }
     if (GATHER) {
         for (int i = tid; i < p.nsrc * GT_ROWS; i += blockDim.x) {
             const int s = i / GT_ROWS, m = i % GT_ROWS;
             const int64_t n = row0 + m;
-            rowptr[s * GT_ROWS + m] = (n < p.N && p.src[s].index) ? gt_src_ptr(p, s, n) : nullptr;
+            rowptr[s * GT_ROWS + m] = (n < p.N && p.src[s].index) ? src_row(p.src[s], n) : nullptr;
         }
     }
     if (tid == 0) {
@@ -331,19 +300,19 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
                 make_float2(fmaf(racc[i], s_scale[c], s_shift[c]), fmaf(racc[i + 1], s_scale[c + 1], s_shift[c + 1]));
         }
         named_bar_sync(2, GT_CONV_THREADS);
-        const bool staged = p.out_mode == 0 || (p.out_mode == 2 && (p.dC & 3) == 0);
+        const bool staged = ep.mode == 0 || (ep.mode == 2 && (ep.dC & 3) == 0);
         if (staged) {
             constexpr int LPR = BN / 4;                                // lanes per output row
             const int c = (tid % LPR) * 4, cg = col0 + c;
-            const bool vec = (p.out_ld & 3) == 0 && (reinterpret_cast<uintptr_t>(p.out) & 15) == 0;
+            const bool vec = (ep.out_ld & 3) == 0 && (reinterpret_cast<uintptr_t>(ep.out) & 15) == 0;
             if (cg < p.Cout) {
                 for (int r = tid / LPR; r < GT_ROWS; r += GT_CONV_THREADS / LPR) {
                     const int64_t nr = rown[r];
                     if (nr < 0) continue;
                     float4 v = *reinterpret_cast<const float4*>(stg + r * SLD + c);
-                    if (p.residual) {
-                        const float* rp = p.residual + (size_t)nr * p.res_ld + cg;
-                        if (cg + 3 < p.Cout && (p.res_ld & 3) == 0 && (reinterpret_cast<uintptr_t>(p.residual) & 15) == 0) {
+                    if (ep.residual) {
+                        const float* rp = ep.residual + (size_t)nr * ep.res_ld + cg;
+                        if (cg + 3 < p.Cout && (ep.res_ld & 3) == 0 && (reinterpret_cast<uintptr_t>(ep.residual) & 15) == 0) {
                             const float4 rv = *reinterpret_cast<const float4*>(rp);
                             v.x += rv.x; v.y += rv.y; v.z += rv.z; v.w += rv.w;
                         } else {
@@ -353,21 +322,21 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
                             if (cg + 3 < p.Cout) v.w += rp[3];
                         }
                     }
-                    v.x = apply_act(v.x, p.act, p.slope); v.y = apply_act(v.y, p.act, p.slope);
-                    v.z = apply_act(v.z, p.act, p.slope); v.w = apply_act(v.w, p.act, p.slope);
+                    v.x = apply_act(v.x, ep.act, ep.slope); v.y = apply_act(v.y, ep.act, ep.slope);
+                    v.z = apply_act(v.z, ep.act, ep.slope); v.w = apply_act(v.w, ep.act, ep.slope);
                     float* o;
-                    if (p.out_mode == 0) {
-                        o = p.out + (size_t)nr * p.out_ld + cg;
+                    if (ep.mode == 0) {
+                        o = ep.out + (size_t)nr * ep.out_ld + cg;
                     } else {
-                        const int64_t per = (int64_t)p.dIH * p.dIW;
+                        const int64_t per = (int64_t)ep.dIH * ep.dIW;
                         const int64_t b = nr / per;
                         const int rr = (int)(nr % per);
-                        const int iy = rr / p.dIW, ix = rr % p.dIW;
-                        const int sub = cg / p.dC, co = cg - sub * p.dC;
-                        const int dy = sub / p.ds, dx = sub - dy * p.ds;
-                        const size_t opix = ((size_t)b * p.dIH * p.ds + (size_t)iy * p.ds + dy) * (p.dIW * p.ds) +
-                                            (size_t)ix * p.ds + dx;
-                        o = p.out + opix * p.out_ld + co;
+                        const int iy = rr / ep.dIW, ix = rr % ep.dIW;
+                        const int sub = cg / ep.dC, co = cg - sub * ep.dC;
+                        const int dy = sub / ep.ds, dx = sub - dy * ep.ds;
+                        const size_t opix = ((size_t)b * ep.dIH * ep.ds + (size_t)iy * ep.ds + dy) * (ep.dIW * ep.ds) +
+                                            (size_t)ix * ep.ds + dx;
+                        o = ep.out + opix * ep.out_ld + co;
                     }
                     if (vec && cg + 3 < p.Cout) {
                         *reinterpret_cast<float4*>(o) = v;
@@ -387,21 +356,21 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
                 const int64_t n = rown[r];
                 if (n < 0 || c >= p.Cout) continue;
                 float x = stg[r * SLD + cl];
-                if (p.residual) x += p.residual[(size_t)n * p.res_ld + c];
-                x = apply_act(x, p.act, p.slope);
-                if (p.out_mode == 1) {
-                    const int64_t b = n / p.plane, pix = n % p.plane;
-                    p.out[((size_t)b * p.Cout + c) * p.plane + pix] = x;
+                if (ep.residual) x += ep.residual[(size_t)n * ep.res_ld + c];
+                x = apply_act(x, ep.act, ep.slope);
+                if (ep.mode == 1) {
+                    const int64_t b = n / ep.plane, pix = n % ep.plane;
+                    ep.out[((size_t)b * p.Cout + c) * ep.plane + pix] = x;
                 } else {
-                    const int64_t per = (int64_t)p.dIH * p.dIW;
+                    const int64_t per = (int64_t)ep.dIH * ep.dIW;
                     const int64_t b = n / per;
                     const int rr = (int)(n % per);
-                    const int iy = rr / p.dIW, ix = rr % p.dIW;
-                    const int sub = c / p.dC, co = c - sub * p.dC;
-                    const int dy = sub / p.ds, dx = sub - dy * p.ds;
-                    const size_t opix = ((size_t)b * p.dIH * p.ds + (size_t)iy * p.ds + dy) * (p.dIW * p.ds) +
-                                        (size_t)ix * p.ds + dx;
-                    p.out[opix * p.out_ld + co] = x;
+                    const int iy = rr / ep.dIW, ix = rr % ep.dIW;
+                    const int sub = c / ep.dC, co = c - sub * ep.dC;
+                    const int dy = sub / ep.ds, dx = sub - dy * ep.ds;
+                    const size_t opix = ((size_t)b * ep.dIH * ep.ds + (size_t)iy * ep.ds + dy) * (ep.dIW * ep.ds) +
+                                        (size_t)ix * ep.ds + dx;
+                    ep.out[opix * ep.out_ld + co] = x;
                 }
             }
         }
@@ -441,19 +410,6 @@ static int make_map(CUtensorMap* map, const void* base, int rank, const uint64_t
     return O3DML_OK;
 }
 
-static int g_num_sms = 0;
-int gt_num_sms() {
-    if (!g_num_sms) {
-        int dev = 0, n = 0;
-        if (cudaGetDevice(&dev) == cudaSuccess &&
-            cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0)
-            g_num_sms = n;
-        else
-            g_num_sms = kNumSMs;
-    }
-    return g_num_sms;
-}
-
 template <int BN, bool GATHER, bool LITE = false>
 static int gemm_tc_launch_bn(const GemmTcParams& p, unsigned grid_x, cudaStream_t st) {
     using C = GtCfg<BN, LITE>;
@@ -473,7 +429,10 @@ static int gemm_tc_launch_bn(const GemmTcParams& p, unsigned grid_x, cudaStream_
 
 constexpr int GT_LITE_MAX_SLICES = 16;   // longest product, in 32-channel k-slices, that runs on the LITE kernels
 
-static int gemm_tc_launch(GemmTcParams& p, const void* wimg, cudaStream_t st) {
+static int gemm_tc_launch(GemmTcParams& p, const void* wimg, int k_pad, int n_pad, cudaStream_t st) {
+    p.Kpad = k_pad;
+    p.Npad = n_pad;
+    O3DML_CHECK(n_pad >= p.Cout, "linear_tc: weight image has fewer rows than out_channels");
     if (p.N <= 0 || p.Cout <= 0) return O3DML_OK;
     O3DML_CHECK(p.Kpad % GT_KS == 0 && p.Kpad >= p.K, "linear_tc: weight image K padding must be a multiple of 32");
     O3DML_CHECK(p.Npad == 32 || p.Npad == 64 || p.Npad % 128 == 0,
@@ -482,6 +441,7 @@ static int gemm_tc_launch(GemmTcParams& p, const void* wimg, cudaStream_t st) {
     bool any_gather = false;
     if (p.mode == 0)
         for (int s = 0; s < p.nsrc; ++s) any_gather = any_gather || p.src[s].index != nullptr;
+    const int sms = device_sm_count();
     int64_t row_tiles = ceil_div<int64_t>(p.N, GT_ROWS);
     if (p.mode == 1) {
         int best_tiles = 1 << 30;
@@ -491,11 +451,11 @@ static int gemm_tc_launch(GemmTcParams& p, const void* wimg, cudaStream_t st) {
     // products of plain row sources, at most 16 k-slices long, that fill the SMs more than once as 64-column tiles run on
     // the LITE kernels, two CTAs per SM (GtCfg); the convolutions (K = 9 C) stay on the one-CTA-per-SM kernels
     const bool lite = p.mode == 0 && !any_gather && p.Kpad / GT_KS <= GT_LITE_MAX_SLICES &&
-                      row_tiles * (p.Npad / (bn == 32 ? 32 : 64)) > gt_num_sms();
+                      row_tiles * (p.Npad / (bn == 32 ? 32 : 64)) > sms;
     if (lite && bn == 128) bn = 64;
     // a grid that fills less than half of the SMs (PointPillars block 3: 27 x 2 CTAs; one cloud per GPU: 6 - 88)
     // runs as 64-column tiles instead: twice the CTAs, each with half the tensor-core work per slice
-    if (bn == 128 && 2 * row_tiles * (p.Npad / 128) <= gt_num_sms()) bn = 64;
+    if (bn == 128 && 2 * row_tiles * (p.Npad / 128) <= sms) bn = 64;
     {   // weight image: fp32 [2 * Npad][Kpad] (TF32 hi rows, then lo rows)
         const uint64_t dims[2] = {(uint64_t)p.Kpad, (uint64_t)2 * p.Npad};
         const uint64_t str[1] = {(uint64_t)p.Kpad * 4};
@@ -574,20 +534,6 @@ static int gemm_tc_launch(GemmTcParams& p, const void* wimg, cudaStream_t st) {
 
 using namespace o3dml;
 
-static int gt_common(GemmTcParams& p, const void* wimg, int k_pad, int n_pad, const float* scale,
-                     const float* shift, const float* residual, int residual_ld, int act, float slope,
-                     float* out, int out_ld, int out_channels) {
-    p.Kpad = k_pad;
-    p.Npad = n_pad;
-    p.scale = scale; p.shift = shift; p.residual = residual; p.res_ld = residual_ld;
-    p.act = act; p.slope = slope; p.out = out; p.out_ld = out_ld; p.Cout = out_channels;
-    O3DML_CHECK(act >= 0 && act <= 2, "linear_tc: unknown activation %d", act);
-    O3DML_CHECK(wimg && out, "linear_tc: null weight image / out");
-    O3DML_CHECK((reinterpret_cast<uintptr_t>(wimg) & 15) == 0, "linear_tc: weight image must be 16-byte aligned");
-    O3DML_CHECK(n_pad >= out_channels, "linear_tc: weight image has fewer rows than out_channels");
-    return O3DML_OK;
-}
-
 extern "C" int o3dml_linear_tc_supported(const o3dml_src_t* srcs, int num_srcs) {
     if (num_srcs < 1 || num_srcs > GT_MAX_SRC) return 0;
     for (int s = 0; s < num_srcs; ++s) {
@@ -604,78 +550,41 @@ extern "C" int o3dml_linear_tc(int64_t num_rows, const o3dml_src_t* srcs, int nu
                                const float* shift, const float* residual, int residual_ld, int act,
                                float slope, float* out, int out_ld, int out_channels,
                                int out_nchw_plane, void* stream) {
-    O3DML_CHECK(num_srcs >= 1 && num_srcs <= GT_MAX_SRC, "linear_tc: 1..3 sources");
-    O3DML_CHECK(o3dml_linear_tc_supported(srcs, num_srcs),
-                "linear_tc: sources need a multiple of 4 channels (32 for all but the last), 16-byte aligned rows");
     GemmTcParams p = {};
     p.N = num_rows;
     p.mode = 0;
     p.nsrc = num_srcs;
-    int k = 0;
-    for (int s = 0; s < num_srcs; ++s) {
-        const o3dml_src_t& S = srcs[s];
-        O3DML_CHECK(S.ld >= S.channels, "linear_tc: bad source %d", s);
-        p.src[s].data = S.data; p.src[s].index = S.index; p.src[s].rows = S.rows;
-        p.src[s].out_rows_per_batch = S.out_rows_per_batch;
-        p.src[s].src_rows_per_batch = S.src_rows_per_batch;
-        p.src[s].channels = S.channels; p.src[s].ld = S.ld; p.src[s].index_is64 = S.index_is64;
-        p.src[s].index_ld = S.index ? (S.index_ld > 0 ? S.index_ld : 1) : 0;
-        p.koff[s] = k;
-        k += S.channels;
-    }
-    for (int s = num_srcs; s <= GT_MAX_SRC; ++s) p.koff[s] = k;
-    p.K = k;
-    int rc = gt_common(p, weight_image, k_pad, n_pad, scale, shift, residual, residual_ld, act, slope, out,
-                       out_ld, out_channels);
+    int rc = set_srcs("linear_tc", srcs, num_srcs, p.src, p.koff);
     if (rc) return rc;
-    if (out_nchw_plane > 0) {
-        p.out_mode = 1;
-        p.plane = out_nchw_plane;
-    }
-    return gemm_tc_launch(p, weight_image, (cudaStream_t)stream);
+    O3DML_CHECK(o3dml_linear_tc_supported(srcs, num_srcs),
+                "linear_tc: sources need a multiple of 4 channels (32 for all but the last), 16-byte aligned rows");
+    rc = set_epilogue("linear_tc", p, weight_image, scale, shift, residual, residual_ld, act, slope, out, out_ld,
+                      out_channels, out_nchw_plane);
+    if (rc) return rc;
+    p.K = p.koff[GT_MAX_SRC];
+    return gemm_tc_launch(p, weight_image, k_pad, n_pad, (cudaStream_t)stream);
 }
 
 extern "C" int o3dml_conv3x3_nhwc_tc(const float* in, int batch, int H, int W, int C, int stride,
                                      const void* weight_image, int k_pad, int n_pad, const float* scale,
                                      const float* shift, int act, float slope, float* out,
                                      int out_channels, void* stream) {
-    O3DML_CHECK(in && batch > 0 && H > 0 && W > 0, "conv3x3_tc: bad input");
-    O3DML_CHECK((C % GT_KS) == 0, "conv3x3_tc: input channels must be a multiple of 32");
-    O3DML_CHECK(stride == 1 || stride == 2, "conv3x3_tc: stride 1 or 2");
-    O3DML_CHECK((reinterpret_cast<uintptr_t>(in) & 15) == 0, "conv3x3_tc: input must be 16-byte aligned");
     GemmTcParams p = {};
-    p.mode = 1;
-    p.nsrc = 1;
-    p.src[0].data = in;
-    p.H = H; p.W = W; p.C = C; p.stride = stride;
-    p.OH = (H + 2 - 3) / stride + 1;
-    p.OW = (W + 2 - 3) / stride + 1;
-    p.N = (int64_t)batch * p.OH * p.OW;
-    p.K = 9 * C;
-    int rc = gt_common(p, weight_image, k_pad, n_pad, scale, shift, nullptr, 0, act, slope, out,
-                       out_channels, out_channels);
+    int rc = set_conv3x3("conv3x3_tc", p, in, batch, H, W, C, stride, GT_KS);
+    if (!rc) rc = set_epilogue("conv3x3_tc", p, weight_image, scale, shift, nullptr, 0, act, slope, out, out_channels,
+                               out_channels, 0);
     if (rc) return rc;
-    return gemm_tc_launch(p, weight_image, (cudaStream_t)stream);
+    return gemm_tc_launch(p, weight_image, k_pad, n_pad, (cudaStream_t)stream);
 }
 
 extern "C" int o3dml_deconv_nhwc_tc(const float* in, int batch, int H, int W, int C, int stride,
                                     const void* weight_image, int k_pad, int n_pad, const float* scale,
                                     const float* shift, int act, float slope, float* out, int out_ld,
                                     int out_channels, void* stream) {
-    O3DML_CHECK(in && batch > 0 && H > 0 && W > 0 && stride >= 1, "deconv_tc: bad input");
-    O3DML_CHECK((C % 4) == 0 && (reinterpret_cast<uintptr_t>(in) & 15) == 0, "deconv_tc: C % 4, aligned input");
     GemmTcParams p = {};
-    p.N = (int64_t)batch * H * W;
-    p.mode = 0;
-    p.nsrc = 1;
-    p.src[0].data = in; p.src[0].rows = p.N; p.src[0].channels = C; p.src[0].ld = C;
-    p.koff[0] = 0;
-    for (int i = 1; i <= GT_MAX_SRC; ++i) p.koff[i] = C;
-    p.K = C;
-    int rc = gt_common(p, weight_image, k_pad, n_pad, scale, shift, nullptr, 0, act, slope, out, out_ld,
-                       stride * stride * out_channels);
+    int rc = set_deconv("deconv_tc", p, weight_image, in, batch, H, W, C, stride, scale, shift, act, slope, out, out_ld,
+                        out_channels);
     if (rc) return rc;
-    p.out_mode = 2;
-    p.ds = stride; p.dIH = H; p.dIW = W; p.dC = out_channels;
-    return gemm_tc_launch(p, weight_image, (cudaStream_t)stream);
+    O3DML_CHECK((C % 4) == 0 && (reinterpret_cast<uintptr_t>(in) & 15) == 0, "deconv_tc: C % 4, aligned input");
+    return gemm_tc_launch(p, weight_image, k_pad, n_pad, (cudaStream_t)stream);
 }

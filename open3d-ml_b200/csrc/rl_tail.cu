@@ -16,7 +16,7 @@
 // Weights: host-packed image (open3d_ml_b200._lib.pack_tail_image): per layer, per 32-wide k-chunk, hi then lo tiles of
 // [N rows][32 floats] in the K-major SWIZZLE_128B layout, copied once per CTA with one cp.async.bulk.
 #include "../../include/o3dml_b200.h"
-#include "common.cuh"
+#include "dense.cuh"
 #include "tc.cuh"
 #include <string.h>
 #include <algorithm>
@@ -31,10 +31,9 @@ constexpr size_t RT_SMEM = RT_WBYTES + RT_THREADS * RT_LD * 4 + 64 + 1024;
 
 struct RlTailParams {
     const float* skip;
-    const float* coarse;
-    const void* idx;
-    int skip_ld, coarse_ld, idx_is64, classes;
-    int64_t N, out_rows_per_batch, src_rows_per_batch, coarse_rows;
+    o3dml_src_t coarse;   // gathered through the interpolation index
+    int skip_ld, classes;
+    int64_t N;
     const float* wimg;
     float* out;
     float slope;
@@ -120,11 +119,7 @@ __global__ void __launch_bounds__(RT_THREADS, 2) rl_tail_kernel(const __grid_con
         const float* s1 = nullptr;
         if (n < p.N) {
             s0 = p.skip + (size_t)n * p.skip_ld;
-            int64_t r = load_index(p.idx, n, p.idx_is64);
-            if (r >= 0) {
-                if (p.out_rows_per_batch > 0) r = r < p.src_rows_per_batch ? r + (n / p.out_rows_per_batch) * p.src_rows_per_batch : -1;
-                if (r >= 0 && r < p.coarse_rows) s1 = p.coarse + (size_t)r * p.coarse_ld;
-            }
+            s1 = src_row(p.coarse, n);
         }
         float4* arow = reinterpret_cast<float4*>(act + tid * RT_LD);
 #pragma unroll
@@ -189,23 +184,20 @@ extern "C" int o3dml_randla_tail(const float* skip, int skip_ld, const float* co
                 "randla_tail: 16-byte aligned rows and weight image");
     if (num_rows <= 0) return O3DML_OK;
     RlTailParams p;
-    p.skip = skip; p.coarse = coarse; p.idx = interp_index;
-    p.skip_ld = skip_ld; p.coarse_ld = coarse_ld; p.idx_is64 = index_is64; p.classes = classes;
-    p.N = num_rows; p.out_rows_per_batch = out_rows_per_batch; p.src_rows_per_batch = src_rows_per_batch;
-    p.coarse_rows = coarse_rows;
+    p.skip = skip; p.skip_ld = skip_ld; p.classes = classes; p.N = num_rows;
+    p.coarse = {coarse, interp_index, coarse_rows, out_rows_per_batch, src_rows_per_batch, RT_K1 / 2, coarse_ld,
+                index_is64, 1};
     p.wimg = (const float*)weight_image; p.out = out; p.slope = slope;
     memcpy(p.scale, h_scale, sizeof(p.scale));
     memcpy(p.shift, h_shift, sizeof(p.shift));
-    static unsigned long long configured = 0;
-    int dev = 0, sms = kNumSMs;
-    O3DML_CUDA(cudaGetDevice(&dev));
-    if (dev >= 64 || !((configured >> dev) & 1ull)) {
+    static PerDeviceOnce once;
+    const int dev = current_device();
+    if (once.need(dev)) {
         O3DML_CUDA(cudaFuncSetAttribute(rl_tail_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RT_SMEM));
-        if (dev < 64) configured |= 1ull << dev;
+        once.done(dev);
     }
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int64_t tiles = ceil_div<int64_t>(num_rows, RT_THREADS);
-    const unsigned grid = (unsigned)std::min<int64_t>(tiles, (int64_t)sms * 2);
+    const unsigned grid = (unsigned)std::min<int64_t>(tiles, (int64_t)device_sm_count() * 2);
     rl_tail_kernel<<<grid, RT_THREADS, RT_SMEM, (cudaStream_t)stream>>>(p);
     O3DML_LAUNCH_CHECK();
     o3dml_count_launches(1);

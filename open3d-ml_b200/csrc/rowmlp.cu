@@ -11,23 +11,16 @@
 // memory, no barrier and no weight traffic at all.  Sources may be a concat of two tensors, the
 // second optionally gathered through an index (decoder: nearest_interpolation).
 #include "../../include/o3dml_b200.h"
-#include "common.cuh"
+#include "dense.cuh"
 #include <string.h>
 
 namespace o3dml {
-
-struct RowSrc {
-    const float* data;
-    const void* index;   // null = identity
-    int64_t rows, out_rows_per_batch, src_rows_per_batch;
-    int32_t ld, index_is64, index_ld, pad;
-};
 
 template <int C0, int C1, int COUT>
 struct alignas(16) RowMlpParams {
     static constexpr int K = C0 + C1;
     static constexpr int CP = (COUT + 3) & ~3;    // padded weight row: 16-byte constant loads
-    RowSrc src[2];
+    o3dml_src_t src[2];
     int64_t N;
     float* out;
     int32_t out_ld, act;
@@ -35,20 +28,6 @@ struct alignas(16) RowMlpParams {
     int32_t pad;
     float w[K * CP + 2 * CP];                     // [K][CP] weight, then scale[CP], shift[CP]
 };
-
-__device__ __forceinline__ const float* row_ptr(const RowSrc& S, int64_t n) {
-    int64_t r = n;
-    if (S.index) {
-        r = load_index(S.index, n * S.index_ld, S.index_is64);
-        if (r < 0) return nullptr;
-        if (S.out_rows_per_batch > 0) {
-            if (r >= S.src_rows_per_batch) return nullptr;
-            r += (n / S.out_rows_per_batch) * S.src_rows_per_batch;
-        }
-        if (r >= S.rows) return nullptr;
-    }
-    return S.data + (size_t)r * S.ld;
-}
 
 template <int C>
 __device__ __forceinline__ void load_row(const float* p, float* x) {
@@ -75,8 +54,8 @@ rowmlp_kernel(const __grid_constant__ RowMlpParams<C0, C1, COUT> p) {
     const int64_t n = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (n >= p.N) return;
     float x[K];
-    load_row<C0>(row_ptr(p.src[0], n), x);
-    if (C1 > 0) load_row<C1>(row_ptr(p.src[1], n), x + C0);
+    load_row<C0>(src_row(p.src[0], n), x);
+    if (C1 > 0) load_row<C1>(src_row(p.src[1], n), x + C0);
     float acc[CP];
 #pragma unroll
     for (int c = 0; c < CP; ++c) acc[c] = 0.f;
@@ -101,7 +80,7 @@ rowmlp_kernel(const __grid_constant__ RowMlpParams<C0, C1, COUT> p) {
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 template <int C0, int C1, int COUT>
-static int rowmlp_launch(int64_t num_rows, const o3dml_src_t* srcs, const float* hw, const float* hs,
+static int rowmlp_launch(int64_t num_rows, const o3dml_src_t (&srcs)[2], const float* hw, const float* hs,
                          const float* ht, int act, float slope, float* out, int out_ld, cudaStream_t st) {
     using P = RowMlpParams<C0, C1, COUT>;
     static_assert(sizeof(P) <= 32000, "kernel parameter block too large");
@@ -114,14 +93,7 @@ static int rowmlp_launch(int64_t num_rows, const o3dml_src_t* srcs, const float*
         if (c % 4 == 0)
             O3DML_CHECK(aligned16(srcs[s].data) && srcs[s].ld % 4 == 0,
                         "linear_rows_small: source %d is not 16-byte aligned", s);
-        p.src[s].data = srcs[s].data;
-        p.src[s].index = srcs[s].index;
-        p.src[s].rows = srcs[s].rows;
-        p.src[s].out_rows_per_batch = srcs[s].out_rows_per_batch;
-        p.src[s].src_rows_per_batch = srcs[s].src_rows_per_batch;
-        p.src[s].ld = srcs[s].ld;
-        p.src[s].index_is64 = srcs[s].index_is64;
-        p.src[s].index_ld = srcs[s].index_ld;
+        p.src[s] = srcs[s];
     }
     if (COUT % 4 == 0)
         O3DML_CHECK(aligned16(out) && out_ld % 4 == 0, "linear_rows_small: output is not 16-byte aligned");
@@ -169,12 +141,16 @@ extern "C" int o3dml_linear_rows_small(int64_t num_rows, const o3dml_src_t* srcs
         else
             cudaGetLastError();
     }
+    o3dml_src_t src[2] = {};
+    int koff[3];
+    int rc = set_srcs("linear_rows_small", srcs, num_srcs, src, koff);
+    if (rc) return rc;
     if (num_rows == 0) return O3DML_OK;
-    const int c0 = srcs[0].channels, c1 = num_srcs == 2 ? srcs[1].channels : 0;
+    const int c0 = src[0].channels, c1 = num_srcs == 2 ? src[1].channels : 0;
     cudaStream_t st = (cudaStream_t)stream;
 #define RM_CASE(A, B, C)                                                                              \
     if (c0 == A && c1 == B && out_channels == C)                                                      \
-        return rowmlp_launch<A, B, C>(num_rows, srcs, h_weight_t, h_scale, h_shift, act, slope, out, \
+        return rowmlp_launch<A, B, C>(num_rows, src, h_weight_t, h_scale, h_shift, act, slope, out, \
                                       out_ld, st);
 #include "rowmlp_shapes.inc"
 #undef RM_CASE

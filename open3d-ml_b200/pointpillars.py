@@ -142,16 +142,7 @@ class PointPillarsB200:
     def _conv(self, x, B, H, W, name, stride, cin, cout):
         OH, OW = (H - 1) // stride + 1, (W - 1) // stride + 1
         out = self._get(name, (B, OH, OW, cout))
-        pw = self.w[name + ".wt"]
-        if cin % 32 == 0:
-            L.check(L.lib().o3dml_conv3x3_nhwc_tc(L.ptr(x), B, H, W, cin, stride, L.ptr(pw.img), pw.k_pad,
-                                                  pw.n_pad, L.ptr(self.w[name + ".s"]),
-                                                  L.ptr(self.w[name + ".t"]), 1, 0.0, L.ptr(out), cout,
-                                                  L.stream()))
-        else:
-            L.check(L.lib().o3dml_conv3x3_nhwc(L.ptr(x), B, H, W, cin, stride, L.ptr(pw.wt),
-                                               L.ptr(self.w[name + ".s"]), L.ptr(self.w[name + ".t"]),
-                                               1, 0.0, L.ptr(out), cout, L.stream()))
+        L.conv3x3(x, self.w[name + ".wt"], out, self.w[name + ".s"], self.w[name + ".t"], stride, act="relu")
         return out, OH, OW
 
     def backbone_neck_head(self, canvas):
@@ -176,17 +167,8 @@ class PointPillarsB200:
         for (p, us, cin, co), (f, h, w_) in zip(self.deblocks, feats):
             if h * us != OH or w_ * us != OW:
                 raise RuntimeError("PointPillarsB200: neck scales do not line up")
-            pw = self.w[p + ".wt"]
-            if cin % 4 == 0:
-                L.check(L.lib().o3dml_deconv_nhwc_tc(L.ptr(f), B, h, w_, cin, us, L.ptr(pw.img), pw.k_pad,
-                                                     pw.n_pad, L.ptr(self.w[p + ".s"]), L.ptr(self.w[p + ".t"]),
-                                                     1, 0.0, neck.data_ptr() + 4 * off, self.neck_channels,
-                                                     co, L.stream()))
-            else:
-                L.check(L.lib().o3dml_deconv_nhwc(L.ptr(f), B, h, w_, cin, us, L.ptr(pw.wt),
-                                                  L.ptr(self.w[p + ".s"]), L.ptr(self.w[p + ".t"]), 1, 0.0,
-                                                  neck.data_ptr() + 4 * off, self.neck_channels, co,
-                                                  L.stream()))
+            L.deconv(f, self.w[p + ".wt"], neck[..., off:off + co], self.w[p + ".s"], self.w[p + ".t"], us,
+                     act="relu")
             off += co
         ch = sum(self.head_split)
         out = torch.empty((B, ch, OH, OW), dtype=torch.float32, device=self.device)

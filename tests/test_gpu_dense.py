@@ -104,13 +104,7 @@ def test_conv3x3_nhwc(B, H, W, C, Co, stride, tc):
     OH, OW = (H - 1) // stride + 1, (W - 1) // stride + 1
     out = torch.empty(B, OH, OW, Co).cuda()
     wt = w.permute(2, 3, 1, 0).reshape(9 * C, Co).contiguous()
-    if tc:
-        pw = L.pack_linear(wt)
-        L.check(L.lib().o3dml_conv3x3_nhwc_tc(L.ptr(x), B, H, W, C, stride, L.ptr(pw.img), pw.k_pad, pw.n_pad,
-                                              L.ptr(s), L.ptr(t), 1, 0.0, L.ptr(out), Co, L.stream()))
-    else:
-        L.check(L.lib().o3dml_conv3x3_nhwc(L.ptr(x), B, H, W, C, stride, L.ptr(wt), L.ptr(s), L.ptr(t), 1, 0.0,
-                                           L.ptr(out), Co, L.stream()))
+    L.conv3x3(x, L.pack_linear(wt) if tc else wt, out, s, t, stride, act="relu")
     ref = F.conv2d(x.permute(0, 3, 1, 2), w, None, stride, 1)
     ref = torch.relu(ref * s.view(1, -1, 1, 1) + t.view(1, -1, 1, 1)).permute(0, 2, 3, 1)
     assert ref.shape == out.shape and rel_err(out, ref) < TOL
@@ -126,14 +120,7 @@ def test_deconv_nhwc_into_concat_buffer(stride, tc):
     neck = torch.zeros(B, H * stride, W * stride, 384).cuda()
     wt = w.permute(0, 2, 3, 1).reshape(C, stride * stride * Co).contiguous()
     s_rep, t_rep = s.repeat(stride * stride), t.repeat(stride * stride)   # keep alive across the call
-    if tc:
-        pw = L.pack_linear(wt)
-        L.check(L.lib().o3dml_deconv_nhwc_tc(L.ptr(x), B, H, W, C, stride, L.ptr(pw.img), pw.k_pad, pw.n_pad,
-                                             L.ptr(s_rep), L.ptr(t_rep), 1, 0.0, neck.data_ptr() + 4 * 128, 384,
-                                             Co, L.stream()))
-    else:
-        L.check(L.lib().o3dml_deconv_nhwc(L.ptr(x), B, H, W, C, stride, L.ptr(wt), L.ptr(s_rep), L.ptr(t_rep), 1,
-                                          0.0, neck.data_ptr() + 4 * 128, 384, Co, L.stream()))
+    L.deconv(x, L.pack_linear(wt) if tc else wt, neck[..., 128:256], s_rep, t_rep, stride, act="relu")
     ref = F.conv_transpose2d(x.permute(0, 3, 1, 2), w, None, stride)
     ref = torch.relu(ref * s.view(1, -1, 1, 1) + t.view(1, -1, 1, 1)).permute(0, 2, 3, 1)
     assert rel_err(neck[..., 128:256], ref) < TOL
@@ -259,3 +246,96 @@ def test_linear_tc_strided_source_view():
     out = torch.empty(5000, 128).cuda()
     L.linear([L.make_src(wide[:, 32:], channels=64, ld=96)], L.pack_linear(w), out, act=None)
     assert rel_err(out, wide[:, 32:].double() @ w.double()) < 3e-6
+
+
+def _gathered(data, n, index=None, index_ld=1, out_rows_per_batch=0, src_rows_per_batch=0):
+    """float64 rows that output rows 0..n-1 read from a source (include/o3dml_b200.h o3dml_src_t; index_ld <= 0 reads
+    as 1): row n itself, or the row its index names, zeros where the id is negative, past src_rows_per_batch
+    (batch-relative) or where the resolved row is not in [0, rows)."""
+    if index is None:
+        return data[:n].double()
+    r = index.reshape(-1)[::max(index_ld, 1)][:n].long()
+    ok = r >= 0
+    if out_rows_per_batch > 0:
+        ok &= r < src_rows_per_batch
+        r = r + (torch.arange(n, device=r.device) // out_rows_per_batch) * src_rows_per_batch
+    ok &= r < data.shape[0]
+    out = torch.zeros(n, data.shape[1], dtype=torch.float64, device=data.device)
+    out[ok] = data[r[ok]].double()
+    return out
+
+
+def _dense_case(name, n):
+    """Two 32-channel sources of the (32 + 32) -> 32 layer: a list of make_src keyword sets (data first)."""
+    g = torch.Generator().manual_seed(11)
+    a, b = rnd(n, 32, seed=12), rnd(n, 32, seed=13)
+    pool = rnd(300, 32, seed=14)
+    if name == "identity":
+        return [dict(data=a), dict(data=b)]
+    if name == "global_int32_column0":               # column 0 of an [n, 3] id matrix
+        nb = torch.randint(0, 300, (n, 3), generator=g).to(torch.int32).cuda()
+        return [dict(data=a), dict(data=pool, index=nb, index_ld=3)]
+    if name == "shadow_ids":                        # ids -1 and == rows read zeros, in both sources
+        i0 = torch.randint(-1, 301, (n,), generator=g).cuda()
+        i1 = torch.randint(-1, 301, (n, 2), generator=g).to(torch.int32).cuda()
+        i0[:2], i1[:2, 0] = torch.tensor([-1, 300]).cuda(), torch.tensor([300, -1], dtype=torch.int32).cuda()
+        return [dict(data=pool, index=i0), dict(data=pool, index=i1, index_ld=2)]
+    if name == "batch_relative_int64":               # ids == src_rows_per_batch and past it read zeros
+        B, nco = 2, 150
+        idx = torch.randint(0, nco + 2, (n,), generator=g).cuda()
+        idx[:2] = torch.tensor([nco, nco + 1]).cuda()
+        return [dict(data=a), dict(data=pool, index=idx, out_rows_per_batch=n // B, src_rows_per_batch=nco)]
+    if name == "index_ld0":                         # index_ld = 0 reads as 1
+        idx = torch.randint(0, 300, (n,), generator=g).to(torch.int32).cuda()
+        return [dict(data=pool, index=idx, index_ld=0), dict(data=b)]
+    raise KeyError(name)
+
+
+ROUTES = {   # _lib.linear's choice for a PackedWeight, forced through its routing constants
+    "simt": ("o3dml_linear", dict(TC_MIN_K=10 ** 9, USE_ROW_MLP=False)),
+    "tc": ("o3dml_linear_tc", dict(TC_MIN_K=8, USE_ROW_MLP=False)),
+    "rows_small": ("o3dml_linear_rows_small", dict(USE_ROW_MLP=True, ROW_MLP_MIN_ROWS=0)),
+}
+
+
+@pytest.mark.parametrize("case", ["identity", "global_int32_column0", "shadow_ids", "batch_relative_int64",
+                                  "index_ld0"])
+@pytest.mark.parametrize("route", list(ROUTES))
+def test_linear_routes_read_sources_alike(route, case, monkeypatch):
+    """The same gathered sources through each of linear's three kernels (gemm.cu, gemm_tc.cu, rowmlp.cu) vs float64."""
+    n = 1000
+    entry, consts = ROUTES[route]
+    for k, v in consts.items():
+        monkeypatch.setattr(L, k, v)
+    h, called = L.lib(), []
+    for name in ("o3dml_linear", "o3dml_linear_tc", "o3dml_linear_rows_small"):
+        fn = getattr(h, name)
+        monkeypatch.setattr(h, name, lambda *a, _fn=fn, _name=name: called.append(_name) or _fn(*a))
+    kws = _dense_case(case, n)
+    srcs = [L.make_src(**kw) for kw in kws]
+    x = torch.cat([_gathered(kw["data"], n, kw.get("index"), kw.get("index_ld", 1), kw.get("out_rows_per_batch", 0),
+                             kw.get("src_rows_per_batch", 0)) for kw in kws], 1)
+    w = rnd(64, 32, seed=15) / 8
+    s, t = rnd(32, seed=16).abs() + 0.5, rnd(32, seed=17)
+    out = torch.full((n, 32), float("nan")).cuda()
+    n0 = L.lib().o3dml_launch_count()
+    L.linear(srcs, L.pack_linear(w), out, s, t, act="leaky", slope=0.2)
+    assert L.lib().o3dml_launch_count() == n0 + 1 and called == [entry]
+    ref = F.leaky_relu((x @ w.double()) * s + t, 0.2)
+    assert rel_err(out, ref) < TOL
+
+
+def test_linear_rows_small_rejects_malformed_sources():
+    """rowmlp.cu takes the source checks of o3dml_linear: ld < channels and null data are errors, not launches."""
+    x = rnd(101, 32, seed=1)
+    out = torch.empty(100, 32).cuda()
+    w = torch.zeros(32, 32)
+    narrow, null = L.make_src(x, channels=32, ld=16, rows=100), L.make_src(x, rows=100)
+    null.data = None
+    for src in (narrow, null):
+        n0 = L.lib().o3dml_launch_count()
+        rc = L.lib().o3dml_linear_rows_small(100, (L.Src * 1)(src), 1, w.data_ptr(), None, None, 0, 0.0, L.ptr(out),
+                                             32, 32, L.stream())
+        assert rc != 0 and L.lib().o3dml_launch_count() == n0
+        with pytest.raises(RuntimeError):
+            L.check(rc)
