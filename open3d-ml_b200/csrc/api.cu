@@ -16,6 +16,6 @@ extern "C" const char* o3dml_last_error(void) { return g_err; }
 extern "C" int o3dml_abi_version(void) { return O3DML_ABI_VERSION; }
 
 static std::atomic<unsigned long long> g_launches{0};
-extern "C" void o3dml_count_launches(int n) { g_launches.fetch_add((unsigned long long)n, std::memory_order_relaxed); }
+void o3dml::count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 extern "C" void o3dml_launch_count_add(unsigned long long n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 extern "C" unsigned long long o3dml_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }

@@ -149,6 +149,8 @@ extern "C" int o3dml_continuous_conv(const float* filters, int size_x, int size_
                 "continuous_conv: null input");
     O3DML_CHECK(size_x >= 1 && size_y >= 1 && size_z >= 1 && in_channels >= 1 && out_channels >= 1 && out_channels <= 1024,
                 "continuous_conv: bad filter shape (out_channels <= 1024)");
+    // one input row is staged in the 48 KB of dynamic shared memory a kernel gets without opting in
+    O3DML_CHECK(in_channels <= 48 * 1024 / (int)sizeof(float), "continuous_conv: in_channels must be <= 12288");
     O3DML_CHECK(coordinate_mapping == 0 || coordinate_mapping == 1,
                 "continuous_conv: coordinate_mapping must be identity (0) or ball_to_cube_radial (1)");
     O3DML_CHECK(interpolation >= 0 && interpolation <= 2, "continuous_conv: interpolation 0 nearest, 1 linear, 2 linear_border");
@@ -163,8 +165,6 @@ extern "C" int o3dml_continuous_conv(const float* filters, int size_x, int size_
     for (int a = 0; a < 3; ++a) p.offset[a] = h_offset ? h_offset[a] : 0.f;
     p.align_corners = align_corners; p.mapping = coordinate_mapping; p.interpolation = interpolation;
     p.normalize = normalize; p.num_out = num_out; p.num_inp = num_inp; p.out = out;
-    cconv_kernel<<<(unsigned)num_out, 128, (size_t)in_channels * sizeof(float), (cudaStream_t)stream>>>(p);
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(1);
+    O3DML_CUDA(launch<cconv_kernel>((unsigned)num_out, 128, (size_t)in_channels * sizeof(float), (cudaStream_t)stream, p));
     return O3DML_OK;
 }

@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <atomic>
+#include <utility>
 
 #define O3DML_OK 0
 #define O3DML_ERR_INVALID 1
@@ -11,7 +13,6 @@
 #define O3DML_ERR_UNSUPPORTED 4
 
 extern "C" void o3dml_set_error(const char* fmt, ...);
-extern "C" void o3dml_count_launches(int n);  // kernels enqueued (bench.py gpu_launches)
 
 #define O3DML_FAIL(code, ...)      \
     do {                           \
@@ -24,31 +25,59 @@ extern "C" void o3dml_count_launches(int n);  // kernels enqueued (bench.py gpu_
         if (!(cond)) O3DML_FAIL(O3DML_ERR_INVALID, __VA_ARGS__); \
     } while (0)
 
-#define O3DML_CUDA(expr)                                                              \
+// variadic so that the commas of a template argument list, launch<k<A, B>>(...), need no extra parentheses
+#define O3DML_CUDA(...)                                                               \
     do {                                                                              \
-        cudaError_t e__ = (expr);                                                     \
+        cudaError_t e__ = (__VA_ARGS__);                                              \
         if (e__ != cudaSuccess)                                                       \
-            O3DML_FAIL(O3DML_ERR_CUDA, "%s failed: %s (%s:%d)", #expr,               \
+            O3DML_FAIL(O3DML_ERR_CUDA, "%s failed: %s (%s:%d)", #__VA_ARGS__,         \
                        cudaGetErrorString(e__), __FILE__, __LINE__);                  \
     } while (0)
-
-#define O3DML_LAUNCH_CHECK() O3DML_CUDA(cudaGetLastError())
 
 namespace o3dml {
 
 constexpr int kNumSMs = 132;  // H100 SXM (fallback when the attribute query fails)
 
-// The opt-in dynamic shared-memory size is a per-device function attribute: `static bool configured` guards set it on
-// the first device only, so a process that drives two GPUs failed on the second.  One bit per device ordinal.
-struct PerDeviceOnce {
-    unsigned long long mask = 0;
-    bool need(int dev) const { return dev < 0 || dev >= 64 || !((mask >> dev) & 1ull); }
-    void done(int dev) { if (dev >= 0 && dev < 64) mask |= 1ull << dev; }
-};
-inline int current_device() {
-    int dev = 0;
-    return cudaGetDevice(&dev) == cudaSuccess ? dev : -1;
+void count_launch();  // adds one to o3dml_launch_count()
+
+// Opts Kernel into `smem` bytes of dynamic shared memory when that is more than the 48 KB default.  The limit is a
+// per-device function attribute, so it is set once per device ordinal (a process may drive several GPUs).
+// Precondition: every launch of one Kernel asks for the same `smem`.
+template <auto Kernel>
+cudaError_t opt_in_smem(size_t smem) {
+    if (smem <= 48 * 1024) return cudaSuccess;
+    static std::atomic<unsigned long long> done{0};  // one bit per device ordinal
+    int dev = -1;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev >= 64) dev = -1;
+    if (dev >= 0 && ((done.load(std::memory_order_relaxed) >> dev) & 1ull)) return cudaSuccess;
+    const cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess && dev >= 0) done.fetch_or(1ull << dev, std::memory_order_relaxed);
+    return e;
 }
+
+// Every kernel of the library is enqueued here, so that o3dml_launch_count() counts exactly the kernels that were
+// enqueued (memsets and copies are not counted).  Returns the launch error; call sites wrap it in O3DML_CUDA so the
+// message names the failing launch.  A failed launch is also cleared from cudaGetLastError(), so that a later,
+// unrelated check does not report it again.
+template <auto Kernel, class... Args>
+cudaError_t launch(dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+    cudaError_t e = opt_in_smem<Kernel>(smem);
+    if (e == cudaSuccess) {
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = grid;
+        cfg.blockDim = block;
+        cfg.dynamicSmemBytes = smem;
+        cfg.stream = st;
+        e = cudaLaunchKernelEx(&cfg, Kernel, std::forward<Args>(args)...);
+    }
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        return e;
+    }
+    count_launch();
+    return cudaSuccess;
+}
+
 inline int device_sm_count() {
     int dev = 0, n = 0;
     if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess &&

@@ -392,27 +392,25 @@ extern "C" int o3dml_pp_detect(const float* cls, int64_t cls_batch_stride, const
     Workspace ws(workspace, workspace_bytes);
     const DetectBuffers d = carve(ws, B, N, K, C, select);
     if (!ws.ok) O3DML_FAIL(O3DML_ERR_WORKSPACE, "pp_detect: workspace too small (%zu needed)", ws.off);
-    int launches = 5;
     if (select) {
         O3DML_CUDA(cudaMemsetAsync(d.hist, 0, ((size_t)kPasses * B * kBins + B) * sizeof(uint32_t), st));
         const dim3 grid((unsigned)ceil_div<int64_t>(N, kSelRows), (unsigned)B);
         for (int pass = 0; pass <= kPasses; ++pass)
-            pp_select_kernel<<<grid, kSelThreads, 0, st>>>(pass, cls, cls_batch_stride, HW, A, C, N, K, d.keys32,
-                                                             d.hist, d.states, d.cand_count, d.cand);
-        launches += kPasses + 1;
+            O3DML_CUDA(launch<pp_select_kernel>(grid, kSelThreads, 0, st, pass, cls, cls_batch_stride, HW, A, C, N, K,
+                                                d.keys32, d.hist, d.states, d.cand_count, d.cand));
     }
     const size_t sort_smem = (size_t)P * sizeof(unsigned long long);
-    pp_topk_decode_kernel<<<B, kSortThreads, select ? sort_smem : 0, st>>>(
-        d.cand, select ? 1 : 0, K, P, cls, cls_batch_stride, reg, reg_batch_stride, dir, dir_batch_stride, HW, A, C,
-        anchors, d.dec, d.dirc, d.sc);
-    pp_class_sort_kernel<<<B * C, kSortThreads, sort_smem, st>>>(d.sc, d.dec, K, P, C, score_thr, d.seg_idx, d.bev,
-                                                                 d.seg_cnt);
-    pp_nms_mask_kernel<<<dim3((unsigned)words_max, (unsigned)words_max, (unsigned)(B * C)), 64, 0, st>>>(
-        d.bev, d.seg_cnt, K, words_max, d.mask);
-    pp_nms_sweep_kernel<<<B * C, 32, 0, st>>>(d.mask, d.seg_idx, d.seg_cnt, K, words_max, d.keep, d.nkeep);
-    pp_output_kernel<<<dim3((unsigned)ceil_div<int64_t>((int64_t)C * K, 256), (unsigned)B), 256, 0, st>>>(
-        d.dec, d.dirc, d.sc, d.keep, d.nkeep, K, C, dir_offset, out_boxes, out_scores, out_labels, d_counts);
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(launches);
+    O3DML_CUDA(launch<pp_topk_decode_kernel>(B, kSortThreads, select ? sort_smem : 0, st, d.cand, select ? 1 : 0, K, P,
+                                             cls, cls_batch_stride, reg, reg_batch_stride, dir, dir_batch_stride, HW,
+                                             A, C, anchors, d.dec, d.dirc, d.sc));
+    O3DML_CUDA(launch<pp_class_sort_kernel>(B * C, kSortThreads, sort_smem, st, d.sc, d.dec, K, P, C, score_thr,
+                                            d.seg_idx, d.bev, d.seg_cnt));
+    O3DML_CUDA(launch<pp_nms_mask_kernel>(dim3((unsigned)words_max, (unsigned)words_max, (unsigned)(B * C)), 64, 0, st,
+                                          d.bev, d.seg_cnt, K, words_max, d.mask));
+    O3DML_CUDA(launch<pp_nms_sweep_kernel>(B * C, 32, 0, st, d.mask, d.seg_idx, d.seg_cnt, K, words_max, d.keep,
+                                           d.nkeep));
+    O3DML_CUDA(launch<pp_output_kernel>(dim3((unsigned)ceil_div<int64_t>((int64_t)C * K, 256), (unsigned)B), 256, 0, st,
+                                        d.dec, d.dirc, d.sc, d.keep, d.nkeep, K, C, dir_offset, out_boxes, out_scores,
+                                        out_labels, d_counts));
     return O3DML_OK;
 }

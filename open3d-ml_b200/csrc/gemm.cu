@@ -265,16 +265,14 @@ static int gemm_launch(GemmParams& p, cudaStream_t st) {
     // widest column tile that the output fills; narrow outputs get the tall tile
     if (p.Cout <= 32) {
         dim3 grid((unsigned)ceil_div<int64_t>(p.N, 256), (unsigned)ceil_div(p.Cout, 32));
-        gemm_gather_kernel<32><<<grid, GEMM_THREADS, 0, st>>>(p);
+        O3DML_CUDA(launch<gemm_gather_kernel<32>>(grid, GEMM_THREADS, 0, st, p));
     } else if (p.Cout <= 64 || p.N >= 4096) {
         dim3 grid((unsigned)ceil_div<int64_t>(p.N, 128), (unsigned)ceil_div(p.Cout, 64));
-        gemm_gather_kernel<64><<<grid, GEMM_THREADS, 0, st>>>(p);
+        O3DML_CUDA(launch<gemm_gather_kernel<64>>(grid, GEMM_THREADS, 0, st, p));
     } else {
         dim3 grid((unsigned)ceil_div<int64_t>(p.N, 64), (unsigned)ceil_div(p.Cout, 128));
-        gemm_gather_kernel<128><<<grid, GEMM_THREADS, 0, st>>>(p);
+        O3DML_CUDA(launch<gemm_gather_kernel<128>>(grid, GEMM_THREADS, 0, st, p));
     }
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(1);
     return O3DML_OK;
 }
 

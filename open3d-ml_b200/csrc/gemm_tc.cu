@@ -413,17 +413,8 @@ static int make_map(CUtensorMap* map, const void* base, int rank, const uint64_t
 template <int BN, bool GATHER, bool LITE = false>
 static int gemm_tc_launch_bn(const GemmTcParams& p, unsigned grid_x, cudaStream_t st) {
     using C = GtCfg<BN, LITE>;
-    static PerDeviceOnce once;
-    const int dev = current_device();
-    if (once.need(dev)) {
-        O3DML_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, GATHER, LITE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        (int)C::SMEM));
-        once.done(dev);
-    }
     dim3 grid(grid_x, (unsigned)(p.Npad / BN));
-    gemm_tc_kernel<BN, GATHER, LITE><<<grid, gt_threads<GATHER>(), C::SMEM, st>>>(p);
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(1);
+    O3DML_CUDA(launch<gemm_tc_kernel<BN, GATHER, LITE>>(grid, gt_threads<GATHER>(), C::SMEM, st, p));
     return O3DML_OK;
 }
 

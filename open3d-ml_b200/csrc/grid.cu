@@ -380,23 +380,25 @@ static int grid_build(const float* pts, int64_t np, const int64_t* psplits, cons
                       int64_t nq, const int64_t* qsplits, int batch, float fixed_cs, int k,
                       GridBuf& g, cudaStream_t st) {
     const int T = 256;
-    grid_init_kernel<<<ceil_div(batch * 6, T), T, 0, st>>>(g.bbox, batch);
-    if (np > 0) grid_bbox_kernel<<<(unsigned)ceil_div<int64_t>(np, T), T, 0, st>>>(pts, np, psplits, batch, g.bbox);
-    grid_setup_kernel<<<1, 32, 0, st>>>(g.bbox, psplits, batch, fixed_cs, k, g.info, g.total_cells);
+    const unsigned pb = (unsigned)ceil_div<int64_t>(np, T);
+    O3DML_CUDA(launch<grid_init_kernel>(ceil_div(batch * 6, T), T, 0, st, g.bbox, batch));
+    if (np > 0) O3DML_CUDA(launch<grid_bbox_kernel>(pb, T, 0, st, pts, np, psplits, batch, g.bbox));
+    O3DML_CUDA(launch<grid_setup_kernel>(1, 32, 0, st, g.bbox, psplits, batch, fixed_cs, k, g.info, g.total_cells));
     O3DML_CUDA(cudaMemsetAsync(g.cell_start, 0, (g.max_cells + 1) * 4, st));
     O3DML_CUDA(cudaMemsetAsync(g.cursor, 0, (g.max_cells + 1) * 4, st));
-    if (np > 0) grid_count_kernel<<<(unsigned)ceil_div<int64_t>(np, T), T, 0, st>>>(pts, np, psplits, batch, g.info, g.cell_of, g.cell_start);
+    if (np > 0)
+        O3DML_CUDA(launch<grid_count_kernel>(pb, T, 0, st, pts, np, psplits, batch, g.info, g.cell_of, g.cell_start));
     O3DML_CUDA(exclusive_scan_u32(g.cell_start, g.cell_start, g.max_cells + 1, nullptr, g.scan_tmp, st));
-    if (np > 0) grid_fill_kernel<<<(unsigned)ceil_div<int64_t>(np, T), T, 0, st>>>(pts, np, g.cell_of, g.cell_start, g.cursor, g.sorted);
+    if (np > 0)
+        O3DML_CUDA(launch<grid_fill_kernel>(pb, T, 0, st, pts, np, g.cell_of, g.cell_start, g.cursor, g.sorted));
     if (nq > 0) {
+        const unsigned qb = (unsigned)ceil_div<int64_t>(nq, T);
         O3DML_CUDA(cudaMemsetAsync(g.qstart, 0, (g.max_cells + 1) * 4, st));
         O3DML_CUDA(cudaMemsetAsync(g.qcursor, 0, (g.max_cells + 1) * 4, st));
-        query_cell_kernel<<<(unsigned)ceil_div<int64_t>(nq, T), T, 0, st>>>(q, nq, qsplits, batch, g.info, g.qcell, g.qstart);
+        O3DML_CUDA(launch<query_cell_kernel>(qb, T, 0, st, q, nq, qsplits, batch, g.info, g.qcell, g.qstart));
         O3DML_CUDA(exclusive_scan_u32(g.qstart, g.qstart, g.max_cells + 1, nullptr, g.scan_tmp, st));
-        query_order_kernel<<<(unsigned)ceil_div<int64_t>(nq, T), T, 0, st>>>(nq, g.qcell, g.qstart, g.qcursor, g.order);
+        O3DML_CUDA(launch<query_order_kernel>(qb, T, 0, st, nq, g.qcell, g.qstart, g.qcursor, g.order));
     }
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(6 + (nq > 0 ? 3 : 0));
     return O3DML_OK;
 }
 
@@ -427,18 +429,16 @@ extern "C" int o3dml_knn_search(const float* points, int64_t num_points,
                         queries_row_splits, (int)batch, 0.f, k, g, st);
     if (rc) return rc;
     const unsigned nb = (unsigned)ceil_div<int64_t>(num_queries, 128);
-#define KNN_LAUNCH(KM)                                                                           \
-    knn_kernel<KM><<<nb, 128, 0, st>>>(queries, num_queries, queries_row_splits, points_row_splits, \
-                                       (int)batch, g.order, g.info, g.cell_start, g.sorted, k,    \
-                                       out_index, index_is64, out_distance2)
+#define KNN_LAUNCH(KM)                                                                                  \
+    O3DML_CUDA(launch<knn_kernel<KM>>(nb, 128, 0, st, queries, num_queries, queries_row_splits,          \
+                                      points_row_splits, (int)batch, g.order, g.info, g.cell_start,     \
+                                      g.sorted, k, out_index, index_is64, out_distance2))
     if (k == 1) KNN_LAUNCH(1);
     else if (k <= 8) KNN_LAUNCH(8);
     else if (k <= 16) KNN_LAUNCH(16);
     else if (k <= 32) KNN_LAUNCH(32);
     else KNN_LAUNCH(64);
 #undef KNN_LAUNCH
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(1);
     return O3DML_OK;
 }
 
@@ -477,14 +477,11 @@ extern "C" int o3dml_radius_count(const float* points, int64_t num_points,
                         queries_row_splits, (int)batch, radius, 0, g, st);
     if (rc) return rc;
     const unsigned nb = (unsigned)ceil_div<int64_t>(num_queries, 128);
-    radius_kernel<0><<<nb, 128, 0, st>>>(queries, num_queries, queries_row_splits, (int)batch, g.order,
-                                         g.info, g.cell_start, g.sorted, radius, counts, nullptr,
-                                         nullptr, nullptr);
+    O3DML_CUDA(launch<radius_kernel<0>>(nb, 128, 0, st, queries, num_queries, queries_row_splits, (int)batch, g.order,
+                                        g.info, g.cell_start, g.sorted, radius, counts, nullptr, nullptr, nullptr));
     O3DML_CUDA(exclusive_scan_u32(counts, counts, num_queries, total, scan_tmp, st));
-    widen_splits_kernel<<<(unsigned)ceil_div<int64_t>(num_queries, 256), 256, 0, st>>>(
-        counts, num_queries, total, neighbors_row_splits, d_total);
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(3);
+    O3DML_CUDA(launch<widen_splits_kernel>((unsigned)ceil_div<int64_t>(num_queries, 256), 256, 0, st, counts,
+                                           num_queries, total, neighbors_row_splits, d_total));
     return O3DML_OK;
 }
 
@@ -503,10 +500,8 @@ extern "C" int o3dml_radius_fill(const float* queries, int64_t num_points, int64
     O3DML_CHECK(neighbors_index != nullptr && neighbors_distance2 != nullptr,
                 "fixed_radius_search: index and distance outputs are both required");
     const unsigned nb = (unsigned)ceil_div<int64_t>(num_queries, 128);
-    radius_kernel<1><<<nb, 128, 0, st>>>(queries, num_queries, queries_row_splits, (int)batch, g.order,
-                                         g.info, g.cell_start, g.sorted, radius, nullptr,
-                                         neighbors_row_splits, neighbors_index, neighbors_distance2);
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(1);
+    O3DML_CUDA(launch<radius_kernel<1>>(nb, 128, 0, st, queries, num_queries, queries_row_splits, (int)batch, g.order,
+                                        g.info, g.cell_start, g.sorted, radius, nullptr, neighbors_row_splits,
+                                        neighbors_index, neighbors_distance2));
     return O3DML_OK;
 }

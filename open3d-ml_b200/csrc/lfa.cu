@@ -266,17 +266,8 @@ template <int D, int STAGE>
 static int lfa_launch(const LfaParams& p, cudaStream_t st) {
     using C = LfaCfg<D>;
     const size_t smem = C::smem_bytes(STAGE);
-    static PerDeviceOnce once;
-    const int dev = current_device();
-    if (once.need(dev)) {
-        O3DML_CUDA(cudaFuncSetAttribute(lfa_pool_kernel<D, STAGE>,
-                                        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        once.done(dev);
-    }
     const unsigned blocks = (unsigned)ceil_div<int64_t>(p.total, C::P);
-    lfa_pool_kernel<D, STAGE><<<blocks, LFA_THREADS, smem, st>>>(p);
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(1);
+    O3DML_CUDA(launch<lfa_pool_kernel<D, STAGE>>(blocks, LFA_THREADS, smem, st, p));
     return O3DML_OK;
 }
 
@@ -440,9 +431,7 @@ static int lfa16c_launch(const LfaParams& p, const Lfa16W& w, cudaStream_t st) {
     const int64_t groups = ceil_div<int64_t>(p.total, L16_PTS);
     const int64_t cap = (int64_t)device_sm_count() * L16C_CTAS;   // resident CTAs; each walks groups with a grid stride
     const unsigned blocks = (unsigned)(groups < cap ? groups : cap);
-    lfa16c_kernel<STAGE><<<blocks, L16_ROWS, 0, st>>>(p, w, groups);
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(1);
+    O3DML_CUDA(launch<lfa16c_kernel<STAGE>>(blocks, L16_ROWS, 0, st, p, w, groups));
     return O3DML_OK;
 }
 

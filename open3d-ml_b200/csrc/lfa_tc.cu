@@ -566,23 +566,16 @@ template <int D, int STAGE>
 static int lfa_tc_launch(const LfaTcParams& p, cudaStream_t st) {
     using C = LtcCfg<D, STAGE>;
     static_assert(C::SMEM <= 227 * 1024, "shared memory budget");
-    static PerDeviceOnce once;
-    const int dev = current_device();
-    if (once.need(dev)) {
-        O3DML_CUDA(cudaFuncSetAttribute(lfa_pool_tc_kernel<D, STAGE>,
-                                        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
-        once.done(dev);
-    }
-    // persistent CTAs: as many as are resident at once (registers and shared memory both limit it)
+    // persistent CTAs: as many as are resident at once (registers and shared memory both limit it).  The occupancy
+    // query counts the opt-in shared memory only once the kernel has been opted in.
+    O3DML_CUDA(opt_in_smem<lfa_pool_tc_kernel<D, STAGE>>(C::SMEM));
     int per_sm = 0;
     O3DML_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lfa_pool_tc_kernel<D, STAGE>, C::NTH, C::SMEM));
     if (per_sm < 1) per_sm = 1;
     if (per_sm > 4) per_sm = 4;
     int64_t grid = (int64_t)device_sm_count() * per_sm;
     if (grid > p.num_tiles) grid = p.num_tiles;
-    lfa_pool_tc_kernel<D, STAGE><<<(unsigned)grid, C::NTH, C::SMEM, st>>>(p);
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(1);
+    O3DML_CUDA(launch<lfa_pool_tc_kernel<D, STAGE>>((unsigned)grid, C::NTH, C::SMEM, st, p));
     return O3DML_OK;
 }
 

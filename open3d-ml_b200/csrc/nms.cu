@@ -133,16 +133,14 @@ extern "C" int o3dml_nms(const float* boxes, const float* scores, int64_t num_bo
     char* tmp = ws.take<char>(radix_sort_temp_bytes(n));
     uint64_t* mask = ws.take<uint64_t>((size_t)n * words);
     if (!ws.ok) O3DML_FAIL(O3DML_ERR_WORKSPACE, "nms: workspace too small (%zu needed)", ws.off);
-    nms_keys_kernel<<<(unsigned)ceil_div<int64_t>(n, 256), 256, 0, st>>>(scores, n, ka);
+    O3DML_CUDA(launch<nms_keys_kernel>((unsigned)ceil_div<int64_t>(n, 256), 256, 0, st, scores, n, ka));
     int in_b = 0;
     O3DML_CUDA(radix_sort_pairs(ka, va, kb, vb, true, n, 32, tmp, st, &in_b));
     const uint32_t* order = in_b ? vb : va;
     O3DML_CUDA(cudaMemsetAsync(mask, 0, (size_t)n * words * 8, st));
     dim3 grid((unsigned)words, (unsigned)words);
-    nms_mask_kernel<<<grid, 64, 0, st>>>(boxes, order, n, iou_threshold, mask, words);
-    nms_sweep_kernel<<<1, 32, (size_t)words * 8, st>>>(mask, order, n, words, keep_indices, d_num_keep);
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(3);
+    O3DML_CUDA(launch<nms_mask_kernel>(grid, 64, 0, st, boxes, order, n, iou_threshold, mask, words));
+    O3DML_CUDA(launch<nms_sweep_kernel>(1, 32, (size_t)words * 8, st, mask, order, n, words, keep_indices, d_num_keep));
     return O3DML_OK;
 }
 
@@ -151,9 +149,7 @@ extern "C" int o3dml_iou_matrix(const float* boxes_a, int64_t num_a, const float
     O3DML_CHECK(mode == 0 || mode == 1, "iou: mode 0 (bev, [.,5]) or 1 (3d, [.,7])");
     if (num_a <= 0 || num_b <= 0) return O3DML_OK;
     O3DML_CHECK(boxes_a && boxes_b && out, "iou: null input");
-    iou_matrix_kernel<<<(unsigned)ceil_div<int64_t>(num_a * num_b, 128), 128, 0, (cudaStream_t)stream>>>(
-        boxes_a, num_a, boxes_b, num_b, mode, out);
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(1);
+    O3DML_CUDA(launch<iou_matrix_kernel>((unsigned)ceil_div<int64_t>(num_a * num_b, 128), 128, 0, (cudaStream_t)stream,
+                                         boxes_a, num_a, boxes_b, num_b, mode, out));
     return O3DML_OK;
 }

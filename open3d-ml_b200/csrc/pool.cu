@@ -150,7 +150,7 @@ kpconv_gather_grouped_kernel(const float* __restrict__ q_pts, const float* __res
                              int64_t n_support, const void* __restrict__ nidx, int idx_is64, int H,
                              const float* __restrict__ x, int Cin, const float* __restrict__ kpts, int K,
                              float extent, int64_t nq, float* __restrict__ out,
-                             const float* __restrict__ offsets = nullptr, int offset_ld = 0) {
+                             const float* __restrict__ offsets, int offset_ld) {
     constexpr int QPW = 32 / LPQ;                       // queries per warp
     __shared__ float4 kp4[(DEFORM ? 8 * QPW : 1) * KP_MAXK];   // DEFORM: [warp][query][kernel point]
     // [warp][4 kernel points][slot]: slot = row ^ (row / LPQ) spreads the QPW rows that are read
@@ -308,11 +308,9 @@ extern "C" int o3dml_gather_max(const float* src, int64_t src_rows, int channels
     O3DML_CHECK(k >= 1, "gather_max: k >= 1");
     if (num_rows <= 0) return O3DML_OK;
     int64_t total = num_rows * (channels / 4);
-    gather_max_kernel<<<(unsigned)ceil_div<int64_t>(total, 256), 256, 0, (cudaStream_t)stream>>>(
-        src, src_rows, channels, src_ld, index, index_is64, num_rows, k, out_rows_per_batch,
-        src_rows_per_batch, shadow_zero, out, out_ld);
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(1);
+    O3DML_CUDA(launch<gather_max_kernel>((unsigned)ceil_div<int64_t>(total, 256), 256, 0, (cudaStream_t)stream, src,
+                                         src_rows, channels, src_ld, index, index_is64, num_rows, k,
+                                         out_rows_per_batch, src_rows_per_batch, shadow_zero, out, out_ld));
     return O3DML_OK;
 }
 
@@ -332,30 +330,27 @@ extern "C" int o3dml_kpconv_gather(const float* query_points, int64_t num_querie
                          ((reinterpret_cast<uintptr_t>(features) | reinterpret_cast<uintptr_t>(weighted_features)) & 15) == 0;
     const bool narrow = in_channels <= 8 && num_support < ((int64_t)1 << 31);
     if (aligned || narrow) {
-#define KPG_LAUNCH(LPQ, NE)                                                                                          \
-    kpconv_gather_grouped_kernel<LPQ, NE><<<(unsigned)ceil_div<int64_t>(num_queries, 8 * (32 / LPQ)), 256, 0, st>>>( \
-        query_points, support_points, num_support, neighbor_index, index_is64, max_neighbors, features,          \
-        in_channels, kernel_points, num_kernel_points, kp_extent, num_queries, weighted_features)
+#define KPG_LAUNCH(LPQ, NE)                                                                                        \
+    O3DML_CUDA(launch<kpconv_gather_grouped_kernel<LPQ, NE>>(                                                      \
+        (unsigned)ceil_div<int64_t>(num_queries, 8 * (32 / LPQ)), 256, 0, st, query_points, support_points,      \
+        num_support, neighbor_index, index_is64, max_neighbors, features, in_channels, kernel_points,          \
+        num_kernel_points, kp_extent, num_queries, weighted_features, nullptr, 0))
         if (!aligned) KPG_LAUNCH(8, 1);
         else if (in_channels <= 32) KPG_LAUNCH(8, 4);
         else if (in_channels <= 64) KPG_LAUNCH(16, 4);
         else KPG_LAUNCH(32, 4);
 #undef KPG_LAUNCH
-        O3DML_LAUNCH_CHECK();
-        o3dml_count_launches(1);
         return O3DML_OK;
     }
-#define KP_LAUNCH(NE)                                                                                   \
-    kpconv_gather_kernel<NE><<<nb, 256, 0, st>>>(query_points, support_points, num_support, neighbor_index, \
-                                                 index_is64, max_neighbors, features, in_channels,          \
-                                                 kernel_points, num_kernel_points, kp_extent, num_queries,  \
-                                                 weighted_features)
+#define KP_LAUNCH(NE)                                                                                         \
+    O3DML_CUDA(launch<kpconv_gather_kernel<NE>>(nb, 256, 0, st, query_points, support_points, num_support,    \
+                                                neighbor_index, index_is64, max_neighbors, features,         \
+                                                in_channels, kernel_points, num_kernel_points, kp_extent,    \
+                                                num_queries, weighted_features))
     if (in_channels <= 32) KP_LAUNCH(1);
     else if (in_channels <= 64) KP_LAUNCH(2);
     else KP_LAUNCH(4);
 #undef KP_LAUNCH
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(1);
     return O3DML_OK;
 }
 
@@ -377,16 +372,15 @@ extern "C" int o3dml_kpconv_gather_deformable(const float* query_points, int64_t
                 "kpconv_deformable: Cin % 4 == 0 with 16-byte aligned rows, or Cin <= 8; fewer than 2^31 supports");
     if (num_queries <= 0) return O3DML_OK;
     cudaStream_t st = (cudaStream_t)stream;
-#define KPD_LAUNCH(LPQ, NE)                                                                                             \
-    kpconv_gather_grouped_kernel<LPQ, NE, true><<<(unsigned)ceil_div<int64_t>(num_queries, 8 * (32 / LPQ)), 256, 0, st>>>( \
-        query_points, support_points, num_support, neighbor_index, index_is64, max_neighbors, features, in_channels,     \
-        kernel_points, num_kernel_points, kp_extent, num_queries, weighted_features, offsets, offset_ld)
+#define KPD_LAUNCH(LPQ, NE)                                                                                        \
+    O3DML_CUDA(launch<kpconv_gather_grouped_kernel<LPQ, NE, true>>(                                                \
+        (unsigned)ceil_div<int64_t>(num_queries, 8 * (32 / LPQ)), 256, 0, st, query_points, support_points,      \
+        num_support, neighbor_index, index_is64, max_neighbors, features, in_channels, kernel_points,          \
+        num_kernel_points, kp_extent, num_queries, weighted_features, offsets, offset_ld))
     if (!aligned) KPD_LAUNCH(8, 1);
     else if (in_channels <= 32) KPD_LAUNCH(8, 4);
     else if (in_channels <= 64) KPD_LAUNCH(16, 4);
     else KPD_LAUNCH(32, 4);
 #undef KPD_LAUNCH
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(1);
     return O3DML_OK;
 }

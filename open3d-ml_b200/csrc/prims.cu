@@ -137,15 +137,11 @@ cudaError_t exclusive_scan_u32(const uint32_t* in, uint32_t* out, int64_t n, uin
         if (total_out) return cudaMemsetAsync(total_out, 0, sizeof(uint32_t), st);
         return cudaSuccess;
     }
-    if (n <= SCAN_TILE) {
-        scan_single_block<<<1, SCAN_THREADS, 0, st>>>(in, out, n, total_out);
-        return cudaGetLastError();
-    }
+    if (n <= SCAN_TILE) return launch<scan_single_block>(1, SCAN_THREADS, 0, st, in, out, n, total_out);
     const int64_t tiles = ceil_div<int64_t>(n, SCAN_TILE);
     cudaError_t e = cudaMemsetAsync(temp, 0, (size_t)(tiles + 1) * sizeof(unsigned long long), st);
     if (e != cudaSuccess) return e;
-    scan_lookback<<<(unsigned)tiles, SCAN_THREADS, 0, st>>>(in, out, n, (unsigned long long*)temp, total_out);
-    return cudaGetLastError();
+    return launch<scan_lookback>((unsigned)tiles, SCAN_THREADS, 0, st, in, out, n, (unsigned long long*)temp, total_out);
 }
 
 // ------------------------------------------------------------ radix sort ----
@@ -264,16 +260,17 @@ cudaError_t radix_sort_pairs(uint64_t* keys_a, uint32_t* vals_a, uint64_t* keys_
     uint32_t* vout = vals_b;
     for (int p = 0; p < passes; ++p) {
         int shift = 8 * p;
-        rs_histogram<<<nblk, RS_THREADS, 0, st>>>(kin, n, shift, hist, nblk);
-        cudaError_t e = exclusive_scan_u32(hist, hist, (int64_t)RS_BINS * nblk, nullptr, scan_tmp, st);
+        cudaError_t e = launch<rs_histogram>(nblk, RS_THREADS, 0, st, kin, n, shift, hist, nblk);
+        if (e == cudaSuccess) e = exclusive_scan_u32(hist, hist, (int64_t)RS_BINS * nblk, nullptr, scan_tmp, st);
+        if (e == cudaSuccess)
+            e = launch<rs_scatter>(nblk, RS_THREADS, 0, st, kin, (p == 0 && vals_are_iota) ? nullptr : vin, kout, vout,
+                                   n, shift, hist, nblk);
         if (e != cudaSuccess) return e;
-        rs_scatter<<<nblk, RS_THREADS, 0, st>>>(kin, (p == 0 && vals_are_iota) ? nullptr : vin, kout,
-                                                vout, n, shift, hist, nblk);
         uint64_t* tk = kin; kin = kout; kout = tk;
         uint32_t* tv = vin; vin = vout; vout = tv;
         *result_in_b ^= 1;
     }
-    return cudaGetLastError();
+    return cudaSuccess;
 }
 
 }  // namespace o3dml

@@ -190,16 +190,8 @@ extern "C" int o3dml_randla_tail(const float* skip, int skip_ld, const float* co
     p.wimg = (const float*)weight_image; p.out = out; p.slope = slope;
     memcpy(p.scale, h_scale, sizeof(p.scale));
     memcpy(p.shift, h_shift, sizeof(p.shift));
-    static PerDeviceOnce once;
-    const int dev = current_device();
-    if (once.need(dev)) {
-        O3DML_CUDA(cudaFuncSetAttribute(rl_tail_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RT_SMEM));
-        once.done(dev);
-    }
     const int64_t tiles = ceil_div<int64_t>(num_rows, RT_THREADS);
     const unsigned grid = (unsigned)std::min<int64_t>(tiles, (int64_t)device_sm_count() * 2);
-    rl_tail_kernel<<<grid, RT_THREADS, RT_SMEM, (cudaStream_t)stream>>>(p);
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(1);
+    O3DML_CUDA(launch<rl_tail_kernel>(grid, RT_THREADS, RT_SMEM, (cudaStream_t)stream, p));
     return O3DML_OK;
 }

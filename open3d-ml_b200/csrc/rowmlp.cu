@@ -109,9 +109,7 @@ static int rowmlp_launch(int64_t num_rows, const o3dml_src_t (&srcs)[2], const f
         p.w[K * CP + c] = hs ? hs[c] : 1.f;
         p.w[K * CP + CP + c] = ht ? ht[c] : 0.f;
     }
-    rowmlp_kernel<C0, C1, COUT><<<(unsigned)ceil_div<int64_t>(num_rows, 256), 256, 0, st>>>(p);
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(1);
+    O3DML_CUDA(launch<rowmlp_kernel<C0, C1, COUT>>((unsigned)ceil_div<int64_t>(num_rows, 256), 256, 0, st, p));
     return O3DML_OK;
 }
 

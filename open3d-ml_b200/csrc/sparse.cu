@@ -125,15 +125,15 @@ extern "C" int o3dml_sparse_conv_neighbors(const float* in_positions, int64_t nu
     const uint64_t* skeys = ka;
     const uint32_t* perm = va;
     if (num_in > 0) {
-        sparse_keys_kernel<<<(unsigned)ceil_div<int64_t>(num_in, 256), 256, 0, st>>>(in_positions, num_in, g.inv_v, ka);
+        O3DML_CUDA(launch<sparse_keys_kernel>((unsigned)ceil_div<int64_t>(num_in, 256), 256, 0, st, in_positions, num_in,
+                                              g.inv_v, ka));
         int in_b = 0;
         O3DML_CUDA(radix_sort_pairs(ka, va, kb, vb, true, num_in, 63, tmp, st, &in_b));
         skeys = in_b ? kb : ka;
         perm = in_b ? vb : va;
     }
-    sparse_neighbors_kernel<<<(unsigned)ceil_div<int64_t>(num_out * kc, 256), 256, 0, st>>>(
-        in_positions, num_in, out_positions, num_out, skeys, perm, g, neighbors, neighbor_count);
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(2);
+    O3DML_CUDA(launch<sparse_neighbors_kernel>((unsigned)ceil_div<int64_t>(num_out * kc, 256), 256, 0, st, in_positions,
+                                               num_in, out_positions, num_out, skeys, perm, g, neighbors,
+                                               neighbor_count));
     return O3DML_OK;
 }

@@ -86,17 +86,14 @@ extern "C" int o3dml_voxel_reduce(const float* points, int point_stride, const f
     if (num_voxels_bound <= 0) return O3DML_OK;
     const int C = 3 + feat_channels;
     const int64_t total = num_voxels_bound * C;
-    voxel_reduce_kernel<<<(unsigned)ceil_div<int64_t>(total, 256), 256, 0, st>>>(
-        points, point_stride, features, feat_channels, feat_stride, voxel_row_splits, voxel_point_indices, d_num_voxels,
-        num_voxels_bound, position_mode, feature_mode, out_points, out_features);
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(1);
-    if (labels) {
-        voxel_label_kernel<<<(unsigned)ceil_div<int64_t>(num_voxels_bound, 128), 128, 0, st>>>(
-            labels, voxel_row_splits, voxel_point_indices, d_num_voxels, num_voxels_bound, out_labels);
-        O3DML_LAUNCH_CHECK();
-        o3dml_count_launches(1);
-    }
+    O3DML_CUDA(launch<voxel_reduce_kernel>((unsigned)ceil_div<int64_t>(total, 256), 256, 0, st, points, point_stride,
+                                           features, feat_channels, feat_stride, voxel_row_splits, voxel_point_indices,
+                                           d_num_voxels, num_voxels_bound, position_mode, feature_mode, out_points,
+                                           out_features));
+    if (labels)
+        O3DML_CUDA(launch<voxel_label_kernel>((unsigned)ceil_div<int64_t>(num_voxels_bound, 128), 128, 0, st, labels,
+                                              voxel_row_splits, voxel_point_indices, d_num_voxels, num_voxels_bound,
+                                              out_labels));
     return O3DML_OK;
 }
 
@@ -119,9 +116,7 @@ extern "C" int o3dml_reduce_subarrays_sum(const float* values, const int64_t* ro
                                           void* stream) {
     if (num_rows <= 0) return O3DML_OK;
     O3DML_CHECK(values && row_splits && out, "reduce_subarrays_sum: null input");
-    o3dml::reduce_subarrays_kernel<<<(unsigned)o3dml::ceil_div<int64_t>(num_rows, 256), 256, 0, (cudaStream_t)stream>>>(
-        values, row_splits, num_rows, out);
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(1);
+    O3DML_CUDA(launch<reduce_subarrays_kernel>((unsigned)ceil_div<int64_t>(num_rows, 256), 256, 0, (cudaStream_t)stream,
+                                               values, row_splits, num_rows, out));
     return O3DML_OK;
 }

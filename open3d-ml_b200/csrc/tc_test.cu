@@ -129,9 +129,9 @@ using namespace o3dml;
 extern "C" int o3dml_tc_mma_rate(int n, int reps, long long* out, void* stream) {
     O3DML_CHECK(n >= 16 && n <= 256 && (n % 16) == 0, "tc_mma_rate: bad N");
     const size_t smem = 2 * 4 * 128 * 16 + 2 * 4 * (size_t)n * 16;
+    // the size varies from call to call, which launch<>() does not track: set it here on every call
     O3DML_CUDA(cudaFuncSetAttribute(tc_mma_rate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    tc_mma_rate_kernel<<<1, 128, smem, (cudaStream_t)stream>>>(n, reps, out);
-    O3DML_LAUNCH_CHECK();
+    O3DML_CUDA(launch<tc_mma_rate_kernel>(1, 128, smem, (cudaStream_t)stream, n, reps, out));
     return O3DML_OK;
 }
 
@@ -143,8 +143,6 @@ extern "C" int o3dml_tc_gemm_test(const float* a, const float* b, float* d, int 
     const size_t smem = (size_t)(k / 8) * 16 * 2 * (128 + n);
     O3DML_CHECK(smem <= 200 * 1024, "tc_gemm_test: operands do not fit in shared memory");
     O3DML_CUDA(cudaFuncSetAttribute(tc_gemm_test_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    tc_gemm_test_kernel<<<1, 128, smem, (cudaStream_t)stream>>>(a, b, d, n, k, terms);
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(1);
+    O3DML_CUDA(launch<tc_gemm_test_kernel>(1, 128, smem, (cudaStream_t)stream, a, b, d, n, k, terms));
     return O3DML_OK;
 }

@@ -387,29 +387,26 @@ extern "C" int o3dml_voxelize(const float* points, int64_t num_points, int point
     const int T = 256;
     const unsigned nb = (unsigned)ceil_div<int64_t>(n, T);
     O3DML_CUDA(cudaMemsetAsync(scalars, 0, 16 * sizeof(uint32_t), st));
-    vox_hash_kernel<<<nb, T, 0, st>>>(points, point_stride, n, row_splits, (int)batch, g, invalid_key,
-                                      keys_a);
+    O3DML_CUDA(launch<vox_hash_kernel>(nb, T, 0, st, points, point_stride, n, row_splits, (int)batch, g, invalid_key,
+                                       keys_a));
     int in_b = 0;
     O3DML_CUDA(radix_sort_pairs(keys_a, vals_a, keys_b, vals_b, true, n, num_bits, sort_tmp, st, &in_b));
     const uint64_t* ks = in_b ? keys_b : keys_a;
     const uint32_t* vs = in_b ? vals_b : vals_a;
-    vox_heads_kernel<<<nb, T, 0, st>>>(ks, n, invalid_key, flags, &scalars[0]);
+    O3DML_CUDA(launch<vox_heads_kernel>(nb, T, 0, st, ks, n, invalid_key, flags, &scalars[0]));
     O3DML_CUDA(exclusive_scan_u32(flags, flags, n, &scalars[1], scan_tmp, st));
-    vox_headpos_kernel<<<nb, T, 0, st>>>(flags, ks, n, invalid_key, head_pos);
-    vox_batch_bounds_kernel<<<1, 256, 0, st>>>(ks, flags, &scalars[1], &scalars[0], (int)batch,
+    O3DML_CUDA(launch<vox_headpos_kernel>(nb, T, 0, st, flags, ks, n, invalid_key, head_pos));
+    O3DML_CUDA(launch<vox_batch_bounds_kernel>(1, 256, 0, st, ks, flags, &scalars[1], &scalars[0], (int)batch,
                                                (uint64_t)g.cells, max_voxels, batch_first, batch_out,
-                                               voxel_batch_splits);
-    vox_counts_kernel<<<nb, T, 0, st>>>(head_pos, &scalars[1], &scalars[0], batch_first, (int)batch,
-                                        max_voxels, max_points_per_voxel, n, kept);
+                                               voxel_batch_splits));
+    O3DML_CUDA(launch<vox_counts_kernel>(nb, T, 0, st, head_pos, &scalars[1], &scalars[0], batch_first, (int)batch,
+                                         max_voxels, max_points_per_voxel, n, kept));
     O3DML_CUDA(exclusive_scan_u32(kept, kept_excl, n, &scalars[2], scan_tmp, st));
-    vox_emit_voxels_kernel<<<nb, T, 0, st>>>(ks, head_pos, &scalars[1], kept_excl, &scalars[2],
-                                             batch_first, batch_out, (int)batch, max_voxels, g, n,
-                                             voxel_coords, voxel_point_row_splits, voxel_batch_id,
-                                             d_counts);
-    vox_emit_points_kernel<<<nb, T, 0, st>>>(ks, vs, flags, head_pos, &scalars[0], kept, kept_excl, n,
-                                             voxel_point_indices);
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(9 + 3 * ((num_bits + 7) / 8));  // scans here are single-block (n < 64 Ki tiles)
+    O3DML_CUDA(launch<vox_emit_voxels_kernel>(nb, T, 0, st, ks, head_pos, &scalars[1], kept_excl, &scalars[2],
+                                              batch_first, batch_out, (int)batch, max_voxels, g, n, voxel_coords,
+                                              voxel_point_row_splits, voxel_batch_id, d_counts));
+    O3DML_CUDA(launch<vox_emit_points_kernel>(nb, T, 0, st, ks, vs, flags, head_pos, &scalars[0], kept, kept_excl, n,
+                                              voxel_point_indices));
     return O3DML_OK;
 }
 
@@ -423,15 +420,13 @@ extern "C" int o3dml_ragged_to_dense(const void* values, int elem_bytes, int64_t
     if (total == 0) return O3DML_OK;
     unsigned nb = (unsigned)ceil_div<int64_t>(total, 256);
     if (elem_bytes == 8)
-        ragged_to_dense_kernel<int64_t><<<nb, 256, 0, st>>>((const int64_t*)values, row_splits, rows,
-                                                           out_col_size, inner, (int64_t)fill_bits,
-                                                           (int64_t)add, (int64_t*)out);
+        O3DML_CUDA(launch<ragged_to_dense_kernel<int64_t>>(nb, 256, 0, st, (const int64_t*)values, row_splits, rows,
+                                                           out_col_size, inner, (int64_t)fill_bits, (int64_t)add,
+                                                           (int64_t*)out));
     else
-        ragged_to_dense_kernel<int32_t><<<nb, 256, 0, st>>>((const int32_t*)values, row_splits, rows,
-                                                           out_col_size, inner, (int32_t)fill_bits,
-                                                           (int32_t)add, (int32_t*)out);
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(1);
+        O3DML_CUDA(launch<ragged_to_dense_kernel<int32_t>>(nb, 256, 0, st, (const int32_t*)values, row_splits, rows,
+                                                           out_col_size, inner, (int32_t)fill_bits, (int32_t)add,
+                                                           (int32_t*)out));
     return O3DML_OK;
 }
 
@@ -453,11 +448,9 @@ extern "C" int o3dml_pp_pfn_scatter(const float* points, int point_stride, int p
     int64_t blocks = ceil_div<int64_t>(warps_needed, 8);
     int64_t cap = (int64_t)device_sm_count() * 8;  // 8 resident CTAs of 256 threads per SM
     if (blocks > cap) blocks = cap;
-    pp_pfn_scatter_kernel<64><<<(unsigned)blocks, 256, 0, st>>>(
-        points, point_stride, point_channels, voxel_coords, voxel_row_splits, voxel_point_indices,
-        voxel_batch_id, d_num_voxels, num_voxels_bound, w_t, bn_scale, bn_shift, vx, vy, x_offset,
-        y_offset, nx, ny, max_points_per_voxel, feat_out, canvas, canvas_nchw);
-    O3DML_LAUNCH_CHECK();
-    o3dml_count_launches(1);
+    O3DML_CUDA(launch<pp_pfn_scatter_kernel<64>>(
+        (unsigned)blocks, 256, 0, st, points, point_stride, point_channels, voxel_coords, voxel_row_splits,
+        voxel_point_indices, voxel_batch_id, d_num_voxels, num_voxels_bound, w_t, bn_scale, bn_shift, vx, vy, x_offset,
+        y_offset, nx, ny, max_points_per_voxel, feat_out, canvas, canvas_nchw));
     return O3DML_OK;
 }
