@@ -8,8 +8,10 @@
  *   - `stream` is a cudaStream_t passed as void*; all work is enqueued on it, no
  *     function synchronises the device or allocates memory;
  *   - scratch memory comes from the caller (`workspace`, sized by the matching
- *     *_workspace_bytes function); outputs are caller-allocated, inputs are never
- *     written or retained;
+ *     *_workspace_bytes function, which returns exactly the bytes the entry uses);
+ *     an entry given too small a workspace returns 2 before it enqueues anything,
+ *     and o3dml_last_error() names the bytes it needed; outputs are
+ *     caller-allocated, inputs are never written or retained;
  *   - return value 0 = success; otherwise o3dml_last_error() describes the failure
  *     (the Python layer raises RuntimeError, as TORCH_CHECK does upstream);
  *   - data-dependent output sizes are reported through small device counters

@@ -25,6 +25,11 @@ extern "C" void o3dml_set_error(const char* fmt, ...);
         if (!(cond)) O3DML_FAIL(O3DML_ERR_INVALID, __VA_ARGS__); \
     } while (0)
 
+#define O3DML_CHECK_WORKSPACE(ws, entry)                                                                    \
+    do {                                                                                                    \
+        if (!(ws).ok) O3DML_FAIL(O3DML_ERR_WORKSPACE, entry ": workspace too small (%zu needed)", (ws).off); \
+    } while (0)
+
 // variadic so that the commas of a template argument list, launch<k<A, B>>(...), need no extra parentheses
 #define O3DML_CUDA(...)                                                               \
     do {                                                                              \
@@ -91,25 +96,27 @@ __host__ __device__ inline T ceil_div(T a, T b) {
     return (a + b - 1) / b;
 }
 
-inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
-
-// Bump allocator over a caller-provided workspace.
+// Bump allocator over a caller-provided workspace, in 256-byte aligned pieces.  Each entry point lays its workspace
+// out in one carve function, carve(Workspace&, sizes...): the entry carves the caller's buffer and checks it with
+// O3DML_CHECK_WORKSPACE before it enqueues anything, and its *_workspace_bytes returns measure(carve, sizes...).
+// `off` adds up every take, whether it fitted or not, so it is both the exact size and what a failed carve needed.
 struct Workspace {
     char* base;
-    size_t size, off;
-    bool ok;
-    Workspace(void* p, size_t n) : base((char*)p), size(n), off(0), ok(true) {}
+    size_t size, off = 0;
+    bool ok = true;  // every take so far fitted; a take that does not returns nullptr, as do all that follow it
+    Workspace(void* p, size_t n) : base((char*)p), size(n) {}
+    template <class Carve, class... Args>
+    static size_t measure(Carve carve, Args... args) {  // the bytes carve(ws, args...) takes; hands out no memory
+        Workspace ws(nullptr, 0);
+        carve(ws, args...);
+        return ws.off;
+    }
     template <typename T>
     T* take(size_t count) {
-        size_t bytes = align_up(count * sizeof(T));
-        if (!base || off + bytes > size) {
-            ok = false;
-            off += bytes;
-            return nullptr;
-        }
-        T* r = (T*)(base + off);
-        off += bytes;
-        return r;
+        const size_t at = off;
+        off += (count * sizeof(T) + 255) / 256 * 256;
+        ok = ok && base && off <= size;
+        return ok ? (T*)(base + at) : nullptr;
     }
 };
 

@@ -366,9 +366,7 @@ extern "C" size_t o3dml_pp_detect_workspace_bytes(int64_t batch, int64_t height,
                                                   int num_classes, int64_t nms_pre) {
     if (detect_check(batch, height, width, num_anchors, num_classes, nms_pre) != O3DML_OK) return 0;
     const int64_t N = height * width * num_anchors, K = std::min<int64_t>(nms_pre, N);
-    Workspace ws(nullptr, 0);
-    carve(ws, batch, N, K, num_classes, N > nms_pre);
-    return ws.off + 256;
+    return Workspace::measure(carve, batch, N, K, num_classes, N > nms_pre);
 }
 
 extern "C" int o3dml_pp_detect(const float* cls, int64_t cls_batch_stride, const float* reg, int64_t reg_batch_stride,
@@ -379,8 +377,6 @@ extern "C" int o3dml_pp_detect(const float* cls, int64_t cls_batch_stride, const
     const int rc = detect_check(batch, height, width, num_anchors, num_classes, nms_pre);
     if (rc != O3DML_OK) return rc;
     if (batch == 0) return O3DML_OK;
-    O3DML_CHECK(cls && reg && dir && anchors && out_boxes && out_scores && out_labels && d_counts,
-                "pp_detect: null input");
     cudaStream_t st = (cudaStream_t)stream;
     const int B = (int)batch, C = num_classes, A = num_anchors, HW = (int)(height * width);
     const int64_t N = (int64_t)HW * A;
@@ -391,7 +387,9 @@ extern "C" int o3dml_pp_detect(const float* cls, int64_t cls_batch_stride, const
     const int words_max = (K + 63) / 64;
     Workspace ws(workspace, workspace_bytes);
     const DetectBuffers d = carve(ws, B, N, K, C, select);
-    if (!ws.ok) O3DML_FAIL(O3DML_ERR_WORKSPACE, "pp_detect: workspace too small (%zu needed)", ws.off);
+    O3DML_CHECK_WORKSPACE(ws, "pp_detect");
+    O3DML_CHECK(cls && reg && dir && anchors && out_boxes && out_scores && out_labels && d_counts,
+                "pp_detect: null input");
     if (select) {
         O3DML_CUDA(cudaMemsetAsync(d.hist, 0, ((size_t)kPasses * B * kBins + B) * sizeof(uint32_t), st));
         const dim3 grid((unsigned)ceil_div<int64_t>(N, kSelRows), (unsigned)B);

@@ -81,10 +81,12 @@ __global__ void grid_bbox_kernel(const float* __restrict__ pts, int64_t n,
     }
 }
 
+// cells grid_setup_kernel allows a batch item of nb points: the host sizes the cell arrays from it, without a sync
+__host__ __device__ inline double grid_cell_cap(int64_t nb) { return 2.0 * (double)nb + 64.0; }
+
 // One thread per batch item picks the cell size.  fixed_cs > 0: radius search (cs = radius);
 // otherwise the k-NN heuristic: the radius expected to hold k points at the mean surface /
-// volume density of the bounding box.  Cells per item are capped at 2*n_b + 64 so that the
-// caller can size the cell arrays without a device->host sync.
+// volume density of the bounding box.  The cell size then grows until the item's cells fit grid_cell_cap.
 __global__ void grid_setup_kernel(const unsigned* __restrict__ bbox,
                                   const int64_t* __restrict__ splits, int batch, float fixed_cs,
                                   int k, GridInfo* __restrict__ info, uint32_t* total_cells) {
@@ -112,7 +114,7 @@ __global__ void grid_setup_kernel(const unsigned* __restrict__ bbox,
                 float cs3 = cbrtf(kk * e0 * e1 * e2 / (4.18879f * (float)nb));
                 cs = fmaxf(fmaxf(cs2, cs3), 1e-6f);
             }
-            const double cap = 2.0 * (double)nb + 64.0;
+            const double cap = grid_cell_cap(nb);
             for (int it = 0; it < 64; ++it) {
                 double c = (floor((double)e[0] / cs) + 1) * (floor((double)e[1] / cs) + 1) *
                            (floor((double)e[2] / cs) + 1);
@@ -344,41 +346,52 @@ struct GridBuf {
     unsigned* bbox; GridInfo* info; uint32_t* total_cells;
     uint32_t *cell_of, *cell_start, *cursor; float4* sorted;
     uint32_t *qcell, *qstart, *qcursor, *order;
-    char* scan_tmp;
+    void* scan_tmp;
     int64_t max_cells;
 };
 
-static size_t grid_bytes(int64_t np, int64_t nq, int64_t batch) {
-    int64_t max_cells = 2 * np + 128 * batch + 64;
-    size_t s = 0;
-    s += align_up(batch * 6 * 4) + align_up(batch * sizeof(GridInfo)) + align_up(64);
-    s += align_up(np * 4) + 2 * align_up((max_cells + 1) * 4) + align_up(np * 16);
-    s += align_up(nq * 4) + 2 * align_up((max_cells + 1) * 4) + align_up(nq * 4);
-    s += scan_temp_bytes(max_cells + 1);
-    return s + 4096;
+// cells of a whole batch: the items' caps add up to 2*np + 64*batch, plus a margin of one cap(0) per item and one more
+static int64_t grid_max_cells(int64_t np, int64_t batch) {
+    return (int64_t)grid_cell_cap(np) + 2 * batch * (int64_t)grid_cell_cap(0);
 }
 
-static int grid_carve(Workspace& ws, int64_t np, int64_t nq, int64_t batch, GridBuf* g) {
-    g->max_cells = 2 * np + 128 * batch + 64;
-    g->bbox = ws.take<unsigned>(batch * 6);
-    g->info = ws.take<GridInfo>(batch);
-    g->total_cells = ws.take<uint32_t>(16);
-    g->cell_of = ws.take<uint32_t>(np);
-    g->cell_start = ws.take<uint32_t>(g->max_cells + 1);
-    g->cursor = ws.take<uint32_t>(g->max_cells + 1);
-    g->sorted = ws.take<float4>(np);
-    g->qcell = ws.take<uint32_t>(nq);
-    g->qstart = ws.take<uint32_t>(g->max_cells + 1);
-    g->qcursor = ws.take<uint32_t>(g->max_cells + 1);
-    g->order = ws.take<uint32_t>(nq);
-    g->scan_tmp = ws.take<char>(scan_temp_bytes(g->max_cells + 1));
-    return ws.ok ? 0 : 1;
+static GridBuf grid_carve(Workspace& ws, int64_t np, int64_t nq, int64_t batch) {
+    GridBuf g;
+    g.max_cells = grid_max_cells(np, batch);
+    g.bbox = ws.take<unsigned>(batch * 6);
+    g.info = ws.take<GridInfo>(batch);
+    g.total_cells = ws.take<uint32_t>(16);
+    g.cell_of = ws.take<uint32_t>(np);
+    g.cell_start = ws.take<uint32_t>(g.max_cells + 1);
+    g.cursor = ws.take<uint32_t>(g.max_cells + 1);
+    g.sorted = ws.take<float4>(np);
+    g.qcell = ws.take<uint32_t>(nq);
+    g.qstart = ws.take<uint32_t>(g.max_cells + 1);
+    g.qcursor = ws.take<uint32_t>(g.max_cells + 1);
+    g.order = ws.take<uint32_t>(nq);
+    g.scan_tmp = scan_carve(ws, g.max_cells + 1);
+    return g;
+}
+
+// Layout of the fixed-radius search: the grid that o3dml_radius_count builds and o3dml_radius_fill reads back, then
+// the per-query counts and their scan.  Both entries carve it, so that fill finds the grid where count left it.
+struct RadiusBuf : GridBuf {
+    uint32_t *counts, *total;
+    void* count_scan_tmp;
+};
+
+static RadiusBuf radius_carve(Workspace& ws, int64_t np, int64_t nq, int64_t batch) {
+    RadiusBuf r{grid_carve(ws, np, nq, batch)};
+    r.counts = ws.take<uint32_t>(nq + 1);
+    r.count_scan_tmp = scan_carve(ws, nq + 1);
+    r.total = ws.take<uint32_t>(16);
+    return r;
 }
 
 // builds the support grid and the cell-ordered query permutation
 static int grid_build(const float* pts, int64_t np, const int64_t* psplits, const float* q,
                       int64_t nq, const int64_t* qsplits, int batch, float fixed_cs, int k,
-                      GridBuf& g, cudaStream_t st) {
+                      const GridBuf& g, cudaStream_t st) {
     const int T = 256;
     const unsigned pb = (unsigned)ceil_div<int64_t>(np, T);
     O3DML_CUDA(launch<grid_init_kernel>(ceil_div(batch * 6, T), T, 0, st, g.bbox, batch));
@@ -407,7 +420,7 @@ static int grid_build(const float* pts, int64_t np, const int64_t* psplits, cons
 using namespace o3dml;
 
 extern "C" size_t o3dml_knn_workspace_bytes(int64_t num_points, int64_t num_queries, int64_t batch) {
-    return grid_bytes(num_points, num_queries, batch);
+    return Workspace::measure(grid_carve, num_points, num_queries, batch);
 }
 
 extern "C" int o3dml_knn_search(const float* points, int64_t num_points,
@@ -422,9 +435,8 @@ extern "C" int o3dml_knn_search(const float* points, int64_t num_points,
     O3DML_CHECK(num_points < ((int64_t)1 << 30), "knn_search: too many points");
     if (num_queries == 0) return O3DML_OK;
     Workspace ws(workspace, workspace_bytes);
-    GridBuf g;
-    if (grid_carve(ws, num_points, num_queries, batch, &g))
-        O3DML_FAIL(O3DML_ERR_WORKSPACE, "knn_search: workspace too small (%zu needed)", ws.off);
+    const GridBuf g = grid_carve(ws, num_points, num_queries, batch);
+    O3DML_CHECK_WORKSPACE(ws, "knn_search");
     int rc = grid_build(points, num_points, points_row_splits, queries, num_queries,
                         queries_row_splits, (int)batch, 0.f, k, g, st);
     if (rc) return rc;
@@ -444,8 +456,7 @@ extern "C" int o3dml_knn_search(const float* points, int64_t num_points,
 
 extern "C" size_t o3dml_radius_workspace_bytes(int64_t num_points, int64_t num_queries,
                                                int64_t batch) {
-    return grid_bytes(num_points, num_queries, batch) + align_up((num_queries + 1) * 4) +
-           scan_temp_bytes(num_queries + 1) + 1024;
+    return Workspace::measure(radius_carve, num_points, num_queries, batch);
 }
 
 // Phase 1: builds the grid (kept in the workspace for phase 2) and writes
@@ -461,13 +472,8 @@ extern "C" int o3dml_radius_count(const float* points, int64_t num_points,
     O3DML_CHECK(batch >= 1 && num_points >= 0 && num_queries >= 0, "fixed_radius_search: bad sizes");
     O3DML_CHECK(num_points < ((int64_t)1 << 30), "fixed_radius_search: too many points");
     Workspace ws(workspace, workspace_bytes);
-    GridBuf g;
-    int bad = grid_carve(ws, num_points, num_queries, batch, &g);
-    uint32_t* counts = ws.take<uint32_t>(num_queries + 1);
-    char* scan_tmp = ws.take<char>(scan_temp_bytes(num_queries + 1));
-    uint32_t* total = ws.take<uint32_t>(16);
-    if (bad || !ws.ok)
-        O3DML_FAIL(O3DML_ERR_WORKSPACE, "fixed_radius_search: workspace too small (%zu needed)", ws.off);
+    const RadiusBuf g = radius_carve(ws, num_points, num_queries, batch);
+    O3DML_CHECK_WORKSPACE(ws, "fixed_radius_search");
     if (num_queries == 0) {
         O3DML_CUDA(cudaMemsetAsync(neighbors_row_splits, 0, sizeof(int64_t), st));
         if (d_total) O3DML_CUDA(cudaMemsetAsync(d_total, 0, sizeof(int64_t), st));
@@ -478,10 +484,10 @@ extern "C" int o3dml_radius_count(const float* points, int64_t num_points,
     if (rc) return rc;
     const unsigned nb = (unsigned)ceil_div<int64_t>(num_queries, 128);
     O3DML_CUDA(launch<radius_kernel<0>>(nb, 128, 0, st, queries, num_queries, queries_row_splits, (int)batch, g.order,
-                                        g.info, g.cell_start, g.sorted, radius, counts, nullptr, nullptr, nullptr));
-    O3DML_CUDA(exclusive_scan_u32(counts, counts, num_queries, total, scan_tmp, st));
-    O3DML_CUDA(launch<widen_splits_kernel>((unsigned)ceil_div<int64_t>(num_queries, 256), 256, 0, st, counts,
-                                           num_queries, total, neighbors_row_splits, d_total));
+                                        g.info, g.cell_start, g.sorted, radius, g.counts, nullptr, nullptr, nullptr));
+    O3DML_CUDA(exclusive_scan_u32(g.counts, g.counts, num_queries, g.total, g.count_scan_tmp, st));
+    O3DML_CUDA(launch<widen_splits_kernel>((unsigned)ceil_div<int64_t>(num_queries, 256), 256, 0, st, g.counts,
+                                           num_queries, g.total, neighbors_row_splits, d_total));
     return O3DML_OK;
 }
 
@@ -494,9 +500,8 @@ extern "C" int o3dml_radius_fill(const float* queries, int64_t num_points, int64
     cudaStream_t st = (cudaStream_t)stream;
     if (num_queries == 0) return O3DML_OK;
     Workspace ws(workspace, workspace_bytes);
-    GridBuf g;
-    if (grid_carve(ws, num_points, num_queries, batch, &g))
-        O3DML_FAIL(O3DML_ERR_WORKSPACE, "fixed_radius_search: workspace too small");
+    const RadiusBuf g = radius_carve(ws, num_points, num_queries, batch);
+    O3DML_CHECK_WORKSPACE(ws, "fixed_radius_search");
     O3DML_CHECK(neighbors_index != nullptr && neighbors_distance2 != nullptr,
                 "fixed_radius_search: index and distance outputs are both required");
     const unsigned nb = (unsigned)ceil_div<int64_t>(num_queries, 128);

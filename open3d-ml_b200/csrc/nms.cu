@@ -100,43 +100,40 @@ __global__ void nms_sweep_kernel(const uint64_t* __restrict__ mask, const uint32
     if (threadIdx.x == 0) *num_keep = kept;
 }
 
+// the sort of the scores, then the [n][words] suppression bit matrix
+static std::pair<RadixSortBufs, uint64_t*> nms_carve(Workspace& ws, int64_t n) {
+    n = n > 0 ? n : 1;
+    const RadixSortBufs sort = radix_sort_carve(ws, n);
+    return {sort, ws.take<uint64_t>((size_t)n * ceil_div<int64_t>(n, 64))};
+}
+
 }  // namespace o3dml
 
 using namespace o3dml;
 
-static size_t nms_bytes(int64_t n) {
-    const int64_t words = ceil_div<int64_t>(n, 64);
-    return 2 * align_up(n * 8) + 2 * align_up(n * 4) + align_up(radix_sort_temp_bytes(n)) +
-           align_up((size_t)n * words * 8) + 1024;
-}
-
-extern "C" size_t o3dml_nms_workspace_bytes(int64_t num_boxes) { return nms_bytes(num_boxes > 0 ? num_boxes : 1); }
+extern "C" size_t o3dml_nms_workspace_bytes(int64_t num_boxes) { return Workspace::measure(nms_carve, num_boxes); }
 
 extern "C" int o3dml_nms(const float* boxes, const float* scores, int64_t num_boxes, float iou_threshold,
                          int64_t* keep_indices, int64_t* d_num_keep, void* workspace, size_t workspace_bytes,
                          void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
-    O3DML_CHECK(num_boxes >= 0 && d_num_keep, "nms: bad arguments");
+    O3DML_CHECK(num_boxes >= 0, "nms: bad arguments");
     if (num_boxes == 0) {
+        O3DML_CHECK(d_num_keep, "nms: bad arguments");
         O3DML_CUDA(cudaMemsetAsync(d_num_keep, 0, sizeof(int64_t), st));
         return O3DML_OK;
     }
-    O3DML_CHECK(boxes && scores && keep_indices, "nms: null input");
     O3DML_CHECK(num_boxes <= 65536, "nms: at most 65 536 boxes (the suppression matrix is N^2 / 8 bytes)");
     const int64_t n = num_boxes, words = ceil_div<int64_t>(n, 64);
     O3DML_CHECK(words * 8 <= 48 * 1024, "nms: too many boxes for the sweep kernel");
     Workspace ws(workspace, workspace_bytes);
-    uint64_t* ka = ws.take<uint64_t>(n);
-    uint64_t* kb = ws.take<uint64_t>(n);
-    uint32_t* va = ws.take<uint32_t>(n);
-    uint32_t* vb = ws.take<uint32_t>(n);
-    char* tmp = ws.take<char>(radix_sort_temp_bytes(n));
-    uint64_t* mask = ws.take<uint64_t>((size_t)n * words);
-    if (!ws.ok) O3DML_FAIL(O3DML_ERR_WORKSPACE, "nms: workspace too small (%zu needed)", ws.off);
-    O3DML_CUDA(launch<nms_keys_kernel>((unsigned)ceil_div<int64_t>(n, 256), 256, 0, st, scores, n, ka));
-    int in_b = 0;
-    O3DML_CUDA(radix_sort_pairs(ka, va, kb, vb, true, n, 32, tmp, st, &in_b));
-    const uint32_t* order = in_b ? vb : va;
+    auto [sort, mask] = nms_carve(ws, n);
+    O3DML_CHECK_WORKSPACE(ws, "nms");
+    O3DML_CHECK(d_num_keep, "nms: bad arguments");
+    O3DML_CHECK(boxes && scores && keep_indices, "nms: null input");
+    O3DML_CUDA(launch<nms_keys_kernel>((unsigned)ceil_div<int64_t>(n, 256), 256, 0, st, scores, n, sort.keys_a));
+    O3DML_CUDA(radix_sort_pairs(sort, true, n, 32, st));
+    const uint32_t* order = sort.vals_a;
     O3DML_CUDA(cudaMemsetAsync(mask, 0, (size_t)n * words * 8, st));
     dim3 grid((unsigned)words, (unsigned)words);
     O3DML_CUDA(launch<nms_mask_kernel>(grid, 64, 0, st, boxes, order, n, iou_threshold, mask, words));

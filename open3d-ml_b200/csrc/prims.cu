@@ -125,9 +125,8 @@ scan_lookback(const uint32_t* __restrict__ in, uint32_t* __restrict__ out, int64
     }
 }
 
-size_t scan_temp_bytes(int64_t n) {
-    int64_t tiles = ceil_div<int64_t>(n, SCAN_TILE);
-    return align_up((size_t)(tiles + 2) * sizeof(unsigned long long));
+void* scan_carve(Workspace& ws, int64_t n) {
+    return ws.take<unsigned long long>((size_t)ceil_div<int64_t>(n, SCAN_TILE) + 2);
 }
 
 // out may alias in.  total_out (device, optional) receives the grand total.
@@ -233,42 +232,36 @@ rs_scatter(const uint64_t* __restrict__ keys_in, const uint32_t* __restrict__ va
     }
 }
 
-size_t radix_sort_temp_bytes(int64_t n) {
-    int64_t nblk = ceil_div<int64_t>(n > 0 ? n : 1, RS_TILE);
-    return align_up((size_t)RS_BINS * nblk * sizeof(uint32_t)) + scan_temp_bytes(RS_BINS * nblk);
+RadixSortBufs radix_sort_carve(Workspace& ws, int64_t n) {
+    const int64_t bins = (int64_t)RS_BINS * ceil_div<int64_t>(n > 0 ? n : 1, RS_TILE);
+    RadixSortBufs b;
+    b.keys_a = ws.take<uint64_t>(n);
+    b.keys_b = ws.take<uint64_t>(n);
+    b.vals_a = ws.take<uint32_t>(n);
+    b.vals_b = ws.take<uint32_t>(n);
+    b.hist = ws.take<uint32_t>(bins);
+    b.scan_tmp = scan_carve(ws, bins);
+    return b;
 }
 
-// Stable sort of bits [0, num_bits) of the keys.  Ping-pongs between the (a)
-// and (b) buffers, starting from (a); *result_in_b tells where the sorted pairs
-// ended up.  vals_are_iota: ignore vals_a on input and use 0..n-1.
-cudaError_t radix_sort_pairs(uint64_t* keys_a, uint32_t* vals_a, uint64_t* keys_b, uint32_t* vals_b,
-                             bool vals_are_iota, int64_t n, int num_bits, void* temp,
-                             cudaStream_t st, int* result_in_b) {
-    *result_in_b = 0;
+// Stable sort of bits [0, num_bits) of the n pairs in (keys_a, vals_a), n <= the n that `b` was carved for.
+// vals_are_iota: ignore vals_a on input and use 0..n-1.  Each pass scatters from the (a) buffers into the (b) buffers
+// and then swaps the two in `b`, so that the sorted pairs end in (keys_a, vals_a).
+cudaError_t radix_sort_pairs(RadixSortBufs& b, bool vals_are_iota, int64_t n, int num_bits, cudaStream_t st) {
     if (n <= 0) return cudaSuccess;
     int nblk = (int)ceil_div<int64_t>(n, RS_TILE);
-    char* t = (char*)temp;
-    uint32_t* hist = (uint32_t*)t;
-    t += align_up((size_t)RS_BINS * nblk * sizeof(uint32_t));
-    void* scan_tmp = t;
-
     int passes = (num_bits + 7) / 8;
     if (passes < 1) passes = 1;
-    uint64_t* kin = keys_a;
-    uint32_t* vin = vals_a;
-    uint64_t* kout = keys_b;
-    uint32_t* vout = vals_b;
     for (int p = 0; p < passes; ++p) {
         int shift = 8 * p;
-        cudaError_t e = launch<rs_histogram>(nblk, RS_THREADS, 0, st, kin, n, shift, hist, nblk);
-        if (e == cudaSuccess) e = exclusive_scan_u32(hist, hist, (int64_t)RS_BINS * nblk, nullptr, scan_tmp, st);
+        cudaError_t e = launch<rs_histogram>(nblk, RS_THREADS, 0, st, b.keys_a, n, shift, b.hist, nblk);
+        if (e == cudaSuccess) e = exclusive_scan_u32(b.hist, b.hist, (int64_t)RS_BINS * nblk, nullptr, b.scan_tmp, st);
         if (e == cudaSuccess)
-            e = launch<rs_scatter>(nblk, RS_THREADS, 0, st, kin, (p == 0 && vals_are_iota) ? nullptr : vin, kout, vout,
-                                   n, shift, hist, nblk);
+            e = launch<rs_scatter>(nblk, RS_THREADS, 0, st, b.keys_a, (p == 0 && vals_are_iota) ? nullptr : b.vals_a,
+                                   b.keys_b, b.vals_b, n, shift, b.hist, nblk);
         if (e != cudaSuccess) return e;
-        uint64_t* tk = kin; kin = kout; kout = tk;
-        uint32_t* tv = vin; vin = vout; vout = tv;
-        *result_in_b ^= 1;
+        std::swap(b.keys_a, b.keys_b);
+        std::swap(b.vals_a, b.vals_b);
     }
     return cudaSuccess;
 }

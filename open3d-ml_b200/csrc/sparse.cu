@@ -83,13 +83,16 @@ __global__ void sparse_neighbors_kernel(const float* __restrict__ in_pos, int64_
     if (found != (int32_t)n && count) atomicAdd(&count[o], 1);
 }
 
+static RadixSortBufs sparse_carve(Workspace& ws, int64_t num_in) {
+    return radix_sort_carve(ws, num_in > 0 ? num_in : 1);
+}
+
 }  // namespace o3dml
 
 using namespace o3dml;
 
 extern "C" size_t o3dml_sparse_conv_workspace_bytes(int64_t num_in) {
-    const int64_t n = num_in > 0 ? num_in : 1;
-    return 2 * align_up(n * 8) + 2 * align_up(n * 4) + align_up(radix_sort_temp_bytes(n)) + 1024;
+    return Workspace::measure(sparse_carve, num_in);
 }
 
 extern "C" int o3dml_sparse_conv_neighbors(const float* in_positions, int64_t num_in, const float* out_positions,
@@ -112,28 +115,18 @@ extern "C" int o3dml_sparse_conv_neighbors(const float* in_positions, int64_t nu
     }
     g.transpose = transpose ? 1 : 0;
     if (num_out == 0) return O3DML_OK;
+    Workspace ws(workspace, workspace_bytes);
+    RadixSortBufs b = sparse_carve(ws, num_in);
+    O3DML_CHECK_WORKSPACE(ws, "sparse_conv");
     O3DML_CHECK(neighbors && out_positions, "sparse_conv: null output");
     if (neighbor_count) O3DML_CUDA(cudaMemsetAsync(neighbor_count, 0, sizeof(int32_t) * num_out, st));
-    Workspace ws(workspace, workspace_bytes);
-    const int64_t n = num_in > 0 ? num_in : 1;
-    uint64_t* ka = ws.take<uint64_t>(n);
-    uint64_t* kb = ws.take<uint64_t>(n);
-    uint32_t* va = ws.take<uint32_t>(n);
-    uint32_t* vb = ws.take<uint32_t>(n);
-    char* tmp = ws.take<char>(radix_sort_temp_bytes(n));
-    if (!ws.ok) O3DML_FAIL(O3DML_ERR_WORKSPACE, "sparse_conv: workspace too small (%zu needed)", ws.off);
-    const uint64_t* skeys = ka;
-    const uint32_t* perm = va;
     if (num_in > 0) {
         O3DML_CUDA(launch<sparse_keys_kernel>((unsigned)ceil_div<int64_t>(num_in, 256), 256, 0, st, in_positions, num_in,
-                                              g.inv_v, ka));
-        int in_b = 0;
-        O3DML_CUDA(radix_sort_pairs(ka, va, kb, vb, true, num_in, 63, tmp, st, &in_b));
-        skeys = in_b ? kb : ka;
-        perm = in_b ? vb : va;
+                                              g.inv_v, b.keys_a));
+        O3DML_CUDA(radix_sort_pairs(b, true, num_in, 63, st));
     }
     O3DML_CUDA(launch<sparse_neighbors_kernel>((unsigned)ceil_div<int64_t>(num_out * kc, 256), 256, 0, st, in_positions,
-                                               num_in, out_positions, num_out, skeys, perm, g, neighbors,
+                                               num_in, out_positions, num_out, b.keys_a, b.vals_a, g, neighbors,
                                                neighbor_count));
     return O3DML_OK;
 }

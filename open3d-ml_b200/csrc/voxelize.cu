@@ -323,20 +323,33 @@ pp_pfn_scatter_kernel(const float* __restrict__ pts, int ld, int C,
     }
 }
 
+struct VoxBuffers {
+    RadixSortBufs sort;
+    uint32_t *flags, *head_pos, *kept, *kept_excl, *batch_first, *batch_out;
+    void* scan_tmp;
+    uint32_t* scalars;  // [0]=n_valid [1]=m_all [2]=kept_total
+};
+
+static VoxBuffers vox_carve(Workspace& ws, int64_t n, int64_t batch) {
+    VoxBuffers b;
+    b.sort = radix_sort_carve(ws, n);
+    b.flags = ws.take<uint32_t>(n + 1);
+    b.head_pos = ws.take<uint32_t>(n + 1);
+    b.kept = ws.take<uint32_t>(n + 1);
+    b.kept_excl = ws.take<uint32_t>(n + 1);
+    b.scan_tmp = scan_carve(ws, n + 1);
+    b.batch_first = ws.take<uint32_t>(batch + 2);
+    b.batch_out = ws.take<uint32_t>(batch + 2);
+    b.scalars = ws.take<uint32_t>(16);
+    return b;
+}
+
 }  // namespace o3dml
 
 using namespace o3dml;
 
 extern "C" size_t o3dml_voxelize_workspace_bytes(int64_t n, int64_t batch) {
-    size_t s = 0;
-    s += 2 * align_up((size_t)n * 8);                    // keys a/b
-    s += 2 * align_up((size_t)n * 4);                    // vals a/b
-    s += radix_sort_temp_bytes(n);
-    s += 4 * align_up((size_t)(n + 1) * 4);              // flags/excl, head_pos, kept, kept_excl
-    s += scan_temp_bytes(n + 1);
-    s += 2 * align_up((size_t)(batch + 2) * 4);          // batch_first, batch_out
-    s += align_up(64);                                   // scalars
-    return s + 1024;
+    return Workspace::measure(vox_carve, n, batch);
 }
 
 extern "C" int o3dml_voxelize(const float* points, int64_t num_points, int point_stride,
@@ -365,20 +378,8 @@ extern "C" int o3dml_voxelize(const float* points, int64_t num_points, int point
         return O3DML_OK;
     }
     Workspace ws(workspace, workspace_bytes);
-    uint64_t* keys_a = ws.take<uint64_t>(n);
-    uint64_t* keys_b = ws.take<uint64_t>(n);
-    uint32_t* vals_a = ws.take<uint32_t>(n);
-    uint32_t* vals_b = ws.take<uint32_t>(n);
-    char* sort_tmp = ws.take<char>(radix_sort_temp_bytes(n));
-    uint32_t* flags = ws.take<uint32_t>(n + 1);
-    uint32_t* head_pos = ws.take<uint32_t>(n + 1);
-    uint32_t* kept = ws.take<uint32_t>(n + 1);
-    uint32_t* kept_excl = ws.take<uint32_t>(n + 1);
-    char* scan_tmp = ws.take<char>(scan_temp_bytes(n + 1));
-    uint32_t* batch_first = ws.take<uint32_t>(batch + 2);
-    uint32_t* batch_out = ws.take<uint32_t>(batch + 2);
-    uint32_t* scalars = ws.take<uint32_t>(16);  // [0]=n_valid [1]=m_all [2]=kept_total
-    if (!ws.ok) O3DML_FAIL(O3DML_ERR_WORKSPACE, "voxelize: workspace too small (%zu needed)", ws.off);
+    VoxBuffers b = vox_carve(ws, n, batch);
+    O3DML_CHECK_WORKSPACE(ws, "voxelize");
 
     const uint64_t invalid_key = (uint64_t)g.cells * (uint64_t)batch;  // sorts last
     int num_bits = 1;
@@ -386,27 +387,27 @@ extern "C" int o3dml_voxelize(const float* points, int64_t num_points, int point
 
     const int T = 256;
     const unsigned nb = (unsigned)ceil_div<int64_t>(n, T);
+    uint32_t* scalars = b.scalars;
     O3DML_CUDA(cudaMemsetAsync(scalars, 0, 16 * sizeof(uint32_t), st));
     O3DML_CUDA(launch<vox_hash_kernel>(nb, T, 0, st, points, point_stride, n, row_splits, (int)batch, g, invalid_key,
-                                       keys_a));
-    int in_b = 0;
-    O3DML_CUDA(radix_sort_pairs(keys_a, vals_a, keys_b, vals_b, true, n, num_bits, sort_tmp, st, &in_b));
-    const uint64_t* ks = in_b ? keys_b : keys_a;
-    const uint32_t* vs = in_b ? vals_b : vals_a;
-    O3DML_CUDA(launch<vox_heads_kernel>(nb, T, 0, st, ks, n, invalid_key, flags, &scalars[0]));
-    O3DML_CUDA(exclusive_scan_u32(flags, flags, n, &scalars[1], scan_tmp, st));
-    O3DML_CUDA(launch<vox_headpos_kernel>(nb, T, 0, st, flags, ks, n, invalid_key, head_pos));
-    O3DML_CUDA(launch<vox_batch_bounds_kernel>(1, 256, 0, st, ks, flags, &scalars[1], &scalars[0], (int)batch,
-                                               (uint64_t)g.cells, max_voxels, batch_first, batch_out,
+                                       b.sort.keys_a));
+    O3DML_CUDA(radix_sort_pairs(b.sort, true, n, num_bits, st));
+    const uint64_t* ks = b.sort.keys_a;
+    const uint32_t* vs = b.sort.vals_a;
+    O3DML_CUDA(launch<vox_heads_kernel>(nb, T, 0, st, ks, n, invalid_key, b.flags, &scalars[0]));
+    O3DML_CUDA(exclusive_scan_u32(b.flags, b.flags, n, &scalars[1], b.scan_tmp, st));
+    O3DML_CUDA(launch<vox_headpos_kernel>(nb, T, 0, st, b.flags, ks, n, invalid_key, b.head_pos));
+    O3DML_CUDA(launch<vox_batch_bounds_kernel>(1, 256, 0, st, ks, b.flags, &scalars[1], &scalars[0], (int)batch,
+                                               (uint64_t)g.cells, max_voxels, b.batch_first, b.batch_out,
                                                voxel_batch_splits));
-    O3DML_CUDA(launch<vox_counts_kernel>(nb, T, 0, st, head_pos, &scalars[1], &scalars[0], batch_first, (int)batch,
-                                         max_voxels, max_points_per_voxel, n, kept));
-    O3DML_CUDA(exclusive_scan_u32(kept, kept_excl, n, &scalars[2], scan_tmp, st));
-    O3DML_CUDA(launch<vox_emit_voxels_kernel>(nb, T, 0, st, ks, head_pos, &scalars[1], kept_excl, &scalars[2],
-                                              batch_first, batch_out, (int)batch, max_voxels, g, n, voxel_coords,
+    O3DML_CUDA(launch<vox_counts_kernel>(nb, T, 0, st, b.head_pos, &scalars[1], &scalars[0], b.batch_first, (int)batch,
+                                         max_voxels, max_points_per_voxel, n, b.kept));
+    O3DML_CUDA(exclusive_scan_u32(b.kept, b.kept_excl, n, &scalars[2], b.scan_tmp, st));
+    O3DML_CUDA(launch<vox_emit_voxels_kernel>(nb, T, 0, st, ks, b.head_pos, &scalars[1], b.kept_excl, &scalars[2],
+                                              b.batch_first, b.batch_out, (int)batch, max_voxels, g, n, voxel_coords,
                                               voxel_point_row_splits, voxel_batch_id, d_counts));
-    O3DML_CUDA(launch<vox_emit_points_kernel>(nb, T, 0, st, ks, vs, flags, head_pos, &scalars[0], kept, kept_excl, n,
-                                              voxel_point_indices));
+    O3DML_CUDA(launch<vox_emit_points_kernel>(nb, T, 0, st, ks, vs, b.flags, b.head_pos, &scalars[0], b.kept,
+                                              b.kept_excl, n, voxel_point_indices));
     return O3DML_OK;
 }
 

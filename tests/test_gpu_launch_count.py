@@ -11,12 +11,9 @@ import pytest
 import torch
 
 from open3d_ml_b200 import _lib as L
+from abi_cases import boxes, knn_case, nms_case, pp_detect_case, radius_case, rnd, sparse_conv_case, voxelize_case
 
 pytestmark = pytest.mark.gpu
-
-
-def rnd(*shape, seed=0):
-    return torch.randn(*shape, generator=torch.Generator().manual_seed(seed)).cuda()
 
 
 def counted_and_traced(call):
@@ -39,24 +36,12 @@ def counted_and_traced(call):
 
 # ---------------------------------------------------------------------------------------------------- the cases
 # Each builder allocates everything its call needs and returns the call: a closure that only enters the library, either
-# directly (returning the entry's status) or through the _lib wrapper that picks the dense kernel and checks.
+# directly (returning the entry's status) or through the _lib wrapper that picks the dense kernel and checks.  The entries
+# that take a workspace are built by abi_cases and run over a workspace of exactly the size their sizing function gives.
 
-def voxelize_inputs(n=500, batch=2, seed=1):
-    pts = (torch.rand(n, 4, generator=torch.Generator().manual_seed(seed)) * 4).cuda()
-    rs = torch.tensor([0, n // 2, n], dtype=torch.int64).cuda() if batch == 2 else torch.tensor([0, n]).cuda()
-    host = [np.full(3, v, np.float32) for v in (0.5, 0.0, 4.0)]      # voxel size, range min, range max
-    out = dict(coords=torch.empty(n, 3, dtype=torch.int32).cuda(), pidx=torch.empty(n, dtype=torch.int64).cuda(),
-               vrs=torch.empty(n + 1, dtype=torch.int64).cuda(), bsp=torch.empty(batch + 1, dtype=torch.int64).cuda(),
-               bid=torch.empty(n, dtype=torch.int32).cuda(), counts=torch.empty(2, dtype=torch.int64).cuda())
-    wsb = L.lib().o3dml_voxelize_workspace_bytes(n, batch)
-    ws = torch.empty(wsb, dtype=torch.uint8).cuda()
-
-    def call():
-        return L.lib().o3dml_voxelize(L.ptr(pts), n, pts.stride(0), L.ptr(rs), batch, host[0].ctypes.data,
-                                      host[1].ctypes.data, host[2].ctypes.data, 32, 1000, L.ptr(out["coords"]),
-                                      L.ptr(out["pidx"]), L.ptr(out["vrs"]), L.ptr(out["bsp"]), L.ptr(out["bid"]),
-                                      L.ptr(out["counts"]), L.ptr(ws), wsb, L.stream())
-    return pts, out, call
+def voxelize_inputs():
+    case = voxelize_case()
+    return case.pts, case.out, case.with_own_workspace()
 
 
 def case_voxelize():
@@ -72,41 +57,19 @@ def case_ragged_to_dense(dtype):
 
 
 def case_knn(num_points):
-    p, q = rnd(num_points, 3, seed=1), rnd(300, 3, seed=2)
-    ps = torch.tensor([0, num_points], dtype=torch.int64).cuda()
-    qs = torch.tensor([0, 300], dtype=torch.int64).cuda()
-    idx, d2 = torch.empty(300, 8, dtype=torch.int32).cuda(), torch.empty(300, 8).cuda()
-    wsb = L.lib().o3dml_knn_workspace_bytes(num_points, 300, 1)
-    ws = torch.empty(wsb, dtype=torch.uint8).cuda()
-    return lambda: L.lib().o3dml_knn_search(L.ptr(p), num_points, L.ptr(ps), L.ptr(q), 300, L.ptr(qs), 1, 8,
-                                            L.ptr(idx), 0, L.ptr(d2), L.ptr(ws), wsb, L.stream())
-
-
-def radius_inputs():
-    p, q = rnd(400, 3, seed=3), rnd(200, 3, seed=4)
-    ps = torch.tensor([0, 200, 400], dtype=torch.int64).cuda()
-    qs = torch.tensor([0, 100, 200], dtype=torch.int64).cuda()
-    nrs, total = torch.empty(201, dtype=torch.int64).cuda(), torch.zeros(1, dtype=torch.int64).cuda()
-    wsb = L.lib().o3dml_radius_workspace_bytes(400, 200, 2)
-    ws = torch.empty(wsb, dtype=torch.uint8).cuda()
-
-    def count():
-        return L.lib().o3dml_radius_count(L.ptr(p), 400, L.ptr(ps), L.ptr(q), 200, L.ptr(qs), 2, 0.8, L.ptr(nrs),
-                                          L.ptr(total), L.ptr(ws), wsb, L.stream())
-    return p, q, qs, nrs, total, ws, wsb, count
+    return knn_case(p_splits=(0, num_points)).with_own_workspace()
 
 
 def case_radius_count():
-    return radius_inputs()[-1]
+    return radius_case().with_own_workspace()
 
 
 def case_radius_fill():
-    p, q, qs, nrs, total, ws, wsb, count = radius_inputs()
-    L.check(count())
-    t = int(total.item())
-    idx, d2 = torch.empty(t, dtype=torch.int32).cuda(), torch.empty(t).cuda()
-    return lambda: L.lib().o3dml_radius_fill(L.ptr(q), 400, 200, L.ptr(qs), 2, 0.8, L.ptr(nrs), L.ptr(idx), L.ptr(d2),
-                                             L.ptr(ws), wsb, L.stream())
+    case = radius_case()
+    ws = torch.empty(case.wsb, dtype=torch.uint8).cuda()
+    L.check(case.run(L.ptr(ws), case.wsb))
+    case.prepare_fill()
+    return lambda: case.fill(L.ptr(ws), case.wsb)
 
 
 def case_voxel_reduce(labels):
@@ -129,15 +92,7 @@ def case_reduce_subarrays_sum():
 
 
 def case_sparse_conv_neighbors(num_in):
-    ip = torch.randint(0, 8, (num_in, 3), generator=torch.Generator().manual_seed(6)).float().cuda()
-    op = torch.randint(0, 8, (100, 3), generator=torch.Generator().manual_seed(7)).float().cuda()
-    off, ks = np.zeros(3, np.float32), np.full(3, 3, np.int32)
-    nbr, cnt = torch.empty(100, 27, dtype=torch.int32).cuda(), torch.empty(100, dtype=torch.int32).cuda()
-    wsb = L.lib().o3dml_sparse_conv_workspace_bytes(num_in)
-    ws = torch.empty(wsb, dtype=torch.uint8).cuda()
-    return lambda: L.lib().o3dml_sparse_conv_neighbors(L.ptr(ip), num_in, L.ptr(op), 100, 1.0, off.ctypes.data,
-                                                       ks.ctypes.data, 0, L.ptr(nbr), L.ptr(cnt), L.ptr(ws), wsb,
-                                                       L.stream())
+    return sparse_conv_case(num_in).with_own_workspace()
 
 
 def case_continuous_conv():
@@ -154,19 +109,8 @@ def case_continuous_conv():
                                                  L.ptr(rs), 0, 0, 0, 1, L.ptr(out), L.stream())
 
 
-def boxes(n, seed):
-    g = torch.Generator().manual_seed(seed)
-    xy = torch.rand(n, 2, generator=g) * 20
-    wh = torch.rand(n, 2, generator=g) * 3 + 0.5
-    return torch.cat([xy, xy + wh, torch.rand(n, 1, generator=g)], 1).cuda()
-
-
 def case_nms():
-    b, s = boxes(300, 12), rnd(300, seed=13)
-    keep, cnt = torch.empty(300, dtype=torch.int64).cuda(), torch.zeros(1, dtype=torch.int64).cuda()
-    wsb = L.lib().o3dml_nms_workspace_bytes(300)
-    ws = torch.empty(wsb, dtype=torch.uint8).cuda()
-    return lambda: L.lib().o3dml_nms(L.ptr(b), L.ptr(s), 300, 0.5, L.ptr(keep), L.ptr(cnt), L.ptr(ws), wsb, L.stream())
+    return nms_case(300).with_own_workspace()
 
 
 def case_iou_matrix():
@@ -176,20 +120,7 @@ def case_iou_matrix():
 
 
 def case_pp_detect(select):
-    B, H, W, A, C = 2, 6, 5, 2, 3
-    nms_pre = 20 if select else 100          # select: H * W * A = 60 rows > nms_pre
-    cls, reg, dr = rnd(B, A * C, H, W, seed=16), rnd(B, A * 7, H, W, seed=17) * 0.1, rnd(B, A * 2, H, W, seed=18)
-    g = torch.Generator().manual_seed(19)
-    anchors = torch.cat([torch.rand(H * W * A, 3, generator=g) * 20, torch.rand(H * W * A, 3, generator=g) + 1,
-                         torch.rand(H * W * A, 1, generator=g)], 1).cuda()
-    K = min(nms_pre, H * W * A)
-    bx, sc = torch.empty(B, C * K, 7).cuda(), torch.empty(B, C * K).cuda()
-    lab, cnt = torch.empty(B, C * K, dtype=torch.int64).cuda(), torch.empty(B, dtype=torch.int64).cuda()
-    wsb = L.lib().o3dml_pp_detect_workspace_bytes(B, H, W, A, C, nms_pre)
-    ws = torch.empty(wsb, dtype=torch.uint8).cuda()
-    return lambda: L.lib().o3dml_pp_detect(L.ptr(cls), cls.stride(0), L.ptr(reg), reg.stride(0), L.ptr(dr),
-                                           dr.stride(0), B, H, W, A, C, L.ptr(anchors), nms_pre, 0.1, 0.78,
-                                           L.ptr(bx), L.ptr(sc), L.ptr(lab), L.ptr(cnt), L.ptr(ws), wsb, L.stream())
+    return pp_detect_case(select).with_own_workspace()
 
 
 def case_pfn_scatter():
