@@ -127,6 +127,11 @@ def act_code(act):
     return {None: 0, "none": 0, "relu": 1, "leaky": 2}[act]
 
 
+def is64(index):
+    """The ABI's index-width flag of an int32 / int64 index tensor."""
+    return 1 if index.dtype == torch.int64 else 0
+
+
 def make_src(data, index=None, index_ld=1, out_rows_per_batch=0, src_rows_per_batch=0,
              channels=None, ld=None, rows=None):
     """data: 2-D float32 CUDA tensor [rows, C] (row stride ld)."""
@@ -138,7 +143,7 @@ def make_src(data, index=None, index_ld=1, out_rows_per_batch=0, src_rows_per_ba
     if index is not None:
         assert index.dtype in (torch.int64, torch.int32) and index.is_cuda
         s.index = index.data_ptr()
-        s.index_is64 = 1 if index.dtype == torch.int64 else 0
+        s.index_is64 = is64(index)
         s.index_ld = index_ld
     s.out_rows_per_batch = out_rows_per_batch
     s.src_rows_per_batch = src_rows_per_batch
@@ -231,6 +236,22 @@ class PackedWeight:
 
 def pack_linear(w_kc):
     return PackedWeight(w_kc)
+
+
+def host_state_dict(state_dict):
+    """A reference state_dict on the host: floating-point entries as fp32 copies, the others as they are."""
+    return {k: v.detach().to("cpu", torch.float32) if v.is_floating_point() else v.cpu()
+            for k, v in state_dict.items()}
+
+
+def fold_bn(sd, prefix, eps, bias=None):
+    """Eval-mode BatchNorm `prefix` after a layer with an optional `bias`, folded in float64 into fp32 (scale, shift):
+    s = w / sqrt(var + eps), t = b - s * mean [+ s * bias]."""
+    s = sd[prefix + ".weight"].double() / torch.sqrt(sd[prefix + ".running_var"].double() + eps)
+    t = sd[prefix + ".bias"].double() - s * sd[prefix + ".running_mean"].double()
+    if bias is not None:
+        t = t + s * bias.double()
+    return s.float(), t.float()
 
 
 TC_MIN_K = 64

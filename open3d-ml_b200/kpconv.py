@@ -75,8 +75,7 @@ class KPFCNNB200:
         self.enc, self.enc_skips, self.dec, self.dec_concats = _plan(cfg)
         if cfg.get("modulated", False) and any(b["deform"] for b in self.enc):
             raise RuntimeError("KPFCNNB200: modulated deformable KPConv is not supported")
-        sd = {k: v.detach().to("cpu", torch.float32) if v.is_floating_point() else v.cpu()
-              for k, v in state_dict.items()}
+        sd = L.host_state_dict(state_dict)
         w = self.w = {}
 
         def put(name, t):
@@ -84,10 +83,8 @@ class KPFCNNB200:
 
         def bn(p, use_bn):
             if use_bn:
-                q = p + ".batch_norm"
-                s = sd[q + ".weight"].double() / torch.sqrt(sd[q + ".running_var"].double() + BN_EPS)
-                t = sd[q + ".bias"].double() - s * sd[q + ".running_mean"].double()
-                put(p + ".s", s.float()), put(p + ".t", t.float())
+                s, t = L.fold_bn(sd, p + ".batch_norm", BN_EPS)
+                put(p + ".s", s), put(p + ".t", t)
             else:
                 put(p + ".t", sd[p + ".bias"])
 
@@ -132,15 +129,14 @@ class KPFCNNB200:
     def _lin(self, p, srcs, n, act, residual=None):
         wt = self.w[p + ".wt"]
         out = torch.empty((n, wt.shape[1]), dtype=torch.float32, device=self.device)
-        bnp = p + ".batch_norm" if (p + ".batch_norm.t") in self.w else p
-        return L.linear(srcs, wt, out, self.w.get(bnp + ".s"), self.w.get(bnp + ".t"),
+        return L.linear(srcs, wt, out, self.w.get(p + ".batch_norm.s"), self.w[p + ".batch_norm.t"],
                         residual=residual, act=act, slope=self.slope)
 
     def _kpconv(self, p, q_pts, s_pts, nidx, x, extent, bn_name, deform=False, probe=None):
         kp = self.w[p + ".kp"]
         K, cin = kp.shape[0], x.shape[1]
         nq = q_pts.shape[0]
-        is64 = 1 if nidx.dtype == torch.int64 else 0
+        is64 = L.is64(nidx)
         events = []
 
         def mark():
@@ -213,9 +209,8 @@ class KPFCNNB200:
                 if strided:
                     sc = torch.empty((q.shape[0], feats.shape[1]), dtype=torch.float32, device=dev)
                     L.check(L.lib().o3dml_gather_max(
-                        L.ptr(feats), feats.shape[0], feats.shape[1], feats.stride(0), L.ptr(nidx),
-                        1 if nidx.dtype == torch.int64 else 0, q.shape[0], nidx.shape[1], 0, 0, 1,
-                        L.ptr(sc), sc.stride(0), L.stream()))
+                        L.ptr(feats), feats.shape[0], feats.shape[1], feats.stride(0), L.ptr(nidx), L.is64(nidx),
+                        q.shape[0], nidx.shape[1], 0, 0, 1, L.ptr(sc), sc.stride(0), L.stream()))
                 if b["in_dim"] != b["out_dim"]:
                     sc = self._lin(p + ".unary_shortcut", [L.make_src(sc)], sc.shape[0], None)
                 x = self._lin(p + ".unary2", [L.make_src(y)], y.shape[0], "leaky", residual=sc)

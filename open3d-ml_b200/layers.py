@@ -33,6 +33,23 @@ def sparse_conv_neighbors(inp_positions, out_positions, voxel_size, offset, kern
     return nbr, cnt
 
 
+def pack_cell_groups(w):
+    """Kernel weights [cells, Cin, Cout] -> [(first cell, end cell, PackedWeight [cells * Cin, Cout])]: the cells
+    grouped three at a time, one gathered GEMM each."""
+    kc, cout = w.shape[0], w.shape[2]
+    return [(a, min(a + 3, kc),L.pack_linear(w[a:a + 3].reshape(-1, cout))) for a in range(0, kc, 3)]
+
+
+def contract_cells(feat, table, groups, out, bias=None):
+    """out [M, Cout] = sum over the cells c of feat[table[:, c]] @ W_c, + bias: one gathered GEMM per group of
+    pack_cell_groups, the first writing out (with the bias), the others adding onto it through their residual.
+    table int32 [M, cells]; an empty cell holds the shadow id feat.shape[0]."""
+    kc = table.shape[1]
+    for gi, (a, b, pw) in enumerate(groups):
+        srcs = [L.make_src(feat, index=table[:, c:], index_ld=kc) for c in range(a, b)]
+        L.linear(srcs, pw, out, None, None if gi else bias, residual=out if gi else None, act=None)
+
+
 class _SparseConvBase(torch.nn.Module):
     TRANSPOSE = False
 
@@ -58,15 +75,12 @@ class _SparseConvBase(torch.nn.Module):
         self._packed = None
 
     def _weights(self, dev):
-        """Kernel cells grouped three at a time into [3 * Cin, Cout] operands (PackedWeight), cached per version."""
+        """pack_cell_groups of the kernel, cached per version."""
         key = (self.kernel._version, self.kernel.data_ptr(), str(dev))
         if self._packed is None or self._packed[0] != key:
-            kc = int(np.prod(self.kernel_size))
-            w = self.kernel.detach().reshape(kc, self.in_channels, self.filters).float().cpu()
-            groups = [(c0, min(c0 + 3, kc)) for c0 in range(0, kc, 3)]
-            packs = [L.pack_linear(w[a:b].reshape((b - a) * self.in_channels, self.filters)) for a, b in groups]
-            self._packed = (key, groups, packs)
-        return self._packed[1], self._packed[2]
+            w = self.kernel.detach().reshape(-1, self.in_channels, self.filters).float().cpu()
+            self._packed = (key, pack_cell_groups(w))
+        return self._packed[1]
 
     def forward(self, inp_features, inp_positions, out_positions, voxel_size, inp_importance=None, **kwargs):
         if inp_importance is not None or kwargs.get("user_neighbors_index") is not None:
@@ -80,14 +94,10 @@ class _SparseConvBase(torch.nn.Module):
         vs = float(torch.as_tensor(voxel_size).reshape(-1)[0]) if not isinstance(voxel_size, (int, float)) else float(voxel_size)
         nbr, cnt = sparse_conv_neighbors(inp_positions, out_positions, vs, self.offset, self.kernel_size,
                                          self.TRANSPOSE, want_count=self.normalize)
-        kc = nbr.shape[1]
         out = torch.zeros((m, self.filters), dtype=torch.float32, device=feat.device)
         if m and n:
-            groups, packs = self._weights(feat.device)
             bias = self.bias.detach().to(feat.device, torch.float32) if self.use_bias and not self.normalize else None
-            for gi, ((a, b), pw) in enumerate(zip(groups, packs)):
-                srcs = [L.make_src(feat, index=nbr[:, c:], index_ld=kc) for c in range(a, b)]
-                L.linear(srcs, pw, out, None, bias if gi == 0 else None, residual=out if gi else None, act=None)
+            contract_cells(feat, nbr, self._weights(feat.device), out, bias)
         elif self.use_bias and not self.normalize:
             out += self.bias.detach().to(out.device)
         if self.normalize:

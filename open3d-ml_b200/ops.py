@@ -22,6 +22,7 @@ import numpy as np
 import torch
 
 from . import _lib as L
+from . import layers
 
 VoxelizeResult = collections.namedtuple(
     "VoxelizeResult",
@@ -129,6 +130,25 @@ def ragged_to_dense(values, row_splits, out_col_size, default_value, _add=0):
     return out if was_cuda else out.cpu()
 
 
+def knn_workspace_bytes(num_points, num_queries, batch):
+    return L.lib().o3dml_knn_workspace_bytes(num_points, num_queries, batch)
+
+
+def knn_search_raw(points, points_row_splits, queries, queries_row_splits, k, out_index, out_distance2=None,
+                   workspace=None):
+    """Sync-free form of knn_search: contiguous CUDA points / queries [N,3] with int64 row splits, dense outputs from
+    the caller (out_index int32 or int64 [Nq, k], out_distance2 float32 [Nq, k] or None), and a uint8 workspace of
+    at least knn_workspace_bytes, allocated here when none is given."""
+    batch = points_row_splits.numel() - 1
+    if workspace is None:
+        wsb = knn_workspace_bytes(points.shape[0], queries.shape[0], batch)
+        workspace = torch.empty((wsb,), dtype=torch.uint8, device=points.device)
+    L.check(L.lib().o3dml_knn_search(L.ptr(points), points.shape[0], L.ptr(points_row_splits), L.ptr(queries),
+                                     queries.shape[0], L.ptr(queries_row_splits), batch, int(k), L.ptr(out_index),
+                                     L.is64(out_index), L.ptr(out_distance2), L.ptr(workspace), workspace.numel(),
+                                     L.stream()))
+
+
 def knn_search(points, queries, k, points_row_splits=None, queries_row_splits=None,
                index_dtype=torch.int32, metric="L2", ignore_query_point=False,
                return_distances=False, allow_short=False):
@@ -155,12 +175,7 @@ def knn_search(points, queries, k, points_row_splits=None, queries_row_splits=No
                            "implemented)" % (short, k))
     idx = torch.empty((q.shape[0], k), dtype=index_dtype, device=dev)
     d2 = torch.empty((q.shape[0], k), dtype=torch.float32, device=dev) if return_distances else None
-    wsb = L.lib().o3dml_knn_workspace_bytes(p.shape[0], q.shape[0], batch)
-    ws = torch.empty((wsb,), dtype=torch.uint8, device=dev)
-    L.check(L.lib().o3dml_knn_search(L.ptr(p), p.shape[0], L.ptr(ps), L.ptr(q), q.shape[0],
-                                     L.ptr(qs), batch, k, L.ptr(idx),
-                                     1 if index_dtype == torch.int64 else 0, L.ptr(d2), L.ptr(ws),
-                                     wsb, L.stream()))
+    knn_search_raw(p, ps, q, qs, k, idx, d2)
     rs = torch.arange(0, (q.shape[0] + 1) * k, k, dtype=torch.int64, device=dev)
     out = KnnResult(idx.reshape(-1), rs,
                     d2.reshape(-1) if d2 is not None else torch.empty(0, device=dev))
@@ -414,9 +429,8 @@ def voxel_pooling(positions, features, voxel_size, position_fn="average", featur
         out = VoxelPoolingResult(pts.new_zeros((0, 3)), feats.new_zeros((0, feats.shape[1])))
         return out if was_cuda else VoxelPoolingResult(*(t.cpu() for t in out))
     vs = float(voxel_size)
-    mm = torch.stack([pts.amin(0), pts.amax(0)]).cpu().numpy().astype(np.float32)
-    origin = (np.floor((mm[0] / np.float32(vs)).astype(np.float32)) * np.float32(vs)).astype(np.float32)
-    coords, pidx, vrs, bsp, _, counts = voxelize_raw(pts, None, [vs, vs, vs], origin, mm[1], INT64_MAX, INT64_MAX)
+    origin, mx = _subsample_range(pts, vs)
+    coords, pidx, vrs, bsp, _, counts = voxelize_raw(pts, None, [vs, vs, vs], origin, mx, INT64_MAX, INT64_MAX)
     m = int(counts[0].item())
     if "nearest_neighbor" in (position_fn, feature_fn):
         # reorder every voxel's point list so that its first entry is the point nearest to the voxel centre
@@ -477,7 +491,7 @@ def continuous_conv(filters, out_positions, extents, offset, inp_positions, inp_
     L.check(L.lib().o3dml_continuous_conv(
         L.ptr(f), sx, sy, sz, cin, cout, L.ptr(op), op.shape[0], L.ptr(ext), 1 if ext.numel() > 1 else 0,
         off.ctypes.data, L.ptr(ip), L.ptr(feat), ip.shape[0], L.ptr(imp), L.ptr(idx),
-        1 if idx.dtype == torch.int64 else 0, L.ptr(nimp), L.ptr(rs), 1 if align_corners else 0,
+        L.is64(idx), L.ptr(nimp), L.ptr(rs), 1 if align_corners else 0,
         _CCONV_MAPPING[coordinate_mapping], 1 if normalize else 0, _CCONV_INTERP[interpolation], L.ptr(out), L.stream()))
     return out if was_cuda else out.cpu()
 
@@ -503,11 +517,7 @@ def sparse_conv(filters, inp_features, inp_importance, neighbors_index, neighbor
     table = torch.full((m, kc), feat.shape[0], dtype=torch.int32, device=feat.device)
     table[rows, _dev(neighbors_kernel_index).long()] = _dev(neighbors_index).to(torch.int32)
     out = torch.zeros((m, cout), dtype=torch.float32, device=feat.device)
-    for gi, c0 in enumerate(range(0, kc, 3)):
-        c1 = min(c0 + 3, kc)
-        pw = L.pack_linear(w[c0:c1].reshape((c1 - c0) * cin, cout))
-        srcs = [L.make_src(feat, index=table[:, c:], index_ld=kc) for c in range(c0, c1)]
-        L.linear(srcs, pw, out, None, None, residual=out if gi else None, act=None)
+    layers.contract_cells(feat, table, layers.pack_cell_groups(w), out)
     if normalize:
         out = out / lens.clamp_min(1).to(torch.float32).unsqueeze(1)
     return out if was_cuda else out.cpu()

@@ -8,7 +8,8 @@ forward, so the runner overlaps them: the inputs of batch k+1 cross PCIe on a
 copy stream while batch k computes, and the result of batch k returns on a second copy
 stream.  Every batch's inputs and results still cross the bus; nothing is cached.
 
-graph_replay() is the CUDA-graph capture and replay the models use for their launch-bound parts.
+graph_replay() is the CUDA-graph capture and replay the models use for their launch-bound parts, and BufferCache
+holds the device buffers that keep those parts allocation-stable.
 """
 import torch
 
@@ -17,11 +18,29 @@ from . import _lib as L
 GRAPH_CACHE_ENTRIES = 8
 
 
-def graph_replay(cache, key, thunk, device):
-    """Replays thunk() from a CUDA graph captured at its first call under `key` and returns a clone of its result (a
-    tensor or a tuple of tensors; the graph's own outputs are overwritten by the next replay).  thunk must be free of
-    host synchronisation and allocation-stable (cached buffers), and the key must name every address it reads.
-    `cache` is the caller's dict; it is cleared when it would exceed GRAPH_CACHE_ENTRIES graphs."""
+class BufferCache:
+    """A model's device buffers: get() makes a new tensor only for a new (name, shape, dtype), so that a buffer keeps
+    its address from call to call and a CUDA graph captured over it stays valid."""
+
+    def __init__(self, device):
+        self.device = device
+        self._bufs = {}
+
+    def get(self, name, shape, dtype=torch.float32):
+        key = (name, tuple(shape), dtype)
+        t = self._bufs.get(key)
+        if t is None:
+            t = self._bufs[key] = torch.empty(key[1], dtype=dtype, device=self.device)
+        return t
+
+
+def graph_replay(cache, name, tensors, thunk, device):
+    """Replays thunk() from a CUDA graph captured at its first call for `name` and the (address, shape, dtype) of
+    `tensors`, and returns a clone of its result (a tensor or a tuple of tensors; the graph's own outputs are
+    overwritten by the next replay).  thunk must be free of host synchronisation and allocation-stable (BufferCache),
+    and `tensors` must hold every input it reads.  `cache` is the caller's dict; it is cleared when it would exceed
+    GRAPH_CACHE_ENTRIES graphs."""
+    key = (name,) + tuple((t.data_ptr(), tuple(t.shape), t.dtype) for t in tensors)
     ent = cache.get(key)
     if ent is None:
         thunk()                          # sizes the cached buffers and sets kernel attributes, neither capturable

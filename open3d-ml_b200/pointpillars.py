@@ -23,15 +23,9 @@ import torch
 
 from . import _lib as L
 from . import ops
-from .pipeline import graph_replay
+from .pipeline import BufferCache, graph_replay
 
 BN_EPS = 1e-3  # point_pillars.py:409,648,724
-
-
-def _fold_bn(sd, prefix, eps=BN_EPS):
-    s = sd[prefix + ".weight"].double() / torch.sqrt(sd[prefix + ".running_var"].double() + eps)
-    t = sd[prefix + ".bias"].double() - s * sd[prefix + ".running_mean"].double()
-    return s.float(), t.float()
 
 
 class PointPillarsB200:
@@ -44,9 +38,9 @@ class PointPillarsB200:
         self.use_graph = bool(use_graph)
         self._graphs = {}
         self.device = dev = torch.device(device or "cuda")
+        self.buf = BufferCache(dev)
         self.cfg = cfg
-        sd = {k: v.detach().to("cpu", torch.float32) if v.is_floating_point() else v.cpu()
-              for k, v in state_dict.items()}
+        sd = L.host_state_dict(state_dict)
         w = self.w = {}
 
         def put(name, t):
@@ -59,7 +53,7 @@ class PointPillarsB200:
         self.pfn_out = lw.shape[0]
         self.point_channels = lw.shape[1] - 5
         put("pfn.wt", lw.t())
-        s, t = _fold_bn(sd, "voxel_encoder.pfn_layers.0.norm")
+        s, t = L.fold_bn(sd, "voxel_encoder.pfn_layers.0.norm", BN_EPS)
         put("pfn.s", s), put("pfn.t", t)
         # backbone
         self.blocks = []
@@ -70,7 +64,7 @@ class PointPillarsB200:
             for conv, bn, st in layers:
                 cw = sd[conv + ".weight"]  # [co, ci, 3, 3]
                 w[conv + ".wt"] = L.pack_linear(cw.permute(2, 3, 1, 0).reshape(9 * cw.shape[1], cw.shape[0]))
-                s, t = _fold_bn(sd, bn)
+                s, t = L.fold_bn(sd, bn, BN_EPS)
                 put(conv + ".s", s), put(conv + ".t", t)
             self.blocks.append([(c, st, sd[c + ".weight"].shape[1], sd[c + ".weight"].shape[0])
                                 for c, _, st in layers])
@@ -83,7 +77,7 @@ class PointPillarsB200:
                 raise RuntimeError("PointPillarsB200: deblock kernel must equal its stride")
             co = dw.shape[1]
             w[p + ".wt"] = L.pack_linear(dw.permute(0, 2, 3, 1).reshape(dw.shape[0], us * us * co))
-            s, t = _fold_bn(sd, p + ".1")
+            s, t = L.fold_bn(sd, p + ".1", BN_EPS)
             put(p + ".s", s.repeat(us * us)), put(p + ".t", t.repeat(us * us))
             self.deblocks.append((p, us, dw.shape[0], co))
         self.neck_channels = sum(d[3] for d in self.deblocks)
@@ -99,16 +93,7 @@ class PointPillarsB200:
         self.x_off = float(self.vx / 2 + r[0])
         self.y_off = float(self.vy / 2 + r[1])
         self.ny, self.nx = cfg["output_shape"]
-        self._buf = {}
         self._anchors = {}
-
-    def _get(self, name, shape, dtype=torch.float32):
-        key = (name, tuple(shape), dtype)
-        t = self._buf.get(key)
-        if t is None:
-            t = torch.empty(shape, dtype=dtype, device=self.device)
-            self._buf[key] = t
-        return t
 
     # ------------------------------------------------------------- front end
     def front_end(self, frames, want_feat=False, canvas_nchw=False):
@@ -125,7 +110,7 @@ class PointPillarsB200:
             cfg["max_voxels"], want_batch_id=True)
         C = self.pfn_out
         shape = (B, C, self.ny, self.nx) if canvas_nchw else (B, self.ny, self.nx, C)
-        canvas = self._get("canvas", shape)
+        canvas = self.buf.get("canvas", shape)
         canvas.zero_()
         bound = min(pts.shape[0], B * int(cfg["max_voxels"]))
         feat = torch.empty((bound, C), dtype=torch.float32, device=dev) if want_feat else None
@@ -141,7 +126,7 @@ class PointPillarsB200:
     # ---------------------------------------------------------- dense layers
     def _conv(self, x, B, H, W, name, stride, cin, cout):
         OH, OW = (H - 1) // stride + 1, (W - 1) // stride + 1
-        out = self._get(name, (B, OH, OW, cout))
+        out = self.buf.get(name, (B, OH, OW, cout))
         L.conv3x3(x, self.w[name + ".wt"], out, self.w[name + ".s"], self.w[name + ".t"], stride, act="relu")
         return out, OH, OW
 
@@ -149,8 +134,7 @@ class PointPillarsB200:
         """SECOND + SECONDFPN + Anchor3DHead on the NHWC canvas -> (cls, reg, dir) in NCHW."""
         if not self.use_graph:
             return self._bnh_eager(canvas)
-        key = (canvas.data_ptr(), tuple(canvas.shape))
-        return graph_replay(self._graphs, key, lambda: self._bnh_eager(canvas), self.device)
+        return graph_replay(self._graphs, "backbone_neck_head", [canvas], lambda: self._bnh_eager(canvas), self.device)
 
     def _bnh_eager(self, canvas):
         B, H, W = canvas.shape[0], canvas.shape[1], canvas.shape[2]
@@ -162,7 +146,7 @@ class PointPillarsB200:
             feats.append((x, H, W))
         us0 = self.deblocks[0][1]
         OH, OW = feats[0][1] * us0, feats[0][2] * us0
-        neck = self._get("neck", (B, OH, OW, self.neck_channels))
+        neck = self.buf.get("neck", (B, OH, OW, self.neck_channels))
         off = 0
         for (p, us, cin, co), (f, h, w_) in zip(self.deblocks, feats):
             if h * us != OH or w_ * us != OW:

@@ -18,7 +18,8 @@ indices); the output is ``[B, N, num_classes]`` like the reference.
 import torch
 
 from . import _lib as L
-from .pipeline import graph_replay
+from . import ops
+from .pipeline import BufferCache, graph_replay
 
 BN_EPS = 1e-6  # randlanet.py:77,499
 # d_out values served by the wgmma kernel (lfa_tc.cu).  d = 16 stays on the FP32 SIMT kernel with its weights in the
@@ -26,14 +27,6 @@ BN_EPS = 1e-6  # randlanet.py:77,499
 # d = 512 (fifth encoder of the 5-level configs, a few hundred points) runs on the tiled SIMT kernel (lfa.cu).
 TC_DIMS = (32, 64, 128, 256)
 SUPPORTED_DIMS = (16, 32, 64, 128, 256, 512)
-
-
-def _fold_bn(sd, prefix, bias=None, eps=BN_EPS):
-    s = sd[prefix + ".weight"].double() / torch.sqrt(sd[prefix + ".running_var"].double() + eps)
-    t = sd[prefix + ".bias"].double() - s * sd[prefix + ".running_mean"].double()
-    if bias is not None:
-        t = t + s * bias.double()
-    return s.float(), t.float()
 
 
 class RandLANetB200:
@@ -45,10 +38,10 @@ class RandLANetB200:
         self._graphs = {}
         self._splits = {}
         self.device = torch.device(device or "cuda")
+        self.buf = BufferCache(self.device)
         self.num_layers = num_layers
         self.k = num_neighbors
-        sd = {k: v.detach().to("cpu", torch.float32) if v.is_floating_point() else v.cpu()
-              for k, v in state_dict.items()}
+        sd = L.host_state_dict(state_dict)
         self.w = {}
         dev = self.device
 
@@ -63,14 +56,14 @@ class RandLANetB200:
             else:        # dense layer: fp32 + tensor-core operand image
                 self.w[p + ".wt"] = L.pack_linear(w)
             if bn:
-                s, t = _fold_bn(sd, p + ".batch_norm", sd[p + ".conv.bias"])
+                s, t = L.fold_bn(sd, p + ".batch_norm", BN_EPS, sd[p + ".conv.bias"])
                 put(p + ".s", s)
                 put(p + ".t", t)
             else:
                 put(p + ".t", sd[p + ".conv.bias"])
 
         self.w["fc0.wt"] = L.pack_linear(sd["fc0.weight"].t())
-        s, t = _fold_bn(sd, "bn0", sd["fc0.bias"])
+        s, t = L.fold_bn(sd, "bn0", BN_EPS, sd["fc0.bias"])
         put("fc0.s", s), put("fc0.t", t)
         self.d_out = []
         for i in range(num_layers):
@@ -101,8 +94,8 @@ class RandLANetB200:
                                                   ".lse2.mlp.s", ".lse2.mlp.t")),
                         self.w["%s.%s.score.wt" % (p, pool)], self.w["%s.%s.score.b" % (p, pool)])
             # mlp2 + shortcut as ONE gemm over [p2 | feat] with the BN scales folded into the rows
-            s2, t2 = _fold_bn(sd, p + ".mlp2.batch_norm", sd[p + ".mlp2.conv.bias"])
-            ss, ts = _fold_bn(sd, p + ".shortcut.batch_norm", sd[p + ".shortcut.conv.bias"])
+            s2, t2 = L.fold_bn(sd, p + ".mlp2.batch_norm", BN_EPS, sd[p + ".mlp2.conv.bias"])
+            ss, ts = L.fold_bn(sd, p + ".shortcut.batch_norm", BN_EPS, sd[p + ".shortcut.conv.bias"])
             w2 = sd[p + ".mlp2.conv.weight"][:, :, 0, 0] * s2[:, None]
             ws = sd[p + ".shortcut.conv.weight"][:, :, 0, 0] * ss[:, None]
             self.w[p + ".out.wt"] = L.pack_linear(torch.cat([w2.t(), ws.t()], 0))
@@ -115,7 +108,6 @@ class RandLANetB200:
         shared_mlp("fc1.3", bn=False)
         self.num_classes = sd["fc1.3.conv.weight"].shape[0]
         self.in_channels = sd["fc0.weight"].shape[1]
-        self._buf = {}
         # ---- fused tail (rl_tail.cu): last decoder layer + fc1 stack in one kernel
         self.tail = None
         pl = "decoder.%d" % (num_layers - 1)
@@ -127,19 +119,10 @@ class RandLANetB200:
             img = L.pack_tail_image([wd, w0, w1, w3], [32, 64, 32, 32]).to(dev)
             sc, sh = torch.ones(4, 64), torch.zeros(4, 64)
             for li, name in enumerate((pl, "fc1.0", "fc1.1")):
-                s_, t_ = _fold_bn(sd, name + ".batch_norm", sd[name + ".conv.bias"])
+                s_, t_ = L.fold_bn(sd, name + ".batch_norm", BN_EPS, sd[name + ".conv.bias"])
                 sc[li, :s_.numel()], sh[li, :t_.numel()] = s_, t_
             sh[3, :self.num_classes] = sd["fc1.3.conv.bias"]
             self.tail = (img, sc.contiguous(), sh.contiguous())
-
-    # ------------------------------------------------------------------ buffers
-    def _get(self, name, rows, ch):
-        key = (name, rows, ch)
-        t = self._buf.get(key)
-        if t is None:
-            t = torch.empty((rows, ch), dtype=torch.float32, device=self.device)
-            self._buf[key] = t
-        return t
 
     def _mlp(self, p, srcs, out, act="leaky", slope=0.2):
         return L.linear(srcs, self.w[p + ".wt"], out, self.w.get(p + ".s"), self.w[p + ".t"],
@@ -150,7 +133,7 @@ class RandLANetB200:
         pool = "pool1" if stage == 1 else "pool2"
         if d in TC_DIMS:
             L.check(L.lib().o3dml_randla_lfa_pool_tc(
-                stage, d, L.ptr(coords), L.ptr(nidx), 1 if nidx.dtype == torch.int64 else 0, self.k,
+                stage, d, L.ptr(coords), L.ptr(nidx), L.is64(nidx), self.k,
                 L.ptr(feat), B, N, L.ptr(w[p + ".lse1.mlp.wt"]), L.ptr(w[p + ".lse1.mlp.s"]),
                 L.ptr(w[p + ".lse1.mlp.t"]),
                 L.ptr(w.get(p + ".lse2.mlp.img")) if stage == 2 else None,
@@ -161,11 +144,11 @@ class RandLANetB200:
             return
         if d == 16:
             L.check(L.lib().o3dml_randla_lfa16_pool(
-                stage, L.ptr(coords), L.ptr(nidx), 1 if nidx.dtype == torch.int64 else 0, self.k,
+                stage, L.ptr(coords), L.ptr(nidx), L.is64(nidx), self.k,
                 L.ptr(feat), B, N, w["%s.lfa16.%d" % (p, stage)].data_ptr(), L.ptr(agg), L.stream()))
             return
         L.check(L.lib().o3dml_randla_lfa_pool(
-            stage, d, L.ptr(coords), L.ptr(nidx), 1 if nidx.dtype == torch.int64 else 0, self.k,
+            stage, d, L.ptr(coords), L.ptr(nidx), L.is64(nidx), self.k,
             L.ptr(feat), B, N, L.ptr(w[p + ".lse1.mlp.wt"]), L.ptr(w[p + ".lse1.mlp.s"]),
             L.ptr(w[p + ".lse1.mlp.t"]),
             L.ptr(w[p + ".lse2.mlp.wt"]) if stage == 2 else None,
@@ -191,7 +174,7 @@ class RandLANetB200:
         inp = self.to_device(inputs)
         feats = inp["features"]
         B, N0, cin = feats.shape
-        x = self._get("fc0", B * N0, self.w["fc0.wt"].shape[1])
+        x = self.buf.get("fc0", (B * N0, self.w["fc0.wt"].shape[1]))
         L.linear([L.make_src(feats.view(B * N0, cin))], self.w["fc0.wt"], x, self.w["fc0.s"],
                  self.w["fc0.t"], act="leaky", slope=0.2)
         skips = []
@@ -204,14 +187,14 @@ class RandLANetB200:
             N = coords.shape[1]
             rows = B * N
             cflat = coords.view(rows, 3)
-            f1 = self._mlp(p + ".mlp1", [L.make_src(x)], self._get(p + ".f1", rows, h))
-            agg1 = self._get(p + ".agg1", rows, d)
+            f1 = self._mlp(p + ".mlp1", [L.make_src(x)], self.buf.get(p + ".f1", (rows, h)))
+            agg1 = self.buf.get(p + ".agg1", (rows, d))
             self._lfa_pool(1, d, cflat, nidx, f1, B, N, p, agg1)
-            p1 = self._mlp(p + ".pool1.mlp", [L.make_src(agg1)], self._get(p + ".p1", rows, h))
-            agg2 = self._get(p + ".agg2", rows, d)
+            p1 = self._mlp(p + ".pool1.mlp", [L.make_src(agg1)], self.buf.get(p + ".p1", (rows, h)))
+            agg2 = self.buf.get(p + ".agg2", (rows, d))
             self._lfa_pool(2, d, cflat, nidx, p1, B, N, p, agg2)
-            p2 = self._mlp(p + ".pool2.mlp", [L.make_src(agg2)], self._get(p + ".p2", rows, d))
-            enc = self._get(p + ".enc", rows, 2 * d)
+            p2 = self._mlp(p + ".pool2.mlp", [L.make_src(agg2)], self.buf.get(p + ".p2", (rows, d)))
+            enc = self.buf.get(p + ".enc", (rows, 2 * d))
             L.linear([L.make_src(p2), L.make_src(x)], self.w[p + ".out.wt"], enc, None,
                      self.w[p + ".out.t"], act="leaky", slope=0.01)
             if taps is not None:
@@ -219,9 +202,8 @@ class RandLANetB200:
                 taps[p] = enc.view(B, N, 2 * d)
             sub = inp["sub_idx"][i]
             ns = sub.shape[1]
-            pooled = self._get(p + ".sub", B * ns, 2 * d)
-            L.check(L.lib().o3dml_gather_max(L.ptr(enc), rows, 2 * d, 2 * d, L.ptr(sub),
-                                             1 if sub.dtype == torch.int64 else 0, B * ns,
+            pooled = self.buf.get(p + ".sub", (B * ns, 2 * d))
+            L.check(L.lib().o3dml_gather_max(L.ptr(enc), rows, 2 * d, 2 * d, L.ptr(sub), L.is64(sub), B * ns,
                                              sub.shape[2], ns, N, 0, L.ptr(pooled), 2 * d,
                                              L.stream()))
             if i == 0:
@@ -229,7 +211,7 @@ class RandLANetB200:
             skips.append((pooled, ns))
             x = pooled
         nlast = skips[-1][1]
-        x = self._mlp("mlp", [L.make_src(x)], self._get("mlp", x.shape[0], x.shape[1]))
+        x = self._mlp("mlp", [L.make_src(x)], self.buf.get("mlp", x.shape))
         ncoarse = nlast
         use_tail = self.tail is not None and taps is None
         for i in range(self.num_layers):
@@ -242,19 +224,19 @@ class RandLANetB200:
                 iv = interp.view(-1)
                 L.check(L.lib().o3dml_randla_tail(
                     L.ptr(skip), skip.stride(0), L.ptr(x), x.stride(0), x.shape[0], L.ptr(iv),
-                    1 if iv.dtype == torch.int64 else 0, nup, ncoarse, B * nup, L.ptr(img), sc.data_ptr(), sh.data_ptr(),
+                    L.is64(iv), nup, ncoarse, B * nup, L.ptr(img), sc.data_ptr(), sh.data_ptr(),
                     0.2, self.num_classes, L.ptr(logits), L.stream()))
                 return logits.view(B, N0, self.num_classes)
             cout = self.w[p + ".wt"].shape[1]
-            out = self._get(p, B * nup, cout)
+            out = self.buf.get(p, (B * nup, cout))
             self._mlp(p, [L.make_src(skip),
                           L.make_src(x, index=interp.view(-1), index_ld=1, out_rows_per_batch=nup,
                                      src_rows_per_batch=ncoarse)], out)
             if taps is not None:
                 taps[p] = out.view(B, nup, cout)
             x, ncoarse = out, nup
-        y = self._mlp("fc1.0", [L.make_src(x)], self._get("fc1.0", x.shape[0], 64))
-        y = self._mlp("fc1.1", [L.make_src(y)], self._get("fc1.1", x.shape[0], 32))
+        y = self._mlp("fc1.0", [L.make_src(x)], self.buf.get("fc1.0", (x.shape[0], 64)))
+        y = self._mlp("fc1.1", [L.make_src(y)], self.buf.get("fc1.1", (x.shape[0], 32)))
         logits = torch.empty((B * N0, self.num_classes), dtype=torch.float32, device=self.device)
         self._mlp("fc1.3", [L.make_src(y)], logits, act=None)
         return logits.view(B, N0, self.num_classes)
@@ -271,29 +253,11 @@ class RandLANetB200:
         return t
 
     def _knn(self, points, queries, k, ps, qs, name):
-        """o3dml_knn_search into cached int32 buffers (global row ids), no host synchronisation."""
-        nq = queries.shape[0]
-        idx = self._geti(name, nq, k)
-        batch = ps.numel() - 1
-        wsb = L.lib().o3dml_knn_workspace_bytes(points.shape[0], nq, batch)
-        ws = self._getb(name + ".ws", wsb)
-        L.check(L.lib().o3dml_knn_search(L.ptr(points), points.shape[0], L.ptr(ps), L.ptr(queries), nq,
-                                         L.ptr(qs), batch, k, L.ptr(idx), 0, None, L.ptr(ws), wsb, L.stream()))
+        """k-NN into cached int32 buffers (global row ids), no host synchronisation."""
+        idx = self.buf.get(name, (queries.shape[0], k), torch.int32)
+        wsb = ops.knn_workspace_bytes(points.shape[0], queries.shape[0], ps.numel() - 1)
+        ops.knn_search_raw(points, ps, queries, qs, k, idx, workspace=self.buf.get(name + ".ws", (wsb,), torch.uint8))
         return idx
-
-    def _geti(self, name, rows, cols):
-        key = (name, rows, cols, "i32")
-        t = self._buf.get(key)
-        if t is None:
-            t = self._buf[key] = torch.empty((rows, cols), dtype=torch.int32, device=self.device)
-        return t
-
-    def _getb(self, name, nbytes):
-        key = (name, nbytes, "u8")
-        t = self._buf.get(key)
-        if t is None:
-            t = self._buf[key] = torch.empty((nbytes,), dtype=torch.uint8, device=self.device)
-        return t
 
     def build_pyramid(self, points):
         """The index pyramid of RandLANet.transform (randlanet.py:218-229: per level k-NN of the cloud in
@@ -311,9 +275,9 @@ class RandLANetB200:
             rs = self._row_splits(B, n)
             nb = self._knn(flat, flat, self.k, rs, rs, "pyr.nb.%d" % i)
             ns = n // self.sub_sampling_ratio[i]
-            sub = self._get("pyr.sub.%d" % i, B * ns, 3).view(B, ns, 3)
+            sub = self.buf.get("pyr.sub.%d" % i, (B * ns, 3)).view(B, ns, 3)
             sub.copy_(pc[:, :ns])
-            pool = self._geti("pyr.pool.%d" % i, B * ns, self.k)
+            pool = self.buf.get("pyr.pool.%d" % i, (B * ns, self.k), torch.int32)
             pool.view(B, ns, self.k).copy_(nb.view(B, n, self.k)[:, :ns])
             up = self._knn(sub.view(B * ns, 3), flat, 1, self._row_splits(B, ns), rs, "pyr.up.%d" % i)
             out["coords"].append(flat.view(1, B * n, 3))
@@ -334,28 +298,22 @@ class RandLANetB200:
         return self.forward(inp).view(B, N, self.num_classes)
 
     # ------------------------------------------------------------- CUDA graph
-    def _graphed(self, name, tensors, thunk):
-        """Replays thunk() from a CUDA graph captured at first use for these tensor addresses (the
-        forward is ~40 launches of 5-60 us: launch-bound from Python at one cloud per GPU)."""
-        if not self.use_graph:
-            return thunk()
-        key = (name,) + tuple((t.data_ptr(), tuple(t.shape), t.dtype) for t in tensors)
-        return graph_replay(self._graphs, key, thunk, self.device)
-
+    # the forward is ~40 launches of 5-60 us: launch-bound from Python at one cloud per GPU
     def forward_graphed(self, inputs):
         """forward() for DEVICE-resident inputs, replayed from a CUDA graph keyed by their addresses."""
         flat = [inputs["features"]] + [t for k in ("coords", "neighbor_indices", "sub_idx", "interp_idx")
                                        for t in inputs[k]]
-        if not all(t.is_cuda for t in flat):
+        if not self.use_graph or not all(t.is_cuda for t in flat):
             return self.forward(inputs)
-        return self._graphed("forward", flat, lambda: self.forward(inputs))
+        return graph_replay(self._graphs, "forward", flat, lambda: self.forward(inputs), self.device)
 
     def forward_points_graphed(self, points, features=None):
         """forward_points() for DEVICE-resident clouds, replayed from a CUDA graph (pyramid + forward)."""
-        if not points.is_cuda or (features is not None and not features.is_cuda):
+        if not self.use_graph or not points.is_cuda or (features is not None and not features.is_cuda):
             return self.forward_points(points, features)
         ts = [points] + ([features] if features is not None else [])
-        return self._graphed("forward_points", ts, lambda: self.forward_points(points, features))
+        return graph_replay(self._graphs, "forward_points", ts, lambda: self.forward_points(points, features),
+                            self.device)
 
 
 def patch_reference_model(model):
