@@ -220,9 +220,13 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
                             if (p.stride == 1) {
                                 tma_load_4d(ah, &p.mapA[0], cc, ox0 - 1 + dx, oy0 - 1 + dy, cb, &full_bar[stage]);
                             } else {   // input pixel 2*o - 1 + d: odd parity for d = 0 (coordinate o - 1) and d = 2 (o)
+                                // A 1-pixel-wide (-high) image has no odd columns (rows), and its odd map is the even
+                                // one (host side).  Its only output column (row) is 0, and tap d = 2 then reads the
+                                // padding: coordinate -1, as for d = 0, which the TMA unit fills with zeros.
                                 const int py = dy != 1, px = dx != 1;
-                                tma_load_4d(ah, &p.mapA[py * 2 + px], cc, ox0 - (dx == 0), oy0 - (dy == 0), cb,
-                                            &full_bar[stage]);
+                                const int x = ox0 - (dx == 0 || (dx == 2 && p.W == 1));
+                                const int y = oy0 - (dy == 0 || (dy == 2 && p.H == 1));
+                                tma_load_4d(ah, &p.mapA[py * 2 + px], cc, x, y, cb, &full_bar[stage]);
                             }
                         }
                     }
@@ -495,7 +499,7 @@ static int gemm_tc_launch(GemmTcParams& p, const void* wimg, int k_pad, int n_pa
             for (int py = 0; py < 2; ++py)
                 for (int px = 0; px < 2; ++px) {
                     const uint64_t wp = (uint64_t)(p.W - px + 1) / 2, hp = (uint64_t)(p.H - py + 1) / 2;
-                    if (wp == 0 || hp == 0) {      // a 1-pixel-wide image has no odd columns: never addressed in range
+                    if (wp == 0 || hp == 0) {      // no odd columns (rows): the producer reads it at -1 only
                         p.mapA[py * 2 + px] = p.mapA[0];
                         continue;
                     }

@@ -27,7 +27,7 @@ gather_max_kernel(const float* __restrict__ src, int64_t src_rows, int C, int ld
     const int c = (int)(t % c4n) * 4;
     const int64_t boff = out_rows_per_batch > 0 ? (row / out_rows_per_batch) * src_rows_per_batch : 0;
     const int64_t lim = out_rows_per_batch > 0 ? src_rows_per_batch : src_rows;
-    float4 best = make_float4(-FLT_MAX, -FLT_MAX, -FLT_MAX, -FLT_MAX);
+    float4 best = make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);   // a max over -inf rows is -inf
     bool any = false;
     for (int j = 0; j < k; ++j) {
         const int64_t r = load_index(idx, row * k + j, idx_is64);

@@ -224,9 +224,13 @@ def kpconv_inputs(cin, nq=200, ns=300, H=20, K=15, seed=34):
     return q, s, nb, x, kp, off, torch.empty(nq, K * cin).cuda()
 
 
-def case_kpconv_gather(cin):
-    """cin 32: grouped kernel on float4 rows; 5: grouped kernel on narrow rows; 10: the shuffle kernel."""
+def case_kpconv_gather(cin, offset=0):
+    """cin 32 / 64 / 256: grouped kernel on float4 rows, 8 / 16 / 32 lanes per query; 5: grouped kernel on narrow rows;
+    10 / 50 / 130: the shuffle kernel with 1 / 2 / 4 channels per lane.  offset 4: the feature rows start 4 bytes past
+    a 16-byte boundary, which the float4 kernels cannot load."""
     q, s, nb, x, kp, _, out = kpconv_inputs(cin)
+    if offset:
+        x = torch.cat([torch.zeros(offset // 4).cuda(), x.reshape(-1)])[offset // 4:].view_as(x)
     return lambda: L.lib().o3dml_kpconv_gather(L.ptr(q), q.shape[0], L.ptr(s), s.shape[0], L.ptr(nb), 1, nb.shape[1],
                                                L.ptr(x), cin, L.ptr(kp), kp.shape[0], 0.12, L.ptr(out), L.stream())
 
@@ -272,6 +276,11 @@ CASES = {
     "kpconv_gather_grouped": lambda: case_kpconv_gather(32),
     "kpconv_gather_narrow": lambda: case_kpconv_gather(5),
     "kpconv_gather_shuffle": lambda: case_kpconv_gather(10),
+    "kpconv_gather_grouped_16": lambda: case_kpconv_gather(64),
+    "kpconv_gather_grouped_32": lambda: case_kpconv_gather(256),
+    "kpconv_gather_shuffle_2": lambda: case_kpconv_gather(50),
+    "kpconv_gather_shuffle_4": lambda: case_kpconv_gather(130),
+    "kpconv_gather_shuffle_unaligned": lambda: case_kpconv_gather(64, offset=4),
     "kpconv_gather_deformable": case_kpconv_gather_deformable,
 }
 
@@ -282,8 +291,15 @@ EXPECTED_KERNEL = {
     "conv3x3_simt": "gemm_gather_kernel", "conv3x3_tc": "gemm_tc_kernel",
     "deconv_simt": "gemm_gather_kernel", "deconv_tc": "gemm_tc_kernel",
     "lfa_simt": "lfa_pool_kernel", "lfa_tc": "lfa_pool_tc_kernel", "lfa16": "lfa16c_kernel",
-    "kpconv_gather_grouped": "kpconv_gather_grouped_kernel", "kpconv_gather_narrow": "kpconv_gather_grouped_kernel",
-    "kpconv_gather_shuffle": "kpconv_gather_kernel",
+    # pool.cu instantiations, as a trace names them with the spaces removed
+    "kpconv_gather_grouped": "kpconv_gather_grouped_kernel<8,4,false>",
+    "kpconv_gather_narrow": "kpconv_gather_grouped_kernel<8,1,false>",
+    "kpconv_gather_grouped_16": "kpconv_gather_grouped_kernel<16,4,false>",
+    "kpconv_gather_grouped_32": "kpconv_gather_grouped_kernel<32,4,false>",
+    "kpconv_gather_shuffle": "kpconv_gather_kernel<1>",
+    "kpconv_gather_shuffle_2": "kpconv_gather_kernel<2>",
+    "kpconv_gather_shuffle_4": "kpconv_gather_kernel<4>",
+    "kpconv_gather_shuffle_unaligned": "kpconv_gather_kernel<2>",
 }
 
 
@@ -302,4 +318,5 @@ def test_launch_count_matches_profiled_kernels(case):
     assert counted == len(names), "%s: o3dml_launch_count grew by %d, the profiler saw %d kernels: %s" % (
         case, counted, len(names), names)
     if case in EXPECTED_KERNEL:
-        assert any(EXPECTED_KERNEL[case] + "<" in n or EXPECTED_KERNEL[case] + "(" in n for n in names), names
+        k = EXPECTED_KERNEL[case]
+        assert any(k + "<" in m or k + "(" in m for m in (n.replace(" ", "") for n in names)), names
