@@ -142,6 +142,21 @@ O3DML_API int o3dml_pp_pfn_scatter(const float* points, int point_stride, int po
                          int max_points_per_voxel, float* feat_out, float* canvas,
                          int canvas_nchw, void* stream);
 
+/* o3dml_pp_pfn_scatter for the two-layer PillarFeatureNet (feat_channels [64, 64], e.g. the nuScenes and Argoverse
+ *   configs): layer 0 w0_t [C+5, 32] with folded BN bn0_scale/shift [32], then layer 1 w1_t [64, 64] =
+ *   linear.weight^T with folded BN bn1_scale/shift [64] on [y0 | max over slots of y0] (point_pillars.py:400-453).
+ *   Every slot takes part in both maxima; only layer 0's input is masked, so a padded slot's layer-1 value is
+ *   relu(BN1(W1 . [relu(BN0(0)) | m0])), which differs per pillar.  Other arguments and checks as above. */
+O3DML_API int o3dml_pp_pfn2_scatter(const float* points, int point_stride, int point_channels,
+                         const int32_t* voxel_coords, const int64_t* voxel_row_splits,
+                         const int64_t* voxel_point_indices, const int32_t* voxel_batch_id,
+                         const int64_t* d_num_voxels, int64_t num_voxels_bound, const float* w0_t,
+                         const float* bn0_scale, const float* bn0_shift, const float* w1_t,
+                         const float* bn1_scale, const float* bn1_shift, int out_channels, float vx,
+                         float vy, float x_offset, float y_offset, int nx, int ny,
+                         int max_points_per_voxel, float* feat_out, float* canvas, int canvas_nchw,
+                         void* stream);
+
 /* Neighbour table of open3d.ml.torch.layers.SparseConv / SparseConvTranspose
  *   (ml3d/torch/models/sparseconvnet.py:344-485): neighbors int32 [num_out, kx*ky*kz] = id of the input point
  *   in kernel cell (x, y, z) (row-major, the layout of the layer's `kernel` parameter [kx, ky, kz, Cin, Cout])

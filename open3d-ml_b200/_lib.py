@@ -52,6 +52,8 @@ _SIGNATURES = {
     "o3dml_pp_detect": (I, [P, L, P, L, P, L, L, L, L, I, I, P, L, F, F, P, P, P, P, P, Z, P]),
     "o3dml_pp_pfn_scatter": (I, [P, I, I, P, P, P, P, P, L, P, P, P, I, F, F, F, F, I, I, I, P, P,
                                  I, P]),
+    "o3dml_pp_pfn2_scatter": (I, [P, I, I, P, P, P, P, P, L, P, P, P, P, P, P, I, F, F, F, F, I, I, I, P, P,
+                                  I, P]),
     "o3dml_linear": (I, [L, ctypes.POINTER(Src), I, P, P, P, P, I, I, F, P, I, I, I, P]),
     "o3dml_conv3x3_nhwc": (I, [P, I, I, I, I, I, P, P, P, I, F, P, I, P]),
     "o3dml_deconv_nhwc": (I, [P, I, I, I, I, I, P, P, P, I, F, P, I, I, P]),

@@ -224,7 +224,31 @@ __global__ void ragged_to_dense_kernel(const T* __restrict__ values,
 // One warp per pillar; lane p owns point slot p (max_num_points <= 32); every
 // lane owns output channels {lane, lane+32, ...}.  Padded slots contribute the
 // per-channel constant relu(BN(0)) to the max (SURVEY.md A1).
-template <int COUT>
+//
+// TWO: the two-layer PillarFeatureNet (feat_channels [64, 64], point_pillars.py:400-453).  Wt / scale / shift are
+// layer 0 ([C+5][32], lane j owns unit j) and l1 is layer 1 (input [y0[p] | m0], 64 -> COUT = 64).  Only layer 0's
+// input is masked, so a padded slot's layer-1 input is [relu(BN0(0)) | m0]: its value depends on the pillar and is
+// computed per pillar (SURVEY.md A13).  Layer 0 runs twice per valid slot (once for m0, once for layer 1) rather
+// than keeping y0 of all slots.
+struct PfnLayer1 {
+    const float* w_t;    // [64][COUT] = linear.weight^T, staged in shared memory
+    const float* scale;  // [COUT]
+    const float* shift;  // [COUT]
+};
+
+constexpr int PFN_MAXCIN = 16;
+
+// relu(BN0(W0 . f[p])) of this lane's layer-0 unit for slot p (the slot's decorated features live in lane p)
+__device__ __forceinline__ float pfn0_unit(const float (&f)[PFN_MAXCIN], const float (&w)[PFN_MAXCIN][1], float sc,
+                                           float sh, int cin, int p) {
+    float acc = 0.f;
+#pragma unroll
+    for (int c = 0; c < PFN_MAXCIN; ++c)
+        if (c < cin) acc = fmaf(__shfl_sync(0xffffffffu, f[c], p), w[c][0], acc);
+    return fmaxf(fmaf(acc, sc, sh), 0.f);
+}
+
+template <int COUT, bool TWO = false>
 __global__ void __launch_bounds__(256)
 pp_pfn_scatter_kernel(const float* __restrict__ pts, int ld, int C,
                       const int32_t* __restrict__ coords,      // [M,3] x,y,z
@@ -232,27 +256,40 @@ pp_pfn_scatter_kernel(const float* __restrict__ pts, int ld, int C,
                       const int64_t* __restrict__ point_indices,
                       const int32_t* __restrict__ voxel_batch,  // [M] or null (batch 0)
                       const int64_t* __restrict__ num_voxels_dev, int64_t num_voxels_host,
-                      const float* __restrict__ Wt,     // [C+5][COUT]
-                      const float* __restrict__ scale,  // [COUT]
-                      const float* __restrict__ shift,  // [COUT]
+                      const float* __restrict__ Wt,     // [C+5][COUT]   (TWO: [C+5][32])
+                      const float* __restrict__ scale,  // [COUT]        (TWO: [32])
+                      const float* __restrict__ shift,  // [COUT]        (TWO: [32])
                       float vx, float vy, float x_off, float y_off, int nx, int ny, int max_pts,
                       float* __restrict__ feat_out,     // [M,COUT] or null
-                      float* __restrict__ canvas, int canvas_nchw) {
+                      float* __restrict__ canvas, int canvas_nchw, PfnLayer1 l1) {
+    static_assert(!TWO || COUT == 64, "the two-layer PFN is built for 64 output channels");
     constexpr int NCH = COUT / 32;
-    constexpr int MAXCIN = 16;
+    constexpr int NW = TWO ? 1 : NCH;  // channels per lane of the first layer
+    constexpr int MAXCIN = PFN_MAXCIN;
     const int lane = threadIdx.x & 31;
     const int64_t M = num_voxels_dev ? *num_voxels_dev : num_voxels_host;
     const int cin = C + 5;
     // weights for this lane's channels, kept in registers across pillars
-    float w[MAXCIN][NCH], sc[NCH], sh[NCH];
+    float w[MAXCIN][NW], sc[NW], sh[NW];
 #pragma unroll
     for (int c = 0; c < MAXCIN; ++c)
 #pragma unroll
-        for (int q = 0; q < NCH; ++q) w[c][q] = (c < cin) ? Wt[c * COUT + q * 32 + lane] : 0.f;
+        for (int q = 0; q < NW; ++q) w[c][q] = (c < cin) ? Wt[c * (NW * 32) + q * 32 + lane] : 0.f;
 #pragma unroll
-    for (int q = 0; q < NCH; ++q) {
+    for (int q = 0; q < NW; ++q) {
         sc[q] = scale[q * 32 + lane];
         sh[q] = shift[q * 32 + lane];
+    }
+    __shared__ float w1s[TWO ? 64 * COUT : 1];
+    float sc1[NCH], sh1[NCH];
+    if constexpr (TWO) {
+        for (int i = threadIdx.x; i < 64 * COUT; i += blockDim.x) w1s[i] = l1.w_t[i];
+#pragma unroll
+        for (int q = 0; q < NCH; ++q) {
+            sc1[q] = l1.scale[q * 32 + lane];
+            sh1[q] = l1.shift[q * 32 + lane];
+        }
+        __syncthreads();
     }
     const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     for (int64_t v = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; v < M; v += warps) {
@@ -285,23 +322,64 @@ pp_pfn_scatter_kernel(const float* __restrict__ pts, int ld, int C,
                     if (c == C + e) f[c] = dec[e];
         }
         float best[NCH];
+        if constexpr (!TWO) {
 #pragma unroll
-        for (int q = 0; q < NCH; ++q) best[q] = (cnt < max_pts) ? fmaxf(sh[q], 0.f) : 0.f;
-        for (int p = 0; p < cnt; ++p) {
-            float acc[NCH];
+            for (int q = 0; q < NCH; ++q) best[q] = (cnt < max_pts) ? fmaxf(sh[q], 0.f) : 0.f;
+            for (int p = 0; p < cnt; ++p) {
+                float acc[NCH];
 #pragma unroll
-            for (int q = 0; q < NCH; ++q) acc[q] = 0.f;
+                for (int q = 0; q < NCH; ++q) acc[q] = 0.f;
 #pragma unroll
-            for (int c = 0; c < MAXCIN; ++c) {
-                if (c < cin) {
-                    float fv = __shfl_sync(0xffffffffu, f[c], p);
+                for (int c = 0; c < MAXCIN; ++c) {
+                    if (c < cin) {
+                        float fv = __shfl_sync(0xffffffffu, f[c], p);
 #pragma unroll
-                    for (int q = 0; q < NCH; ++q) acc[q] = fmaf(fv, w[c][q], acc[q]);
+                        for (int q = 0; q < NCH; ++q) acc[q] = fmaf(fv, w[c][q], acc[q]);
+                    }
+                }
+#pragma unroll
+                for (int q = 0; q < NCH; ++q)
+                    best[q] = fmaxf(best[q], fmaxf(fmaf(acc[q], sc[q], sh[q]), 0.f));
+            }
+        } else {
+            // layer 0: m0 = max over all max_pts slots, padded ones giving relu(BN0(0))
+            const bool padded = cnt < max_pts;
+            const float pad0 = fmaxf(sh[0], 0.f);
+            float m0 = padded ? pad0 : 0.f;
+            for (int p = 0; p < cnt; ++p) m0 = fmaxf(m0, pfn0_unit(f, w, sc[0], sh[0], cin, p));
+            // layer 1: W1[:, 32:] . m0 is shared by every slot; the padded slot's value is the same product on
+            // [relu(BN0(0)) | m0]
+            float base[NCH], pad[NCH];
+#pragma unroll
+            for (int q = 0; q < NCH; ++q) base[q] = pad[q] = 0.f;
+#pragma unroll 8
+            for (int k = 0; k < 32; ++k) {
+                const float mk = __shfl_sync(0xffffffffu, m0, k);
+                const float pk = __shfl_sync(0xffffffffu, pad0, k);
+#pragma unroll
+                for (int q = 0; q < NCH; ++q) {
+                    base[q] = fmaf(mk, w1s[(32 + k) * COUT + q * 32 + lane], base[q]);
+                    pad[q] = fmaf(pk, w1s[k * COUT + q * 32 + lane], pad[q]);
                 }
             }
 #pragma unroll
             for (int q = 0; q < NCH; ++q)
-                best[q] = fmaxf(best[q], fmaxf(fmaf(acc[q], sc[q], sh[q]), 0.f));
+                best[q] = padded ? fmaxf(fmaf(pad[q] + base[q], sc1[q], sh1[q]), 0.f) : 0.f;
+            for (int p = 0; p < cnt; ++p) {
+                const float y0 = pfn0_unit(f, w, sc[0], sh[0], cin, p);
+                float acc[NCH];
+#pragma unroll
+                for (int q = 0; q < NCH; ++q) acc[q] = 0.f;
+#pragma unroll 8
+                for (int k = 0; k < 32; ++k) {
+                    const float yk = __shfl_sync(0xffffffffu, y0, k);
+#pragma unroll
+                    for (int q = 0; q < NCH; ++q) acc[q] = fmaf(yk, w1s[k * COUT + q * 32 + lane], acc[q]);
+                }
+#pragma unroll
+                for (int q = 0; q < NCH; ++q)
+                    best[q] = fmaxf(best[q], fmaxf(fmaf(acc[q] + base[q], sc1[q], sh1[q]), 0.f));
+            }
         }
         if (feat_out) {
 #pragma unroll
@@ -431,15 +509,16 @@ extern "C" int o3dml_ragged_to_dense(const void* values, int elem_bytes, int64_t
     return O3DML_OK;
 }
 
-extern "C" int o3dml_pp_pfn_scatter(const float* points, int point_stride, int point_channels,
-                                    const int32_t* voxel_coords, const int64_t* voxel_row_splits,
-                                    const int64_t* voxel_point_indices, const int32_t* voxel_batch_id,
-                                    const int64_t* d_num_voxels, int64_t num_voxels_bound,
-                                    const float* w_t, const float* bn_scale, const float* bn_shift,
-                                    int out_channels, float vx, float vy, float x_offset,
-                                    float y_offset, int nx, int ny, int max_points_per_voxel,
-                                    float* feat_out, float* canvas, int canvas_nchw, void* stream) {
-    cudaStream_t st = (cudaStream_t)stream;
+// The argument checks and the launch of both PFN entries; TWO selects the two-layer kernel (l1 unused otherwise).
+template <bool TWO>
+static int pp_pfn_scatter_launch(const float* points, int point_stride, int point_channels,
+                                 const int32_t* voxel_coords, const int64_t* voxel_row_splits,
+                                 const int64_t* voxel_point_indices, const int32_t* voxel_batch_id,
+                                 const int64_t* d_num_voxels, int64_t num_voxels_bound, const float* w_t,
+                                 const float* bn_scale, const float* bn_shift, PfnLayer1 l1, int out_channels,
+                                 float vx, float vy, float x_offset, float y_offset, int nx, int ny,
+                                 int max_points_per_voxel, float* feat_out, float* canvas, int canvas_nchw,
+                                 cudaStream_t st) {
     O3DML_CHECK(point_channels >= 3 && point_channels <= 11, "pfn: 3..11 point channels supported");
     O3DML_CHECK(max_points_per_voxel >= 1 && max_points_per_voxel <= 32,
                 "pfn: max_points_per_voxel must be <= 32 for the fused kernel");
@@ -449,9 +528,39 @@ extern "C" int o3dml_pp_pfn_scatter(const float* points, int point_stride, int p
     int64_t blocks = ceil_div<int64_t>(warps_needed, 8);
     int64_t cap = (int64_t)device_sm_count() * 8;  // 8 resident CTAs of 256 threads per SM
     if (blocks > cap) blocks = cap;
-    O3DML_CUDA(launch<pp_pfn_scatter_kernel<64>>(
+    O3DML_CUDA(launch<pp_pfn_scatter_kernel<64, TWO>>(
         (unsigned)blocks, 256, 0, st, points, point_stride, point_channels, voxel_coords, voxel_row_splits,
         voxel_point_indices, voxel_batch_id, d_num_voxels, num_voxels_bound, w_t, bn_scale, bn_shift, vx, vy, x_offset,
-        y_offset, nx, ny, max_points_per_voxel, feat_out, canvas, canvas_nchw));
+        y_offset, nx, ny, max_points_per_voxel, feat_out, canvas, canvas_nchw, l1));
     return O3DML_OK;
+}
+
+extern "C" int o3dml_pp_pfn_scatter(const float* points, int point_stride, int point_channels,
+                                    const int32_t* voxel_coords, const int64_t* voxel_row_splits,
+                                    const int64_t* voxel_point_indices, const int32_t* voxel_batch_id,
+                                    const int64_t* d_num_voxels, int64_t num_voxels_bound,
+                                    const float* w_t, const float* bn_scale, const float* bn_shift,
+                                    int out_channels, float vx, float vy, float x_offset,
+                                    float y_offset, int nx, int ny, int max_points_per_voxel,
+                                    float* feat_out, float* canvas, int canvas_nchw, void* stream) {
+    return pp_pfn_scatter_launch<false>(points, point_stride, point_channels, voxel_coords, voxel_row_splits,
+                                        voxel_point_indices, voxel_batch_id, d_num_voxels, num_voxels_bound, w_t,
+                                        bn_scale, bn_shift, PfnLayer1{}, out_channels, vx, vy, x_offset, y_offset, nx,
+                                        ny, max_points_per_voxel, feat_out, canvas, canvas_nchw, (cudaStream_t)stream);
+}
+
+extern "C" int o3dml_pp_pfn2_scatter(const float* points, int point_stride, int point_channels,
+                                     const int32_t* voxel_coords, const int64_t* voxel_row_splits,
+                                     const int64_t* voxel_point_indices, const int32_t* voxel_batch_id,
+                                     const int64_t* d_num_voxels, int64_t num_voxels_bound, const float* w0_t,
+                                     const float* bn0_scale, const float* bn0_shift, const float* w1_t,
+                                     const float* bn1_scale, const float* bn1_shift, int out_channels, float vx,
+                                     float vy, float x_offset, float y_offset, int nx, int ny,
+                                     int max_points_per_voxel, float* feat_out, float* canvas, int canvas_nchw,
+                                     void* stream) {
+    return pp_pfn_scatter_launch<true>(points, point_stride, point_channels, voxel_coords, voxel_row_splits,
+                                       voxel_point_indices, voxel_batch_id, d_num_voxels, num_voxels_bound, w0_t,
+                                       bn0_scale, bn0_shift, PfnLayer1{w1_t, bn1_scale, bn1_shift}, out_channels, vx,
+                                       vy, x_offset, y_offset, nx, ny, max_points_per_voxel, feat_out, canvas,
+                                       canvas_nchw, (cudaStream_t)stream);
 }

@@ -2,7 +2,8 @@
 ``PointPillars.forward`` (ml3d/torch/models/point_pillars.py:102-134):
 
     voxelize (all frames in ONE batched call, no per-frame Python loop, :112-128, :328-382)
-    -> pillar gather + decoration + PFN + max + scatter-to-BEV in one kernel (:417-616),
+    -> pillar gather + decoration + PFN (one layer, or the two of feat_channels [64, 64]) + max + scatter-to-BEV in
+       one kernel (:400-616),
        reading the CSR voxel lists directly (the [M,32,4] pillar tensor never exists)
     -> SECOND / SECONDFPN / Anchor3DHead as NHWC implicit-GEMM convolutions (:619-841)
 
@@ -46,15 +47,24 @@ class PointPillarsB200:
         def put(name, t):
             w[name] = t.to(dev, torch.float32).contiguous()
 
-        # PFN (single layer): linear.weight [64, C+5]
-        lw = sd["voxel_encoder.pfn_layers.0.linear.weight"]
-        if "voxel_encoder.pfn_layers.1.linear.weight" in sd:
-            raise RuntimeError("PointPillarsB200: only single-layer PillarFeatureNet is fused")
-        self.pfn_out = lw.shape[0]
+        # PFN: one layer, linear.weight [64, C+5], or two (feat_channels [64, 64]): [32, C+5] then [64, 64]
+        pfn = []
+        while "voxel_encoder.pfn_layers.%d.linear.weight" % len(pfn) in sd:
+            pfn.append(sd["voxel_encoder.pfn_layers.%d.linear.weight" % len(pfn)])
+        lw = pfn[0]
         self.point_channels = lw.shape[1] - 5
-        put("pfn.wt", lw.t())
-        s, t = L.fold_bn(sd, "voxel_encoder.pfn_layers.0.norm", BN_EPS)
-        put("pfn.s", s), put("pfn.t", t)
+        if len(pfn) == 2 and tuple(lw.shape) == (32, lw.shape[1]) and tuple(pfn[1].shape) == (64, 64):
+            self.pfn_layers = 2
+        elif len(pfn) == 1:
+            self.pfn_layers = 1
+        else:
+            raise RuntimeError("PointPillarsB200: PillarFeatureNet with linear weights %s is not fused (one layer, or "
+                               "two of [32, C+5] and [64, 64])" % [list(x.shape) for x in pfn])
+        self.pfn_out = pfn[-1].shape[0]
+        for i, x in enumerate(pfn):
+            put("pfn%d.wt" % i, x.t())
+            s, t = L.fold_bn(sd, "voxel_encoder.pfn_layers.%d.norm" % i, BN_EPS)
+            put("pfn%d.s" % i, s), put("pfn%d.t" % i, t)
         # backbone
         self.blocks = []
         for i, (n, stride) in enumerate(zip(cfg["layer_nums"], cfg["layer_strides"])):
@@ -114,14 +124,25 @@ class PointPillarsB200:
         canvas.zero_()
         bound = min(pts.shape[0], B * int(cfg["max_voxels"]))
         feat = torch.empty((bound, C), dtype=torch.float32, device=dev) if want_feat else None
-        L.check(L.lib().o3dml_pp_pfn_scatter(
-            L.ptr(pts), pts.stride(0), self.point_channels, L.ptr(coords), L.ptr(vrs), L.ptr(pidx),
-            L.ptr(bid), L.ptr(counts), bound, L.ptr(self.w["pfn.wt"]), L.ptr(self.w["pfn.s"]),
-            L.ptr(self.w["pfn.t"]), C, self.vx, self.vy, self.x_off, self.y_off, self.nx, self.ny,
-            int(cfg["max_num_points"]), L.ptr(feat), L.ptr(canvas), 1 if canvas_nchw else 0,
-            L.stream()))
-        return canvas, dict(coords=coords, point_indices=pidx, row_splits=vrs, batch_splits=bsp,
-                            batch_id=bid, counts=counts, feat=feat, points=pts)
+        vox = dict(coords=coords, point_indices=pidx, row_splits=vrs, batch_splits=bsp, batch_id=bid, counts=counts,
+                   feat=feat, points=pts, bound=bound)
+        self.pfn_scatter(vox, canvas, canvas_nchw)
+        return canvas, vox
+
+    def pfn_scatter(self, vox, canvas, canvas_nchw=False):
+        """The pillar feature net + scatter of front_end (one launch): the voxel buffers `vox` of front_end into
+        vox["feat"] (may be None) and `canvas`."""
+        w = self.w
+        voxels = (L.ptr(vox["points"]), vox["points"].stride(0), self.point_channels, L.ptr(vox["coords"]),
+                  L.ptr(vox["row_splits"]), L.ptr(vox["point_indices"]), L.ptr(vox["batch_id"]), L.ptr(vox["counts"]),
+                  vox["bound"], L.ptr(w["pfn0.wt"]), L.ptr(w["pfn0.s"]), L.ptr(w["pfn0.t"]))
+        rest = (self.pfn_out, self.vx, self.vy, self.x_off, self.y_off, self.nx, self.ny,
+                int(self.cfg["max_num_points"]), L.ptr(vox["feat"]), L.ptr(canvas), 1 if canvas_nchw else 0, L.stream())
+        if self.pfn_layers == 2:
+            L.check(L.lib().o3dml_pp_pfn2_scatter(*voxels, L.ptr(w["pfn1.wt"]), L.ptr(w["pfn1.s"]),
+                                                  L.ptr(w["pfn1.t"]), *rest))
+        else:
+            L.check(L.lib().o3dml_pp_pfn_scatter(*voxels, *rest))
 
     # ---------------------------------------------------------- dense layers
     def _conv(self, x, B, H, W, name, stride, cin, cout):
