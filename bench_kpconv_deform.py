@@ -4,10 +4,10 @@ run eagerly on the same GPU.
     python bench_kpconv_deform.py [--steps N] [--warmup W]
 
 Workload: 4 m spheres cropped from synthetic LiDAR frames (synth.semantickitti_cloud), grid-subsampled at 0.08 m and
-stacked to batch_limit = 20 000 points (tests/kpconv_deform_support.paris_clouds, seed 1000); the batch is built on
-the device by kpconv.build_batch with the deform radii of kpconv.layer_radii.  Weights: the manifest of
+stacked to batch_limit = 20 000 points (tests/helpers.paris_clouds, seed 1000); the batch is built on the device by
+kpconv.build_batch with the deform radii of kpconv.layer_radii.  Weights: the manifest of
 tests/golden/boundary_kpconv_deform_class.npz, seed 1.  The fused forward is timed with CUDA events per step after
-warm-up (median over --steps), in two runs alternating with the eager port (tests/kpconv_deform_support.kpfcnn_forward,
+warm-up (median over --steps), in two runs alternating with the eager port (oracle/models_torch.kpfcnn_forward,
 median over --steps / 10).  For every deformable KPConv it reports H (neighbour row width), the fraction of valid
 neighbours the re-selection keeps, and the median time of its four steps: offset gather (rigid kpconv_gather), offset
 GEMM, deformable gather, GEMM + BN + LeakyReLU.  Prints one JSON line and writes nothing.
@@ -54,21 +54,21 @@ def main():
         raise SystemExit("bench_kpconv_deform.py measures on a CUDA device; none is visible")
     import open3d_ml_b200 as M
     from open3d_ml_b200.kpconv import build_batch
-    from oracle import weights
-    import kpconv_deform_support as KD
+    from oracle import models_torch as MT, weights
+    from helpers import paris_clouds
     torch.cuda.set_device(0)
     info = gpu_info()
     g = np.load(os.path.join(ROOT, "tests", "golden", "boundary_kpconv_deform_class.npz"))
     cfg = json.loads(str(g["cfg"]))
     sd = weights.seeded_state_dict(json.loads(str(g["manifest"])), 1)
-    clouds = KD.paris_clouds(1000)
+    clouds = paris_clouds(1000)
     batch = build_batch(clouds, cfg)
     net = M.KPFCNNB200(sd, cfg)
     sdc = {k: v.cuda() for k, v in sd.items()}
 
     def port():
         with torch.no_grad():
-            return KD.kpfcnn_forward(sdc, batch, cfg)
+            return MT.kpfcnn_forward(sdc, batch, cfg)
     for _ in range(args.warmup):
         net(batch)
     port()
@@ -90,7 +90,7 @@ def main():
     convs = []
     for c in probe:
         dkp = c["offsets"].view(-1, c["kernel_points"].shape[0], 3) * c["extent"] + c["kernel_points"]
-        _, kept = KD.deform_influence(c["q_pts"], c["s_pts"], c["neighbors"], dkp, c["extent"])
+        kept = MT.kp_kept(c["q_pts"], c["s_pts"], c["neighbors"], dkp, c["extent"])
         valid = (c["neighbors"] >= 0) & (c["neighbors"] < c["s_pts"].shape[0])
         med = np.median(np.array(per[c["name"]]), axis=0)
         convs.append(dict(conv=c["name"], queries=int(c["q_pts"].shape[0]), H=int(c["neighbors"].shape[1]),

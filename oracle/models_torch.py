@@ -2,11 +2,14 @@
 
 Plain-PyTorch (CPU, float32) restatement of the three reference forwards on the
 hot path, driven by the reference's own ``state_dict`` keys, in point-major
-(channels-last) layout.  It exists because /root/reference cannot travel to the
-GPU box: tests/test_oracle_models.py pins every function here against the
-UNMODIFIED reference classes (imported through oracle/refshim.py) in this
-container, and against the committed golden fixtures everywhere.  On the GPU
-box it is the parity checker for full-size inputs and the "port" CPU baseline.
+(channels-last) layout.  It is the one port of the reference in the repository:
+it exists because the reference tree does not travel to the GPU machines.
+tests/test_oracle_models.py, test_oracle_kpconv_deform.py and
+test_oracle_pointpillars_configs.py pin it against the UNMODIFIED reference
+classes (imported through oracle/refshim.py) where the reference is installed,
+and against the committed golden fixtures everywhere.  On a GPU it is the parity
+checker for full-size inputs, the kernel tests' float64 reference and the
+"port" CPU baseline.
 
 Reference lines followed:
   RandLANet.forward            ml3d/torch/models/randlanet.py:241-298
@@ -17,16 +20,18 @@ Reference lines followed:
   random_sample / nearest_interpolation   randlanet.py:300-350
   PointPillars.forward         ml3d/torch/models/point_pillars.py:102-134
   PointPillarsVoxelization     point_pillars.py:328-382
-  PillarFeatureNet / PFNLayer  point_pillars.py:417-555
+  PillarFeatureNet / PFNLayer  point_pillars.py:400-555 (one or more layers)
   PointPillarsScatter          point_pillars.py:577-616
   SECOND / SECONDFPN / head    point_pillars.py:619-841
   KPFCNN.forward               ml3d/torch/models/kpconv.py:270-291
-  KPConv.forward (rigid)       kpconv.py:1005-1159
+  KPFCNN heads (reduce_fc or not)   kpconv.py:229-251
+  KPConv.forward (rigid and deformable, modulated = False)   kpconv.py:1005-1159
   Unary/Resnet/Simple blocks   kpconv.py:1213-1464, max_pool/closest_pool :821-858
 
-Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline /
-``--impl reference`` legs may import this module.
+Only tests/, __graft_entry__.smoke(), bench.py's cpu_baseline / ``--impl reference``
+legs and the side benches (bench_kpconv_deform.py) may import this module.
 """
+import itertools
 import math
 
 import numpy as np
@@ -178,24 +183,35 @@ def pp_voxelize(points, cfg, voxelize=None):
     return pillars[ok], coords[ok], counts[ok]
 
 
-def pp_pfn(pillars, counts, coords4, sd, cfg):
-    """PillarFeatureNet with a single PFNLayer: -> [M,64] (point_pillars.py:512-555,417-453).
-    Padded slots take part in the max (SURVEY.md A1)."""
-    vx, vy = cfg["voxel_size"][0], cfg["voxel_size"][1]
-    x_off = vx / 2 + cfg["point_cloud_range"][0]
-    y_off = vy / 2 + cfg["point_cloud_range"][1]
+def pp_decorate(pillars, counts, cx, cy, vx, vy, x_off, y_off):
+    """PillarFeatureNet's decoration (point_pillars.py:512-555): pillars [M,P,C] with counts [M] points and cell
+    x / y [M] -> [M,P,C+5] = [point, point - pillar mean (f_cluster), x / y - cell centre (f_center)], the padded
+    slots zeroed."""
     cnt = counts.to(pillars.dtype).view(-1, 1, 1)
     mean = pillars[:, :, :3].sum(1, keepdim=True) / cnt
     f_cluster = pillars[:, :, :3] - mean
     f_center = torch.stack([
-        pillars[:, :, 0] - (coords4[:, 3].to(pillars.dtype).unsqueeze(1) * vx + x_off),
-        pillars[:, :, 1] - (coords4[:, 2].to(pillars.dtype).unsqueeze(1) * vy + y_off)], -1)
+        pillars[:, :, 0] - (cx.to(pillars.dtype).unsqueeze(1) * vx + x_off),
+        pillars[:, :, 1] - (cy.to(pillars.dtype).unsqueeze(1) * vy + y_off)], -1)
     f = torch.cat([pillars, f_cluster, f_center], -1)
-    slot = torch.arange(pillars.shape[1]).view(1, -1)
-    f = f * (slot < counts.view(-1, 1)).unsqueeze(-1).to(f.dtype)
-    y = f @ sd["voxel_encoder.pfn_layers.0.linear.weight"].t()
-    y = torch.relu(bn_eval(y, sd, "voxel_encoder.pfn_layers.0.norm", PP_BN_EPS))
-    return y.max(dim=1)[0]
+    slot = torch.arange(pillars.shape[1], device=pillars.device).view(1, -1)
+    return f * (slot < counts.view(-1, 1)).unsqueeze(-1).to(f.dtype)
+
+
+def pp_pfn(pillars, counts, coords4, sd, cfg):
+    """PillarFeatureNet with its PFNLayers: -> [M,64] (point_pillars.py:400-555).  Only the decoration is masked:
+    every slot, padded ones included, takes part in every layer's max (SURVEY.md A1), and a layer that is not the
+    last passes cat(y[p], max over slots of y) on."""
+    vx, vy = cfg["voxel_size"][0], cfg["voxel_size"][1]
+    f = pp_decorate(pillars, counts, coords4[:, 3], coords4[:, 2], vx, vy,
+                    vx / 2 + cfg["point_cloud_range"][0], vy / 2 + cfg["point_cloud_range"][1])
+    for i in itertools.count():
+        p = "voxel_encoder.pfn_layers.%d" % i
+        y = torch.relu(bn_eval(f @ sd[p + ".linear.weight"].t(), sd, p + ".norm", PP_BN_EPS))
+        m = y.max(dim=1, keepdim=True)[0]
+        if "voxel_encoder.pfn_layers.%d.linear.weight" % (i + 1) not in sd:
+            return m.squeeze(1)
+        f = torch.cat([y, m.expand_as(y)], 2)
 
 
 def pp_scatter(vfeat, coords4, batch, ny, nx):
@@ -251,21 +267,61 @@ def pointpillars_forward(sd, frames, cfg, voxelize=None, taps=None):
 
 
 # =============================================================================
-# KPConv / KPFCNN (rigid, linear influence, sum aggregation: SURVEY.md A11)
+# KPConv / KPFCNN (linear influence, sum aggregation: SURVEY.md A11; rigid and deformable, not modulated)
 # =============================================================================
 KP_BN_EPS = 1e-5  # nn.BatchNorm1d default (kpconv.py:1231)
 
 
-def kp_conv(q_pts, s_pts, nidx, x, kpts, weights, extent):
-    """KPConv.forward, rigid path (kpconv.py:1044-1159). nidx [Nq,H] with shadow = len(s_pts)."""
+def kp_d2(q_pts, s_pts, nidx, kpts):
+    """[Nq,H,K] squared distances of the neighbours nidx [Nq,H], relative to their query, to the kernel points kpts:
+    [K,3] (rigid) or [Nq,K,3] (deformed, per query).  Every id outside [0, ns) reads the shadow point at 1e6."""
+    ns = s_pts.shape[0]
     s_pts = torch.cat([s_pts, torch.full_like(s_pts[:1], 1e6)])
-    nb = s_pts[nidx] - q_pts.unsqueeze(1)  # [Nq,H,3]
-    diff = nb.unsqueeze(2) - kpts  # [Nq,H,K,3]
-    d2 = (diff * diff).sum(-1)
-    w = torch.clamp(1 - torch.sqrt(d2) / extent, min=0.0).transpose(1, 2)  # [Nq,K,H]
+    nb = s_pts[torch.where((nidx >= 0) & (nidx < ns), nidx, ns)] - q_pts.unsqueeze(1)  # [Nq,H,3]
+    diff = nb.unsqueeze(2) - kpts.unsqueeze(-3)  # [Nq,H,K,3]
+    return (diff * diff).sum(-1)
+
+
+def kp_kept(q_pts, s_pts, nidx, kpts, extent):
+    """The deformable conv's re-selection (kpconv.py:1071-1103): [Nq,H], true where d2 < extent^2 for some kernel
+    point."""
+    return (kp_d2(q_pts, s_pts, nidx, kpts) < extent ** 2).any(2)
+
+
+def kp_gather(q_pts, s_pts, nidx, x, kpts, extent, keep=None):
+    """The [Nq,K,Cin] operand of KPConv.forward (kpconv.py:1044-1159): sum over the neighbours n of
+    max(0, 1 - |s[n] - q - kp| / extent) * x[n].  Ids outside [0, ns) and the neighbours that keep [Nq,H] drops read
+    the shadow row, whose feature is zero: a non-finite feature of a dropped neighbour does not reach the sum."""
+    ns = s_pts.shape[0]
+    w = torch.clamp(1 - torch.sqrt(kp_d2(q_pts, s_pts, nidx, kpts)) / extent, min=0.0).transpose(1, 2)  # [Nq,K,H]
+    ok = (nidx >= 0) & (nidx < ns)
+    if keep is not None:
+        ok = ok & keep
     x = torch.cat([x, torch.zeros_like(x[:1])])
-    wf = w @ x[nidx]  # [Nq,K,Cin]
-    return torch.einsum("nkc,kcd->nd", wf, weights)
+    return w @ x[torch.where(ok, nidx, ns)]
+
+
+def kp_conv(q_pts, s_pts, nidx, x, kpts, weights, extent, keep=None):
+    """KPConv.forward: the gathered operand contracted with weights [K,Cin,Cout]."""
+    return torch.einsum("nkc,kcd->nd", kp_gather(q_pts, s_pts, nidx, x, kpts, extent, keep), weights)
+
+
+def kp_conv_deform(q_pts, s_pts, nidx, x, sd, p, extent, stats=None):
+    """Deformable KPConv.forward (kpconv.py:1011-1159) from the state_dict keys under p (...KPConv).  The offset conv
+    (a rigid KPConv with 3K outputs) + offset_bias, scaled by the extent and added to the kernel points, each step
+    rounded on its own, moves the kernel points per query; the conv then re-selects and gathers at the moved points.
+    Both convs read offset_conv.kernel_points: KPConv.kernel_points is the same Parameter (kpconv.py:977-978), and
+    load_state_dict loads the child's key last.  stats[p] gets the kept / dropped valid neighbours and the median
+    offset in extents."""
+    kpts = sd[p + ".offset_conv.kernel_points"]
+    off = kp_conv(q_pts, s_pts, nidx, x, kpts, sd[p + ".offset_conv.weights"], extent) + sd[p + ".offset_bias"]
+    dkp = off.view(-1, kpts.shape[0], 3) * extent + kpts
+    kept = kp_kept(q_pts, s_pts, nidx, dkp, extent)
+    if stats is not None:
+        valid = (nidx >= 0) & (nidx < s_pts.shape[0])
+        stats[p] = dict(kept=int(kept.sum()), dropped=int((valid & ~kept).sum()),
+                        median_offset=float((dkp - kpts).norm(dim=-1).median()) / extent)
+    return kp_conv(q_pts, s_pts, nidx, x, dkp, sd[p + ".weights"], extent, kept)
 
 
 def kp_bn(x, sd, p, use_bn):
@@ -322,9 +378,10 @@ def kpfcnn_plan(cfg):
                 head_in=out_dim)
 
 
-def kpfcnn_forward(sd, batch, cfg, taps=None):
+def kpfcnn_forward(sd, batch, cfg, taps=None, stats=None):
     """batch: dict(features [N0,Cf], points[l] [N_l,3], neighbors[l] [N_l,H], pools[l], upsamples[l])
-    -> logits [N0, C] (kpconv.py:270-291)."""
+    -> logits [N0, C] (kpconv.py:270-291), with rigid and deformable blocks and either head.  stats collects
+    kp_conv_deform's diagnostics per deformable conv."""
     plan = kpfcnn_plan(cfg)
     use_bn, slope = cfg.get("use_batch_norm", True), cfg.get("l_relu", 0.1)
     x = batch["features"]
@@ -338,18 +395,19 @@ def kpfcnn_forward(sd, batch, cfg, taps=None):
         q = batch["points"][L + 1] if strided else batch["points"][L]
         s = batch["points"][L]
         nidx = batch["pools"][L] if strided else batch["neighbors"][L]
+
+        def conv(y):
+            if "deform" in b["kind"]:
+                return kp_conv_deform(q, s, nidx, y, sd, p + ".KPConv", b["extent"], stats)
+            return kp_conv(q, s, nidx, y, sd[p + ".KPConv.kernel_points"], sd[p + ".KPConv.weights"], b["extent"])
         if "simple" in b["kind"]:
-            y = kp_conv(q, s, nidx, x, sd[p + ".KPConv.kernel_points"], sd[p + ".KPConv.weights"],
-                        b["extent"])
-            x = lrelu(kp_bn(y, sd, p + ".batch_norm", use_bn), slope)
+            x = lrelu(kp_bn(conv(x), sd, p + ".batch_norm", use_bn), slope)
         elif "resnetb" in b["kind"]:
             feats = x
             y = feats
             if b["in_dim"] != b["out_dim"] // 4:
                 y = kp_unary(y, sd, p + ".unary1", use_bn, True, slope)
-            y = kp_conv(q, s, nidx, y, sd[p + ".KPConv.kernel_points"], sd[p + ".KPConv.weights"],
-                        b["extent"])
-            y = lrelu(kp_bn(y, sd, p + ".batch_norm_conv", use_bn), slope)
+            y = lrelu(kp_bn(conv(y), sd, p + ".batch_norm_conv", use_bn), slope)
             y = kp_unary(y, sd, p + ".unary2", use_bn, False, slope)
             sc = kp_max_pool(feats, nidx) if strided else feats
             if b["in_dim"] != b["out_dim"]:
@@ -371,8 +429,12 @@ def kpfcnn_forward(sd, batch, cfg, taps=None):
             raise NotImplementedError(b["kind"])
         if taps is not None:
             taps[p] = x
-    # head (non reduce_fc): both UnaryBlocks are built without BN and WITH LeakyReLU
-    # (kpconv.py:236-247: no_relu keeps its default False on head_softmax)
+    if cfg.get("reduce_fc", False):
+        # kpconv.py:229-240: head_mlp with BN (always) and LeakyReLU, head_softmax with a bias and no activation
+        x = kp_unary(x, sd, "head_mlp", True, True, slope)
+        return kp_unary(x, sd, "head_softmax", False, False, slope)
+    # kpconv.py:241-251: both UnaryBlocks without BN and WITH LeakyReLU (no_relu keeps its default False on
+    # head_softmax)
     x = kp_unary(x, sd, "head_mlp", False, True, slope)
     return kp_unary(x, sd, "head_softmax", False, True, slope)
 

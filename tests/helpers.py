@@ -1,5 +1,6 @@
 """Shared builders for the model parity tests: seeded weights + seeded inputs,
-re-derived exactly as tests/golden/make_golden.py derived them."""
+re-derived exactly as tests/golden/make_golden.py derived them, and the
+Paris-Lille3D-shaped clouds of the deformable KPConv tests and benchmark."""
 import os
 
 import numpy as np
@@ -60,3 +61,22 @@ def kp_batch_tensors(bd):
     for k in ("points", "neighbors", "pools", "upsamples"):
         tb[k] = [torch.from_numpy(a) for a in bd[k]]
     return tb
+
+
+def paris_clouds(seed, batch_limit=20000, in_radius=4.0, dl=0.08, n=200000):
+    """Paris-Lille3D-shaped input: 4 m spheres cropped from synthetic LiDAR frames around points within 15 m of the
+    sensor, grid-subsampled at 0.08 m (features: the constant 1 of in_features_dim = 1) and stacked while the total
+    stays within batch_limit points.  -> list of (points [n,3], features [n,1]) float32 numpy clouds."""
+    rng = np.random.default_rng(seed)
+    clouds, total = [], 0
+    for s in range(seed, seed + 64):
+        pc = synth.semantickitti_cloud(n, s)
+        near = pc[np.linalg.norm(pc[:, :2], axis=1) < 15.0]
+        c = near[rng.integers(len(near))]
+        crop = pc[np.linalg.norm(pc - c, axis=1) < in_radius] - c
+        pts = synth.grid_subsample(crop, dl).astype(np.float32)
+        if total + len(pts) > batch_limit:
+            break
+        clouds.append((pts, np.ones((len(pts), 1), np.float32)))
+        total += len(pts)
+    return clouds

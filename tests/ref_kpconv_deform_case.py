@@ -7,7 +7,7 @@ Run as a script in a fresh process:
     python tests/ref_kpconv_deform_case.py [--ops oracle] [--record DIR]
 
 `--ops oracle` binds the CPU oracle (no GPU needed).  The script asserts that the torch port
-(tests/kpconv_deform_support.py) matches the reference to < 1e-5 on the logits and on every deformable encoder
+(oracle/models_torch.kpfcnn_forward) matches the reference to < 1e-5 on the logits and on every deformable encoder
 block; against a GPU library it also runs KPFCNNB200 on the same batch.  Prints one JSON line.
 """
 import json
@@ -23,7 +23,7 @@ import ref_boundary_cases as rbc  # noqa: E402  (puts the repository root on sys
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
-import kpconv_deform_support as KD  # noqa: E402
+from oracle import models_torch as MT  # noqa: E402
 
 # a 4 m Paris-Lille3D sphere at 0.08 m has ~10 000 points; these keep the fixture under ~2 MB
 IN_RADIUS, MAX_IN_POINTS, BATCH_LIMIT = 2.0, 4000, 4000
@@ -60,7 +60,7 @@ def run(root, dev):
               upsamples=list(b.upsamples))
     port_taps, stats = {}, {}
     with torch.no_grad():
-        port = KD.kpfcnn_forward(sd, bd, dict(net.cfg), taps=port_taps, stats=stats)
+        port = MT.kpfcnn_forward(sd, bd, dict(net.cfg), taps=port_taps, stats=stats)
     errs = dict(logits=rbc.rel(port, ref))
     for i in deform:
         errs["encoder_blocks.%d" % i] = rbc.rel(port_taps["encoder_blocks.%d" % i], taps[i])

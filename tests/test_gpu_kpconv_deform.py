@@ -1,6 +1,6 @@
-"""o3dml_kpconv_gather_deformable against a float64 torch restatement of the offsets and the neighbour
-re-selection (tests/kpconv_deform_support.py), and KPFCNNB200 on the deformable Paris-Lille3D config against the
-unmodified reference (tests/golden/boundary_kpconv_deform_class.npz) and the torch port."""
+"""o3dml_kpconv_gather_deformable against the torch port's deformable gather and neighbour re-selection in float64
+(oracle/models_torch.py), and KPFCNNB200 on the deformable Paris-Lille3D config against the unmodified reference
+(tests/golden/boundary_kpconv_deform_class.npz) and the torch port."""
 import ctypes
 import json
 
@@ -8,8 +8,9 @@ import numpy as np
 import pytest
 import torch
 
-import kpconv_deform_support as KD
 from conftest import rel_err
+from helpers import paris_clouds
+from oracle import models_torch as MT
 from test_oracle_kpconv_deform import fixture, sampled_rel_err
 
 pytestmark = pytest.mark.gpu
@@ -63,8 +64,8 @@ def case(cin, H, seed, strided=False, is64=True, nq=300, ns=400, off_scale=0.5):
 def want_deform(q, s, nidx, x, kp, off, extent=EXT):
     d = lambda t: t.double().cpu()  # noqa: E731
     dkp = d(off[:, :3 * K]).view(-1, K, 3) * extent + d(kp)
-    n = d(nidx.long())
-    return KD.deform_gather(d(q), d(s), n.long(), d(x), dkp, extent).reshape(q.shape[0], -1)
+    q, s, n = d(q), d(s), nidx.long().cpu()
+    return MT.kp_gather(q, s, n, d(x), dkp, extent, MT.kp_kept(q, s, n, dkp, extent)).reshape(q.shape[0], -1)
 
 
 def row_err(got, want):
@@ -92,8 +93,8 @@ def test_offsets_away_from_every_neighbour_give_zero_rows():
 
 def test_inf_feature_propagates_only_from_kept_neighbours():
     q, s, nidx, x, kp, off = case(32, 40, 6)
-    _, kept = KD.deform_influence(q.double().cpu(), s.double().cpu(), nidx.cpu(),
-                                  off[:, :3 * K].double().cpu().view(-1, K, 3) * EXT + kp.double().cpu(), EXT)
+    kept = MT.kp_kept(q.double().cpu(), s.double().cpu(), nidx.cpu(),
+                      off[:, :3 * K].double().cpu().view(-1, K, 3) * EXT + kp.double().cpu(), EXT)
     valid = (nidx.cpu() >= 0) & (nidx.cpu() < s.shape[0])
     r = 10
     nk = int(nidx[r, int(torch.nonzero(kept[r])[0])])
@@ -169,9 +170,9 @@ def paris_cfg():
 
 def test_build_batch_paris_lille3d_matches_the_oracle_pyramid_at_deform_radii():
     from open3d_ml_b200.kpconv import build_batch, layer_radii
-    from oracle import ops as O, models_torch as MT
+    from oracle import ops as O
     cfg = paris_cfg()
-    clouds = KD.paris_clouds(300, batch_limit=8000)
+    clouds = paris_clouds(300, batch_limit=8000)
     b = build_batch(clouds, cfg)
     P = np.concatenate([c[0] for c in clouds])
     lens = [len(c[0]) for c in clouds]
@@ -190,12 +191,12 @@ def test_kpfcnn_b200_paris_lille3d_batch_matches_the_port():
     import open3d_ml_b200 as M
     from open3d_ml_b200.kpconv import build_batch
     _, sd, _, cfg = fixture()
-    b = build_batch(KD.paris_clouds(400), cfg)
+    b = build_batch(paris_clouds(400), cfg)
     got = M.KPFCNNB200(sd, cfg)(b)
     sdc = {k: v.cuda().double() if v.is_floating_point() else v.cuda() for k, v in sd.items()}
     b64 = dict(b, features=b["features"].double(), points=[p.double() for p in b["points"]])
     with torch.no_grad():
-        want = KD.kpfcnn_forward(sdc, b64, cfg)
+        want = MT.kpfcnn_forward(sdc, b64, cfg)
     err = rel_err(got, want)
     print("paris batch rel err %.3g over %d points" % (err, b["points"][0].shape[0]))
     assert err < BATCH_TOL
@@ -205,7 +206,7 @@ def test_forward_does_not_sync_the_host():
     import open3d_ml_b200 as M
     from open3d_ml_b200.kpconv import build_batch
     _, sd, _, cfg = fixture()
-    b = build_batch(KD.paris_clouds(500, batch_limit=8000), cfg)
+    b = build_batch(paris_clouds(500, batch_limit=8000), cfg)
     net = M.KPFCNNB200(sd, cfg)
     want = net(b).clone()                    # first call caches what the GEMMs keep on the host
     torch.cuda.synchronize()

@@ -1,10 +1,12 @@
-"""KPConv's neighbour gather + kernel-point correlation (pool.cu o3dml_kpconv_gather) and the index max pool
-(o3dml_gather_max) against float64 restatements, at every kernel instantiation the entry dispatches to and at the
-index, shape and scheduling edges where such kernels go wrong."""
+"""KPConv's neighbour gather + kernel-point correlation (pool.cu o3dml_kpconv_gather) against the torch port's gather
+(oracle/models_torch.kp_gather) in float64, and the index max pool (o3dml_gather_max) against a restatement, at every
+kernel instantiation the entry dispatches to and at the index, shape and scheduling edges where such kernels go
+wrong."""
 import pytest
 import torch
 
 from open3d_ml_b200 import _lib as L
+from oracle import models_torch as MT
 
 from conftest import rel_err
 
@@ -12,39 +14,6 @@ EXTENT = 0.125
 # Against float64 on an H100 80GB HBM3 (400 W power limit), the largest rel_err of the gathered tensor over all cases
 # below was 2.25e-7; the bound keeps about 5x of margin.
 KPG_TOL = 1.2e-6
-
-
-def kpconv_gather_reference(q_pts, s_pts, nidx, x, kpts, extent):
-    """A[q, k * Cin + c] = sum_h infl[q, k, h] * x[n_h, c] with infl = max(0, 1 - |s[n_h] - q - kp_k| / extent), zero for
-    ids < 0 or >= ns: the rigid, linear-influence, sum-aggregated KPConv.forward, in float64."""
-    q, s, x, kp = q_pts.double(), s_pts.double(), x.double(), kpts.double()
-    ns, nq, H = s.shape[0], q.shape[0], nidx.shape[1]
-    K, C = kp.shape[0], x.shape[1]
-    ok = (nidx >= 0) & (nidx < ns)
-    n = torch.where(ok, nidx, 0).long()
-    d = (s[n] - q.unsqueeze(1)).unsqueeze(2) - kp                          # [nq, H, K, 3]
-    infl = torch.clamp(1 - d.norm(dim=-1) / extent, min=0.0) * ok.unsqueeze(-1)
-    xs = x[n] * ok.unsqueeze(-1)
-    if H == 0:
-        return torch.zeros(nq, K * C, dtype=torch.float64, device=x.device)
-    return torch.einsum("qhk,qhc->qkc", infl, xs).reshape(nq, K * C)
-
-
-def test_reference_matches_oracle_kp_conv():
-    """The restatement above equals oracle.models_torch.kp_conv (shadow id == ns) in float64, identity weights."""
-    from oracle import models_torch as MT
-    g = torch.Generator().manual_seed(1)
-    nq, ns, H, K, C = 40, 60, 9, 15, 3
-    s = (torch.rand(ns, 3, generator=g, dtype=torch.float64) - 0.5) * 0.3
-    q = (torch.rand(nq, 3, generator=g, dtype=torch.float64) - 0.5) * 0.3
-    nb = torch.randint(0, ns + 1, (nq, H), generator=g)
-    x = torch.randn(ns, C, generator=g, dtype=torch.float64)
-    kp = (torch.rand(K, 3, generator=g, dtype=torch.float64) - 0.5) * 0.3
-    w = torch.eye(K * C, dtype=torch.float64).view(K, C, K * C)
-    ref = MT.kp_conv(q, s, nb, x, kp, w, EXTENT)
-    got = kpconv_gather_reference(q, s, nb, x, kp, EXTENT)
-    assert float((got - ref).abs().max()) <= 1e-12 * float(ref.abs().max())
-    assert float(got.abs().max()) > 0
 
 
 # in_channels, byte offset of the feature rows -> the lanes that share one query in the kernel the entry runs: the
@@ -98,7 +67,7 @@ def kpconv_gather_errors(cin, offset, int32):
                 q, s, nb, x, kp = _case(cin, H, K, nq, offset=offset, int32=int32, seed=K * 1000 + H * 10 + nq)
                 out = torch.full((nq + 5, K * cin), float("nan")).cuda()
                 L.check(_run(q, s, nb, x, kp, EXTENT, out))
-                ref = kpconv_gather_reference(q, s, nb, x, kp, EXTENT)
+                ref = MT.kp_gather(q.double(), s.double(), nb, x.double(), kp.double(), EXTENT).flatten(1)
                 assert bool(out[nq:].isnan().all()), (K, H, nq)
                 errs[(K, H, nq)] = rel_err(out[:nq], ref)
     return errs

@@ -1,13 +1,14 @@
-"""The fused pillar feature net + BEV scatter (voxelize.cu pp_pfn_scatter_kernel) against a float64 restatement of the
-reference's PillarFeatureNet + PFNLayer + PointPillarsScatter: dense [M, max_points, C] pillars, a mask over the padded
-slots, the mean over num_points and f_center from coords * voxel_size + offset.  The voxel CSR comes from the CUDA
-voxelize, which is bit-exact against the oracle (test_gpu_ops.py)."""
+"""The fused pillar feature net + BEV scatter (voxelize.cu pp_pfn_scatter_kernel) against the reference's
+PillarFeatureNet + PFNLayer + PointPillarsScatter in float64: dense [M, max_points, C] pillars gathered from the voxel
+CSR, decorated by the torch port (oracle/models_torch.pp_decorate), then the layer in the kernel's folded-BN form.  The
+voxel CSR comes from the CUDA voxelize, which is bit-exact against the oracle (test_gpu_ops.py)."""
 import numpy as np
 import pytest
 import torch
 
 from open3d_ml_b200 import _lib as L
 from open3d_ml_b200 import ops
+from oracle import models_torch as MT
 
 from conftest import rel_err
 
@@ -42,20 +43,22 @@ def _frame(n, C, max_pts, g):
     return torch.cat([xyz, extra], 1)
 
 
-def pfn_reference(pts, coords, vrs, pidx, M, max_pts, wt, scale, shift, vx, vy, x_off, y_off):
-    """[M, 64] float64 pillar features, the reference's own form (point_pillars.py PillarFeatureNet / PFNLayer)."""
+def pillar_decoration(pts, coords, vrs, pidx, M, max_pts, vx, vy, x_off, y_off):
+    """The first M pillars of the voxel CSR as dense float64 [M, P, C] pillars (padded slots zero), decorated by the
+    torch port: -> ([M, P, C+5] with the padded slots zeroed, the slot mask [M, P])."""
     rs = vrs[:M + 1].long()
     cnt = rs[1:] - rs[:-1]
     slot = torch.arange(max_pts, device=pts.device).view(1, -1)
     mask = slot < cnt.view(-1, 1)
     src = torch.where(mask, pidx[(rs[:-1].view(-1, 1) + slot).clamp_max(pidx.numel() - 1)], -1)
-    feats = torch.cat([torch.zeros_like(pts[:1]), pts]).double()
-    pillars = feats[src + 1]                                                   # [M, P, C], padded slots zero
-    mean = pillars[:, :, :3].sum(1, keepdim=True) / cnt.double().view(-1, 1, 1)
-    f_cluster = pillars[:, :, :3] - mean
+    pillars = torch.cat([torch.zeros_like(pts[:1]), pts]).double()[src + 1]
     c = coords[:M].double()
-    f_center = torch.stack([pillars[:, :, 0] - (c[:, 0:1] * vx + x_off), pillars[:, :, 1] - (c[:, 1:2] * vy + y_off)], -1)
-    f = torch.cat([pillars, f_cluster, f_center], -1) * mask.unsqueeze(-1).double()
+    return MT.pp_decorate(pillars, cnt, c[:, 0], c[:, 1], vx, vy, x_off, y_off), mask
+
+
+def pfn_reference(pts, coords, vrs, pidx, M, max_pts, wt, scale, shift, vx, vy, x_off, y_off):
+    """[M, 64] float64 pillar features (point_pillars.py PillarFeatureNet / PFNLayer)."""
+    f, _ = pillar_decoration(pts, coords, vrs, pidx, M, max_pts, vx, vy, x_off, y_off)
     y = torch.relu((f @ wt.double()) * scale.double() + shift.double())
     return y.max(1)[0]
 

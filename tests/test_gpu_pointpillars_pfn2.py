@@ -1,9 +1,9 @@
 """The fused two-layer pillar feature net + BEV scatter (o3dml_pp_pfn2_scatter, voxelize.cu pp_pfn_scatter_kernel<64,
-true>) against a float64 restatement of the reference's PillarFeatureNet with feat_channels [64, 64]
-(point_pillars.py:400-555) in its dense [M, max_points, C] form: layer 0 (32 units) on the masked decoration, its max
-over ALL slots m0, then layer 1 on cat(y0[p], m0) and the max over all slots again.  A padded slot's layer-1 input is
-[relu(BN0(0)) | m0], so its value differs per pillar; the cases make it decide many maxima.  Frames, canvas and
-scatter checks as in test_gpu_pointpillars_kernels.py."""
+true>) against the reference's PillarFeatureNet with feat_channels [64, 64] (point_pillars.py:400-555) in float64 in
+its dense [M, max_points, C] form: the torch port's masked decoration, layer 0 (32 units) on it, its max over ALL
+slots m0, then layer 1 on cat(y0[p], m0) and the max over all slots again.  A padded slot's layer-1 input is
+[relu(BN0(0)) | m0], so its value differs per pillar; the cases make it decide many maxima.  Frames, pillar gather,
+canvas and scatter checks as in test_gpu_pointpillars_kernels.py."""
 import numpy as np
 import pytest
 import torch
@@ -12,28 +12,13 @@ from open3d_ml_b200 import _lib as L
 from open3d_ml_b200 import ops
 
 from conftest import rel_err
-from test_gpu_pointpillars_kernels import COUT, NX, NY, RANGE, VOXEL, _frame, scatter_reference
+from test_gpu_pointpillars_kernels import COUT, NX, NY, RANGE, VOXEL, _frame, pillar_decoration, scatter_reference
 
 pytestmark = pytest.mark.gpu
 
 # Against float64 on an H100 80GB HBM3 (700 W power limit), the largest rel_err of the pillar features over the cases
 # below was 3.9e-7; the bound keeps about 5x of margin.
 PFN2_TOL = 2e-6
-
-
-def decorate(pts, coords, vrs, pidx, M, max_pts, vx, vy, x_off, y_off):
-    """[M, P, C+5] float64 decorated pillars with the padded slots zeroed, and the slot mask [M, P]."""
-    rs = vrs[:M + 1].long()
-    cnt = rs[1:] - rs[:-1]
-    slot = torch.arange(max_pts, device=pts.device).view(1, -1)
-    mask = slot < cnt.view(-1, 1)
-    src = torch.where(mask, pidx[(rs[:-1].view(-1, 1) + slot).clamp_max(pidx.numel() - 1)], -1)
-    feats = torch.cat([torch.zeros_like(pts[:1]), pts]).double()
-    pillars = feats[src + 1]
-    mean = pillars[:, :, :3].sum(1, keepdim=True) / cnt.double().view(-1, 1, 1)
-    c = coords[:M].double()
-    f_center = torch.stack([pillars[:, :, 0] - (c[:, 0:1] * vx + x_off), pillars[:, :, 1] - (c[:, 1:2] * vy + y_off)], -1)
-    return torch.cat([pillars, pillars[:, :, :3] - mean, f_center], -1) * mask.unsqueeze(-1).double(), mask
 
 
 def pfn2_reference(f, w0, s0, t0, w1, s1, t1):
@@ -99,7 +84,7 @@ def test_pfn2_scatter_vs_float64(C, max_pts):
 
     vx, vy = VOXEL[0], VOXEL[1]
     x_off, y_off = float(np.float32(vx / 2 + RANGE[0])), float(np.float32(vy / 2 + RANGE[1]))
-    f, mask = decorate(pts, coords, vrs, pidx, M, max_pts, vx, vy, x_off, y_off)
+    f, mask = pillar_decoration(pts, coords, vrs, pidx, M, max_pts, vx, vy, x_off, y_off)
     ref, y1 = pfn2_reference(f, *wts)
     err = rel_err(feat[:M], ref)
     assert err < PFN2_TOL, err

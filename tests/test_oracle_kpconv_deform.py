@@ -1,5 +1,5 @@
-"""Deformable KPConv without a GPU: the torch restatement (tests/kpconv_deform_support.py) against the unmodified
-reference's outputs stored in tests/golden/boundary_kpconv_deform_class.npz (Paris-Lille3D config, recorded by
+"""Deformable KPConv without a GPU: the torch port (oracle/models_torch.py) against the unmodified reference's
+outputs stored in tests/golden/boundary_kpconv_deform_class.npz (Paris-Lille3D config, recorded by
 tests/ref_kpconv_deform_case.py), the tied-kernel-point rule, and kpconv.layer_radii against the radii
 KPConvBatch.segmentation_inputs picks (concat_batcher.py:209-262)."""
 import json
@@ -9,9 +9,8 @@ import numpy as np
 import pytest
 import torch
 
-import kpconv_deform_support as KD
 from conftest import GOLDEN
-from oracle import weights
+from oracle import models_torch as MT, weights
 from open3d_ml_b200.kpconv import layer_radii
 
 # largest error of the port against the reference on this fixture: 2.6e-6 (logits), 2.7e-6 (blocks)
@@ -39,7 +38,7 @@ def port():
     g, sd, batch, cfg = fixture()
     taps, stats = {}, {}
     with torch.no_grad():
-        out = KD.kpfcnn_forward(sd, batch, cfg, taps=taps, stats=stats)
+        out = MT.kpfcnn_forward(sd, batch, cfg, taps=taps, stats=stats)
     return g, out, taps, stats
 
 
@@ -66,15 +65,15 @@ def test_port_follows_offset_conv_kernel_points():
     assert not torch.equal(sd[p + ".kernel_points"], sd[p + ".offset_conv.kernel_points"])   # seeded apart
     base = {}
     with torch.no_grad():
-        KD.kpfcnn_forward(sd, batch, cfg, taps=base)
+        MT.kpfcnn_forward(sd, batch, cfg, taps=base)
         other = dict(sd)
         other[p + ".kernel_points"] = sd[p + ".kernel_points"] * 3.0 + 1.0
         moved = {}
-        KD.kpfcnn_forward(other, batch, cfg, taps=moved)
+        MT.kpfcnn_forward(other, batch, cfg, taps=moved)
         assert torch.equal(moved["encoder_blocks.5"], base["encoder_blocks.5"])
         swapped = dict(sd)
         swapped[p + ".offset_conv.kernel_points"] = sd[p + ".kernel_points"]
-        KD.kpfcnn_forward(swapped, batch, cfg, taps=moved)
+        MT.kpfcnn_forward(swapped, batch, cfg, taps=moved)
         assert not torch.allclose(moved["encoder_blocks.5"], base["encoder_blocks.5"])
 
 

@@ -1,4 +1,4 @@
-"""The oracle forward with a PillarFeatureNet of one or two layers (pp_configs_support.pointpillars_forward) and the
+"""The oracle forward with a PillarFeatureNet of one or two layers (oracle/models_torch.pointpillars_forward) and the
 oracle box decoding (detect_support.pp_get_bboxes) against the UNMODIFIED reference PointPillars built from its
 nuScenes, Argoverse and Lyft ymls, recorded in tests/golden/pointpillars_config_<k>.npz
 (`python tests/ref_pointpillars_configs.py --ops oracle --record tests/golden`).  Runs without a GPU."""
@@ -10,7 +10,8 @@ import torch
 
 from detect_support import pp_detect_maps, pp_get_bboxes
 from open3d_ml_b200.pointpillars import grid_anchors
-from pp_configs_support import CONFIGS, DETECT_CASES, fixture, load, pointpillars_forward
+from oracle.models_torch import pointpillars_forward
+from pp_configs_support import CONFIGS, DETECT_CASES, fixture, load
 from test_oracle_detect import assert_margins
 
 TOL = 2e-5  # float32 re-association between two CPU implementations, relative to the output's max |value|
