@@ -185,6 +185,42 @@ O3DML_API int o3dml_continuous_conv(const float* filters, int size_x, int size_y
                                     int align_corners, int coordinate_mapping, int normalize, int interpolation,
                                     float* out, void* stream);
 
+/* open3d.ml.torch.ops.continuous_conv_transpose (op surface named by the north star; no call site in the reference),
+ *   the exact adjoint of o3dml_continuous_conv: for output j with the inputs i = neighbors_index[e] of its list
+ *   [neighbors_row_splits[j], neighbors_row_splits[j+1]),
+ *   out[j] = oimp_j * sum_e nimp_e * s_i * W(map((out_pos[j] - inp_pos[i]) * 2 / extent_i + offset))^T f[i]
+ *   with extent_i = extents[extents_per_point ? i : 0], oimp = out_importance and nimp = neighbors_importance (NULL:
+ *   ones), s_i = 1 / inp_neighbors_importance_sum[i] under normalize (NULL: 1 / the length of row i of
+ *   inp_neighbors_row_splits; one of the two is required), 1 for a zero divisor and without normalize.  Filter
+ *   layout, mapping, interpolation and limits as in o3dml_continuous_conv; fp32 sums in list order.  inp_positions /
+ *   inp_features may be NULL when num_inp == 0. */
+O3DML_API int o3dml_continuous_conv_transpose(const float* filters, int size_x, int size_y, int size_z,
+                                              int in_channels, int out_channels, const float* out_positions,
+                                              int64_t num_out, const float* out_importance, const float* extents,
+                                              int extents_per_point, const float* h_offset,
+                                              const float* inp_positions, const float* inp_features, int64_t num_inp,
+                                              const float* inp_neighbors_importance_sum,
+                                              const int64_t* inp_neighbors_row_splits, const void* neighbors_index,
+                                              int index_is64, const float* neighbors_importance,
+                                              const int64_t* neighbors_row_splits, int align_corners,
+                                              int coordinate_mapping, int normalize, int interpolation, float* out,
+                                              void* stream);
+
+/* open3d.ml.torch.ops.invert_neighbors_list(num_points, inp_neighbors_index, inp_neighbors_row_splits,
+ *   inp_neighbors_attributes) (no call site in the reference; pairs with the transposed convolution above):
+ *   num_inp rows of num_entries ids in [0, num_points) regrouped by id.  neighbors_index [num_entries] (int32 or
+ *   int64, as the input) holds, for every row j, the input rows i that contain j, once per occurrence, ordered by
+ *   (i, position in row i): a stable sort of the entries by id.  neighbors_row_splits int64 [num_points + 1].
+ *   Entries whose id is out of range are dropped: they follow the last row, in input order, and
+ *   neighbors_row_splits[num_points] counts the entries kept.  permutation int64 [num_entries]: the input entry at
+ *   each output position (the caller permutes per-entry attributes with it).  num_entries < 2^32. */
+O3DML_API size_t o3dml_invert_neighbors_list_workspace_bytes(int64_t num_entries);
+O3DML_API int o3dml_invert_neighbors_list(int64_t num_points, const void* inp_neighbors_index, int index_is64,
+                                          const int64_t* inp_neighbors_row_splits, int64_t num_inp,
+                                          int64_t num_entries, void* neighbors_index, int64_t* neighbors_row_splits,
+                                          int64_t* permutation, void* workspace, size_t workspace_bytes,
+                                          void* stream);
+
 /* ------------------------------------------- detection post-processing ---- */
 
 /* open3d.ml.torch.ops.nms(boxes, scores, nms_overlap_thresh) -- rotated-BEV greedy NMS

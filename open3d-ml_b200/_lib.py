@@ -45,6 +45,10 @@ _SIGNATURES = {
     "o3dml_sparse_conv_workspace_bytes": (Z, [L]),
     "o3dml_sparse_conv_neighbors": (I, [P, L, P, L, F, P, P, I, P, P, P, Z, P]),
     "o3dml_continuous_conv": (I, [P, I, I, I, I, I, P, L, P, I, P, P, P, L, P, P, I, P, P, I, I, I, I, P, P]),
+    "o3dml_continuous_conv_transpose": (I, [P, I, I, I, I, I, P, L, P, P, I, P, P, P, L, P, P, P, I, P, P, I, I, I, I,
+                                            P, P]),
+    "o3dml_invert_neighbors_list_workspace_bytes": (Z, [L]),
+    "o3dml_invert_neighbors_list": (I, [L, P, I, P, L, L, P, P, P, P, Z, P]),
     "o3dml_nms_workspace_bytes": (Z, [L]),
     "o3dml_nms": (I, [P, P, L, F, P, P, P, Z, P]),
     "o3dml_iou_matrix": (I, [P, L, P, L, I, P, P]),

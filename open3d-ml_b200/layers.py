@@ -159,3 +159,50 @@ class ContinuousConv(torch.nn.Module):
         if self.use_bias:
             out = out + self.bias.detach().to(out.device)
         return self.activation(out) if self.activation is not None else out
+
+
+class ContinuousConvTranspose(ContinuousConv):
+    """open3d.ml.torch.layers.ContinuousConvTranspose: the constructor, parameters (`kernel` [Sz, Sy, Sx, Cin, Cout],
+    `bias`) and `offset` buffer of ContinuousConv, so state_dicts load either way.  forward = one fixed-radius search
+    of the outputs around each input (radius = extent / 2), ops.invert_neighbors_list of its lists and
+    ops.continuous_conv_transpose; under `normalize` input i is scaled by 1 / its neighbour count.  One host read
+    (the search's count); inference only."""
+
+    def __init__(self, in_channels, filters, kernel_size, window_function=None, use_dense_layer_for_center=False,
+                 **kwargs):
+        if window_function is not None or use_dense_layer_for_center:
+            raise RuntimeError("ContinuousConvTranspose: window_function and use_dense_layer_for_center are not "
+                               "implemented")
+        super().__init__(in_channels, filters, kernel_size, **kwargs)
+        self._offset_host = None
+
+    def _host_offset(self):
+        """The `offset` buffer on the host, read once per version: the op takes it by value, and a module moved to
+        the GPU would otherwise pay a device->host read per call."""
+        key = (self.offset.data_ptr(), self.offset._version, str(self.offset.device))
+        if self._offset_host is None or self._offset_host[0] != key:
+            self._offset_host = (key, self.offset.detach().cpu())
+        return self._offset_host[1]
+
+    def forward(self, inp_features, inp_positions, out_positions, extents, out_importance=None, **kwargs):
+        from . import ops
+        for k in ("inp_neighbors_index", "inp_neighbors_importance_sum", "inp_neighbors_row_splits",
+                  "user_neighbors_index", "user_neighbors_row_splits", "user_neighbors_importance"):
+            if kwargs.get(k) is not None:
+                raise RuntimeError("ContinuousConvTranspose: %s is not implemented (the layer runs its own search)" % k)
+        ext = torch.as_tensor(extents, dtype=torch.float32).reshape(-1)
+        if ext.numel() != 1:
+            raise RuntimeError("ContinuousConvTranspose: one extent for all points (per-point extents: use "
+                               "ops.continuous_conv_transpose)")
+        ret_dev = inp_features.device
+        op, ip = ops._dev(out_positions.float()), ops._dev(inp_positions.float())
+        r = ops.fixed_radius_search(op, ip, float(ext[0]) * 0.5, return_distances=False)
+        inv = ops.invert_neighbors_list(op.shape[0], r.neighbors_index, r.neighbors_row_splits, torch.empty(0))
+        out = ops.continuous_conv_transpose(self.kernel.detach(), op, out_importance, ext, self._host_offset(), ip,
+                                            ops._dev(inp_features), r.neighbors_index, None, r.neighbors_row_splits,
+                                            inv.neighbors_index, None, inv.neighbors_row_splits, self.align_corners,
+                                            self.coordinate_mapping, self.normalize, self.interpolation)
+        if self.use_bias:
+            out = out + self.bias.detach().to(out.device)
+        out = self.activation(out) if self.activation is not None else out
+        return out.to(ret_dev)

@@ -496,6 +496,105 @@ def continuous_conv(filters, out_positions, extents, offset, inp_positions, inp_
     return out if was_cuda else out.cpu()
 
 
+InvertNeighborsListResult = collections.namedtuple(
+    "InvertNeighborsListResult", "neighbors_index neighbors_row_splits neighbors_attributes")
+
+
+def invert_neighbors_list(num_points, inp_neighbors_index, inp_neighbors_row_splits, inp_neighbors_attributes):
+    """open3d.ml.torch.ops.invert_neighbors_list: num_inp rows of ids in [0, num_points) -> num_points rows of the
+    input rows that contain each id, once per occurrence, by (input row, position in it): a stable sort by id.  Ids out
+    of range are dropped (they follow the last row; neighbors_row_splits[-1] counts the entries kept).  The attributes
+    ([E, ...], any dtype) are permuted the same way; an empty attributes tensor stays empty.  No host read."""
+    was_cuda = inp_neighbors_index.is_cuda
+    idx = _dev(inp_neighbors_index).reshape(-1).contiguous()
+    if idx.dtype not in (torch.int32, torch.int64):
+        raise RuntimeError("invert_neighbors_list: inp_neighbors_index must be int32 or int64")
+    if inp_neighbors_row_splits.dtype != torch.int64:
+        raise RuntimeError("row_splits must be int64")
+    rs = _dev(inp_neighbors_row_splits).contiguous()
+    num_points, e, num_inp = int(num_points), idx.numel(), rs.numel() - 1
+    if num_points < 0 or num_inp < 0:
+        raise RuntimeError("invert_neighbors_list: num_points must be >= 0 and row_splits non-empty")
+    attrs = inp_neighbors_attributes
+    if attrs.numel() and attrs.shape[0] != e:
+        raise RuntimeError("invert_neighbors_list: attributes must have one row per neighbour entry")
+    dev = idx.device
+    out_idx = torch.empty((e,), dtype=idx.dtype, device=dev)
+    out_rs = torch.empty((num_points + 1,), dtype=torch.int64, device=dev)
+    perm = torch.empty((e,), dtype=torch.int64, device=dev)
+    wsb = L.lib().o3dml_invert_neighbors_list_workspace_bytes(e)
+    ws = torch.empty((wsb,), dtype=torch.uint8, device=dev)
+    L.check(L.lib().o3dml_invert_neighbors_list(num_points, L.ptr(idx), L.is64(idx), L.ptr(rs), num_inp, e,
+                                                L.ptr(out_idx), L.ptr(out_rs), L.ptr(perm), L.ptr(ws), wsb,
+                                                L.stream()))
+    out_attrs = _dev(attrs)[perm] if attrs.numel() else attrs
+    if was_cuda:
+        return InvertNeighborsListResult(out_idx, out_rs, out_attrs)
+    return InvertNeighborsListResult(out_idx.cpu(), out_rs.cpu(), out_attrs.cpu())
+
+
+def continuous_conv_transpose(filters, out_positions, out_importance, extents, offset, inp_positions, inp_features,
+                              inp_neighbors_index, inp_neighbors_importance_sum, inp_neighbors_row_splits,
+                              neighbors_index, neighbors_importance, neighbors_row_splits, align_corners=False,
+                              coordinate_mapping="ball_to_cube_radial", normalize=False, interpolation="linear",
+                              max_temp_mem_MB=64):
+    """open3d.ml.torch.ops.continuous_conv_transpose (raw op; contract in csrc/cconv.cu), the adjoint of
+    continuous_conv: filters [Sz, Sy, Sx, Cin, Cout] as there, inp_features [num_inp, Cin] -> [num_out, Cout].
+    neighbors_* list the inputs of each output (invert_neighbors_list of the forward lists); extents [1] or
+    [num_inp]; empty importance tensors mean "all ones".  Under normalize input i is scaled by
+    1 / inp_neighbors_importance_sum[i], or by 1 / the length of its row of inp_neighbors_row_splits when that sum
+    is empty.  inp_neighbors_index is taken for signature parity and not read.  No host read."""
+    name = "continuous_conv_transpose"
+    if coordinate_mapping not in _CCONV_MAPPING:
+        raise RuntimeError("%s: coordinate_mapping '%s' is not implemented (identity, ball_to_cube_radial)"
+                           % (name, coordinate_mapping))
+    if interpolation not in _CCONV_INTERP:
+        raise RuntimeError("%s: unknown interpolation '%s'" % (name, interpolation))
+    if filters.dim() != 5:
+        raise RuntimeError("%s: filters must have shape [Sz, Sy, Sx, Cin, Cout]" % name)
+    was_cuda = inp_features.is_cuda
+    f = _dev(filters).to(torch.float32).contiguous()
+    op, ip = _dev(out_positions).to(torch.float32).contiguous(), _dev(inp_positions).to(torch.float32).contiguous()
+    feat = _dev(inp_features).to(torch.float32).contiguous()
+    num_out, num_inp = op.shape[0], ip.shape[0]
+    ext = _dev(torch.as_tensor(extents, dtype=torch.float32).reshape(-1)).contiguous()
+    if ext.numel() != 1 and (ext.numel() != num_inp or num_inp == 0):
+        raise RuntimeError("%s: extents must have 1 or num_inp elements" % name)
+    off = np.ascontiguousarray(torch.as_tensor(offset).detach().cpu().numpy(), dtype=np.float32).reshape(3)
+
+    def opt(t, n, what):
+        if t is None or t.numel() == 0:
+            return None
+        t = _dev(t).float().reshape(-1).contiguous()
+        if t.numel() != n:
+            raise RuntimeError("%s: %s must be empty or have %d elements" % (name, what, n))
+        return t
+    oimp = opt(out_importance, num_out, "out_importance")
+    isum = opt(inp_neighbors_importance_sum, num_inp, "inp_neighbors_importance_sum")
+    nimp = opt(neighbors_importance, neighbors_index.numel(), "neighbors_importance")
+    irs = None
+    if inp_neighbors_row_splits is not None and inp_neighbors_row_splits.numel():
+        irs = _dev(inp_neighbors_row_splits).to(torch.int64).contiguous()
+        if irs.numel() != num_inp + 1:
+            raise RuntimeError("%s: inp_neighbors_row_splits must have num_inp + 1 elements" % name)
+    idx = _dev(neighbors_index).contiguous()
+    if idx.dtype not in (torch.int32, torch.int64):
+        raise RuntimeError("%s: neighbors_index must be int32 or int64" % name)
+    rs = _dev(neighbors_row_splits).to(torch.int64).contiguous()
+    if rs.numel() != num_out + 1:
+        raise RuntimeError("%s: neighbors_row_splits must have num_out + 1 elements" % name)
+    sz, sy, sx, cin, cout = f.shape
+    if feat.dim() != 2 or feat.shape[0] != num_inp or feat.shape[1] != cin:
+        raise RuntimeError("%s: feature channels do not match the filter" % name)
+    out = torch.empty((num_out, cout), dtype=torch.float32, device=f.device)
+    L.check(L.lib().o3dml_continuous_conv_transpose(
+        L.ptr(f), sx, sy, sz, cin, cout, L.ptr(op), num_out, L.ptr(oimp), L.ptr(ext), 1 if ext.numel() > 1 else 0,
+        off.ctypes.data, L.ptr(ip), L.ptr(feat), num_inp, L.ptr(isum), L.ptr(irs), L.ptr(idx), L.is64(idx),
+        L.ptr(nimp), L.ptr(rs), 1 if align_corners else 0, _CCONV_MAPPING[coordinate_mapping], 1 if normalize else 0,
+        _CCONV_INTERP[interpolation], L.ptr(out), L.stream()))
+    return out if was_cuda else out.cpu()
+
+
 def sparse_conv(filters, inp_features, inp_importance, neighbors_index, neighbors_kernel_index, neighbors_importance,
                 neighbors_row_splits, normalize=False, max_temp_mem_MB=64):
     """open3d.ml.torch.ops.sparse_conv (raw op): out[o] = sum_j filters[kernel_index[j]]^T f[neighbors_index[j]] over

@@ -132,11 +132,12 @@ def install(ml3d_root=None):
             nms=O.nms,
             reduce_subarrays_sum=O.reduce_subarrays_sum,
             voxel_pooling=O.voxel_pooling,
-            continuous_conv=O.continuous_conv, sparse_conv=O.sparse_conv)
+            continuous_conv=O.continuous_conv, continuous_conv_transpose=O.continuous_conv_transpose,
+            invert_neighbors_list=O.invert_neighbors_list, sparse_conv=O.sparse_conv)
     from . import layers as LY
     _module("open3d.ml.torch.layers", FixedRadiusSearch=O.FixedRadiusSearch, KNNSearch=O.KNNSearch,
             SparseConv=LY.SparseConv, SparseConvTranspose=LY.SparseConvTranspose,
-            ContinuousConv=LY.ContinuousConv)
+            ContinuousConv=LY.ContinuousConv, ContinuousConvTranspose=LY.ContinuousConvTranspose)
     _module("open3d.ml.contrib", subsample=O.subsample, subsample_batch=O.subsample_batch,
             iou_bev_cpu=O.iou_bev, iou_bev_cuda=O.iou_bev, iou_3d_cpu=O.iou_3d, iou_3d_cuda=O.iou_3d)
     vis = _module("open3d.visualization")
