@@ -105,6 +105,47 @@ O3DML_API int o3dml_radius_fill(const float* queries, int64_t num_points, int64_
                       float* neighbors_distance2, void* workspace, size_t workspace_bytes,
                       void* stream);
 
+/* Distance metrics of the general searches below (DESIGN.md section 2): with d = query - point per axis,
+ * L2 = (dx*dx + dy*dy) + dz*dz (returned squared), L1 = (|dx| + |dy|) + |dz|, LINF = max(max(|dx|, |dy|), |dz|),
+ * all in float32 without FMA.  Rows ascend by (distance, index). */
+#define O3DML_METRIC_L2 0
+#define O3DML_METRIC_L1 1
+#define O3DML_METRIC_LINF 2
+
+/* open3d.ml.torch.ops.fixed_radius_search / radius_search and layers.FixedRadiusSearch / RadiusSearch with every
+ * option: the two phases of o3dml_radius_count / _fill (same workspace, o3dml_radius_workspace_bytes, left untouched
+ * between them), which are their L2 / one-radius / int32 case.  A point is kept when distance <= t, t = r * r for L2
+ * and r otherwise.  radii float32 [num_queries] (may be NULL: every query takes `radius`, which must be > 0): a
+ * negative, NaN or infinite radius gives an empty row.  ignore_query_point skips every point whose three coordinates
+ * equal the query's.  Both phases take the same radius, radii, metric and ignore_query_point.  Fill: neighbors_index
+ * int32 or int64 (index_is64) [total]; neighbors_distance float32 [total], divided by t (L2) or r (L1, LINF) under
+ * normalize_distances. */
+O3DML_API int o3dml_radius_search_count(const float* points, int64_t num_points, const int64_t* points_row_splits,
+                                        const float* queries, int64_t num_queries,
+                                        const int64_t* queries_row_splits, int64_t batch, float radius,
+                                        const float* radii, int metric, int ignore_query_point,
+                                        int64_t* neighbors_row_splits, int64_t* d_total, void* workspace,
+                                        size_t workspace_bytes, void* stream);
+O3DML_API int o3dml_radius_search_fill(const float* queries, int64_t num_points, int64_t num_queries,
+                                       const int64_t* queries_row_splits, int64_t batch, float radius,
+                                       const float* radii, int metric, int ignore_query_point,
+                                       int normalize_distances, const int64_t* neighbors_row_splits,
+                                       void* neighbors_index, int index_is64, float* neighbors_distance,
+                                       void* workspace, size_t workspace_bytes, void* stream);
+
+/* open3d.ml.torch.ops.knn_search / layers.KNNSearch with a metric and ignore_query_point; o3dml_knn_search is its
+ * L2 case without ignore_query_point.  Without ignore_query_point: out_index [num_queries, k] and out_distance
+ * [num_queries, k] (may be NULL) as there, out_row_splits and d_total unused.  With it a row may hold fewer than k
+ * neighbours: out_index / out_distance hold the rows back to back (room for num_queries * k entries),
+ * out_row_splits int64 [num_queries + 1] places them and d_total (int64 [1], may be NULL) is their total. */
+O3DML_API size_t o3dml_knn_search_metric_workspace_bytes(int64_t num_points, int64_t num_queries, int64_t batch,
+                                                         int k, int ignore_query_point);
+O3DML_API int o3dml_knn_search_metric(const float* points, int64_t num_points, const int64_t* points_row_splits,
+                                      const float* queries, int64_t num_queries, const int64_t* queries_row_splits,
+                                      int64_t batch, int k, int metric, int ignore_query_point, void* out_index,
+                                      int index_is64, float* out_distance, int64_t* out_row_splits,
+                                      int64_t* d_total, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Per-voxel reduction over the CSR voxel lists of o3dml_voxelize: the second half of
  *   open3d.ml.contrib.subsample / subsample_batch (barycentre grid subsampling,
  *   ml3d/datasets/utils/dataprocessing.py:14-49, ml3d/torch/models/kpconv.py:2037-2164) and of

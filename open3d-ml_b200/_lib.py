@@ -40,6 +40,10 @@ _SIGNATURES = {
     "o3dml_radius_workspace_bytes": (Z, [L, L, L]),
     "o3dml_radius_count": (I, [P, L, P, P, L, P, L, F, P, P, P, Z, P]),
     "o3dml_radius_fill": (I, [P, L, L, P, L, F, P, P, P, P, Z, P]),
+    "o3dml_radius_search_count": (I, [P, L, P, P, L, P, L, F, P, I, I, P, P, P, Z, P]),
+    "o3dml_radius_search_fill": (I, [P, L, L, P, L, F, P, I, I, I, P, P, I, P, P, Z, P]),
+    "o3dml_knn_search_metric_workspace_bytes": (Z, [L, L, L, I, I]),
+    "o3dml_knn_search_metric": (I, [P, L, P, P, L, P, L, I, I, I, P, I, P, P, P, P, Z, P]),
     "o3dml_voxel_reduce": (I, [P, I, P, I, I, P, P, P, P, L, I, I, P, P, P, P]),
     "o3dml_reduce_subarrays_sum": (I, [P, P, L, P, P]),
     "o3dml_sparse_conv_workspace_bytes": (Z, [L]),

@@ -8,8 +8,8 @@ CUDA library or a CUDA device raises RuntimeError (there is no CPU fallback).
 __version__ = "0.1.0"
 
 from . import ops, synth, shard  # noqa: F401,E402
-from .ops import (voxelize, ragged_to_dense, knn_search, fixed_radius_search,  # noqa: F401,E402
-                  FixedRadiusSearch, KNNSearch, NearestNeighborSearch, subsample, subsample_batch,
+from .ops import (voxelize, ragged_to_dense, knn_search, fixed_radius_search, radius_search,  # noqa: F401,E402
+                  FixedRadiusSearch, RadiusSearch, KNNSearch, NearestNeighborSearch, subsample, subsample_batch,
                   nms, iou_bev, iou_3d)
 
 

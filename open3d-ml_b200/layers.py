@@ -120,21 +120,31 @@ class SparseConvTranspose(_SparseConvBase):
 
 
 class ContinuousConv(torch.nn.Module):
-    """open3d.ml.torch.layers.ContinuousConv: fixed-radius search (radius = extent / 2) + ops.continuous_conv.
-    kernel parameter [Sz, Sy, Sx, Cin, Cout] (`kernel`), optional `bias`; inference only."""
+    """open3d.ml.torch.layers.ContinuousConv: radius search (radius = extent / 2, in `radius_search_metric`, skipping
+    points equal to the output point under `radius_search_ignore_query_points`) + ops.continuous_conv.  One extent:
+    fixed_radius_search; one per output point: radius_search with those radii.  `window_function`, when given, maps
+    the normalised distances (distance / (r * r) for L2, distance / r otherwise) to the neighbour importance.
+    user_neighbors_index / _row_splits / _importance replace the search and the window.  kernel parameter
+    [Sz, Sy, Sx, Cin, Cout] (`kernel`), optional `bias`; inference only."""
 
     def __init__(self, in_channels, filters, kernel_size, activation=None, use_bias=True, kernel_initializer=None,
                  bias_initializer=None, align_corners=True, coordinate_mapping="ball_to_cube_radial",
                  interpolation="linear", normalize=True, radius_search_ignore_query_points=False,
-                 radius_search_metric="L2", offset=None, **kwargs):
+                 radius_search_metric="L2", offset=None, window_function=None, use_dense_layer_for_center=False,
+                 **kwargs):
         super().__init__()
-        if radius_search_metric != "L2" or radius_search_ignore_query_points:
-            raise RuntimeError("ContinuousConv: only the L2 radius search including the query point")
+        if use_dense_layer_for_center:
+            raise RuntimeError("ContinuousConv: use_dense_layer_for_center is not implemented")
+        from . import ops
+        ops._metric(radius_search_metric, "ContinuousConv")
         ks = [int(k) for k in kernel_size]
         self.in_channels, self.filters, self.kernel_size = int(in_channels), int(filters), ks
         self.activation, self.use_bias = activation, bool(use_bias)
         self.align_corners, self.coordinate_mapping = bool(align_corners), coordinate_mapping
         self.interpolation, self.normalize = interpolation, bool(normalize)
+        self.radius_search_metric = radius_search_metric
+        self.radius_search_ignore_query_points = bool(radius_search_ignore_query_points)
+        self.window_function = window_function
         self.register_buffer("offset", torch.zeros(3) if offset is None else
                              torch.as_tensor(offset, dtype=torch.float32).reshape(3).clone())
         kernel = torch.empty(*ks, self.in_channels, self.filters)
@@ -146,15 +156,38 @@ class ContinuousConv(torch.nn.Module):
                 bias_initializer(bias)
             self.bias = torch.nn.Parameter(bias)
 
-    def forward(self, inp_features, inp_positions, out_positions, extents, inp_importance=None, **kwargs):
+    def _search(self):
+        return dict(metric=self.radius_search_metric, ignore_query_point=self.radius_search_ignore_query_points)
+
+    def forward(self, inp_features, inp_positions, out_positions, extents, inp_importance=None,
+                user_neighbors_index=None, user_neighbors_row_splits=None, user_neighbors_importance=None, **kwargs):
         from . import ops
         ext = torch.as_tensor(extents, dtype=torch.float32).reshape(-1)
-        if ext.numel() != 1:
-            raise RuntimeError("ContinuousConv: one extent for all points (per-point extents: use ops.continuous_conv)")
-        r = ops.fixed_radius_search(inp_positions.float(), out_positions.float(), float(ext[0]) * 0.5,
-                                    return_distances=False)
+        window = self.window_function
+        if user_neighbors_index is not None:
+            if user_neighbors_row_splits is None:
+                raise RuntimeError("ContinuousConv: user_neighbors_index needs user_neighbors_row_splits")
+            idx, splits, importance = user_neighbors_index, user_neighbors_row_splits, user_neighbors_importance
+        elif ext.numel() == 1:
+            r = float(ext[0]) * 0.5
+            res = ops.fixed_radius_search(inp_positions.float(), out_positions.float(), r,
+                                          return_distances=window is not None, **self._search())
+            idx, splits, importance = res.neighbors_index, res.neighbors_row_splits, None
+            if window is not None:
+                r32 = np.float32(r)
+                scale = r32 * r32 if self.radius_search_metric == "L2" else r32
+                importance = window(res.neighbors_distance / torch.tensor(scale, device=res.neighbors_distance.device))
+        else:
+            if ext.numel() != out_positions.shape[0]:
+                raise RuntimeError("ContinuousConv: extents must have 1 or num_out elements")
+            res = ops.radius_search(inp_positions.float(), out_positions.float(), ext * 0.5,
+                                    return_distances=window is not None, normalize_distances=window is not None,
+                                    **self._search())
+            idx, splits, importance = res.neighbors_index, res.neighbors_row_splits, None
+            if window is not None:
+                importance = window(res.neighbors_distance)
         out = ops.continuous_conv(self.kernel.detach(), out_positions, ext, self.offset, inp_positions, inp_features,
-                                  inp_importance, r.neighbors_index, None, r.neighbors_row_splits,
+                                  inp_importance, idx, importance, splits,
                                   self.align_corners, self.coordinate_mapping, self.normalize, self.interpolation)
         if self.use_bias:
             out = out + self.bias.detach().to(out.device)
@@ -196,7 +229,7 @@ class ContinuousConvTranspose(ContinuousConv):
                                "ops.continuous_conv_transpose)")
         ret_dev = inp_features.device
         op, ip = ops._dev(out_positions.float()), ops._dev(inp_positions.float())
-        r = ops.fixed_radius_search(op, ip, float(ext[0]) * 0.5, return_distances=False)
+        r = ops.fixed_radius_search(op, ip, float(ext[0]) * 0.5, return_distances=False, **self._search())
         inv = ops.invert_neighbors_list(op.shape[0], r.neighbors_index, r.neighbors_row_splits, torch.empty(0))
         out = ops.continuous_conv_transpose(self.kernel.detach(), op, out_importance, ext, self._host_offset(), ip,
                                             ops._dev(inp_features), r.neighbors_index, None, r.neighbors_row_splits,

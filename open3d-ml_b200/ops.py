@@ -9,6 +9,8 @@ Same names, argument meaning, result field names and error behaviour
     ragged_to_dense   point_pillars.py:364-366, kpconv.py:2030-2032
     knn_search        ml3d/torch/models/point_transformer.py:724-734
     FixedRadiusSearch ml3d/torch/models/kpconv.py:2021-2026
+    radius_search / RadiusSearch, and the metric / ignore_query_point / index_dtype options of the
+                      searches (no call site; contract in DESIGN.md section 2)
     NearestNeighborSearch  ml3d/datasets/utils/dataprocessing.py:99-103
 
 Inputs may live on the CPU (the reference's dataloaders call these ops with
@@ -149,15 +151,30 @@ def knn_search_raw(points, points_row_splits, queries, queries_row_splits, k, ou
                                      L.stream()))
 
 
+_METRICS = {"L2": 0, "L1": 1, "Linf": 2}
+
+
+def _metric(metric, name):
+    if metric not in _METRICS:
+        raise RuntimeError("%s: metric must be one of L1, L2, Linf (got %r)" % (name, metric))
+    return _METRICS[metric]
+
+
+def _index_dtype(index_dtype, name):
+    if index_dtype not in (torch.int32, torch.int64):
+        raise RuntimeError("%s: index_dtype must be torch.int32 or torch.int64" % name)
+    return index_dtype
+
+
 def knn_search(points, queries, k, points_row_splits=None, queries_row_splits=None,
                index_dtype=torch.int32, metric="L2", ignore_query_point=False,
                return_distances=False, allow_short=False):
-    """open3d.ml.torch.ops.knn_search.  Rows ascend by (distance, index); distances are squared
-    L2 as upstream returns them for metric='L2'."""
-    if metric != "L2":
-        raise RuntimeError("knn_search: only metric='L2' is implemented")
-    if ignore_query_point:
-        raise RuntimeError("knn_search: ignore_query_point is not implemented")
+    """open3d.ml.torch.ops.knn_search.  Rows ascend by (distance, index) in `metric` (L1, L2, Linf); L2 distances are
+    squared, as upstream returns them.  Dense [Nq * k] rows with row splits 0, k, 2k, ...; with ignore_query_point
+    (points equal to the query are skipped) a row may hold fewer than k neighbours, and the rows are ragged (one
+    device->host read of their total)."""
+    m = _metric(metric, "knn_search")
+    _index_dtype(index_dtype, "knn_search")
     _check_points(points), _check_points(queries, "queries")
     was_cuda = points.is_cuda
     p, q = _dev(points).contiguous(), _dev(queries).contiguous()
@@ -173,18 +190,38 @@ def knn_search(points, queries, k, points_row_splits=None, queries_row_splits=No
     if short < k:      # allow_short=True keeps the C-ABI behaviour: -1 / +inf padded dense rows
         raise RuntimeError("knn_search: a batch item has %d points, fewer than k = %d (ragged results are not "
                            "implemented)" % (short, k))
-    idx = torch.empty((q.shape[0], k), dtype=index_dtype, device=dev)
-    d2 = torch.empty((q.shape[0], k), dtype=torch.float32, device=dev) if return_distances else None
-    knn_search_raw(p, ps, q, qs, k, idx, d2)
-    rs = torch.arange(0, (q.shape[0] + 1) * k, k, dtype=torch.int64, device=dev)
+    nq = q.shape[0]
+    if m == 0 and not ignore_query_point:
+        idx = torch.empty((nq, k), dtype=index_dtype, device=dev)
+        d2 = torch.empty((nq, k), dtype=torch.float32, device=dev) if return_distances else None
+        knn_search_raw(p, ps, q, qs, k, idx, d2)
+        rs = torch.arange(0, (nq + 1) * k, k, dtype=torch.int64, device=dev)
+    else:
+        ig = 1 if ignore_query_point else 0
+        idx = torch.empty((nq * k,), dtype=index_dtype, device=dev)
+        d2 = torch.empty((nq * k,), dtype=torch.float32, device=dev) if return_distances else None
+        rs = torch.arange(0, (nq + 1) * k, k, dtype=torch.int64, device=dev) if not ig else \
+            torch.empty((nq + 1,), dtype=torch.int64, device=dev)
+        total = torch.zeros((1,), dtype=torch.int64, device=dev)
+        wsb = L.lib().o3dml_knn_search_metric_workspace_bytes(p.shape[0], nq, batch, k, ig)
+        ws = torch.empty((wsb,), dtype=torch.uint8, device=dev)
+        L.check(L.lib().o3dml_knn_search_metric(L.ptr(p), p.shape[0], L.ptr(ps), L.ptr(q), nq, L.ptr(qs), batch, k, m,
+                                                ig, L.ptr(idx), L.is64(idx), L.ptr(d2), L.ptr(rs), L.ptr(total),
+                                                L.ptr(ws), wsb, L.stream()))
+        if ig:
+            t = int(total.item())
+            idx, d2 = idx[:t], (d2[:t] if d2 is not None else None)
     out = KnnResult(idx.reshape(-1), rs,
                     d2.reshape(-1) if d2 is not None else torch.empty(0, device=dev))
     return out if was_cuda else KnnResult(*(t.cpu() for t in out))
 
 
-def fixed_radius_search(points, queries, radius, points_row_splits=None, queries_row_splits=None,
-                        return_distances=True):
-    """Two-phase radius search (count, one device->host read of the total, fill)."""
+def _radius_search(name, points, queries, radius, radii, points_row_splits, queries_row_splits, index_dtype, metric,
+                   ignore_query_point, return_distances, normalize_distances):
+    """Two-phase radius search (count, one device->host read of the total, fill) with one radius (radii None) or
+    one per query."""
+    m = _metric(metric, name)
+    _index_dtype(index_dtype, name)
     _check_points(points), _check_points(queries, "queries")
     was_cuda = points.is_cuda
     p, q = _dev(points).contiguous(), _dev(queries).contiguous()
@@ -192,38 +229,78 @@ def fixed_radius_search(points, queries, radius, points_row_splits=None, queries
     ps, qs = _splits(points_row_splits, p.shape[0], dev), _splits(queries_row_splits, q.shape[0], dev)
     batch = ps.numel() - 1
     if qs.numel() - 1 != batch:
-        raise RuntimeError("fixed_radius_search: row splits disagree on the batch size")
+        raise RuntimeError("%s: row splits disagree on the batch size" % name)
     nq = q.shape[0]
+    if radii is not None:
+        radii = _dev(torch.as_tensor(radii)).reshape(-1).contiguous()
+        if radii.dtype != torch.float32 or radii.numel() != nq:
+            raise RuntimeError("%s: radii must be float32 with one radius per query (%d)" % (name, nq))
+    ig, norm = 1 if ignore_query_point else 0, 1 if normalize_distances else 0
     nrs = torch.empty((nq + 1,), dtype=torch.int64, device=dev)
     total = torch.zeros((1,), dtype=torch.int64, device=dev)
     wsb = L.lib().o3dml_radius_workspace_bytes(p.shape[0], nq, batch)
     ws = torch.empty((wsb,), dtype=torch.uint8, device=dev)
-    L.check(L.lib().o3dml_radius_count(L.ptr(p), p.shape[0], L.ptr(ps), L.ptr(q), nq, L.ptr(qs),
-                                       batch, float(radius), L.ptr(nrs), L.ptr(total), L.ptr(ws),
-                                       wsb, L.stream()))
+    L.check(L.lib().o3dml_radius_search_count(L.ptr(p), p.shape[0], L.ptr(ps), L.ptr(q), nq, L.ptr(qs), batch,
+                                              float(radius), L.ptr(radii), m, ig, L.ptr(nrs), L.ptr(total), L.ptr(ws),
+                                              wsb, L.stream()))
     t = int(total.item())
-    idx = torch.empty((t,), dtype=torch.int32, device=dev)
-    d2 = torch.empty((t,), dtype=torch.float32, device=dev)
-    L.check(L.lib().o3dml_radius_fill(L.ptr(q), p.shape[0], nq, L.ptr(qs), batch, float(radius),
-                                      L.ptr(nrs), L.ptr(idx), L.ptr(d2), L.ptr(ws), wsb, L.stream()))
-    out = RadiusResult(idx, nrs, d2 if return_distances else torch.empty(0, device=dev))
+    idx = torch.empty((t,), dtype=index_dtype, device=dev)
+    d = torch.empty((t,), dtype=torch.float32, device=dev)
+    if t:      # with no neighbour at all there is nothing to fill (and the empty outputs have no address)
+        L.check(L.lib().o3dml_radius_search_fill(L.ptr(q), p.shape[0], nq, L.ptr(qs), batch, float(radius),
+                                                 L.ptr(radii), m, ig, norm, L.ptr(nrs), L.ptr(idx), L.is64(idx),
+                                                 L.ptr(d), L.ptr(ws), wsb, L.stream()))
+    out = RadiusResult(idx, nrs, d if return_distances else torch.empty(0, device=dev))
     return out if was_cuda else RadiusResult(*(t_.cpu() for t_ in out))
 
 
+def fixed_radius_search(points, queries, radius, points_row_splits=None, queries_row_splits=None,
+                        return_distances=True, index_dtype=torch.int32, metric="L2", ignore_query_point=False):
+    """open3d.ml.torch.ops.fixed_radius_search: the points within `radius` (> 0) of each query in `metric` (L1, L2,
+    Linf; L2 distances squared), rows by (distance, index); ignore_query_point skips points equal to the query.  Two
+    phases (count, one device->host read of the total, fill)."""
+    return _radius_search("fixed_radius_search", points, queries, radius, None, points_row_splits, queries_row_splits,
+                          index_dtype, metric, ignore_query_point, return_distances, False)
+
+
+def radius_search(points, queries, radii, points_row_splits=None, queries_row_splits=None, index_dtype=torch.int32,
+                  metric="L2", ignore_query_point=False, return_distances=False, normalize_distances=False):
+    """open3d.ml.torch.ops.radius_search: fixed_radius_search with one radius per query, radii float32 [Nq].  A
+    negative, NaN or infinite radius gives an empty row; r = 0 keeps the points equal to the query.
+    normalize_distances returns distance / (r * r) for L2 and distance / r otherwise (NaN for r = 0)."""
+    return _radius_search("radius_search", points, queries, 0.0, radii, points_row_splits, queries_row_splits,
+                          index_dtype, metric, ignore_query_point, return_distances, normalize_distances)
+
+
 class FixedRadiusSearch(torch.nn.Module):
-    """open3d.ml.torch.layers.FixedRadiusSearch (kpconv.py:2021-2026)."""
+    """open3d.ml.torch.layers.FixedRadiusSearch (kpconv.py:2021-2026).  A prebuilt hash_table is accepted and not
+    used: the search builds its own grid."""
 
     def __init__(self, metric="L2", ignore_query_point=False, return_distances=False,
                  max_hash_table_size=32 * 2**20, index_dtype=torch.int32, **kwargs):
         super().__init__()
-        if metric != "L2" or ignore_query_point:
-            raise RuntimeError("FixedRadiusSearch: only metric='L2', ignore_query_point=False")
-        self.return_distances = return_distances
+        _metric(metric, "FixedRadiusSearch")
+        self.kw = dict(metric=metric, ignore_query_point=ignore_query_point,
+                       return_distances=return_distances, index_dtype=_index_dtype(index_dtype, "FixedRadiusSearch"))
 
     def forward(self, points, queries, radius, points_row_splits=None, queries_row_splits=None,
                 hash_table_size_factor=1 / 64, hash_table=None):
-        return fixed_radius_search(points, queries, radius, points_row_splits, queries_row_splits,
-                                   self.return_distances)
+        return fixed_radius_search(points, queries, radius, points_row_splits, queries_row_splits, **self.kw)
+
+
+class RadiusSearch(torch.nn.Module):
+    """open3d.ml.torch.layers.RadiusSearch: radius_search with one radius per query."""
+
+    def __init__(self, metric="L2", ignore_query_point=False, return_distances=False, normalize_distances=False,
+                 index_dtype=torch.int32, **kwargs):
+        super().__init__()
+        _metric(metric, "RadiusSearch")
+        self.kw = dict(metric=metric, ignore_query_point=ignore_query_point, return_distances=return_distances,
+                       normalize_distances=normalize_distances,
+                       index_dtype=_index_dtype(index_dtype, "RadiusSearch"))
+
+    def forward(self, points, queries, radii, points_row_splits=None, queries_row_splits=None):
+        return radius_search(points, queries, radii, points_row_splits, queries_row_splits, **self.kw)
 
 
 class KNNSearch(torch.nn.Module):
@@ -232,8 +309,9 @@ class KNNSearch(torch.nn.Module):
     def __init__(self, metric="L2", ignore_query_point=False, return_distances=False,
                  index_dtype=torch.int32, **kwargs):
         super().__init__()
+        _metric(metric, "KNNSearch")
         self.kw = dict(metric=metric, ignore_query_point=ignore_query_point,
-                       return_distances=return_distances, index_dtype=index_dtype)
+                       return_distances=return_distances, index_dtype=_index_dtype(index_dtype, "KNNSearch"))
 
     def forward(self, points, queries, k, points_row_splits=None, queries_row_splits=None):
         return knn_search(points, queries, k, points_row_splits, queries_row_splits, **self.kw)

@@ -128,14 +128,15 @@ def install(ml3d_root=None):
     ml = _module("open3d.ml")
     mlt = _module("open3d.ml.torch")
     _module("open3d.ml.torch.ops", voxelize=O.voxelize, ragged_to_dense=O.ragged_to_dense,
-            knn_search=O.knn_search, fixed_radius_search=O.fixed_radius_search,
+            knn_search=O.knn_search, fixed_radius_search=O.fixed_radius_search, radius_search=O.radius_search,
             nms=O.nms,
             reduce_subarrays_sum=O.reduce_subarrays_sum,
             voxel_pooling=O.voxel_pooling,
             continuous_conv=O.continuous_conv, continuous_conv_transpose=O.continuous_conv_transpose,
             invert_neighbors_list=O.invert_neighbors_list, sparse_conv=O.sparse_conv)
     from . import layers as LY
-    _module("open3d.ml.torch.layers", FixedRadiusSearch=O.FixedRadiusSearch, KNNSearch=O.KNNSearch,
+    _module("open3d.ml.torch.layers", FixedRadiusSearch=O.FixedRadiusSearch, RadiusSearch=O.RadiusSearch,
+            KNNSearch=O.KNNSearch,
             SparseConv=LY.SparseConv, SparseConvTranspose=LY.SparseConvTranspose,
             ContinuousConv=LY.ContinuousConv, ContinuousConvTranspose=LY.ContinuousConvTranspose)
     _module("open3d.ml.contrib", subsample=O.subsample, subsample_batch=O.subsample_batch,
