@@ -31,6 +31,32 @@ def test_library_builds_loads_and_exports_everything():
     assert _lib.lib().o3dml_last_error() is not None
 
 
+# the exports that enqueue nothing: version, error and counter functions, sizing functions and capability queries
+ENQUEUE_NOTHING = (
+    "o3dml_abi_version", "o3dml_last_error", "o3dml_launch_count", "o3dml_launch_count_add",
+    "o3dml_voxelize_workspace_bytes", "o3dml_knn_workspace_bytes", "o3dml_radius_workspace_bytes",
+    "o3dml_knn_search_metric_workspace_bytes", "o3dml_sparse_conv_workspace_bytes",
+    "o3dml_invert_neighbors_list_workspace_bytes", "o3dml_nms_workspace_bytes", "o3dml_pp_detect_workspace_bytes",
+    "o3dml_linear_tc_supported", "o3dml_linear_rows_small_supported", "o3dml_randla_tail_supported",
+)
+
+
+def test_contract_tables_cover_every_export():
+    """Every export is reached by a launch-count case or enqueues nothing, and every sizing function is checked by an
+    exact-workspace case on the GPU and by a refusal row without one."""
+    from open3d_ml_b200 import _lib
+    from abi_cases import LAUNCH_CASES, REFUSAL_ROWS, WORKSPACE_CASES
+    exports, quiet = set(_lib.EXPORTS), set(ENQUEUE_NOTHING)
+    launched = {entry for entry, _ in LAUNCH_CASES.values()}
+    sizing = {name for name in exports if name.endswith("_workspace_bytes")}
+    for what, names in [("not exported", (launched | quiet) - exports),
+                        ("both launched and enqueuing nothing", launched & quiet),
+                        ("no launch-count case", exports - launched - quiet),
+                        ("no exact-workspace case", sizing - {s for s, _ in WORKSPACE_CASES.values()}),
+                        ("no refusal row", sizing - {s for s, _ in REFUSAL_ROWS.values()})]:
+        assert not names, "%s: %s" % (what, ", ".join(sorted(names)))
+
+
 def test_sass_is_sm90a_only():
     import subprocess
     from open3d_ml_b200 import build

@@ -1,12 +1,8 @@
 """continuous_conv_transpose, invert_neighbors_list and layers.ContinuousConvTranspose on the GPU: the op against the
 float64 oracle over the forward's parameter grid and at its shape and input edges, the inversion bit-equal to its
-oracle, the layer against oracle search + inversion + transpose and as the adjoint of the forward layer, the launch
-counts of both entries against a profiler trace (in a process of its own), and the inversion's exact workspace."""
-import json
-import os
-import subprocess
-import sys
-
+oracle and its refusal of 2^32 entries, and the layer against oracle search + inversion + transpose and as the
+adjoint of the forward layer.  The launch counts and exact workspaces of both C entries are checked with every other
+entry's (tests/abi_cases.py)."""
 import numpy as np
 import pytest
 import torch
@@ -15,9 +11,7 @@ import open3d_ml_b200 as M
 from open3d_ml_b200 import _lib as L, layers as LY
 from oracle import ops as O
 import cconv_transpose_oracle as R
-from abi_cases import WsCase
-from conftest import ROOT, rel_err
-from test_gpu_launch_count import counted_and_traced
+from conftest import rel_err
 
 pytestmark = pytest.mark.gpu
 
@@ -293,109 +287,6 @@ def test_layer_refusals_and_state_dict():
 
 
 # --------------------------------------------------------------------------------------------------- the C ABI
-def invert_case(num_entries, num_points=3000, rows=None, seed=48):
-    """o3dml_invert_neighbors_list over num_entries ids in rows of up to 8, a tenth of them out of range."""
-    rng = np.random.default_rng(seed)
-    rows = rows if rows is not None else max(1, num_entries // 4)
-    lens = np.zeros(rows, np.int64)
-    if num_entries:
-        cuts = np.sort(rng.integers(0, num_entries + 1, rows - 1))
-        lens = np.diff(np.concatenate([[0], cuts, [num_entries]]))
-    splits = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
-    idx = rng.integers(-1, num_points + num_points // 10, num_entries).astype(np.int32)
-    d_idx, d_splits = T(idx), T(splits)
-    out = dict(idx=torch.empty(num_entries, dtype=torch.int32).cuda(),
-               rs=torch.empty(num_points + 1, dtype=torch.int64).cuda(),
-               perm=torch.empty(num_entries, dtype=torch.int64).cuda())
-
-    def run(ws, nbytes):
-        return L.lib().o3dml_invert_neighbors_list(num_points, L.ptr(d_idx), 0, L.ptr(d_splits), rows, num_entries,
-                                                   L.ptr(out["idx"]), L.ptr(out["rs"]), L.ptr(out["perm"]), ws,
-                                                   nbytes, L.stream())
-    case = WsCase(L.lib().o3dml_invert_neighbors_list_workspace_bytes(num_entries), run, list(out.values()))
-    case.ref = R.invert_neighbors_list(num_points, idx.astype(np.int64), splits)
-    return case
-
-
-def transpose_call():
-    rng = np.random.default_rng(49)
-    n, m, cin, cout = 80, 50, 4, 8
-    ip, op, fidx, fsplits, tidx, tsplits, perm = graph(rng, n, m, 0.5)
-    f, o, i = T(rng.standard_normal((2, 2, 2, cin, cout)).astype(np.float32)), T(op), T(ip)
-    feat, ext = T(rng.standard_normal((n, cin)).astype(np.float32)), torch.tensor([0.5]).cuda()
-    off = np.zeros(3, np.float32)
-    idx, rs, fs = T(tidx.astype(np.int32)), T(tsplits), T(fsplits)
-    out = torch.empty(m, cout).cuda()
-    return lambda: L.lib().o3dml_continuous_conv_transpose(
-        L.ptr(f), 2, 2, 2, cin, cout, L.ptr(o), m, None, L.ptr(ext), 0, off.ctypes.data, L.ptr(i), L.ptr(feat), n,
-        None, L.ptr(fs), L.ptr(idx), 0, None, L.ptr(rs), 1, 1, 1, 1, L.ptr(out), L.stream())
-
-
-LAUNCH_CASES = {
-    "continuous_conv_transpose": transpose_call,
-    "invert_neighbors_list": lambda: invert_case(5000).with_own_workspace(),
-    "invert_neighbors_list_no_entries": lambda: invert_case(0, rows=10).with_own_workspace(),
-}
-
-
-def profile_launch_cases():
-    """{case: (counter delta, kernel names in the trace)} of one call of each LAUNCH_CASES entry."""
-    out = {}
-    for case, build in LAUNCH_CASES.items():
-        call = build()
-        for _ in range(3):      # a session now and then delivers no records at all (see test_gpu_launch_count)
-            counted, names = counted_and_traced(call)
-            if names:
-                break
-        out[case] = (counted, names)
-    return out
-
-
-@pytest.fixture(scope="module")
-def launch_profiles():
-    """profile_launch_cases run in a process of its own.  A profiling session opened in the pytest process before
-    test_gpu_launch_count.py runs makes that module's sessions lose the first kernel records of each call, so no session
-    is opened here."""
-    code = "import json, test_gpu_cconv_transpose as t; print(json.dumps(t.profile_launch_cases()))"
-    env = dict(os.environ, PYTHONPATH=os.pathsep.join([ROOT, os.path.join(ROOT, "tests")]))
-    r = subprocess.run([sys.executable, "-c", code], cwd=ROOT, env=env, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stderr[-4000:]
-    return json.loads(r.stdout.strip().splitlines()[-1])
-
-
-@pytest.mark.parametrize("case", list(LAUNCH_CASES))
-def test_launch_count_matches_profiled_kernels(case, launch_profiles):
-    counted, names = launch_profiles[case]
-    assert names and counted == len(names), (case, counted, names)
-    squashed = [n.replace(" ", "") for n in names]
-    if case == "continuous_conv_transpose":
-        assert any("cconv_kernel<true>" in n for n in squashed), names
-    else:
-        assert any("inv_splits_kernel" in n for n in squashed), names
-
-
-TAIL, PATTERN = 4096, 0xA5
-
-
-@pytest.mark.parametrize("num_entries", [0, 9000])
-def test_invert_exact_workspace_suffices_and_one_byte_less_is_refused(num_entries):
-    """9 000 entries span five 2 048-key sort blocks; the key bound (about 3 300) takes two 8-bit passes."""
-    case = invert_case(num_entries)
-    wsb = case.wsb
-    buf = torch.full((wsb + TAIL,), PATTERN, dtype=torch.uint8, device="cuda")
-    for t in case.outputs:
-        t.zero_()
-    L.check(case.run(L.ptr(buf), wsb))
-    torch.cuda.synchronize()
-    idx, rs, perm = (t.cpu().numpy() for t in case.outputs)
-    assert np.array_equal(idx, case.ref[0]) and np.array_equal(rs, case.ref[1]) and np.array_equal(perm, case.ref[2])
-    assert bool((buf[wsb:] == PATTERN).all()), "wrote past its %d-byte workspace" % wsb
-    n0 = L.lib().o3dml_launch_count()
-    assert case.run(L.ptr(buf), wsb - 1) == 2, L.lib().o3dml_last_error().decode()
-    assert ("(%d needed)" % wsb) in L.lib().o3dml_last_error().decode()
-    assert L.lib().o3dml_launch_count() == n0
-
-
 def test_invert_refuses_2_to_the_32_entries():
     rs = torch.zeros(2, dtype=torch.int64).cuda()
     out_rs = torch.empty(11, dtype=torch.int64).cuda()

@@ -1,10 +1,9 @@
 """The general neighbour searches on the GPU: radius_search (one radius per query), the L1 / Linf metrics,
 ignore_query_point, normalize_distances and index_dtype of fixed_radius_search / radius_search / knn_search, bit-equal
 to the oracle (oracle/search.py c_search_*) on uniform, LiDAR-like and room clouds; the layers from CPU and CUDA tensors
-and through the shim; repeatability; launch counts against a profiler trace (in a process of its own); exact
-workspaces; layers.ContinuousConv with the new search options, window and user lists; and the adjoint identity of
-ContinuousConvTranspose with an L1 search that ignores query points."""
-import json
+and through the shim; repeatability; layers.ContinuousConv with the new search options, window and user lists; and the
+adjoint identity of ContinuousConvTranspose with an L1 search that ignores query points.  The launch counts and exact
+workspaces of the C entries are checked with every other entry's (tests/abi_cases.py)."""
 import os
 import subprocess
 import sys
@@ -14,10 +13,9 @@ import pytest
 import torch
 
 import open3d_ml_b200 as M
-from open3d_ml_b200 import _lib as L, layers as LY, synth
+from open3d_ml_b200 import layers as LY, synth
 from oracle import ops as O, search as S
 from conftest import ROOT, rel_err
-from test_gpu_launch_count import counted_and_traced
 
 pytestmark = pytest.mark.gpu
 
@@ -210,132 +208,6 @@ def test_runs_repeat_bit_for_bit():
         for x, y in zip(first, run()):
             assert torch.equal(x, y) or (x.dtype.is_floating_point and torch.equal(x.isnan(), y.isnan()) and
                                          torch.equal(x.nan_to_num(), y.nan_to_num()))
-
-
-# ------------------------------------------------------------------------------------------------ the C ABI
-class SearchCase:
-    """One o3dml_radius_search_count + _fill (radii given) or one o3dml_knn_search_metric call, inputs on the GPU."""
-
-    def __init__(self, what, num_points=2000, num_queries=900, batch_splits=((0, 1200, 2000), (0, 500, 900))):
-        rng = np.random.default_rng(9)
-        self.what = what
-        self.p = T(rng.random((num_points, 3)).astype(np.float32))
-        self.q = T(rng.random((num_queries, 3)).astype(np.float32))
-        self.ps, self.qs = T(np.array(batch_splits[0], np.int64)), T(np.array(batch_splits[1], np.int64))
-        self.np, self.nq, self.batch = num_points, num_queries, len(batch_splits[0]) - 1
-        self.radii = T(rng.uniform(0.02, 0.08, num_queries).astype(np.float32))
-        self.rs = torch.empty(num_queries + 1, dtype=torch.int64).cuda()
-        self.total = torch.zeros(1, dtype=torch.int64).cuda()
-        self.k = 12
-        if what == "knn":
-            self.wsb = L.lib().o3dml_knn_search_metric_workspace_bytes(num_points, num_queries, self.batch, self.k, 1)
-            self.idx = torch.empty(num_queries * self.k, dtype=torch.int64).cuda()
-            self.d = torch.empty(num_queries * self.k).cuda()
-        else:
-            self.wsb = L.lib().o3dml_radius_workspace_bytes(num_points, num_queries, self.batch)
-
-    def count(self, ws, nbytes):
-        if self.what == "knn":
-            return L.lib().o3dml_knn_search_metric(L.ptr(self.p), self.np, L.ptr(self.ps), L.ptr(self.q), self.nq,
-                                                   L.ptr(self.qs), self.batch, self.k, 1, 1, L.ptr(self.idx), 1,
-                                                   L.ptr(self.d), L.ptr(self.rs), L.ptr(self.total), ws, nbytes,
-                                                   L.stream())
-        return L.lib().o3dml_radius_search_count(L.ptr(self.p), self.np, L.ptr(self.ps), L.ptr(self.q), self.nq,
-                                                 L.ptr(self.qs), self.batch, 0.0, L.ptr(self.radii), 2, 1,
-                                                 L.ptr(self.rs), L.ptr(self.total), ws, nbytes, L.stream())
-
-    def prepare_fill(self):
-        t = int(self.total.item())
-        self.idx, self.d = torch.zeros(t, dtype=torch.int64).cuda(), torch.zeros(t).cuda()
-
-    def fill(self, ws, nbytes):
-        return L.lib().o3dml_radius_search_fill(L.ptr(self.q), self.np, self.nq, L.ptr(self.qs), self.batch, 0.0,
-                                                L.ptr(self.radii), 2, 1, 1, L.ptr(self.rs), L.ptr(self.idx), 1,
-                                                L.ptr(self.d), ws, nbytes, L.stream())
-
-    def reference(self):
-        p, q = self.p.cpu().numpy(), self.q.cpu().numpy()
-        ps, qs = self.ps.cpu().numpy(), self.qs.cpu().numpy()
-        if self.what == "knn":
-            idx, d, n = S.c_search_knn(p, q, self.k, ps, qs, 1, True)
-            keep = np.arange(self.k)[None, :] < n[:, None]
-            return idx[keep], np.concatenate([[0], np.cumsum(n)]), d[keep]
-        return S.c_search_radius(p, q, 0.0, self.radii.cpu().numpy(), ps, qs, 2, True, True)
-
-
-def launch_call(what):
-    case = SearchCase(what)
-    ws = torch.empty(case.wsb, dtype=torch.uint8).cuda()
-    if what == "radius_fill":
-        L.check(case.count(L.ptr(ws), case.wsb))
-        case.prepare_fill()
-        return lambda: case.fill(L.ptr(ws), case.wsb)
-    return lambda: case.count(L.ptr(ws), case.wsb)
-
-
-LAUNCH_CASES = {
-    "radius_search_count": lambda: launch_call("radius_count"),
-    "radius_search_fill": lambda: launch_call("radius_fill"),
-    "knn_search_metric_ignore": lambda: launch_call("knn"),
-}
-EXPECT = {"radius_search_count": "radius_kernel<0,2,true,true>", "radius_search_fill": "radius_kernel<1,2,true,true>",
-          "knn_search_metric_ignore": "knn_compact_kernel"}
-
-
-def profile_launch_cases():
-    out = {}
-    for case, build in LAUNCH_CASES.items():
-        call = build()
-        for _ in range(3):      # a session now and then delivers no records at all (see test_gpu_launch_count)
-            counted, names = counted_and_traced(call)
-            if names:
-                break
-        out[case] = (counted, names)
-    return out
-
-
-@pytest.fixture(scope="module")
-def launch_profiles():
-    """profile_launch_cases in a process of its own, for the reason given in test_gpu_cconv_transpose.py."""
-    code = "import json, test_gpu_search as t; print(json.dumps(t.profile_launch_cases()))"
-    env = dict(os.environ, PYTHONPATH=os.pathsep.join([ROOT, os.path.join(ROOT, "tests")]))
-    r = subprocess.run([sys.executable, "-c", code], cwd=ROOT, env=env, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stderr[-4000:]
-    return json.loads(r.stdout.strip().splitlines()[-1])
-
-
-@pytest.mark.parametrize("case", list(LAUNCH_CASES))
-def test_launch_count_matches_profiled_kernels(case, launch_profiles):
-    counted, names = launch_profiles[case]
-    assert names and counted == len(names), (case, counted, names)
-    assert any(EXPECT[case] in n.replace(" ", "") for n in names), names
-
-
-TAIL, PATTERN = 4096, 0xA5
-
-
-@pytest.mark.parametrize("what", ["radius", "knn"])
-def test_exact_workspace_suffices_and_one_byte_less_is_refused(what):
-    case = SearchCase(what)
-    wsb = case.wsb
-    buf = torch.full((wsb + TAIL,), PATTERN, dtype=torch.uint8, device="cuda")
-    L.check(case.count(L.ptr(buf), wsb))
-    if what == "radius":
-        case.prepare_fill()
-        L.check(case.fill(L.ptr(buf), wsb))
-    torch.cuda.synchronize()
-    ref_idx, ref_rs, ref_d = case.reference()
-    t = int(case.total.item())
-    assert np.array_equal(case.rs.cpu().numpy(), ref_rs) and t == ref_rs[-1]
-    assert np.array_equal(case.idx[:t].cpu().numpy(), ref_idx)
-    assert np.array_equal(case.d[:t].cpu().numpy(), ref_d)
-    assert bool((buf[wsb:] == PATTERN).all()), "wrote past its %d-byte workspace" % wsb
-    calls = [case.count] + ([case.fill] if what == "radius" else [])
-    for call in calls:
-        n0 = L.lib().o3dml_launch_count()
-        assert call(L.ptr(buf), wsb - 1) == 2, L.lib().o3dml_last_error().decode()
-        assert ("(%d needed)" % wsb) in L.lib().o3dml_last_error().decode()
-        assert L.lib().o3dml_launch_count() == n0
 
 
 # ------------------------------------------------------------------------------------------- ContinuousConv

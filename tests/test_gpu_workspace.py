@@ -2,32 +2,23 @@
 scratch paths: scans above one 4 096-element tile (the look-back path, which uses its temp), radix sorts over several
 2 048-key blocks, batches with an empty item, NMS over more than 64 boxes, box decoding with and without top-k
 selection.  The exact workspace sits at the front of a larger buffer whose tail holds a byte pattern: the outputs must
-be bit-equal to those of a run with twice the workspace, and the tail must be untouched.  One byte less is refused
-(status 2) before anything is enqueued."""
+be bit-equal to those of a run with twice the workspace, and the tail must be untouched.  Where a case has an oracle,
+the outputs must equal it too; a k-NN output whose rows are packed at its front is compared over their length.  One
+byte less is refused (status 2) before anything is enqueued.  The cases are abi_cases.WORKSPACE_CASES."""
+import numpy as np
 import pytest
 import torch
 
 from open3d_ml_b200 import _lib as L
-from abi_cases import knn_case, nms_case, pp_detect_case, radius_case, sparse_conv_case, voxelize_case
+from abi_cases import WORKSPACE_CASES
 
 pytestmark = pytest.mark.gpu
 
 TAIL, PATTERN = 4096, 0xA5
 
-CASES = {
-    "voxelize": lambda: voxelize_case(splits=(0, 20000, 20000, 40000), voxel=0.1, max_voxels=30000),
-    "knn": lambda: knn_case(p_splits=(0, 3000, 3000, 6000), q_splits=(0, 2500, 5000, 5000)),
-    "radius": lambda: radius_case(p_splits=(0, 3000, 3000, 6000), q_splits=(0, 2500, 5000, 5000), radius=0.3),
-    "sparse_conv_neighbors": lambda: sparse_conv_case(5000),
-    "sparse_conv_neighbors_no_inputs": lambda: sparse_conv_case(0),
-    "nms": lambda: nms_case(3000),
-    "pp_detect": lambda: pp_detect_case(False),
-    "pp_detect_select": lambda: pp_detect_case(True),
-}
-
 
 def calls(case):
-    """The entries a case runs, in order: o3dml_radius_fill follows o3dml_radius_count on the same workspace."""
+    """The entries a case runs, in order: a fill follows its count on the same workspace."""
     return [case.run, case.fill] if hasattr(case, "fill") else [case.run]
 
 
@@ -45,9 +36,11 @@ def run(case, ws, nbytes):
     return out
 
 
-@pytest.mark.parametrize("name", list(CASES))
+@pytest.mark.parametrize("name", list(WORKSPACE_CASES))
 def test_exact_workspace_suffices_and_one_byte_less_is_refused(name):
-    case = CASES[name]()
+    sizing, build = WORKSPACE_CASES[name]
+    case = build()
+    assert case.sizing == sizing, name
     wsb = case.wsb
     big = torch.empty(2 * wsb, dtype=torch.uint8, device="cuda")
     want = run(case, L.ptr(big), 2 * wsb)
@@ -57,6 +50,11 @@ def test_exact_workspace_suffices_and_one_byte_less_is_refused(name):
     for a, b in zip(got, want):
         assert torch.equal(a.view(torch.uint8), b.view(torch.uint8)), name
     assert bool((buf[wsb:] == PATTERN).all()), "%s wrote past its %d-byte workspace" % (name, wsb)
+    if case.reference:
+        ref = case.reference()
+        assert len(ref) == len(got), name
+        for i, (a, r) in enumerate(zip(got, ref)):
+            assert np.array_equal(a.cpu().numpy()[:len(r)], r), "%s: output %d differs from the oracle" % (name, i)
 
     n0 = L.lib().o3dml_launch_count()
     for call in calls(case):
