@@ -230,24 +230,27 @@ __global__ void __launch_bounds__(64) pp_nms_mask_kernel(const float* __restrict
     const int seg = blockIdx.z, ib = blockIdx.y, jb = blockIdx.x;
     const int n = seg_cnt[seg], words = (n + 63) >> 6;
     if (jb < ib || jb >= words) return;
-    __shared__ RBox sb[64];
-    __shared__ float sr[64];
+    __shared__ RBoxXY sb[64];
+    __shared__ float3 sc[64];      // absolute centre and bounding radius, for the early-out only
     const float* base = bev + (size_t)seg * K * 5;
     const int j0 = jb * 64;
     if (j0 + (int)threadIdx.x < n) {
-        const RBox q = rbox_xyxyr(base + (size_t)(j0 + threadIdx.x) * 5);
+        const RBoxXY q = rbox_xyxyr(base + (size_t)(j0 + threadIdx.x) * 5);
+        const float w = q.x1 - q.x0, h = q.y1 - q.y0;
         sb[threadIdx.x] = q;
-        sr[threadIdx.x] = 0.5f * sqrtf(q.w * q.w + q.h * q.h);
+        sc[threadIdx.x] = make_float3(0.5f * (q.x0 + q.x1), 0.5f * (q.y0 + q.y1), 0.5f * sqrtf(w * w + h * h));
     }
     __syncthreads();
     const int i = ib * 64 + threadIdx.x;
     if (i >= n) return;
-    const RBox a = rbox_xyxyr(base + (size_t)i * 5);
-    const float ra = 0.5f * sqrtf(a.w * a.w + a.h * a.h);
+    const RBoxXY a = rbox_xyxyr(base + (size_t)i * 5);
+    const float aw = a.x1 - a.x0, ah = a.y1 - a.y0, ra = 0.5f * sqrtf(aw * aw + ah * ah);
+    const float acx = 0.5f * (a.x0 + a.x1), acy = 0.5f * (a.y0 + a.y1);
     unsigned long long bits = 0;
     const int cnt = min(64, n - j0);
     for (int k = (ib == jb ? threadIdx.x + 1 : 0); k < cnt; ++k) {
-        const float dx = a.cx - sb[k].cx, dy = a.cy - sb[k].cy, rr = 1.001f * (ra + sr[k]) + 1e-6f;
+        const float3 c = sc[k];
+        const float dx = acx - c.x, dy = acy - c.y, rr = 1.001f * (ra + c.z) + 1e-6f;
         if (dx * dx + dy * dy > rr * rr) continue;
         if (rbox_iou(a, sb[k]) > kNmsIou) bits |= 1ull << k;
     }

@@ -7,7 +7,8 @@
 //       call sites: ml3d/metrics/mAP.py:85-89, ml3d/datasets/utils/operations.py:430
 // Contract (upstream Open3D is not vendored: parity unpinned, oracle/ops_ref.c restates the same):
 //   * a box is the rectangle centre (cx, cy), size (w, h) rotated by r about its centre; the overlap of two
-//     boxes is the area of the intersection polygon (Sutherland-Hodgman clipping, shoelace area) in fp32;
+//     boxes is the area of the intersection polygon (Sutherland-Hodgman clipping, shoelace area) in fp32, clipped in
+//     a frame centred on the first box and clamped to the smaller box's area (so IoU is in [0, 1]);
 //   * nms: boxes are visited by descending score (ties: lower index first); a box is kept unless its IoU with an
 //     already kept box exceeds thr; the result lists the kept ORIGINAL indices in visiting order;
 //   * iou_3d: (x, z) is the ground plane with footprint (w, l) and heading ry, y the vertical axis with the box
@@ -38,8 +39,10 @@ __global__ void iou_matrix_kernel(const float* __restrict__ a, int64_t na, const
         const float inter2 = rbox_intersection(ra, rb);
         const float ymax = fminf(p[1], q[1]), ymin = fmaxf(p[1] - p[4], q[1] - q[4]);
         const float ih = fmaxf(ymax - ymin, 0.f);
-        const float inter = inter2 * ih;
-        const float uni = p[3] * p[4] * p[5] + q[3] * q[4] * q[5] - inter;
+        // the volumes as plain products (no FMA), the intersection clamped to the smaller: IoU <= 1, as in rbox_iou
+        const float va = __fmul_rn(__fmul_rn(p[3], p[4]), p[5]), vb = __fmul_rn(__fmul_rn(q[3], q[4]), q[5]);
+        const float inter = fminf(inter2 * ih, fmaxf(fminf(va, vb), 0.f));     // >= 0 with a side <= 0
+        const float uni = va + vb - inter;
         out[t] = uni > 0.f ? inter / uni : 0.f;
     }
 }
@@ -49,6 +52,7 @@ __global__ void nms_keys_kernel(const float* __restrict__ scores, int64_t n, uin
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     uint32_t u = __float_as_uint(scores[i]);
+    if (u == 0x80000000u) u = 0u;                      // -0.0 == +0.0: equal scores, visited by index
     u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);    // ascending order of u == ascending order of the float
     keys[i] = (uint64_t)(~u);                          // descending score
 }
@@ -58,25 +62,17 @@ __global__ void nms_mask_kernel(const float* __restrict__ boxes, const uint32_t*
                                 uint64_t* __restrict__ mask, int64_t words) {
     const int64_t ib = blockIdx.y, jb = blockIdx.x;
     if (jb < ib) return;
-    __shared__ float sb[64][5];
+    __shared__ RBoxXY sb[64];
     const int64_t j0 = jb * 64;
-    if (j0 + threadIdx.x < n) {
-        const float* q = boxes + (size_t)order[j0 + threadIdx.x] * 5;
-#pragma unroll
-        for (int k = 0; k < 5; ++k) sb[threadIdx.x][k] = q[k];
-    }
+    if (j0 + threadIdx.x < n) sb[threadIdx.x] = rbox_xyxyr(boxes + (size_t)order[j0 + threadIdx.x] * 5);
     __syncthreads();
     const int64_t i = ib * 64 + threadIdx.x;
     if (i >= n) return;
-    const float* p = boxes + (size_t)order[i] * 5;
-    const RBox a = rbox_xywhr(0.5f * (p[0] + p[2]), 0.5f * (p[1] + p[3]), p[2] - p[0], p[3] - p[1], p[4]);
+    const RBoxXY a = rbox_xyxyr(boxes + (size_t)order[i] * 5);
     uint64_t bits = 0;
     const int cnt = (int)min((int64_t)64, n - j0);
-    for (int k = (ib == jb ? threadIdx.x + 1 : 0); k < cnt; ++k) {
-        const RBox b = rbox_xywhr(0.5f * (sb[k][0] + sb[k][2]), 0.5f * (sb[k][1] + sb[k][3]), sb[k][2] - sb[k][0],
-                                  sb[k][3] - sb[k][1], sb[k][4]);
-        if (rbox_iou(a, b) > thr) bits |= 1ull << k;
-    }
+    for (int k = (ib == jb ? threadIdx.x + 1 : 0); k < cnt; ++k)
+        if (rbox_iou(a, sb[k]) > thr) bits |= 1ull << k;
     mask[i * words + jb] = bits;
 }
 

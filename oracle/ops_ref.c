@@ -295,12 +295,16 @@ static void rbox_corners(const rbox_t *b, double *x, double *y) {
         y[i] = b->cy + dx[i] * b->s + dy[i] * b->c;
     }
 }
+/* clipped in a frame centred on a; at most min(area a, area b) */
 static double rbox_intersection(const rbox_t *a, const rbox_t *b) {
     if (!(a->w > 0) || !(a->h > 0) || !(b->w > 0) || !(b->h > 0)) return 0.0;
     double px[16], py[16], qx[16], qy[16], bx[4], by[4];
     int n = 4;
-    rbox_corners(a, px, py);
-    rbox_corners(b, bx, by);
+    rbox_t a0 = *a, b0 = *b;
+    a0.cx = 0; a0.cy = 0;
+    b0.cx = b->cx - a->cx; b0.cy = b->cy - a->cy;
+    rbox_corners(&a0, px, py);
+    rbox_corners(&b0, bx, by);
     for (int e = 0; e < 4 && n > 0; ++e) {
         double x0 = bx[e], y0 = by[e], ex = bx[(e + 1) & 3] - x0, ey = by[(e + 1) & 3] - y0;
         int m = 0;
@@ -325,7 +329,9 @@ static double rbox_intersection(const rbox_t *a, const rbox_t *b) {
         int j = (i + 1 == n) ? 0 : i + 1;
         area += px[i] * py[j] - px[j] * py[i];
     }
-    return area > 0 ? 0.5 * area : 0.0;
+    area = area > 0 ? 0.5 * area : 0.0;
+    const double amin = fmin(a->w * a->h, b->w * b->h);
+    return area < amin ? area : amin;
 }
 static double rbox_iou(const rbox_t *a, const rbox_t *b) {
     double inter = rbox_intersection(a, b);
@@ -349,8 +355,9 @@ EXPORT int oracle_iou_matrix(const float *a, int64_t na, const float *b, int64_t
                 double ya = (double)p[1] - p[4], yb = (double)q[1] - q[4];
                 double ymin = ya > yb ? ya : yb;
                 double ih = ymax - ymin > 0 ? ymax - ymin : 0;
-                double inter = inter2 * ih;
-                double uni = (double)p[3] * p[4] * p[5] + (double)q[3] * q[4] * q[5] - inter;
+                double va = (double)p[3] * p[4] * p[5], vb = (double)q[3] * q[4] * q[5];
+                double inter = fmin(inter2 * ih, fmax(fmin(va, vb), 0.0));
+                double uni = va + vb - inter;
                 out[i * nb + j] = (float)(uni > 0 ? inter / uni : 0.0);
             }
         }

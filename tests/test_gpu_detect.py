@@ -104,9 +104,9 @@ def compare_with_oracle(net, cls, reg, dir_, C, head, name, exact_ties=False, to
     return boxes, labels
 
 
-# The Waymo case runs at B = 1 only: its smallest |IoU - 0.01| over 3 x 4096 boxes per frame falls below IOU_NOISE
-# once several frames are pooled.
-@pytest.mark.parametrize("name,B", [(n, B) for n in EDGE for B in ((1,) if n == "waymo" else (1, 3, 8))])
+# The Waymo case runs at B <= 3: its smallest |IoU - 0.01| over 3 x 4096 boxes per frame is 5.6e-6 at B = 3 and
+# 1.5e-6 at B = 8, below IOU_NOISE.
+@pytest.mark.parametrize("name,B", [(n, B) for n in EDGE for B in ((1, 3) if n == "waymo" else (1, 3, 8))])
 def test_fused_get_bboxes_matches_oracle(name, B):
     spec = EDGE[name]
     head = fixture_heads()[spec["head"]]

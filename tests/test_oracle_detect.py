@@ -10,10 +10,11 @@ import torch
 
 from detect_support import pp_detect_maps, pp_get_bboxes
 from helpers import golden
+from rbox_cases import IOU_TOL
 from open3d_ml_b200.pointpillars import grid_anchors
 
 FP32_NOISE = 1e-6          # scores are in [0, 1]: a few ulps of 1.0; the yaw fraction is O(1)
-IOU_NOISE = 1e-5           # IoU of metre-sized boxes from fp32 corners at |x| <= 75 m: a few 1e-6
+IOU_NOISE = IOU_TOL        # |IoU_fp32 - IoU_f64| of the rotated-box kernels, measured in tests/test_gpu_rbox.py
 
 
 def detect_case(g, case):
