@@ -36,7 +36,7 @@ __global__ void voxel_reduce_kernel(const float* __restrict__ pts, int pld, cons
     for (int64_t j = s; j < e; ++j) {
         const float x = src[(size_t)pidx[j] * ld];
         if (mode == 0) acc = __fadd_rn(acc, x);
-        else if (mode == 1) acc = fmaxf(acc, x);
+        else if (mode == 1) acc = (x > acc || x != x) ? x : acc;  // a NaN stays (fmaxf would drop it)
         else if (j == s) acc = x;
     }
     if (mode == 0) acc = __fdiv_rn(acc, (float)(e - s));

@@ -185,20 +185,26 @@ __global__ void vox_emit_points_kernel(const uint64_t* __restrict__ ks,
     if (rank < kept[v]) point_indices[(size_t)kept_excl[v] + rank] = vs[j];
 }
 
+// 0, or 1: voxel size not positive, 2: more than 2^40 cells, 3: a non-finite extent (an infinite or NaN range bound,
+// or a voxel size whose inverse overflows).  The extent is bounded before it is converted to int64 and the cell count
+// after every multiply, both without overflow.
 static int vox_make_grid(const float* vs, const float* rmin, const float* rmax, VoxGrid* g) {
+    constexpr int64_t MAX_CELLS = (int64_t)1 << 40;
     g->cells = 1;
     for (int d = 0; d < 3; ++d) {
         if (!(vs[d] > 0.f)) return 1;
         volatile float iv = 1.0f / vs[d];
         volatile float span = rmax[d] - rmin[d];
         volatile float c = span * iv;
+        if (!isfinite(c)) return 3;
+        if (c > (float)MAX_CELLS) return 2;
         int64_t e = (int64_t)ceilf(c);
         if (e < 1) e = 1;
         g->inv[d] = iv;
         g->rmin[d] = rmin[d];
         g->rmax[d] = rmax[d];
         g->ext1[d] = e + 1;
-        if (g->cells > (int64_t)1 << 40) return 2;
+        if (g->cells > MAX_CELLS / (e + 1)) return 2;  // cells * (e + 1) > MAX_CELLS
         g->cells *= (e + 1);
     }
     return 0;
@@ -444,8 +450,9 @@ extern "C" int o3dml_voxelize(const float* points, int64_t num_points, int point
     O3DML_CHECK(max_points_per_voxel >= 1 && max_voxels >= 1, "voxelize: caps must be >= 1");
     VoxGrid g;
     int rc = vox_make_grid(h_voxel_size, h_range_min, h_range_max, &g);
-    O3DML_CHECK(rc == 0, rc == 1 ? "voxelize: voxel_size must be positive"
-                                 : "voxelize: grid too large (> 2^40 cells)");
+    O3DML_CHECK(rc == 0, rc == 1   ? "voxelize: voxel_size must be positive"
+                         : rc == 2 ? "voxelize: grid too large (> 2^40 cells)"
+                                   : "voxelize: range and voxel_size must give a finite grid");
     O3DML_CHECK((double)g.cells * (double)batch < 4.0e18, "voxelize: grid x batch too large");
     const int64_t n = num_points;
     if (n == 0) {

@@ -368,10 +368,21 @@ def voxel_reduce(points, features, labels, vrs, pidx, counts=None, num_voxels=No
 
 
 def _subsample_range(pts, dl):
-    """Grid origin = floor(min / dl) * dl (float32), upper bound = max: ONE device->host read."""
+    """Grid origin = the largest float32 <= floor(min / dl) * dl, upper bound = max: ONE device->host read.
+
+    The origin is worked out in float64 with dl at its float32 value.  k * dl is then exact (a 24-bit significand
+    times an integer, exact while |min / dl| < 2^29), so the one rounding of min / dl is corrected by a comparison, and the origin is rounded down
+    to float32: origin <= min on every axis, so voxelize's `origin <= p` test keeps the cloud's minimum.  A float32
+    product rounded to nearest can land above min (min = -58.2, dl = 0.04 gives -58.199997) and drop that point."""
     mm = torch.stack([pts.amin(0), pts.amax(0)]).cpu().numpy().astype(np.float32)
-    dl = np.float32(dl)
-    origin = (np.floor((mm[0] / dl).astype(np.float32)) * dl).astype(np.float32)
+    if not np.isfinite(mm).all():
+        raise RuntimeError("subsample: the points must be finite (min %s, max %s)" % (mm[0], mm[1]))
+    mn, d = mm[0].astype(np.float64), np.float64(np.float32(dl))
+    k = np.floor(mn / d)
+    k -= k * d > mn
+    o64 = k * d
+    origin = o64.astype(np.float32)
+    origin = np.where(origin > o64, np.nextafter(origin, np.float32(-np.inf)), origin).astype(np.float32)
     return origin, mm[1]
 
 

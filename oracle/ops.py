@@ -242,12 +242,20 @@ def np_radius(points, queries, radius, points_row_splits=None, queries_row_split
 # grid subsampling (contract: ops_ref.c, "grid subsampling")
 # ----------------------------------------------------------------------------
 def subsample_range(points, dl):
-    """range_min / range_max of the voxel grid: origin = floor(min / dl) * dl in float32."""
+    """range_min / range_max of the voxel grid: origin = the largest float32 <= floor(min / dl) * dl, the product
+    exact in float64 with dl at its float32 value, so origin <= min; non-finite points raise RuntimeError."""
     points = _f32(points)
-    dl = np.float32(dl)
     mn, mx = points.min(0), points.max(0)
-    origin = (np.floor((mn / dl).astype(np.float32)) * dl).astype(np.float32)
-    return origin, mx.astype(np.float32)
+    if not (np.isfinite(mn).all() and np.isfinite(mx).all()):
+        raise RuntimeError("subsample: the points must be finite")
+    d = np.float64(np.float32(dl))
+    m64 = mn.astype(np.float64)
+    k = np.floor(m64 / d)
+    k = np.where(k * d > m64, k - 1, k)        # min / d rounded up onto an integer
+    o64 = k * d
+    origin = o64.astype(np.float32)
+    origin = np.where(origin.astype(np.float64) > o64, np.nextafter(origin, np.float32(-np.inf)), origin)
+    return origin.astype(np.float32), mx.astype(np.float32)
 
 
 def c_subsample_batch(points, batches_len, features=None, classes=None, sampleDl=0.1, max_p=0):

@@ -237,9 +237,11 @@ EXPORT int oracle_voxelize(const float *points, const int64_t *row_splits, int64
  * subsample_batch, call sites ml3d/datasets/utils/dataprocessing.py:14-49 and
  * ml3d/torch/models/kpconv.py:2037-2164; upstream = KPConv's grid_subsampling.cpp, barycentre
  * method).  PARITY UNPINNED (no golden vectors in the reference).  Contract fixed here:
- *   - voxels come from oracle_voxelize with range_min = floor(min(points) / dl) * dl over ALL batch
- *     items, range_max = max(points), no caps -> ascending linear index per batch item;
+ *   - voxels come from oracle_voxelize with range_min = the largest float32 <= floor(min(points) / dl) * dl
+ *     over ALL batch items (oracle/ops.py subsample_range), range_max = max(points), no caps -> ascending
+ *     linear index per batch item;
  *   - barycentre / feature mean = sequential float32 sum in ascending point id, one division;
+ *   - max: a NaN input makes the voxel's max NaN;
  *   - label = most frequent label of the voxel, ties -> smallest label.
  * mode: 0 mean, 1 max, 2 first. */
 EXPORT int oracle_voxel_reduce(const float *points, int point_stride, const float *features, int F,
@@ -255,7 +257,7 @@ EXPORT int oracle_voxel_reduce(const float *points, int point_stride, const floa
             for (int64_t j = s; j < e; ++j) {
                 float x = is_pos ? points[pidx[j] * point_stride + c] : features[pidx[j] * F + (c - 3)];
                 if (mode == 0) acc = acc + x;
-                else if (mode == 1) acc = x > acc ? x : acc;
+                else if (mode == 1) acc = (x > acc || x != x) ? x : acc; /* NaN propagates */
                 else if (j == s) acc = x;
             }
             if (mode == 0) acc = acc / (float)(e - s);
