@@ -133,6 +133,11 @@ def stream():
     return torch.cuda.current_stream().cuda_stream
 
 
+def workspace(nbytes, device):
+    """An entry point's scratch buffer: `nbytes` (its o3dml_*_workspace_bytes) of uint8 on `device`."""
+    return torch.empty((nbytes,), dtype=torch.uint8, device=device)
+
+
 def act_code(act):
     return {None: 0, "none": 0, "relu": 1, "leaky": 2}[act]
 

@@ -16,20 +16,20 @@ from . import _lib as L
 def sparse_conv_neighbors(inp_positions, out_positions, voxel_size, offset, kernel_size, transpose=False,
                           want_count=False):
     """int32 [M, kx*ky*kz] table (shadow id = N) and, optionally, the per-output count of non-empty cells."""
+    from . import ops
     L.require_cuda()
     ip = inp_positions.to("cuda", torch.float32).contiguous()
     op = out_positions.to("cuda", torch.float32).contiguous()
     n, m = ip.shape[0], op.shape[0]
     ks = np.asarray(kernel_size, dtype=np.int32).reshape(3)
-    off = np.ascontiguousarray(torch.as_tensor(offset).detach().cpu().numpy(), dtype=np.float32).reshape(3)
+    off = ops._host3(offset, "offset")
     kc = int(ks.prod())
     nbr = torch.empty((m, kc), dtype=torch.int32, device=ip.device)
     cnt = torch.empty((m,), dtype=torch.int32, device=ip.device) if want_count else None
-    wsb = L.lib().o3dml_sparse_conv_workspace_bytes(n)
-    ws = torch.empty((wsb,), dtype=torch.uint8, device=ip.device)
+    ws = L.workspace(L.lib().o3dml_sparse_conv_workspace_bytes(n), ip.device)
     L.check(L.lib().o3dml_sparse_conv_neighbors(L.ptr(ip), n, L.ptr(op), m, float(voxel_size), off.ctypes.data,
                                                 ks.ctypes.data, 1 if transpose else 0, L.ptr(nbr), L.ptr(cnt),
-                                                L.ptr(ws), wsb, L.stream()))
+                                                L.ptr(ws), ws.numel(), L.stream()))
     return nbr, cnt
 
 
@@ -50,6 +50,26 @@ def contract_cells(feat, table, groups, out, bias=None):
         L.linear(srcs, pw, out, None, None if gi else bias, residual=out if gi else None, act=None)
 
 
+def _kernel_and_bias(layer, kernel_initializer, bias_initializer):
+    """The `kernel` [*kernel_size, in_channels, filters] and, under use_bias, `bias` parameters of a conv layer, with
+    upstream's default initialisers (kernel uniform in [-0.05, 0.05], bias zero)."""
+    kernel = torch.empty(*layer.kernel_size, layer.in_channels, layer.filters)
+    (kernel_initializer or (lambda t: torch.nn.init.uniform_(t, -0.05, 0.05)))(kernel)
+    layer.kernel = torch.nn.Parameter(kernel)
+    if layer.use_bias:
+        bias = torch.zeros(layer.filters)
+        if bias_initializer is not None:
+            bias_initializer(bias)
+        layer.bias = torch.nn.Parameter(bias)
+
+
+def _bias_activation(layer, out, bias=True):
+    """A conv layer's epilogue: + bias (unless already applied, `bias` False), then the activation."""
+    if bias and layer.use_bias:
+        out = out + layer.bias.detach().to(out.device)
+    return layer.activation(out) if layer.activation is not None else out
+
+
 class _SparseConvBase(torch.nn.Module):
     TRANSPOSE = False
 
@@ -64,14 +84,7 @@ class _SparseConvBase(torch.nn.Module):
         if offset is None:      # upstream default: centred for odd kernels, shifted by half a voxel for even ones
             offset = torch.zeros(3) if ks[0] % 2 else torch.full((3,), -0.5)
         self.register_buffer("offset", torch.as_tensor(offset, dtype=torch.float32).reshape(3).clone())
-        kernel = torch.empty(*ks, self.in_channels, self.filters)
-        (kernel_initializer or (lambda t: torch.nn.init.uniform_(t, -0.05, 0.05)))(kernel)
-        self.kernel = torch.nn.Parameter(kernel)
-        if self.use_bias:
-            bias = torch.zeros(self.filters)
-            if bias_initializer is not None:
-                bias_initializer(bias)
-            self.bias = torch.nn.Parameter(bias)
+        _kernel_and_bias(self, kernel_initializer, bias_initializer)
         self._packed = None
 
     def _weights(self, dev):
@@ -87,26 +100,21 @@ class _SparseConvBase(torch.nn.Module):
             raise RuntimeError("SparseConv: importance / user neighbours are not implemented")
         if torch.is_grad_enabled() and (inp_features.requires_grad or self.kernel.requires_grad and self.training):
             raise RuntimeError("open3d_ml_b200: SparseConv is inference-only (call under torch.no_grad() / eval())")
+        from . import ops
         L.require_cuda()
-        ret_dev = inp_features.device
         feat = inp_features.detach().to("cuda", torch.float32).contiguous()
         n, m = feat.shape[0], out_positions.shape[0]
         vs = float(torch.as_tensor(voxel_size).reshape(-1)[0]) if not isinstance(voxel_size, (int, float)) else float(voxel_size)
         nbr, cnt = sparse_conv_neighbors(inp_positions, out_positions, vs, self.offset, self.kernel_size,
                                          self.TRANSPOSE, want_count=self.normalize)
         out = torch.zeros((m, self.filters), dtype=torch.float32, device=feat.device)
+        fused_bias = bool(m and n and self.use_bias and not self.normalize)     # added by the GEMM's epilogue
         if m and n:
-            bias = self.bias.detach().to(feat.device, torch.float32) if self.use_bias and not self.normalize else None
+            bias = self.bias.detach().to(feat.device, torch.float32) if fused_bias else None
             contract_cells(feat, nbr, self._weights(feat.device), out, bias)
-        elif self.use_bias and not self.normalize:
-            out += self.bias.detach().to(out.device)
         if self.normalize:
             out = out / cnt.clamp_min(1).to(torch.float32).unsqueeze(1)
-            if self.use_bias:
-                out = out + self.bias.detach().to(out.device)
-        if self.activation is not None:
-            out = self.activation(out)
-        return out.to(ret_dev)
+        return ops._back(_bias_activation(self, out, bias=not fused_bias), inp_features.device)
 
 
 class SparseConv(_SparseConvBase):
@@ -147,14 +155,16 @@ class ContinuousConv(torch.nn.Module):
         self.window_function = window_function
         self.register_buffer("offset", torch.zeros(3) if offset is None else
                              torch.as_tensor(offset, dtype=torch.float32).reshape(3).clone())
-        kernel = torch.empty(*ks, self.in_channels, self.filters)
-        (kernel_initializer or (lambda t: torch.nn.init.uniform_(t, -0.05, 0.05)))(kernel)
-        self.kernel = torch.nn.Parameter(kernel)
-        if self.use_bias:
-            bias = torch.zeros(self.filters)
-            if bias_initializer is not None:
-                bias_initializer(bias)
-            self.bias = torch.nn.Parameter(bias)
+        _kernel_and_bias(self, kernel_initializer, bias_initializer)
+        self._offset_host = None
+
+    def _host_offset(self):
+        """The `offset` buffer on the host, read once per version: the ops take it by value, and a module moved to
+        the GPU would otherwise pay a device->host read per call."""
+        key = (self.offset.data_ptr(), self.offset._version, str(self.offset.device))
+        if self._offset_host is None or self._offset_host[0] != key:
+            self._offset_host = (key, self.offset.detach().cpu())
+        return self._offset_host[1]
 
     def _search(self):
         return dict(metric=self.radius_search_metric, ignore_query_point=self.radius_search_ignore_query_points)
@@ -186,12 +196,10 @@ class ContinuousConv(torch.nn.Module):
             idx, splits, importance = res.neighbors_index, res.neighbors_row_splits, None
             if window is not None:
                 importance = window(res.neighbors_distance)
-        out = ops.continuous_conv(self.kernel.detach(), out_positions, ext, self.offset, inp_positions, inp_features,
-                                  inp_importance, idx, importance, splits,
+        out = ops.continuous_conv(self.kernel.detach(), out_positions, ext, self._host_offset(), inp_positions,
+                                  inp_features, inp_importance, idx, importance, splits,
                                   self.align_corners, self.coordinate_mapping, self.normalize, self.interpolation)
-        if self.use_bias:
-            out = out + self.bias.detach().to(out.device)
-        return self.activation(out) if self.activation is not None else out
+        return _bias_activation(self, out)
 
 
 class ContinuousConvTranspose(ContinuousConv):
@@ -207,15 +215,6 @@ class ContinuousConvTranspose(ContinuousConv):
             raise RuntimeError("ContinuousConvTranspose: window_function and use_dense_layer_for_center are not "
                                "implemented")
         super().__init__(in_channels, filters, kernel_size, **kwargs)
-        self._offset_host = None
-
-    def _host_offset(self):
-        """The `offset` buffer on the host, read once per version: the op takes it by value, and a module moved to
-        the GPU would otherwise pay a device->host read per call."""
-        key = (self.offset.data_ptr(), self.offset._version, str(self.offset.device))
-        if self._offset_host is None or self._offset_host[0] != key:
-            self._offset_host = (key, self.offset.detach().cpu())
-        return self._offset_host[1]
 
     def forward(self, inp_features, inp_positions, out_positions, extents, out_importance=None, **kwargs):
         from . import ops
@@ -227,7 +226,6 @@ class ContinuousConvTranspose(ContinuousConv):
         if ext.numel() != 1:
             raise RuntimeError("ContinuousConvTranspose: one extent for all points (per-point extents: use "
                                "ops.continuous_conv_transpose)")
-        ret_dev = inp_features.device
         op, ip = ops._dev(out_positions.float()), ops._dev(inp_positions.float())
         r = ops.fixed_radius_search(op, ip, float(ext[0]) * 0.5, return_distances=False, **self._search())
         inv = ops.invert_neighbors_list(op.shape[0], r.neighbors_index, r.neighbors_row_splits, torch.empty(0))
@@ -235,7 +233,4 @@ class ContinuousConvTranspose(ContinuousConv):
                                             ops._dev(inp_features), r.neighbors_index, None, r.neighbors_row_splits,
                                             inv.neighbors_index, None, inv.neighbors_row_splits, self.align_corners,
                                             self.coordinate_mapping, self.normalize, self.interpolation)
-        if self.use_bias:
-            out = out + self.bias.detach().to(out.device)
-        out = self.activation(out) if self.activation is not None else out
-        return out.to(ret_dev)
+        return ops._back(_bias_activation(self, out), inp_features.device)

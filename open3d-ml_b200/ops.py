@@ -42,6 +42,14 @@ def _dev(t):
     return t if t.is_cuda else t.cuda(non_blocking=True)
 
 
+def _back(out, dev):
+    """An op's result -- a tensor, None or a namedtuple of them -- handed back on `dev`, the device of the caller's
+    input: results computed on the GPU are copied to the host for a host caller; host tensors stay as they are."""
+    def back(t):
+        return t if t is None or not t.is_cuda else t.to(dev)
+    return out._make(map(back, out)) if isinstance(out, tuple) else back(out)
+
+
 def _host3(x, what):
     a = np.ascontiguousarray(torch.as_tensor(x).detach().cpu().numpy(), dtype=np.float32).reshape(-1)
     if a.size != 3:
@@ -56,12 +64,17 @@ def _check_points(points, name="points"):
         raise RuntimeError("%s must be float32" % name)
 
 
-def _splits(row_splits, n, device):
-    if row_splits is None:
-        return torch.tensor([0, n], dtype=torch.int64, device=device)
+def _row_splits(row_splits):
     if row_splits.dtype != torch.int64:
         raise RuntimeError("row_splits must be int64")
-    return row_splits.to(device).contiguous()
+    return _dev(row_splits).contiguous()
+
+
+def _splits(row_splits, n, device):
+    """_row_splits, or one batch item of n rows when row_splits is None."""
+    if row_splits is None:
+        return torch.tensor([0, n], dtype=torch.int64, device=device)
+    return _row_splits(row_splits)
 
 
 def voxelize_raw(points, row_splits, voxel_size, points_range_min, points_range_max,
@@ -84,37 +97,31 @@ def voxelize_raw(points, row_splits, voxel_size, points_range_min, points_range_
     bsp = torch.empty((batch + 1,), dtype=torch.int64, device=dev)
     bid = torch.empty((n,), dtype=torch.int32, device=dev) if want_batch_id else None
     counts = torch.empty((2,), dtype=torch.int64, device=dev)
-    wsb = L.lib().o3dml_voxelize_workspace_bytes(n, batch)
-    ws = torch.empty((wsb,), dtype=torch.uint8, device=dev)
+    ws = L.workspace(L.lib().o3dml_voxelize_workspace_bytes(n, batch), dev)
     L.check(L.lib().o3dml_voxelize(
         L.ptr(points), n, points.stride(0), L.ptr(rs), batch, vs.ctypes.data, rmin.ctypes.data,
         rmax.ctypes.data, int(min(max_points_per_voxel, INT64_MAX)), int(min(max_voxels, INT64_MAX)),
         L.ptr(coords), L.ptr(pidx), L.ptr(vrs), L.ptr(bsp), L.ptr(bid), L.ptr(counts), L.ptr(ws),
-        wsb, L.stream()))
+        ws.numel(), L.stream()))
     return coords, pidx, vrs, bsp, bid, counts
 
 
 def voxelize(points, row_splits, voxel_size, points_range_min, points_range_max,
              max_points_per_voxel=INT64_MAX, max_voxels=INT64_MAX):
     """open3d.ml.torch.ops.voxelize -- one device->host read (the voxel count)."""
-    was_cuda = points.is_cuda
     coords, pidx, vrs, bsp, _, counts = voxelize_raw(points, row_splits, voxel_size,
                                                      points_range_min, points_range_max,
                                                      max_points_per_voxel, max_voxels)
     m, kept = (int(v) for v in counts.tolist())
-    out = VoxelizeResult(coords[:m], pidx[:kept], vrs[:m + 1], bsp)
-    return out if was_cuda else VoxelizeResult(*(t.cpu() for t in out))
+    return _back(VoxelizeResult(coords[:m], pidx[:kept], vrs[:m + 1], bsp), points.device)
 
 
 def ragged_to_dense(values, row_splits, out_col_size, default_value, _add=0):
     """open3d.ml.torch.ops.ragged_to_dense for integer / float32 values of shape [L] or [L, ...]."""
-    was_cuda = values.is_cuda
     v = _dev(values).contiguous()
     if v.element_size() not in (4, 8):
         raise RuntimeError("ragged_to_dense: 4- or 8-byte element types only")
-    rs = _dev(row_splits)
-    if rs.dtype != torch.int64:
-        raise RuntimeError("row_splits must be int64")
+    rs = _row_splits(row_splits)
     rows = rs.numel() - 1
     inner = 1
     for s in v.shape[1:]:
@@ -129,7 +136,7 @@ def ragged_to_dense(values, row_splits, out_col_size, default_value, _add=0):
         bits = int(fill.item())
     L.check(L.lib().o3dml_ragged_to_dense(L.ptr(v), v.element_size(), inner, L.ptr(rs), rows,
                                           int(out_col_size), bits, int(_add), L.ptr(out), L.stream()))
-    return out if was_cuda else out.cpu()
+    return _back(out, values.device)
 
 
 def knn_workspace_bytes(num_points, num_queries, batch):
@@ -143,8 +150,7 @@ def knn_search_raw(points, points_row_splits, queries, queries_row_splits, k, ou
     at least knn_workspace_bytes, allocated here when none is given."""
     batch = points_row_splits.numel() - 1
     if workspace is None:
-        wsb = knn_workspace_bytes(points.shape[0], queries.shape[0], batch)
-        workspace = torch.empty((wsb,), dtype=torch.uint8, device=points.device)
+        workspace = L.workspace(knn_workspace_bytes(points.shape[0], queries.shape[0], batch), points.device)
     L.check(L.lib().o3dml_knn_search(L.ptr(points), points.shape[0], L.ptr(points_row_splits), L.ptr(queries),
                                      queries.shape[0], L.ptr(queries_row_splits), batch, int(k), L.ptr(out_index),
                                      L.is64(out_index), L.ptr(out_distance2), L.ptr(workspace), workspace.numel(),
@@ -166,6 +172,20 @@ def _index_dtype(index_dtype, name):
     return index_dtype
 
 
+def _search_args(name, points, queries, points_row_splits, queries_row_splits, index_dtype, metric):
+    """The checks every search makes, in order, and its inputs on the device: (metric code, points, queries, their
+    row splits, batch size)."""
+    m = _metric(metric, name)
+    _index_dtype(index_dtype, name)
+    _check_points(points), _check_points(queries, "queries")
+    p, q = _dev(points).contiguous(), _dev(queries).contiguous()
+    ps, qs = _splits(points_row_splits, p.shape[0], p.device), _splits(queries_row_splits, q.shape[0], p.device)
+    batch = ps.numel() - 1
+    if qs.numel() - 1 != batch:
+        raise RuntimeError("%s: row splits disagree on the batch size" % name)
+    return m, p, q, ps, qs, batch
+
+
 def knn_search(points, queries, k, points_row_splits=None, queries_row_splits=None,
                index_dtype=torch.int32, metric="L2", ignore_query_point=False,
                return_distances=False, allow_short=False):
@@ -173,16 +193,9 @@ def knn_search(points, queries, k, points_row_splits=None, queries_row_splits=No
     squared, as upstream returns them.  Dense [Nq * k] rows with row splits 0, k, 2k, ...; with ignore_query_point
     (points equal to the query are skipped) a row may hold fewer than k neighbours, and the rows are ragged (one
     device->host read of their total)."""
-    m = _metric(metric, "knn_search")
-    _index_dtype(index_dtype, "knn_search")
-    _check_points(points), _check_points(queries, "queries")
-    was_cuda = points.is_cuda
-    p, q = _dev(points).contiguous(), _dev(queries).contiguous()
+    m, p, q, ps, qs, batch = _search_args("knn_search", points, queries, points_row_splits, queries_row_splits,
+                                          index_dtype, metric)
     dev = p.device
-    ps, qs = _splits(points_row_splits, p.shape[0], dev), _splits(queries_row_splits, q.shape[0], dev)
-    batch = ps.numel() - 1
-    if qs.numel() - 1 != batch:
-        raise RuntimeError("knn_search: row splits disagree on the batch size")
     k = int(k)
     # upstream returns ragged (shorter) rows when a batch item holds fewer than k points; this op returns dense
     # [Nq, k] rows, so refuse instead of handing out -1 padded indices that a caller would gather with
@@ -203,33 +216,25 @@ def knn_search(points, queries, k, points_row_splits=None, queries_row_splits=No
         rs = torch.arange(0, (nq + 1) * k, k, dtype=torch.int64, device=dev) if not ig else \
             torch.empty((nq + 1,), dtype=torch.int64, device=dev)
         total = torch.zeros((1,), dtype=torch.int64, device=dev)
-        wsb = L.lib().o3dml_knn_search_metric_workspace_bytes(p.shape[0], nq, batch, k, ig)
-        ws = torch.empty((wsb,), dtype=torch.uint8, device=dev)
+        ws = L.workspace(L.lib().o3dml_knn_search_metric_workspace_bytes(p.shape[0], nq, batch, k, ig), dev)
         L.check(L.lib().o3dml_knn_search_metric(L.ptr(p), p.shape[0], L.ptr(ps), L.ptr(q), nq, L.ptr(qs), batch, k, m,
                                                 ig, L.ptr(idx), L.is64(idx), L.ptr(d2), L.ptr(rs), L.ptr(total),
-                                                L.ptr(ws), wsb, L.stream()))
+                                                L.ptr(ws), ws.numel(), L.stream()))
         if ig:
             t = int(total.item())
             idx, d2 = idx[:t], (d2[:t] if d2 is not None else None)
     out = KnnResult(idx.reshape(-1), rs,
                     d2.reshape(-1) if d2 is not None else torch.empty(0, device=dev))
-    return out if was_cuda else KnnResult(*(t.cpu() for t in out))
+    return _back(out, points.device)
 
 
 def _radius_search(name, points, queries, radius, radii, points_row_splits, queries_row_splits, index_dtype, metric,
                    ignore_query_point, return_distances, normalize_distances):
     """Two-phase radius search (count, one device->host read of the total, fill) with one radius (radii None) or
     one per query."""
-    m = _metric(metric, name)
-    _index_dtype(index_dtype, name)
-    _check_points(points), _check_points(queries, "queries")
-    was_cuda = points.is_cuda
-    p, q = _dev(points).contiguous(), _dev(queries).contiguous()
+    m, p, q, ps, qs, batch = _search_args(name, points, queries, points_row_splits, queries_row_splits, index_dtype,
+                                          metric)
     dev = p.device
-    ps, qs = _splits(points_row_splits, p.shape[0], dev), _splits(queries_row_splits, q.shape[0], dev)
-    batch = ps.numel() - 1
-    if qs.numel() - 1 != batch:
-        raise RuntimeError("%s: row splits disagree on the batch size" % name)
     nq = q.shape[0]
     if radii is not None:
         radii = _dev(torch.as_tensor(radii)).reshape(-1).contiguous()
@@ -238,20 +243,18 @@ def _radius_search(name, points, queries, radius, radii, points_row_splits, quer
     ig, norm = 1 if ignore_query_point else 0, 1 if normalize_distances else 0
     nrs = torch.empty((nq + 1,), dtype=torch.int64, device=dev)
     total = torch.zeros((1,), dtype=torch.int64, device=dev)
-    wsb = L.lib().o3dml_radius_workspace_bytes(p.shape[0], nq, batch)
-    ws = torch.empty((wsb,), dtype=torch.uint8, device=dev)
+    ws = L.workspace(L.lib().o3dml_radius_workspace_bytes(p.shape[0], nq, batch), dev)
     L.check(L.lib().o3dml_radius_search_count(L.ptr(p), p.shape[0], L.ptr(ps), L.ptr(q), nq, L.ptr(qs), batch,
                                               float(radius), L.ptr(radii), m, ig, L.ptr(nrs), L.ptr(total), L.ptr(ws),
-                                              wsb, L.stream()))
+                                              ws.numel(), L.stream()))
     t = int(total.item())
     idx = torch.empty((t,), dtype=index_dtype, device=dev)
     d = torch.empty((t,), dtype=torch.float32, device=dev)
     if t:      # with no neighbour at all there is nothing to fill (and the empty outputs have no address)
         L.check(L.lib().o3dml_radius_search_fill(L.ptr(q), p.shape[0], nq, L.ptr(qs), batch, float(radius),
                                                  L.ptr(radii), m, ig, norm, L.ptr(nrs), L.ptr(idx), L.is64(idx),
-                                                 L.ptr(d), L.ptr(ws), wsb, L.stream()))
-    out = RadiusResult(idx, nrs, d if return_distances else torch.empty(0, device=dev))
-    return out if was_cuda else RadiusResult(*(t_.cpu() for t_ in out))
+                                                 L.ptr(d), L.ptr(ws), ws.numel(), L.stream()))
+    return _back(RadiusResult(idx, nrs, d if return_distances else torch.empty(0, device=dev)), points.device)
 
 
 def fixed_radius_search(points, queries, radius, points_row_splits=None, queries_row_splits=None,
@@ -443,18 +446,15 @@ def nms(boxes, scores, nms_overlap_thresh):
         raise RuntimeError("nms: boxes must have shape [N,5], got %s" % (tuple(boxes.shape),))
     if scores.dim() != 1 or scores.shape[0] != boxes.shape[0]:
         raise RuntimeError("nms: scores must have shape [N]")
-    was_cuda = boxes.is_cuda
     b = _dev(boxes).to(torch.float32).contiguous()
     s = _dev(scores).to(torch.float32).contiguous()
     n = b.shape[0]
     keep = torch.empty((n,), dtype=torch.int64, device=b.device)
     cnt = torch.zeros((1,), dtype=torch.int64, device=b.device)
-    wsb = L.lib().o3dml_nms_workspace_bytes(n)
-    ws = torch.empty((wsb,), dtype=torch.uint8, device=b.device)
+    ws = L.workspace(L.lib().o3dml_nms_workspace_bytes(n), b.device)
     L.check(L.lib().o3dml_nms(L.ptr(b), L.ptr(s), n, float(nms_overlap_thresh), L.ptr(keep), L.ptr(cnt), L.ptr(ws),
-                              wsb, L.stream()))
-    out = keep[:int(cnt.item())]
-    return out if was_cuda else out.cpu()
+                              ws.numel(), L.stream()))
+    return _back(keep[:int(cnt.item())], boxes.device)
 
 
 def _iou(a, b, mode, width):
@@ -484,16 +484,12 @@ def reduce_subarrays_sum(values, row_splits):
     """open3d.ml.torch.ops.reduce_subarrays_sum (ml3d/torch/models/sparseconvnet.py:318-324)."""
     if values.dim() != 1:
         raise RuntimeError("reduce_subarrays_sum: values must be 1-D")
-    if row_splits.dtype != torch.int64:
-        raise RuntimeError("row_splits must be int64")
-    was_cuda = values.is_cuda
+    rs = _row_splits(row_splits)
     v = _dev(values).to(torch.float32).contiguous()
-    rs = _dev(row_splits).contiguous()
     rows = rs.numel() - 1
     out = torch.empty((max(rows, 0),), dtype=torch.float32, device=v.device)
     L.check(L.lib().o3dml_reduce_subarrays_sum(L.ptr(v), L.ptr(rs), rows, L.ptr(out), L.stream()))
-    out = out.to(values.dtype)
-    return out if was_cuda else out.cpu()
+    return _back(out.to(values.dtype), values.device)
 
 
 VoxelPoolingResult = collections.namedtuple("VoxelPoolingResult", "pooled_positions pooled_features")
@@ -509,14 +505,12 @@ def voxel_pooling(positions, features, voxel_size, position_fn="average", featur
     if position_fn not in ("average", "nearest_neighbor", "center") or feature_fn not in ("average", "max", "nearest_neighbor"):
         raise RuntimeError("voxel_pooling: unknown position_fn / feature_fn")
     _check_points(positions, "positions")
-    was_cuda = positions.is_cuda
     pts = _dev(positions).contiguous()
     feats = _dev(features).to(torch.float32).contiguous()
     if feats.dim() != 2 or feats.shape[0] != pts.shape[0]:
         raise RuntimeError("voxel_pooling: features must have shape [N, C]")
     if pts.shape[0] == 0:
-        out = VoxelPoolingResult(pts.new_zeros((0, 3)), feats.new_zeros((0, feats.shape[1])))
-        return out if was_cuda else VoxelPoolingResult(*(t.cpu() for t in out))
+        return _back(VoxelPoolingResult(pts.new_zeros((0, 3)), feats.new_zeros((0, feats.shape[1]))), positions.device)
     vs = float(voxel_size)
     origin, mx = _subsample_range(pts, vs)
     coords, pidx, vrs, bsp, _, counts = voxelize_raw(pts, None, [vs, vs, vs], origin, mx, INT64_MAX, INT64_MAX)
@@ -535,12 +529,40 @@ def voxel_pooling(positions, features, voxel_size, position_fn="average", featur
     op, of, _ = voxel_reduce(pts, feats, None, vrs, pidx, counts, m, position_mode=pm, feature_mode=fm)
     if position_fn == "center":
         op = (coords[:m].to(torch.float32) + 0.5) * vs + torch.from_numpy(origin).to(pts.device)
-    out = VoxelPoolingResult(op, of)
-    return out if was_cuda else VoxelPoolingResult(*(t.cpu() for t in out))
+    return _back(VoxelPoolingResult(op, of), positions.device)
 
 
 _CCONV_MAPPING = {"identity": 0, "ball_to_cube_radial": 1}
 _CCONV_INTERP = {"nearest_neighbor": 0, "linear": 1, "linear_border": 2}
+
+
+def _cconv_args(name, filters, out_positions, extents, offset, inp_positions, inp_features, neighbors_index,
+                neighbors_row_splits, coordinate_mapping, interpolation, extents_per_inp):
+    """The arguments continuous_conv and its transpose share, checked and on the device: (filters, out_positions,
+    inp_positions, inp_features, extents, host offset, neighbors_index, neighbors_row_splits).  Per-point extents
+    count the outputs, or the inputs when `extents_per_inp` (the transpose, which also refuses them with no input)."""
+    if coordinate_mapping not in _CCONV_MAPPING:
+        raise RuntimeError("%s: coordinate_mapping '%s' is not implemented (identity, ball_to_cube_radial)"
+                           % (name, coordinate_mapping))
+    if interpolation not in _CCONV_INTERP:
+        raise RuntimeError("%s: unknown interpolation '%s'" % (name, interpolation))
+    if filters.dim() != 5:
+        raise RuntimeError("%s: filters must have shape [Sz, Sy, Sx, Cin, Cout]" % name)
+    f = _dev(filters).to(torch.float32).contiguous()
+    op, ip = _dev(out_positions).to(torch.float32).contiguous(), _dev(inp_positions).to(torch.float32).contiguous()
+    feat = _dev(inp_features).to(torch.float32).contiguous()
+    ext = _dev(torch.as_tensor(extents, dtype=torch.float32).reshape(-1)).contiguous()
+    n, side = (ip.shape[0], "num_inp") if extents_per_inp else (op.shape[0], "num_out")
+    if ext.numel() != 1 and (ext.numel() != n or extents_per_inp and n == 0):
+        raise RuntimeError("%s: extents must have 1 or %s elements" % (name, side))
+    off = _host3(offset, "offset")
+    idx = _dev(neighbors_index).contiguous()
+    if idx.dtype not in (torch.int32, torch.int64):
+        raise RuntimeError("%s: neighbors_index must be int32 or int64" % name)
+    rs = _dev(neighbors_row_splits).to(torch.int64).contiguous()
+    if rs.numel() != op.shape[0] + 1:
+        raise RuntimeError("%s: neighbors_row_splits must have num_out + 1 elements" % name)
+    return f, op, ip, feat, ext, off, idx, rs
 
 
 def continuous_conv(filters, out_positions, extents, offset, inp_positions, inp_features, inp_importance,
@@ -549,30 +571,12 @@ def continuous_conv(filters, out_positions, extents, offset, inp_positions, inp_
                     max_temp_mem_MB=64):
     """open3d.ml.torch.ops.continuous_conv (raw op; contract in csrc/cconv.cu).  filters [Sz, Sy, Sx, Cin, Cout];
     empty importance tensors mean "all ones"; extents [1] or [num_out]."""
-    if coordinate_mapping not in _CCONV_MAPPING:
-        raise RuntimeError("continuous_conv: coordinate_mapping '%s' is not implemented (identity, ball_to_cube_radial)"
-                           % coordinate_mapping)
-    if interpolation not in _CCONV_INTERP:
-        raise RuntimeError("continuous_conv: unknown interpolation '%s'" % interpolation)
-    if filters.dim() != 5:
-        raise RuntimeError("continuous_conv: filters must have shape [Sz, Sy, Sx, Cin, Cout]")
-    was_cuda = inp_features.is_cuda
-    f = _dev(filters).to(torch.float32).contiguous()
-    op, ip = _dev(out_positions).to(torch.float32).contiguous(), _dev(inp_positions).to(torch.float32).contiguous()
-    feat = _dev(inp_features).to(torch.float32).contiguous()
-    ext = _dev(torch.as_tensor(extents, dtype=torch.float32).reshape(-1)).contiguous()
-    if ext.numel() not in (1, op.shape[0]):
-        raise RuntimeError("continuous_conv: extents must have 1 or num_out elements")
-    off = np.ascontiguousarray(torch.as_tensor(offset).detach().cpu().numpy(), dtype=np.float32).reshape(3)
+    f, op, ip, feat, ext, off, idx, rs = _cconv_args(
+        "continuous_conv", filters, out_positions, extents, offset, inp_positions, inp_features, neighbors_index,
+        neighbors_row_splits, coordinate_mapping, interpolation, extents_per_inp=False)
     imp = None if inp_importance is None or inp_importance.numel() == 0 else _dev(inp_importance).float().contiguous()
     nimp = (None if neighbors_importance is None or neighbors_importance.numel() == 0
             else _dev(neighbors_importance).float().contiguous())
-    idx = _dev(neighbors_index).contiguous()
-    if idx.dtype not in (torch.int32, torch.int64):
-        raise RuntimeError("continuous_conv: neighbors_index must be int32 or int64")
-    rs = _dev(neighbors_row_splits).to(torch.int64).contiguous()
-    if rs.numel() != op.shape[0] + 1:
-        raise RuntimeError("continuous_conv: neighbors_row_splits must have num_out + 1 elements")
     sz, sy, sx, cin, cout = f.shape
     if feat.shape[1] != cin:
         raise RuntimeError("continuous_conv: feature channels do not match the filter")
@@ -582,7 +586,7 @@ def continuous_conv(filters, out_positions, extents, offset, inp_positions, inp_
         off.ctypes.data, L.ptr(ip), L.ptr(feat), ip.shape[0], L.ptr(imp), L.ptr(idx),
         L.is64(idx), L.ptr(nimp), L.ptr(rs), 1 if align_corners else 0,
         _CCONV_MAPPING[coordinate_mapping], 1 if normalize else 0, _CCONV_INTERP[interpolation], L.ptr(out), L.stream()))
-    return out if was_cuda else out.cpu()
+    return _back(out, inp_features.device)
 
 
 InvertNeighborsListResult = collections.namedtuple(
@@ -594,13 +598,10 @@ def invert_neighbors_list(num_points, inp_neighbors_index, inp_neighbors_row_spl
     input rows that contain each id, once per occurrence, by (input row, position in it): a stable sort by id.  Ids out
     of range are dropped (they follow the last row; neighbors_row_splits[-1] counts the entries kept).  The attributes
     ([E, ...], any dtype) are permuted the same way; an empty attributes tensor stays empty.  No host read."""
-    was_cuda = inp_neighbors_index.is_cuda
     idx = _dev(inp_neighbors_index).reshape(-1).contiguous()
     if idx.dtype not in (torch.int32, torch.int64):
         raise RuntimeError("invert_neighbors_list: inp_neighbors_index must be int32 or int64")
-    if inp_neighbors_row_splits.dtype != torch.int64:
-        raise RuntimeError("row_splits must be int64")
-    rs = _dev(inp_neighbors_row_splits).contiguous()
+    rs = _row_splits(inp_neighbors_row_splits)
     num_points, e, num_inp = int(num_points), idx.numel(), rs.numel() - 1
     if num_points < 0 or num_inp < 0:
         raise RuntimeError("invert_neighbors_list: num_points must be >= 0 and row_splits non-empty")
@@ -611,15 +612,12 @@ def invert_neighbors_list(num_points, inp_neighbors_index, inp_neighbors_row_spl
     out_idx = torch.empty((e,), dtype=idx.dtype, device=dev)
     out_rs = torch.empty((num_points + 1,), dtype=torch.int64, device=dev)
     perm = torch.empty((e,), dtype=torch.int64, device=dev)
-    wsb = L.lib().o3dml_invert_neighbors_list_workspace_bytes(e)
-    ws = torch.empty((wsb,), dtype=torch.uint8, device=dev)
+    ws = L.workspace(L.lib().o3dml_invert_neighbors_list_workspace_bytes(e), dev)
     L.check(L.lib().o3dml_invert_neighbors_list(num_points, L.ptr(idx), L.is64(idx), L.ptr(rs), num_inp, e,
-                                                L.ptr(out_idx), L.ptr(out_rs), L.ptr(perm), L.ptr(ws), wsb,
+                                                L.ptr(out_idx), L.ptr(out_rs), L.ptr(perm), L.ptr(ws), ws.numel(),
                                                 L.stream()))
     out_attrs = _dev(attrs)[perm] if attrs.numel() else attrs
-    if was_cuda:
-        return InvertNeighborsListResult(out_idx, out_rs, out_attrs)
-    return InvertNeighborsListResult(out_idx.cpu(), out_rs.cpu(), out_attrs.cpu())
+    return _back(InvertNeighborsListResult(out_idx, out_rs, out_attrs), inp_neighbors_index.device)
 
 
 def continuous_conv_transpose(filters, out_positions, out_importance, extents, offset, inp_positions, inp_features,
@@ -634,22 +632,10 @@ def continuous_conv_transpose(filters, out_positions, out_importance, extents, o
     1 / inp_neighbors_importance_sum[i], or by 1 / the length of its row of inp_neighbors_row_splits when that sum
     is empty.  inp_neighbors_index is taken for signature parity and not read.  No host read."""
     name = "continuous_conv_transpose"
-    if coordinate_mapping not in _CCONV_MAPPING:
-        raise RuntimeError("%s: coordinate_mapping '%s' is not implemented (identity, ball_to_cube_radial)"
-                           % (name, coordinate_mapping))
-    if interpolation not in _CCONV_INTERP:
-        raise RuntimeError("%s: unknown interpolation '%s'" % (name, interpolation))
-    if filters.dim() != 5:
-        raise RuntimeError("%s: filters must have shape [Sz, Sy, Sx, Cin, Cout]" % name)
-    was_cuda = inp_features.is_cuda
-    f = _dev(filters).to(torch.float32).contiguous()
-    op, ip = _dev(out_positions).to(torch.float32).contiguous(), _dev(inp_positions).to(torch.float32).contiguous()
-    feat = _dev(inp_features).to(torch.float32).contiguous()
+    f, op, ip, feat, ext, off, idx, rs = _cconv_args(
+        name, filters, out_positions, extents, offset, inp_positions, inp_features, neighbors_index,
+        neighbors_row_splits, coordinate_mapping, interpolation, extents_per_inp=True)
     num_out, num_inp = op.shape[0], ip.shape[0]
-    ext = _dev(torch.as_tensor(extents, dtype=torch.float32).reshape(-1)).contiguous()
-    if ext.numel() != 1 and (ext.numel() != num_inp or num_inp == 0):
-        raise RuntimeError("%s: extents must have 1 or num_inp elements" % name)
-    off = np.ascontiguousarray(torch.as_tensor(offset).detach().cpu().numpy(), dtype=np.float32).reshape(3)
 
     def opt(t, n, what):
         if t is None or t.numel() == 0:
@@ -666,12 +652,6 @@ def continuous_conv_transpose(filters, out_positions, out_importance, extents, o
         irs = _dev(inp_neighbors_row_splits).to(torch.int64).contiguous()
         if irs.numel() != num_inp + 1:
             raise RuntimeError("%s: inp_neighbors_row_splits must have num_inp + 1 elements" % name)
-    idx = _dev(neighbors_index).contiguous()
-    if idx.dtype not in (torch.int32, torch.int64):
-        raise RuntimeError("%s: neighbors_index must be int32 or int64" % name)
-    rs = _dev(neighbors_row_splits).to(torch.int64).contiguous()
-    if rs.numel() != num_out + 1:
-        raise RuntimeError("%s: neighbors_row_splits must have num_out + 1 elements" % name)
     sz, sy, sx, cin, cout = f.shape
     if feat.dim() != 2 or feat.shape[0] != num_inp or feat.shape[1] != cin:
         raise RuntimeError("%s: feature channels do not match the filter" % name)
@@ -681,7 +661,7 @@ def continuous_conv_transpose(filters, out_positions, out_importance, extents, o
         off.ctypes.data, L.ptr(ip), L.ptr(feat), num_inp, L.ptr(isum), L.ptr(irs), L.ptr(idx), L.is64(idx),
         L.ptr(nimp), L.ptr(rs), 1 if align_corners else 0, _CCONV_MAPPING[coordinate_mapping], 1 if normalize else 0,
         _CCONV_INTERP[interpolation], L.ptr(out), L.stream()))
-    return out if was_cuda else out.cpu()
+    return _back(out, inp_features.device)
 
 
 def sparse_conv(filters, inp_features, inp_importance, neighbors_index, neighbors_kernel_index, neighbors_importance,
@@ -692,7 +672,6 @@ def sparse_conv(filters, inp_features, inp_importance, neighbors_index, neighbor
     if (inp_importance is not None and inp_importance.numel()) or \
             (neighbors_importance is not None and neighbors_importance.numel()):
         raise RuntimeError("sparse_conv: importance is not implemented")
-    was_cuda = inp_features.is_cuda
     w = filters.detach().float().cpu()
     cin, cout = w.shape[-2], w.shape[-1]
     w = w.reshape(-1, cin, cout)
@@ -708,4 +687,4 @@ def sparse_conv(filters, inp_features, inp_importance, neighbors_index, neighbor
     layers.contract_cells(feat, table, layers.pack_cell_groups(w), out)
     if normalize:
         out = out / lens.clamp_min(1).to(torch.float32).unsqueeze(1)
-    return out if was_cuda else out.cpu()
+    return _back(out, inp_features.device)

@@ -243,7 +243,7 @@ class PointPillarsB200:
         scores = torch.empty((B, C * K), dtype=torch.float32, device=dev)
         labels = torch.empty((B, C * K), dtype=torch.int64, device=dev)
         counts = torch.empty((B,), dtype=torch.int64, device=dev)
-        ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+        ws = L.workspace(ws_bytes, dev)
         anchors = self.anchors(H, W, dev)
         c, r, d = maps
         L.check(lib.o3dml_pp_detect(L.ptr(c), c.stride(0), L.ptr(r), r.stride(0), L.ptr(d), d.stride(0), B, H, W, A, C,
