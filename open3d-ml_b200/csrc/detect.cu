@@ -6,14 +6,15 @@
 //      row ascending); otherwise keep all rows in row order.  K = min(nms_pre, N);
 //   3. BBoxCoder.decode of the kept rows against the cached anchors; direction = argmax of the two logits (ties: 0);
 //   4. per class: kept rows with score_c > score_thr, greedy rotated-BEV NMS at IoU 0.01 (the constant of
-//      objdet_helper.py:346) with the nms op's rules (rbox.cuh, visiting by descending score_c, ties by position in
-//      the step-2 order, suppressed when IoU > 0.01);
+//      objdet_helper.py:346) by the nms op's kernels (nms_segments in rbox.cuh, visiting by descending score_c, ties by
+//      position in the step-2 order, suppressed when IoU > 0.01);
 //   5. output per frame: class 0's survivors in visiting order, then class 1's, ...; yaw corrected with
 //      limit_period(yaw - dir_offset, 1, pi) + dir_offset + pi * dir (point_pillars.py:1020-1023), padded to C * K
 //      rows (zeros, label -1).
 // Launches (independent of B and C): top-k by a 5-pass radix select on the unique 55-bit key
 // (score bits << 23 | (2^23 - 1 - row)) -- one memset + 6 launches, skipped when N <= nms_pre -- then sort + decode,
-// per-class segment sort, suppression matrix, sweep and output: 5 launches.  No host synchronisation, no allocation.
+// per-class segment sort, the suppression matrix and sweep of nms.cu over all (frame, class) segments, and output:
+// 5 launches.  No host synchronisation, no allocation.
 #include <algorithm>
 
 #include "../../include/o3dml_b200.h"
@@ -151,12 +152,14 @@ __device__ void bitonic_sort_desc(unsigned long long* s, int n) {
     }
 }
 
-// one block per frame: the top-k order (or row order), then decode of the K kept rows.
+// one block per frame: the top-k order (or row order), then decode of the K kept rows and their BEV boxes
+// (x - w/2, y - l/2, x + w/2, y + l/2, r) (objdet_helper.py:69-99), which every class's NMS reads.
 // BBoxCoder.decode (objdet_helper.py:287-313) with every product and sum rounded on its own, as torch computes it.
 __global__ void __launch_bounds__(kSortThreads) pp_topk_decode_kernel(
     const unsigned long long* __restrict__ cand, int select, int K, int P, const float* __restrict__ cls, int64_t cls_bs,
     const float* __restrict__ reg, int64_t reg_bs, const float* __restrict__ dirm, int64_t dir_bs, int HW, int A, int C,
-    const float* __restrict__ anchors, float* __restrict__ dec, int* __restrict__ dirc, float* __restrict__ sc) {
+    const float* __restrict__ anchors, float* __restrict__ dec, float* __restrict__ bev, int* __restrict__ dirc,
+    float* __restrict__ sc) {
     extern __shared__ unsigned long long sk[];
     const int b = blockIdx.x;
     if (select) {
@@ -181,6 +184,9 @@ __global__ void __launch_bounds__(kSortThreads) pp_topk_decode_kernel(
         o[4] = __fmul_rn(expf(dl[4 * HW]), la);
         o[5] = hg;
         o[6] = __fadd_rn(dl[6 * HW], an[6]);
+        const float hw = o[3] / 2.f, hl = o[4] / 2.f;
+        float* q = bev + ((size_t)b * K + i) * 5;
+        q[0] = o[0] - hw; q[1] = o[1] - hl; q[2] = o[0] + hw; q[3] = o[1] + hl; q[4] = o[6];
         const float* dp = dirm + (size_t)b * dir_bs + (size_t)a * 2 * HW + pos;
         dirc[(size_t)b * K + i] = dp[HW] > dp[0] ? 1 : 0;
         const float* cp = cls + (size_t)b * cls_bs + (size_t)a * C * HW + pos;
@@ -188,11 +194,11 @@ __global__ void __launch_bounds__(kSortThreads) pp_topk_decode_kernel(
     }
 }
 
-// one block per (frame, class): the kept rows above score_thr by (score_c descending, position ascending), and their
-// BEV boxes (x - w/2, y - l/2, x + w/2, y + l/2, r) (objdet_helper.py:69-99)
-__global__ void __launch_bounds__(kSortThreads) pp_class_sort_kernel(
-    const float* __restrict__ sc, const float* __restrict__ dec, int K, int P, int C, float score_thr,
-    int* __restrict__ seg_idx, float* __restrict__ bev, int* __restrict__ seg_cnt) {
+// one block per (frame, class): the positions of the kept rows above score_thr by (score_c descending, position
+// ascending), the NMS segment of the class
+__global__ void __launch_bounds__(kSortThreads) pp_class_sort_kernel(const float* __restrict__ sc, int K, int P, int C,
+                                                                     float score_thr, int* __restrict__ seg_idx,
+                                                                     int* __restrict__ seg_cnt) {
     extern __shared__ unsigned long long sk[];
     __shared__ int cnt;
     const int seg = blockIdx.x, b = seg / C, c = seg - b * C;
@@ -212,72 +218,9 @@ __global__ void __launch_bounds__(kSortThreads) pp_class_sort_kernel(
     __syncthreads();
     bitonic_sort_desc(sk, P);
     const int m = cnt;
-    for (int j = threadIdx.x; j < m; j += blockDim.x) {
-        const int k = (int)(0xFFFFFFFFu - (uint32_t)(sk[j] & 0xFFFFFFFFull));
-        seg_idx[(size_t)seg * K + j] = k;
-        const float* d = dec + ((size_t)b * K + k) * 7;
-        const float hw = d[3] / 2.f, hl = d[4] / 2.f;
-        float* q = bev + ((size_t)seg * K + j) * 5;
-        q[0] = d[0] - hw; q[1] = d[1] - hl; q[2] = d[0] + hw; q[3] = d[1] + hl; q[4] = d[6];
-    }
+    for (int j = threadIdx.x; j < m; j += blockDim.x)
+        seg_idx[(size_t)seg * K + j] = (int)(0xFFFFFFFFu - (uint32_t)(sk[j] & 0xFFFFFFFFull));
     if (threadIdx.x == 0) seg_cnt[seg] = m;
-}
-
-// suppression matrix of every segment in one grid (x: column block, y: row block, z: segment).  Pairs whose
-// bounding circles are disjoint (with a margin far above fp32 rounding) have IoU exactly 0 <= thr: no clipping.
-__global__ void __launch_bounds__(64) pp_nms_mask_kernel(const float* __restrict__ bev, const int* __restrict__ seg_cnt,
-                                                         int K, int words_max, unsigned long long* __restrict__ mask) {
-    const int seg = blockIdx.z, ib = blockIdx.y, jb = blockIdx.x;
-    const int n = seg_cnt[seg], words = (n + 63) >> 6;
-    if (jb < ib || jb >= words) return;
-    __shared__ RBoxXY sb[64];
-    __shared__ float3 sc[64];      // absolute centre and bounding radius, for the early-out only
-    const float* base = bev + (size_t)seg * K * 5;
-    const int j0 = jb * 64;
-    if (j0 + (int)threadIdx.x < n) {
-        const RBoxXY q = rbox_xyxyr(base + (size_t)(j0 + threadIdx.x) * 5);
-        const float w = q.x1 - q.x0, h = q.y1 - q.y0;
-        sb[threadIdx.x] = q;
-        sc[threadIdx.x] = make_float3(0.5f * (q.x0 + q.x1), 0.5f * (q.y0 + q.y1), 0.5f * sqrtf(w * w + h * h));
-    }
-    __syncthreads();
-    const int i = ib * 64 + threadIdx.x;
-    if (i >= n) return;
-    const RBoxXY a = rbox_xyxyr(base + (size_t)i * 5);
-    const float aw = a.x1 - a.x0, ah = a.y1 - a.y0, ra = 0.5f * sqrtf(aw * aw + ah * ah);
-    const float acx = 0.5f * (a.x0 + a.x1), acy = 0.5f * (a.y0 + a.y1);
-    unsigned long long bits = 0;
-    const int cnt = min(64, n - j0);
-    for (int k = (ib == jb ? threadIdx.x + 1 : 0); k < cnt; ++k) {
-        const float3 c = sc[k];
-        const float dx = acx - c.x, dy = acy - c.y, rr = 1.001f * (ra + c.z) + 1e-6f;
-        if (dx * dx + dy * dy > rr * rr) continue;
-        if (rbox_iou(a, sb[k]) > kNmsIou) bits |= 1ull << k;
-    }
-    mask[((size_t)seg * K + i) * words_max + jb] = bits;
-}
-
-// one warp per segment: the greedy sweep of nms.cu over the segment's bit matrix
-__global__ void __launch_bounds__(32) pp_nms_sweep_kernel(const unsigned long long* __restrict__ mask,
-                                                          const int* __restrict__ seg_idx, const int* __restrict__ seg_cnt,
-                                                          int K, int words_max, int* __restrict__ keep,
-                                                          int* __restrict__ nkeep) {
-    __shared__ unsigned long long remv[kMaxK / 64];
-    const int seg = blockIdx.x, n = seg_cnt[seg], words = (n + 63) >> 6;
-    for (int w = threadIdx.x; w < words; w += 32) remv[w] = 0;
-    __syncwarp();
-    const unsigned long long* m = mask + (size_t)seg * K * words_max;
-    int kept = 0;
-    for (int i = 0; i < n; ++i) {
-        const int wi = i >> 6;
-        if (!((remv[wi] >> (i & 63)) & 1ull)) {
-            if (threadIdx.x == 0) keep[(size_t)seg * K + kept] = seg_idx[(size_t)seg * K + i];
-            ++kept;
-            for (int w = wi + threadIdx.x; w < words; w += 32) remv[w] |= m[(size_t)i * words_max + w];
-        }
-        __syncwarp();
-    }
-    if (threadIdx.x == 0) nkeep[seg] = kept;
 }
 
 // padded per-frame output: class offsets, yaw correction, zero fill with label -1
@@ -322,7 +265,7 @@ struct DetectBuffers {
     unsigned long long* cand;
     float *dec, *sc, *bev;
     int *dirc, *seg_idx, *seg_cnt, *keep, *nkeep;
-    unsigned long long* mask;
+    uint64_t* mask;
 };
 
 DetectBuffers carve(Workspace& ws, int64_t B, int64_t N, int64_t K, int64_t C, bool select) {
@@ -337,12 +280,12 @@ DetectBuffers carve(Workspace& ws, int64_t B, int64_t N, int64_t K, int64_t C, b
         d.cand = ws.take<unsigned long long>((size_t)(B * K));
     }
     d.dec = ws.take<float>((size_t)(B * K * 7));
+    d.bev = ws.take<float>((size_t)(B * K * 5));
     d.dirc = ws.take<int>((size_t)(B * K));
     d.sc = ws.take<float>((size_t)(B * K * C));
     d.seg_idx = ws.take<int>((size_t)(B * C * K));
-    d.bev = ws.take<float>((size_t)(B * C * K * 5));
     d.seg_cnt = ws.take<int>((size_t)(B * C));
-    d.mask = ws.take<unsigned long long>((size_t)(B * C * K * words_max));
+    d.mask = ws.take<uint64_t>((size_t)(B * C * K * words_max));
     d.keep = ws.take<int>((size_t)(B * C * K));
     d.nkeep = ws.take<int>((size_t)(B * C));
     return d;
@@ -387,7 +330,6 @@ extern "C" int o3dml_pp_detect(const float* cls, int64_t cls_batch_stride, const
     const bool select = N > nms_pre;
     int P = 1;
     while (P < K) P <<= 1;
-    const int words_max = (K + 63) / 64;
     Workspace ws(workspace, workspace_bytes);
     const DetectBuffers d = carve(ws, B, N, K, C, select);
     O3DML_CHECK_WORKSPACE(ws, "pp_detect");
@@ -403,13 +345,12 @@ extern "C" int o3dml_pp_detect(const float* cls, int64_t cls_batch_stride, const
     const size_t sort_smem = (size_t)P * sizeof(unsigned long long);
     O3DML_CUDA(launch<pp_topk_decode_kernel>(B, kSortThreads, select ? sort_smem : 0, st, d.cand, select ? 1 : 0, K, P,
                                              cls, cls_batch_stride, reg, reg_batch_stride, dir, dir_batch_stride, HW,
-                                             A, C, anchors, d.dec, d.dirc, d.sc));
-    O3DML_CUDA(launch<pp_class_sort_kernel>(B * C, kSortThreads, sort_smem, st, d.sc, d.dec, K, P, C, score_thr,
-                                            d.seg_idx, d.bev, d.seg_cnt));
-    O3DML_CUDA(launch<pp_nms_mask_kernel>(dim3((unsigned)words_max, (unsigned)words_max, (unsigned)(B * C)), 64, 0, st,
-                                          d.bev, d.seg_cnt, K, words_max, d.mask));
-    O3DML_CUDA(launch<pp_nms_sweep_kernel>(B * C, 32, 0, st, d.mask, d.seg_idx, d.seg_cnt, K, words_max, d.keep,
-                                           d.nkeep));
+                                             A, C, anchors, d.dec, d.bev, d.dirc, d.sc));
+    O3DML_CUDA(launch<pp_class_sort_kernel>(B * C, kSortThreads, sort_smem, st, d.sc, K, P, C, score_thr, d.seg_idx,
+                                            d.seg_cnt));
+    // one segment per (frame, class), reading its frame's BEV boxes
+    O3DML_CUDA(nms_segments(d.bev, (int64_t)K * 5, C, d.seg_idx, K, d.seg_cnt, K, B * C, kNmsIou, d.mask, d.keep, K,
+                            d.nkeep, st));
     O3DML_CUDA(launch<pp_output_kernel>(dim3((unsigned)ceil_div<int64_t>((int64_t)C * K, 256), (unsigned)B), 256, 0, st,
                                         d.dec, d.dirc, d.sc, d.keep, d.nkeep, K, C, dir_offset, out_boxes, out_scores,
                                         out_labels, d_counts));

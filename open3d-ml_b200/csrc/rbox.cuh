@@ -1,5 +1,5 @@
-// rbox.cuh -- rotated-rectangle overlap in fp32, shared by the NMS op (nms.cu) and the fused detection
-// post-processing (detect.cu), so that both decide "IoU > thr" with the same arithmetic.
+// rbox.cuh -- rotated-rectangle overlap in fp32 and the greedy NMS launcher, shared by the NMS op (nms.cu) and the
+// fused detection post-processing (detect.cu), so that both decide "IoU > thr" with the same kernels.
 //   A box is the rectangle centre (cx, cy), size (w, h) rotated by r about its centre; the overlap of two boxes
 //   is the area of the intersection polygon (Sutherland-Hodgman clipping, shoelace area).
 //   The clipping runs in a frame centred on the first box: at LiDAR ranges (70 m) absolute corner coordinates carry
@@ -9,6 +9,7 @@
 //   The intersection is clamped to the smaller area, so that 0 <= IoU <= 1 holds under fp32 rounding.
 #pragma once
 #include <cuda_runtime.h>
+#include <stdint.h>
 
 namespace o3dml {
 
@@ -101,7 +102,8 @@ __device__ __forceinline__ float rbox_iou(const RBox& a, const RBox& b) {
     return uni > 0.f ? inter / uni : 0.f;
 }
 
-// the (x0, y0, x1, y1, r) form, in a frame centred on a
+// the (x0, y0, x1, y1, r) form, in a frame centred on a.  For degenerate boxes (km-long slivers) the fp32 result
+// depends on FMA contraction, which shifts if the caller also computes these corner differences or this offset.
 __device__ __forceinline__ float rbox_iou(const RBoxXY& a, const RBoxXY& b) {
     RBox ra, rb;
     ra.cx = 0.f; ra.cy = 0.f; ra.w = a.x1 - a.x0; ra.h = a.y1 - a.y0; ra.c = a.c; ra.s = a.s;
@@ -109,5 +111,14 @@ __device__ __forceinline__ float rbox_iou(const RBoxXY& a, const RBoxXY& b) {
     rb.w = b.x1 - b.x0; rb.h = b.y1 - b.y0; rb.c = b.c; rb.s = b.s;
     return rbox_iou(ra, rb);
 }
+
+// Greedy NMS of `segments` box lists in two launches (nms.cu).  Segment s visits ids[s * ids_stride + i] for i below
+// counts[s] (n_max when counts is null), (x0, y0, x1, y1, r) rows of boxes + (s / segs_per_set) * set_stride, and
+// writes the ids it keeps, in visiting order, to keep + s * keep_stride and their number to num_keep[s].
+// mask: segments * n_max * ceil(n_max / 64) words of scratch, not cleared.  Out is int or int64_t.
+template <typename Out>
+cudaError_t nms_segments(const float* boxes, int64_t set_stride, int segs_per_set, const int* ids, int64_t ids_stride,
+                         const int* counts, int n_max, int segments, float thr, uint64_t* mask, Out* keep,
+                         int64_t keep_stride, Out* num_keep, cudaStream_t st);
 
 }  // namespace o3dml

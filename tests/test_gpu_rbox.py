@@ -166,6 +166,33 @@ def test_nms_duplicates_at_thr_one_and_negative_threshold():
         assert nms_both(bx, sc, -0.01).tolist() == want
 
 
+def test_nms_at_zero_threshold():
+    """thr = 0, the lowest threshold at which pairs with disjoint bounding circles skip the clipping.  Pairs 12 m apart
+    at x ~ 60-170 m: unit squares sharing an edge or a corner, 0.25 m apart, with bounding circles 0.5 m apart, just
+    inside (corners 2^-10 * sqrt 2 apart) and just outside (4x that) the early-out margin, a turned pedestrian pair
+    1 mm apart -- all IoU 0, all kept -- and squares overlapping by a 2^-10 m strip or corner and 8 m boxes overlapping
+    by 2^-6 m at their ends, which lose their second box.  Then chains of overlapping boxes."""
+    t = 2.0 ** -10
+    pairs = [((1, 1, 0), (1, 0)), ((1, 1, 0), (1, 1)), ((1, 1, 0), (0, 1.25)), ((1, 1, 0), (1.5, 0)),
+             ((1, 1, 0), (1 + t, 1 + t)), ((1, 1, 0), (1 + 4 * t, 1 + 4 * t)),
+             ((1, 1, 0), (1 - t, 0)), ((1, 1, 0), (1 - t, 1 - t)), ((8, 0.5, 0), (8 - 16 * t, 0)),
+             ((0.625, 0.75, 0.3), (0.626 * math.cos(0.3), 0.626 * math.sin(0.3)))]
+    rows = []
+    for p, ((w, h, r), (dx, dy)) in enumerate(pairs):
+        x, y = 60.5 + 12 * p, -39.5
+        rows += [[x, y, w, h, r], [x + dx, y + dy, w, h, r]]
+    boxes = to_xyxyr(rows)
+    scores = np.repeat(1 - np.arange(len(pairs)) / 32, 2).astype(np.float32)
+    scores[1::2] -= 1 / 64                                         # visiting order = index order
+    want = [i for i in range(len(boxes)) if i not in (13, 15, 17)]
+    assert O.c_nms(boxes, scores, 0.0)[0].tolist() == want
+    assert nms_both(boxes, scores, 0.0).tolist() == want
+    boxes, scores = chain_clusters(300, seed=5)
+    ref, _ = O.c_nms(boxes, scores, 0.0)
+    assert len(ref) < 300
+    assert np.array_equal(nms_both(boxes, scores, 0.0), ref)
+
+
 def test_nms_at_its_limit():
     """65 536 boxes: 32 768 well-separated pairs of duplicates, distinct scores: at thr 0.5 exactly the higher-scored
     copy of each pair survives, by descending score.  65 537 boxes are refused."""
