@@ -11,6 +11,9 @@ README.md:313-314 / set_open3d_ml_root.sh:1-3 of the reference.  With it,
 runs the reference's models, dataloaders and pipelines with every native op on the
 sm_90a kernels.  Symbols that the reference imports at module load but that are outside
 the hot path (SURVEY.md Appendix B checklist) raise NotImplementedError when CALLED.
+
+The natives come from a table, module name -> attributes; ``_library_bindings()`` is this
+library's.  The test oracle passes its own table to drive the same reference flows on the CPU.
 """
 import importlib
 import os
@@ -102,16 +105,51 @@ class _AliasFinder:
         return ModuleSpec(name, _Loader(), is_package=hasattr(mod, "__path__"))
 
 
-_INSTALLED = False
+def _library_bindings():
+    from . import layers as LY, ops as O
+    return {
+        "open3d.core": dict(Tensor=O._O3CTensor),
+        "open3d.core.nns": dict(NearestNeighborSearch=O.NearestNeighborSearch),
+        "open3d.ml.torch.ops": dict(
+            voxelize=O.voxelize, ragged_to_dense=O.ragged_to_dense,
+            knn_search=O.knn_search, fixed_radius_search=O.fixed_radius_search, radius_search=O.radius_search,
+            nms=O.nms,
+            reduce_subarrays_sum=O.reduce_subarrays_sum,
+            voxel_pooling=O.voxel_pooling,
+            continuous_conv=O.continuous_conv, continuous_conv_transpose=O.continuous_conv_transpose,
+            invert_neighbors_list=O.invert_neighbors_list, sparse_conv=O.sparse_conv),
+        "open3d.ml.torch.layers": dict(
+            FixedRadiusSearch=O.FixedRadiusSearch, RadiusSearch=O.RadiusSearch,
+            KNNSearch=O.KNNSearch,
+            SparseConv=LY.SparseConv, SparseConvTranspose=LY.SparseConvTranspose,
+            ContinuousConv=LY.ContinuousConv, ContinuousConvTranspose=LY.ContinuousConvTranspose),
+        "open3d.ml.contrib": dict(
+            subsample=O.subsample, subsample_batch=O.subsample_batch,
+            iou_bev_cpu=O.iou_bev, iou_bev_cuda=O.iou_bev, iou_3d_cpu=O.iou_3d, iou_3d_cuda=O.iou_3d),
+    }
 
 
-def install(ml3d_root=None):
-    """Registers the fabricated ``open3d`` package.  Idempotent.  Does not touch CUDA."""
+_INSTALLED = None      # the table of the installed package
+
+
+def install(ml3d_root=None, bindings=None):
+    """Registers the fabricated ``open3d`` package.  Idempotent; a second call with another
+    table raises.  Does not touch CUDA.
+
+    ``bindings`` (default: this library's table) maps each fabricated module to its attributes;
+    a symbol of the library's table that it lacks raises NotImplementedError when called."""
     global _INSTALLED
-    if _INSTALLED:
+    library = _library_bindings()
+    table = library if bindings is None else bindings
+    if _INSTALLED is not None:
+        if table != _INSTALLED:
+            raise RuntimeError("open3d_ml_b200.shim: already installed with other bindings")
         return
-    import torch
-    from . import ops as O
+
+    def attrs(name):
+        out = {s: _not_on_hot_path(name + "." + s) for s in library[name]}
+        out.update(table.get(name, {}))
+        return out
 
     root = ml3d_root or os.environ.get("OPEN3D_ML_ROOT")
     if "open3d" in sys.modules and not getattr(sys.modules["open3d"], "_o3dml_b200_shim", False):
@@ -119,34 +157,16 @@ def install(ml3d_root=None):
     _module("open3d", _o3dml_b200_shim=True, __version__="0.0+o3dml_b200",
             _build_config={"BUILD_PYTORCH_OPS": True, "BUILD_TENSORFLOW_OPS": False,
                            "BUILD_GUI": False, "BUILD_CUDA_MODULE": True})
-    core = _module("open3d.core", Tensor=O._O3CTensor)
+    ml = _module("open3d.ml")
+    mlt = _module("open3d.ml.torch")
+    for name in library:
+        _module(name, **attrs(name))
     # device_count() = 0 keeps the reference from importing the CUDA-only PointNet++/PVCNN ops
     # (pointnet2_utils.py:35-36, roipool3d_utils.py:3-4, pvcnn.py:13-14), which are off the path
     _module("open3d.core.cuda", device_count=lambda: 0)
-    _module("open3d.core.nns", NearestNeighborSearch=O.NearestNeighborSearch)
-    core.nns, core.cuda = sys.modules["open3d.core.nns"], sys.modules["open3d.core.cuda"]
-    ml = _module("open3d.ml")
-    mlt = _module("open3d.ml.torch")
-    _module("open3d.ml.torch.ops", voxelize=O.voxelize, ragged_to_dense=O.ragged_to_dense,
-            knn_search=O.knn_search, fixed_radius_search=O.fixed_radius_search, radius_search=O.radius_search,
-            nms=O.nms,
-            reduce_subarrays_sum=O.reduce_subarrays_sum,
-            voxel_pooling=O.voxel_pooling,
-            continuous_conv=O.continuous_conv, continuous_conv_transpose=O.continuous_conv_transpose,
-            invert_neighbors_list=O.invert_neighbors_list, sparse_conv=O.sparse_conv)
-    from . import layers as LY
-    _module("open3d.ml.torch.layers", FixedRadiusSearch=O.FixedRadiusSearch, RadiusSearch=O.RadiusSearch,
-            KNNSearch=O.KNNSearch,
-            SparseConv=LY.SparseConv, SparseConvTranspose=LY.SparseConvTranspose,
-            ContinuousConv=LY.ContinuousConv, ContinuousConvTranspose=LY.ContinuousConvTranspose)
-    _module("open3d.ml.contrib", subsample=O.subsample, subsample_batch=O.subsample_batch,
-            iou_bev_cpu=O.iou_bev, iou_bev_cuda=O.iou_bev, iou_3d_cpu=O.iou_3d, iou_3d_cuda=O.iou_3d)
-    vis = _module("open3d.visualization")
-    tb = _module("open3d.visualization.tensorboard_plugin")
-    _module("open3d.visualization.tensorboard_plugin.summary")
-    vis.tensorboard_plugin = tb
-    for n in ("open3d.geometry", "open3d.utility", "open3d.io", "open3d.t", "open3d.t.io",
-              "open3d.visualization.gui", "open3d.visualization.rendering"):
+    for n in ("open3d.visualization", "open3d.visualization.tensorboard_plugin",
+              "open3d.visualization.tensorboard_plugin.summary", "open3d.geometry", "open3d.utility", "open3d.io",
+              "open3d.t", "open3d.t.io", "open3d.visualization.gui", "open3d.visualization.rendering"):
         _module(n)
     # third-party packages the reference imports at module load and this image lacks
     try:
@@ -180,4 +200,4 @@ def install(ml3d_root=None):
                 return sys.modules["open3d.ml.torch." + attr]
             return mlt_get(attr)
         mlt.__getattr__ = mlt_getattr
-    _INSTALLED = True
+    _INSTALLED = table

@@ -16,8 +16,13 @@ SRC = os.environ.get("OPEN3D_ML_ROOT", "/root/reference")
 DST = os.path.join(HERE, "_ref")
 
 
+def live_root():
+    """The unmodified reference tree itself ($OPEN3D_ML_ROOT or /root/reference), or None where it is absent."""
+    return SRC if os.path.isdir(os.path.join(SRC, "ml3d")) else None
+
+
 def snapshot(force=False):
-    if not os.path.isdir(os.path.join(SRC, "ml3d")):
+    if live_root() is None:
         return None
     stamp = os.path.join(DST, ".stamp")
     if os.path.exists(stamp) and not force:
@@ -40,11 +45,7 @@ def snapshot(force=False):
 
 def ref_root():
     """Where the unmodified reference tree can be imported from: the live tree here, the snapshot on the GPU box."""
-    if os.path.isdir(os.path.join(SRC, "ml3d")):
-        return SRC
-    if os.path.isdir(os.path.join(DST, "ml3d")):
-        return DST
-    return None
+    return live_root() or (DST if os.path.isdir(os.path.join(DST, "ml3d")) else None)
 
 
 if __name__ == "__main__":

@@ -1,220 +1,132 @@
 """oracle/refshim.py -- TEST INFRASTRUCTURE, NOT PRODUCT CODE.
 
-Makes the UNMODIFIED reference model code under /root/reference importable in
-this container (torch CPU only) so that it can be used as the model-layer
-oracle and to generate the golden fixtures under tests/golden/
-(SURVEY.md section 8c, Appendix B).  The reference's third-party native ops
-(`open3d.ml.torch.ops`, `open3d.core.nns`, ...) are bound to the CPU oracle in
-oracle/ops.py; packages that are simply absent from this image (`addict`,
-`matplotlib`, ...) get minimal stand-ins.
-
-/root/reference does not exist on the GPU box: nothing that runs there may
-call `install()`.
+Makes the UNMODIFIED reference model code importable in this container (torch CPU only) so that it can be used
+as the model-layer oracle and to generate the golden fixtures under tests/golden/ (SURVEY.md section 8c,
+Appendix B).  The `open3d` package is the one open3d_ml_b200.shim fabricates, with the reference's third-party
+native ops (`open3d.ml.torch.ops`, `open3d.core.nns`, ...) bound to the CPU oracle in oracle/ops.py by BINDINGS.
 """
 import collections
-import importlib.abc
-import importlib.machinery
 import os
-import sys
-import types
 
 import numpy as np
+import torch
 
-REF_ROOT = os.environ.get("OPEN3D_ML_ROOT", "/root/reference")
+from . import ops as O
+from .make_ref_snapshot import live_root, ref_root
 
 
 def available():
-    return os.path.isdir(os.path.join(REF_ROOT, "ml3d"))
+    """Whether the unmodified reference tree itself is present (not only its oracle/_ref snapshot)."""
+    return live_root() is not None
 
 
-class _AttrDict(dict):
-    """Stand-in for addict.Dict (ml3d/utils/config.py:9)."""
+class Tensor:
+    def __init__(self, a):
+        self.a = np.asarray(a)
 
-    def __init__(self, *args, **kwargs):
-        super().__init__()
-        for a in args:
-            if a:
-                for k, v in dict(a).items():
-                    self[k] = self._conv(v)
-        for k, v in kwargs.items():
-            self[k] = self._conv(v)
+    @staticmethod
+    def from_numpy(a):
+        return Tensor(a)
 
-    @classmethod
-    def _conv(cls, v):
-        if isinstance(v, dict) and not isinstance(v, cls):
-            return cls(v)
-        if isinstance(v, (list, tuple)):
-            return type(v)(cls._conv(x) for x in v)
-        return v
-
-    def __getattr__(self, k):
-        if k.startswith("__"):
-            raise AttributeError(k)
-        if k not in self:
-            self[k] = type(self)()
-        return self[k]
-
-    def __setattr__(self, k, v):
-        self[k] = self._conv(v)
-
-    def __missing__(self, k):
-        v = type(self)()
-        self[k] = v
-        return v
-
-    def to_dict(self):
-        return {k: (v.to_dict() if isinstance(v, _AttrDict) else v) for k, v in self.items()}
-
-    def copy(self):
-        return type(self)(self)
+    def numpy(self):
+        return self.a
 
 
-class _Finder(importlib.abc.MetaPathFinder, importlib.abc.Loader):
-    PREFIXES = ("open3d", "matplotlib", "pyquaternion", "openvino", "addict")
+class NearestNeighborSearch:
+    """dataprocessing.py:99-103"""
 
-    def find_spec(self, name, path=None, target=None):
-        if name.split(".")[0] in self.PREFIXES:
-            return importlib.machinery.ModuleSpec(name, self, is_package=True)
-        return None
+    def __init__(self, pts):
+        self.p = pts.numpy()
 
-    def create_module(self, spec):
-        m = types.ModuleType(spec.name)
-        m.__path__ = []
-        return m
+    def knn_index(self):
+        return True
 
-    def exec_module(self, module):
-        _populate(module)
+    def knn_search(self, q, k):
+        i, d = O.np_knn(self.p, q.numpy(), k)
+        return Tensor(i.astype(np.int64)), Tensor(d)
 
 
-def _populate(m):
-    import torch
-    from . import ops as O
-    name = m.__name__
-
-    def _lazy(attr, _n=name):
-        # `import open3d` followed by `open3d.core.cuda...` (pointnet2_utils.py:35)
-        if attr.startswith("__"):
-            raise AttributeError(attr)
-        import importlib
-        return importlib.import_module(_n + "." + attr)
-    if name != "addict":
-        m.__getattr__ = _lazy
-    if name == "addict":
-        m.Dict = _AttrDict
-    elif name == "open3d":
-        m._build_config = {"BUILD_PYTORCH_OPS": True, "BUILD_TENSORFLOW_OPS": False,
-                           "BUILD_GUI": False, "BUILD_CUDA_MODULE": False}
-        m.__version__ = "0.0-oracle"
-    elif name == "open3d.core.cuda":
-        m.device_count = lambda: 0
-    elif name == "open3d.core":
-        class Tensor:
-            def __init__(self, a):
-                self.a = np.asarray(a)
-
-            @staticmethod
-            def from_numpy(a):
-                return Tensor(a)
-
-            def numpy(self):
-                return self.a
-        m.Tensor = Tensor
-    elif name == "open3d.core.nns":
-        class NearestNeighborSearch:
-            """dataprocessing.py:99-103"""
-
-            def __init__(self, pts):
-                self.p = pts.numpy()
-
-            def knn_index(self):
-                return True
-
-            def knn_search(self, q, k):
-                from open3d.core import Tensor
-                i, d = O.np_knn(self.p, q.numpy(), k)
-                return Tensor(i.astype(np.int64)), Tensor(d)
-        m.NearestNeighborSearch = NearestNeighborSearch
-    elif name == "open3d.ml.torch.ops":
-        V = collections.namedtuple("VoxelizeResult", "voxel_coords voxel_point_indices "
-                                   "voxel_point_row_splits voxel_batch_splits")
-
-        def voxelize(points, row_splits, voxel_size, points_range_min, points_range_max,
-                     max_points_per_voxel=2**62, max_voxels=2**62):
-            r = O.c_voxelize(points.detach().cpu().numpy(), row_splits.cpu().numpy(),
-                             voxel_size.numpy(), points_range_min.numpy(),
-                             points_range_max.numpy(), max_points_per_voxel, max_voxels)
-            return V(*(torch.from_numpy(r[k]) for k in V._fields))
-
-        def ragged_to_dense(values, row_splits, out_col_size, default_value):
-            return torch.from_numpy(O.np_ragged_to_dense(values.numpy(), row_splits.numpy(),
-                                                         int(out_col_size),
-                                                         default_value.numpy()))
-
-        def _todo(*a, **k):
-            raise NotImplementedError("not on the hot path (SURVEY.md 2.2)")
-        def nms(boxes, scores, thr):
-            keep, _ = O.c_nms(boxes.detach().cpu().numpy(), scores.detach().cpu().numpy(), float(thr))
-            return torch.from_numpy(keep).to(boxes.device)
-        m.voxelize, m.ragged_to_dense, m.nms = voxelize, ragged_to_dense, nms
-        m.knn_search = m.reduce_subarrays_sum = _todo
-    elif name == "open3d.ml.torch.layers":
-        R = collections.namedtuple("FixedRadiusSearchResult",
-                                   "neighbors_index neighbors_row_splits neighbors_distance")
-
-        class FixedRadiusSearch:
-            """kpconv.py:2021-2026 (rows ordered by (d2, idx), DESIGN.md)."""
-
-            def __call__(self, points, queries, radius, points_row_splits, queries_row_splits):
-                i, rs, d = O.c_radius(points.numpy(), queries.numpy(), radius,
-                                      points_row_splits.numpy(), queries_row_splits.numpy())
-                return R(torch.from_numpy(i), torch.from_numpy(rs), torch.from_numpy(d))
-        m.FixedRadiusSearch = FixedRadiusSearch
-        m.SparseConv = m.SparseConvTranspose = type("SparseConvStub", (torch.nn.Module,), {})
-    elif name == "open3d.ml.contrib":
-        def _todo(*a, **k):
-            raise NotImplementedError("not on the hot path (SURVEY.md 2.2)")
-        def subsample_batch(points, batches_len, features=None, classes=None, sampleDl=0.1,
-                            method="barycenter", max_p=0, verbose=0):
-            r = O.c_subsample_batch(points, batches_len, features, classes, sampleDl, max_p)
-            if classes is not None:
-                r = r[:-1] + (r[-1].astype(np.asarray(classes).dtype),)
-            return r
-
-        def subsample(points, features=None, classes=None, sampleDl=0.1, verbose=0):
-            r = subsample_batch(points, [len(points)], features, classes, sampleDl)
-            out = (r[0],) + tuple(r[2:])
-            return out[0] if len(out) == 1 else out
-        m.subsample, m.subsample_batch = subsample, subsample_batch
-        m.iou_bev_cpu = m.iou_bev_cuda = lambda a, b: O.c_iou_matrix(a, b, 0)
-        m.iou_3d_cpu = m.iou_3d_cuda = lambda a, b: O.c_iou_matrix(a, b, 1)
-    elif name == "open3d.visualization.tensorboard_plugin":
-        m.summary = types.ModuleType(name + ".summary")
-    elif name in ("matplotlib.pyplot", "matplotlib.cm", "matplotlib"):
-        m.get_cmap = lambda *a, **k: None
+_V = collections.namedtuple("VoxelizeResult", "voxel_coords voxel_point_indices "
+                            "voxel_point_row_splits voxel_batch_splits")
 
 
-_INSTALLED = False
+def voxelize(points, row_splits, voxel_size, points_range_min, points_range_max,
+             max_points_per_voxel=2**62, max_voxels=2**62):
+    r = O.c_voxelize(points.detach().cpu().numpy(), row_splits.cpu().numpy(),
+                     voxel_size.numpy(), points_range_min.numpy(),
+                     points_range_max.numpy(), max_points_per_voxel, max_voxels)
+    return _V(*(torch.from_numpy(r[k]) for k in _V._fields))
+
+
+def ragged_to_dense(values, row_splits, out_col_size, default_value):
+    return torch.from_numpy(O.np_ragged_to_dense(values.numpy(), row_splits.numpy(),
+                                                 int(out_col_size),
+                                                 default_value.numpy()))
+
+
+def nms(boxes, scores, thr):
+    keep, _ = O.c_nms(boxes.detach().cpu().numpy(), scores.detach().cpu().numpy(), float(thr))
+    return torch.from_numpy(keep).to(boxes.device)
+
+
+_R = collections.namedtuple("FixedRadiusSearchResult",
+                            "neighbors_index neighbors_row_splits neighbors_distance")
+
+
+class FixedRadiusSearch:
+    """kpconv.py:2021-2026 (rows ordered by (d2, idx), DESIGN.md)."""
+
+    def __call__(self, points, queries, radius, points_row_splits, queries_row_splits):
+        i, rs, d = O.c_radius(points.numpy(), queries.numpy(), radius,
+                              points_row_splits.numpy(), queries_row_splits.numpy())
+        return _R(torch.from_numpy(i), torch.from_numpy(rs), torch.from_numpy(d))
+
+
+def subsample_batch(points, batches_len, features=None, classes=None, sampleDl=0.1,
+                    method="barycenter", max_p=0, verbose=0):
+    r = O.c_subsample_batch(points, batches_len, features, classes, sampleDl, max_p)
+    if classes is not None:
+        r = r[:-1] + (r[-1].astype(np.asarray(classes).dtype),)
+    return r
+
+
+def subsample(points, features=None, classes=None, sampleDl=0.1, verbose=0):
+    r = subsample_batch(points, [len(points)], features, classes, sampleDl)
+    out = (r[0],) + tuple(r[2:])
+    return out[0] if len(out) == 1 else out
+
+
+def _iou_bev(a, b):
+    return O.c_iou_matrix(a, b, 0)
+
+
+def _iou_3d(a, b):
+    return O.c_iou_matrix(a, b, 1)
+
+
+BINDINGS = {
+    "open3d.core": dict(Tensor=Tensor),
+    "open3d.core.nns": dict(NearestNeighborSearch=NearestNeighborSearch),
+    "open3d.ml.torch.ops": dict(voxelize=voxelize, ragged_to_dense=ragged_to_dense, nms=nms),
+    "open3d.ml.torch.layers": dict(FixedRadiusSearch=FixedRadiusSearch),
+    "open3d.ml.contrib": dict(subsample=subsample, subsample_batch=subsample_batch,
+                              iou_bev_cpu=_iou_bev, iou_bev_cuda=_iou_bev, iou_3d_cpu=_iou_3d, iou_3d_cuda=_iou_3d),
+}
 
 
 def install():
-    """Idempotent.  After this, `import ml3d.torch` works (reference code)."""
-    global _INSTALLED
-    if _INSTALLED:
-        return
-    if not available():
-        raise RuntimeError("reference tree not found at %s" % REF_ROOT)
-    try:
-        import addict  # noqa: F401
-        _Finder.PREFIXES = tuple(p for p in _Finder.PREFIXES if p != "addict")
-    except ImportError:
-        pass
-    sys.meta_path.insert(0, _Finder())
-    sys.path.insert(0, REF_ROOT)
-    _INSTALLED = True
+    """Idempotent.  After this, `import open3d.ml.torch` and `import ml3d.torch` work (reference code).
+    -> the reference root."""
+    from open3d_ml_b200 import shim
+    root = ref_root()
+    if root is None:
+        raise RuntimeError("no reference tree (see oracle/make_ref_snapshot.py)")
+    shim.install(root, BINDINGS)
+    return root
 
 
 def load_cfg(yml_name):
     """Reference config loader (ml3d/utils/config.py:210-241) on a shipped yml."""
-    install()
+    root = install()
     from ml3d.utils import Config
-    return Config.load_from_file(os.path.join(REF_ROOT, "ml3d", "configs", yml_name))
+    return Config.load_from_file(os.path.join(root, "ml3d", "configs", yml_name))

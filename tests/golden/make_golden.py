@@ -18,10 +18,13 @@ import numpy as np
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, os.path.dirname(HERE))
 sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
 
-from oracle import refshim, weights, models_torch as MT, ops as O  # noqa: E402
+from oracle import refshim, weights, models_torch as MT  # noqa: E402
 from open3d_ml_b200 import synth  # noqa: E402
+from open3d_ml_b200.pointpillars import cfg_from_reference  # noqa: E402
+import helpers as H  # noqa: E402
 
 SEED = 1234
 
@@ -31,14 +34,6 @@ def sample_idx(n, m, seed):
 
 
 # ------------------------------------------------------------------ RandLA-Net
-def randla_inputs(B, N, seed0):
-    per = [MT.randlanet_build_inputs(synth.semantickitti_cloud(N, seed0 + b)) for b in range(B)]
-    inp = {k: [torch.from_numpy(np.stack([p[k][i] for p in per])) for i in range(4)]
-           for k in ("coords", "neighbor_indices", "sub_idx", "interp_idx")}
-    inp["features"] = inp["coords"][0].clone()
-    return inp
-
-
 def make_randlanet():
     from ml3d.torch.models import RandLANet
     cfg = refshim.load_cfg("randlanet_semantickitti.yml")
@@ -51,7 +46,7 @@ def make_randlanet():
     sd = weights.seeded_state_dict(man, SEED)
     net.load_state_dict(sd, strict=True)
     B, N = 2, 2048
-    inp = randla_inputs(B, N, 100)
+    inp = H.randla_inputs(B, N, 100)
     taps = {}
     hooks = []
     for i in range(4):
@@ -112,19 +107,9 @@ def make_randlanet_s3dis():
 PP_SMALL = dict(point_cloud_range=[0, -10.24, -3, 20.48, 10.24, 1], output_shape=[128, 128])
 
 
-def pp_cfg_dict(cfg_model):
-    return dict(point_cloud_range=list(cfg_model["point_cloud_range"]),
-                voxel_size=list(cfg_model["voxelize"]["voxel_size"]),
-                max_num_points=cfg_model["voxelize"]["max_num_points"],
-                max_voxels=cfg_model["voxelize"]["max_voxels"][1],
-                output_shape=list(cfg_model["scatter"]["output_shape"]),
-                layer_nums=list(cfg_model["backbone"]["layer_nums"]),
-                layer_strides=list(cfg_model["backbone"]["layer_strides"]),
-                upsample_strides=list(cfg_model["neck"]["upsample_strides"]))
-
-
 def make_pointpillars():
     from ml3d.torch.models import PointPillars
+    from ml3d.utils import Config
 
     class Batch:
         pass
@@ -132,11 +117,12 @@ def make_pointpillars():
     for tag, yml in (("kitti", "pointpillars_kitti.yml"), ("waymo", "pointpillars_waymo.yml")):
         cfg = refshim.load_cfg(yml)
         m = cfg.model.to_dict() if hasattr(cfg.model, "to_dict") else dict(cfg.model)
+        pcfg = {k: v for k, v in cfg_from_reference(m).items() if k not in ("head", "num_classes")}
         net = PointPillars(device="cpu", **cfg.model)
         net.eval()
         man = weights.manifest_from_state_dict(net.state_dict())
         weights.save_manifest(os.path.join(HERE, "pointpillars_%s.manifest.json" % tag), man,
-                              dict(source="ml3d/configs/" + yml, cfg=pp_cfg_dict(m)))
+                              dict(source="ml3d/configs/" + yml, cfg=pcfg))
         if tag != "kitti":
             continue
         sd = weights.seeded_state_dict(man, SEED)
@@ -155,7 +141,7 @@ def make_pointpillars():
         h.remove(), h2.remove()
         pt = {}
         with torch.no_grad():
-            port = MT.pointpillars_forward(sd, frames, pp_cfg_dict(m), taps=pt)
+            port = MT.pointpillars_forward(sd, frames, pcfg, taps=pt)
         for a, bb in zip(port, outs):
             e = (a - bb).abs().max().item() / bb.abs().max().item()
             print("pointpillars: port vs reference rel err %.3e" % e)
@@ -179,7 +165,7 @@ def make_pointpillars():
         m2 = json.loads(json.dumps(m))
         m2["point_cloud_range"] = PP_SMALL["point_cloud_range"]
         m2["scatter"]["output_shape"] = PP_SMALL["output_shape"]
-        net2 = PointPillars(device="cpu", **refshim._AttrDict(m2))
+        net2 = PointPillars(device="cpu", **Config(m2))
         net2.eval()
         net2.load_state_dict(sd, strict=True)
         f2 = [torch.from_numpy(synth.lidar_frame(6000, 210, tuple(PP_SMALL["point_cloud_range"])))]
@@ -192,39 +178,6 @@ def make_pointpillars():
 
 
 # ------------------------------------------------------------------ KPConv
-KP_SMALL_ROOM = (1.6, 1.2, 1.0)
-
-
-def kp_batch(clouds, cfg):
-    """5-level pyramid like KPConvBatch.segmentation_inputs (concat_batcher.py:186-305) with the
-    grid subsampling replaced by open3d_ml_b200.synth.grid_subsample (inputs only)."""
-    pts = [np.concatenate([c[0] for c in clouds])]
-    lens = [[len(c[0]) for c in clouds]]
-    feats = np.concatenate([c[1] for c in clouds])
-    r = cfg["first_subsampling_dl"] * cfg["conv_radius"]
-    dl = cfg["first_subsampling_dl"]
-    out = dict(features=feats, points=[], neighbors=[], pools=[], upsamples=[], lengths=[])
-    cur = [c[0] for c in clouds]
-    for L in range(cfg["num_layers"]):
-        P = np.concatenate(cur)
-        ln = [len(c) for c in cur]
-        out["points"].append(P)
-        out["lengths"].append(ln)
-        out["neighbors"].append(MT.kp_batch_neighbors(P, P, ln, ln, r).astype(np.int64))
-        if L < cfg["num_layers"] - 1:
-            dl2 = 2 * dl
-            nxt = [synth.grid_subsample(c, dl2) for c in cur]
-            Q = np.concatenate(nxt)
-            lq = [len(c) for c in nxt]
-            out["pools"].append(MT.kp_batch_neighbors(Q, P, lq, ln, r).astype(np.int64))
-            out["upsamples"].append(MT.kp_batch_neighbors(P, Q, ln, lq, 2 * r).astype(np.int64))
-            cur, dl, r = nxt, dl2, r * 2
-        else:
-            out["pools"].append(np.zeros((0, 1), np.int64))
-            out["upsamples"].append(np.zeros((0, 1), np.int64))
-    return out
-
-
 def make_kpconv():
     from ml3d.torch.models import KPFCNN
     cfg = refshim.load_cfg("kpconv_s3dis.yml")
@@ -246,8 +199,8 @@ def make_kpconv():
                           dict(source="ml3d/configs/kpconv_s3dis.yml", cfg=kcfg))
     sd = weights.seeded_state_dict(man, SEED)
     net.load_state_dict(sd, strict=True)
-    clouds = [synth.room_cloud(3000, 300, room=KP_SMALL_ROOM), synth.room_cloud(2000, 301, room=KP_SMALL_ROOM)]
-    bd = kp_batch(clouds, kcfg)
+    clouds = [synth.room_cloud(3000, 300, room=H.KP_SMALL_ROOM), synth.room_cloud(2000, 301, room=H.KP_SMALL_ROOM)]
+    bd = H.kp_batch(clouds, kcfg)
 
     class B:
         pass

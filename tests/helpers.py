@@ -1,5 +1,5 @@
-"""Shared builders for the model parity tests: seeded weights + seeded inputs,
-re-derived exactly as tests/golden/make_golden.py derived them, and the
+"""Shared builders for the model parity tests: seeded weights + seeded inputs, the same
+builders tests/golden/make_golden.py recorded the fixtures with, and the
 Paris-Lille3D-shaped clouds of the deformable KPConv tests and benchmark."""
 import os
 
@@ -31,7 +31,8 @@ def randla_inputs(B, N, seed0, knn=None):
 
 
 def kp_batch(clouds, cfg, radius_search=None):
-    """Same pyramid as tests/golden/make_golden.py:kp_batch."""
+    """5-level pyramid like KPConvBatch.segmentation_inputs (concat_batcher.py:186-305) with the
+    grid subsampling replaced by open3d_ml_b200.synth.grid_subsample (inputs only)."""
     r = cfg["first_subsampling_dl"] * cfg["conv_radius"]
     dl = cfg["first_subsampling_dl"]
     out = dict(features=np.concatenate([c[1] for c in clouds]), points=[], neighbors=[], pools=[],

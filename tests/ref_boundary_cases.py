@@ -25,15 +25,14 @@ import torch  # noqa: E402
 
 
 def install(ops):
+    """Binds the CUDA library (`ops` "b200") or the CPU oracle ("oracle") under the reference tree.  -> its root."""
     from oracle.make_ref_snapshot import ref_root
     root = ref_root()
     if root is None:
         print(json.dumps(dict(skipped="no reference tree (neither /root/reference nor oracle/_ref)")))
         sys.exit(0)
     if ops == "oracle":
-        os.environ["OPEN3D_ML_ROOT"] = root
         from oracle import refshim
-        refshim.REF_ROOT = root
         refshim.install()
     else:
         from open3d_ml_b200 import shim
@@ -41,20 +40,9 @@ def install(ops):
     return root
 
 
-def ref_modules():
-    """(ml3d torch namespace, Config): through the fabricated `open3d` package with the product shim, directly
-    from the ml3d tree in the oracle dry run (oracle/refshim.py does not re-export the tree under open3d.ml)."""
-    if OPS == "oracle":
-        import ml3d.torch as m
-        from ml3d.utils import Config
-    else:
-        import open3d.ml.torch as m
-        from open3d.ml.utils import Config
-    return m, Config
-
-
 SEED = 1234
 REC = {}          # arrays of the case for --record
+RECORD = None     # --record DIR
 
 
 def seed_weights(net):
@@ -91,7 +79,8 @@ def case_pointpillars_class(root, dev):
     """Unmodified PointPillars (its own torch layers) fed by the shim's voxelize / ragged_to_dense, against the
     fused PointPillarsB200 built from the same state_dict; then inference_end (anchors, top-k, decode, rotated
     NMS through the shim's nms)."""
-    ml3d, Config = ref_modules()
+    import open3d.ml.torch as ml3d
+    from open3d.ml.utils import Config
     from open3d_ml_b200 import synth
     cfg = Config.load_from_file(os.path.join(root, "ml3d", "configs", "pointpillars_kitti.yml"))
     torch.manual_seed(0)
@@ -141,7 +130,8 @@ def _randla_inputs(net, n, seed):
 def case_randlanet_patch(root, dev):
     """patch_reference_model(RandLANet): the unmodified class with its forward on the fused CUDA path, against the
     same class on the CPU; inputs come from the class's own preprocess / transform (k-NN through the shim)."""
-    ml3d, Config = ref_modules()
+    import open3d.ml.torch as ml3d
+    from open3d.ml.utils import Config
     cfg = Config.load_from_file(os.path.join(root, "ml3d", "configs", "randlanet_semantickitti.yml"))
     cfg.model["num_points"] = 8192
     torch.manual_seed(0)
@@ -173,7 +163,8 @@ def case_randlanet_patch(root, dev):
 def case_semseg_inference(root, dev):
     """SemanticSegmentation.run_inference (semantic_segmentation.py:122-187) on a 20 000-point synthetic cloud,
     unmodified pipeline + dataloader + sampler; natives used: subsample x2, NearestNeighborSearch / knn_search."""
-    ml3d, Config = ref_modules()
+    import open3d.ml.torch as ml3d
+    from open3d.ml.utils import Config
     from open3d_ml_b200 import synth
     cfg = Config.load_from_file(os.path.join(root, "ml3d", "configs", "randlanet_semantickitti.yml"))
     cfg.model["num_points"] = 4096
@@ -199,7 +190,7 @@ def case_semseg_inference(root, dev):
 def case_kpconv_class(root, dev):
     """Unmodified KPFCNN (eval) on a batch built by its own preprocess / transform / ConcatBatcher (grid subsampling
     and the 13 radius searches through the shim), against KPFCNNB200 from the same state_dict and batch."""
-    ml3d, _ = ref_modules()
+    import open3d.ml.torch as ml3d
     from open3d_ml_b200 import synth
     os.chdir(tempfile.mkdtemp())
     np.random.seed(3)
@@ -234,16 +225,32 @@ def case_kpconv_class(root, dev):
     return out
 
 
-OPS = "b200"
+def record(name):
+    """Writes REC to DIR/name under --record DIR."""
+    if RECORD is not None:
+        np.savez_compressed(os.path.join(RECORD, name), **REC)
+
+
+def main(case, run):
+    """The recorders' command line: binds the ops `--ops` names, runs run(root, device) and prints its RESULT line."""
+    global RECORD
+    ops = "oracle" if "--ops" in sys.argv and sys.argv[sys.argv.index("--ops") + 1] == "oracle" else "b200"
+    if "--record" in sys.argv:
+        RECORD = sys.argv[sys.argv.index("--record") + 1]
+    root = install(ops)
+    dev = "cpu" if ops == "oracle" or not torch.cuda.is_available() else "cuda"
+    res = run(root, dev)
+    print("RESULT " + json.dumps(dict(case=case, ops=ops, device=dev, **res)))
+
+
 CASES = dict(ref_tests=case_ref_tests, pointpillars_class=case_pointpillars_class, randlanet_patch=case_randlanet_patch,
              semseg_inference=case_semseg_inference, kpconv_class=case_kpconv_class)
 
 if __name__ == "__main__":
     case = sys.argv[1]
-    OPS = ops = "oracle" if "--ops" in sys.argv and sys.argv[sys.argv.index("--ops") + 1] == "oracle" else "b200"
-    root = install(ops)
-    dev = "cpu" if ops == "oracle" or not torch.cuda.is_available() else "cuda"
-    res = CASES[case](root, dev)
-    if "--record" in sys.argv:
-        np.savez_compressed(os.path.join(sys.argv[sys.argv.index("--record") + 1], "boundary_%s.npz" % case), **REC)
-    print("RESULT " + json.dumps(dict(case=case, ops=ops, device=dev, **res)))
+
+    def run(root, dev):
+        res = CASES[case](root, dev)
+        record("boundary_%s.npz" % case)
+        return res
+    main(case, run)

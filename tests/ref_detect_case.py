@@ -1,6 +1,6 @@
 """Records tests/golden/boundary_pointpillars_detect.npz: the UNMODIFIED reference Anchor3DHead.get_bboxes on the
 seeded synthetic head maps of detect_support.PP_DETECT_CASES, driven through the drop-in boundary exactly as
-tests/ref_boundary_cases.py drives the other reference flows (whose install / ref_modules it reuses).  Run as a script in a
+tests/ref_boundary_cases.py drives the other reference flows (whose command line it reuses).  Run as a script in a
 fresh process:
 
     python tests/ref_detect_case.py [--ops oracle] [--record DIR]
@@ -31,7 +31,8 @@ def run(root, dev):
     PointPillars.inference_end after patch_reference_model."""
     import importlib
     from open3d_ml_b200.pointpillars import cfg_from_reference
-    ml3d, Config = rbc.ref_modules()
+    import open3d.ml.torch as ml3d
+    from open3d.ml.utils import Config
     pp_mod = importlib.import_module(ml3d.models.PointPillars.__module__)
     cfgs = {k: Config.load_from_file(os.path.join(root, "ml3d", "configs", "pointpillars_%s.yml" % k))
             for k in ("kitti", "waymo")}
@@ -73,15 +74,9 @@ def run(root, dev):
                 box_err=max([float((g.cpu() - r).abs().max()) for g, r in zip(got[0], boxes) if len(r)] + [0.0]),
                 inference_end_counts=[len(r) for r in res],
                 inference_end_names=[[bb.label_class for bb in r[:3]] for r in res])
+    rbc.record("boundary_pointpillars_detect.npz")
     return out
 
 
 if __name__ == "__main__":
-    rbc.OPS = ops = "oracle" if "--ops" in sys.argv and sys.argv[sys.argv.index("--ops") + 1] == "oracle" else "b200"
-    root = rbc.install(ops)
-    dev = "cpu" if ops == "oracle" or not torch.cuda.is_available() else "cuda"
-    res = run(root, dev)
-    if "--record" in sys.argv:
-        np.savez_compressed(os.path.join(sys.argv[sys.argv.index("--record") + 1], "boundary_pointpillars_detect.npz"),
-                            **rbc.REC)
-    print("RESULT " + json.dumps(dict(case="pointpillars_detect", ops=ops, device=dev, **res)))
+    rbc.main("pointpillars_detect", run)

@@ -1,7 +1,7 @@
 """Records tests/golden/boundary_kpconv_deform_class.npz: the UNMODIFIED reference KPFCNN built from
 ml3d/configs/kpconv_parislille3d.yml (deformable layers 2-4, reduce_fc head), on a batch its own preprocess /
 transform / ConcatBatcher built through the drop-in boundary (so the neighbourhoods are the deform-radius ones), with
-seeded manifest weights.  Reuses tests/ref_boundary_cases.py's install / ref_modules / seed_weights / record_output.
+seeded manifest weights.  Reuses tests/ref_boundary_cases.py's command line, seed_weights and record_output.
 Run as a script in a fresh process:
 
     python tests/ref_kpconv_deform_case.py [--ops oracle] [--record DIR]
@@ -30,7 +30,8 @@ IN_RADIUS, MAX_IN_POINTS, BATCH_LIMIT = 2.0, 4000, 4000
 
 
 def run(root, dev):
-    ml3d, Config = rbc.ref_modules()
+    import open3d.ml.torch as ml3d
+    from open3d.ml.utils import Config
     from open3d_ml_b200 import synth
     os.chdir(tempfile.mkdtemp())          # KPFCNN writes kernels/dispositions/*.npy into the CWD
     cfg = Config.load_from_file(os.path.join(root, "ml3d", "configs", "kpconv_parislille3d.yml"))
@@ -80,15 +81,9 @@ def run(root, dev):
         import open3d_ml_b200 as M
         got = M.KPFCNNB200(net.state_dict(), dict(net.cfg))(b)
         out["fused_rel_err"] = rbc.rel(got, ref)
+    rbc.record("boundary_kpconv_deform_class.npz")
     return out
 
 
 if __name__ == "__main__":
-    rbc.OPS = ops = "oracle" if "--ops" in sys.argv and sys.argv[sys.argv.index("--ops") + 1] == "oracle" else "b200"
-    root = rbc.install(ops)
-    dev = "cpu" if ops == "oracle" or not torch.cuda.is_available() else "cuda"
-    res = run(root, dev)
-    if "--record" in sys.argv:
-        np.savez_compressed(os.path.join(sys.argv[sys.argv.index("--record") + 1], "boundary_kpconv_deform_class.npz"),
-                            **rbc.REC)
-    print("RESULT " + json.dumps(dict(case="kpconv_deform_class", ops=ops, device=dev, **res)))
+    rbc.main("kpconv_deform_class", run)

@@ -1,7 +1,7 @@
 """Records tests/golden/pointpillars_config_<k>.npz for k in nuscenes, argoverse, lyft: the UNMODIFIED reference
 PointPillars built from its yml (nuScenes and Argoverse with a two-layer PillarFeatureNet) with seeded weights, and
 the unmodified Anchor3DHead.get_bboxes of its head on seeded head maps, driven through the drop-in boundary exactly
-as tests/ref_boundary_cases.py drives the other reference flows (whose install / ref_modules / seed_weights /
+as tests/ref_boundary_cases.py drives the other reference flows (whose command line, seed_weights and
 record_output it reuses).  Run as a script in a fresh process:
 
     python tests/ref_pointpillars_configs.py [--ops oracle] [--record DIR]
@@ -31,9 +31,10 @@ from detect_support import pp_detect_maps  # noqa: E402
 from pp_configs_support import CONFIGS, DETECT_CASES, digest, fixture, synth_frame  # noqa: E402
 
 
-def run(root, dev, record_dir=None):
+def run(root, dev):
     from open3d_ml_b200.pointpillars import cfg_from_reference
-    ml3d, Config = rbc.ref_modules()
+    import open3d.ml.torch as ml3d
+    from open3d.ml.utils import Config
     pp_mod = importlib.import_module(ml3d.models.PointPillars.__module__)
     torch.backends.cuda.matmul.allow_tf32 = False
     torch.backends.cudnn.allow_tf32 = False
@@ -96,14 +97,9 @@ def run(root, dev, record_dir=None):
                 rbc.REC[key + "boxes"] = boxes[b].numpy()
                 rbc.REC[key + "scores"] = scores[b].numpy()
                 rbc.REC[key + "labels"] = labels[b].numpy()
-        if record_dir is not None:
-            np.savez_compressed(os.path.join(record_dir, os.path.basename(fixture(k))), **rbc.REC)
+        rbc.record(os.path.basename(fixture(k)))
     return out
 
 
 if __name__ == "__main__":
-    rbc.OPS = ops = "oracle" if "--ops" in sys.argv and sys.argv[sys.argv.index("--ops") + 1] == "oracle" else "b200"
-    root = rbc.install(ops)
-    dev = "cpu" if ops == "oracle" or not torch.cuda.is_available() else "cuda"
-    res = run(root, dev, sys.argv[sys.argv.index("--record") + 1] if "--record" in sys.argv else None)
-    print("RESULT " + json.dumps(dict(case="pointpillars_configs", ops=ops, device=dev, **res)))
+    rbc.main("pointpillars_configs", run)
