@@ -81,6 +81,14 @@ _SIGNATURES = {
     "o3dml_kpconv_gather_deformable": (I, [P, L, P, L, P, I, I, P, I, P, I, F, P, I, P, P]),
 }
 EXPORTS = tuple(_SIGNATURES)           # the product ABI: exactly what include/o3dml_b200.h declares
+# the PVCNN entries of the product ABI: exactly what include/o3dml_b200_pvcnn.h declares
+_PVCNN_SIGNATURES = {
+    "o3dml_pv_voxel_cells": (I, [P, I, I, I, F, P, P, P, P]),
+    "o3dml_pv_cell_mean": (I, [P, P, L, P, I, I, I, P, P]),
+    "o3dml_conv3x3x3_ndhwc_tc": (I, [P, I, I, I, I, I, P, I, I, P, P, I, F, P, I, P]),
+    "o3dml_trilinear_devoxelize": (I, [P, I, I, I, P, I, I, I, P, I, P, P, P]),
+}
+PVCNN_EXPORTS = tuple(_PVCNN_SIGNATURES)
 # bring-up / profiling hooks (include/o3dml_b200_bringup.h): exported by the library, not part of the product ABI
 _BRINGUP_SIGNATURES = {
     "o3dml_tc_gemm_test": (I, [P, P, P, I, I, I, P]),
@@ -106,7 +114,8 @@ def lib():
                         "There is no CPU fallback." % (LIB_PATH, e)) from e
                 raise
         h = ctypes.CDLL(LIB_PATH)
-        for name, (res, args) in list(_SIGNATURES.items()) + list(_BRINGUP_SIGNATURES.items()):
+        for name, (res, args) in (list(_SIGNATURES.items()) + list(_PVCNN_SIGNATURES.items()) +
+                                  list(_BRINGUP_SIGNATURES.items())):
             fn = getattr(h, name)
             fn.restype, fn.argtypes = res, args
         if h.o3dml_abi_version() != ABI_VERSION:
@@ -340,6 +349,17 @@ def conv3x3(x, weight, out, scale=None, shift=None, stride=1, act=None, slope=0.
         wt = weight.wt if isinstance(weight, PackedWeight) else weight
         check(lib().o3dml_conv3x3_nhwc(ptr(x), B, H, W, C, stride, ptr(wt), ptr(scale), ptr(shift), act_code(act),
                                        float(slope), ptr(out), co, stream()))
+    return out
+
+
+def conv3x3x3(x, weight, out, scale=None, shift=None, act=None, slope=0.0):
+    """out = act(scale * conv3x3x3(x) + shift): padding 1, stride 1, x [B, X, Y, Z, C] and out [B, X, Y, Z, Cout]
+    contiguous channels-last grids, C % 32 == 0.  `weight` is the PackedWeight of [27 C, Cout], row
+    ((kx * 3 + ky) * 3 + kz) * C + c.  There is one kernel, on the tensor cores."""
+    B, X, Y, Z, C = x.shape
+    check(lib().o3dml_conv3x3x3_ndhwc_tc(ptr(x), B, X, Y, Z, C, ptr(weight.img), weight.k_pad, weight.n_pad,
+                                         ptr(scale), ptr(shift), act_code(act), float(slope), ptr(out), out.shape[4],
+                                         stream()))
     return out
 
 

@@ -1,8 +1,8 @@
 """Package body of open3d_ml_b200 (see open3d_ml_b200/__init__.py).
 
 Hopper (sm_90a) operators behind the `open3d.ml.torch.ops` surface used by
-Open3D-ML's PyTorch models, plus fused forwards for PointPillars, RandLA-Net and
-KPFCNN.  Importing the package does not touch CUDA; calling any operator without the
+Open3D-ML's PyTorch models, plus fused forwards for PointPillars, RandLA-Net,
+KPFCNN and PVCNN.  Importing the package does not touch CUDA; calling any operator without the
 CUDA library or a CUDA device raises RuntimeError (there is no CPU fallback).
 """
 __version__ = "0.1.0"
@@ -24,6 +24,9 @@ def __getattr__(name):
     if name in ("KPFCNNB200",):
         from .kpconv import KPFCNNB200
         return KPFCNNB200
+    if name in ("PVCNNB200",):
+        from .pvcnn import PVCNNB200
+        return PVCNNB200
     if name in ("PipelinedRunner",):
         from .pipeline import PipelinedRunner
         return PipelinedRunner

@@ -98,6 +98,46 @@ inline int set_conv3x3(const char* fn, P& p, const float* in, int batch, int H, 
     return O3DML_OK;
 }
 
+// A 3x3x3 convolution, padding 1, stride 1, over a channels-last grid [batch, X, Y, Z, C] (z fastest among the
+// spatial axes) as an implicit GEMM: one row per output voxel, K = 27 C, weight row ((kx * 3 + ky) * 3 + kz) * C + c.
+// A CTA owns a PZ x PY x PX = `rows` box of output voxels with power-of-two sides: the shape with the fewest boxes,
+// then the most compact one (its 27 shifted copies overlap most in L2), then the longest run along z.
+template <class P>
+inline int set_conv3x3x3(const char* fn, P& p, const float* in, int batch, int X, int Y, int Z, int C, int c_multiple,
+                         int rows) {
+    O3DML_CHECK(in && batch > 0 && X > 0 && Y > 0 && Z > 0, "%s: bad input", fn);
+    O3DML_CHECK((C % c_multiple) == 0 && C > 0, "%s: input channels must be a multiple of %d", fn, c_multiple);
+    O3DML_CHECK((reinterpret_cast<uintptr_t>(in) & 15) == 0, "%s: input must be 16-byte aligned", fn);
+    O3DML_CHECK((int64_t)batch * X * Y * Z < ((int64_t)1 << 31), "%s: 2^31 or more voxels", fn);
+    p.mode = 2;
+    p.nsrc = 1;
+    p.src[0].data = in;
+    p.X = X; p.Y = Y; p.Z = Z; p.C = C;
+    p.N = (int64_t)batch * X * Y * Z;
+    p.K = 27 * C;
+    int lr = 0;
+    while ((1 << lr) < rows) ++lr;
+    int64_t best_tiles = -1;
+    int best_sum = 0;
+    for (int lz = 0; lz <= lr; ++lz)
+        for (int ly = 0; lz + ly <= lr; ++ly) {
+            const int pz = 1 << lz, py = 1 << ly, px = rows >> (lz + ly);
+            const int64_t tiles = (int64_t)ceil_div(Z, pz) * ceil_div(Y, py) * ceil_div(X, px);
+            const int sum = pz + py + px;
+            if (best_tiles < 0 || tiles < best_tiles || (tiles == best_tiles && sum < best_sum) ||
+                (tiles == best_tiles && sum == best_sum && lz > p.lpz)) {
+                best_tiles = tiles;
+                best_sum = sum;
+                p.lpz = lz;
+                p.lpy = ly;
+            }
+        }
+    p.tiles_z = ceil_div(Z, 1 << p.lpz);
+    p.tiles_y = ceil_div(Y, 1 << p.lpy);
+    p.tiles_x = ceil_div(X, rows >> (p.lpz + p.lpy));
+    return O3DML_OK;
+}
+
 // A transposed convolution with kernel == stride over an NHWC input is a 1x1 product over the input pixels (one
 // identity source of C channels, stride^2 * out_channels columns) whose output is pixel-shuffled.  scale / shift come
 // tiled to [stride^2 * out_channels].

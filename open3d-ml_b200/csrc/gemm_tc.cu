@@ -13,7 +13,8 @@
 //   * identity row sources and the 3x3 convolution taps are fetched by ONE cp.async.bulk.tensor per
 //     slice (2-D {channels, rows} map; 4-D {C, W, H, B} map whose box is a PW x PH patch of output
 //     pixels shifted by the tap -- negative / overflowing coordinates are zero-filled by the TMA unit,
-//     which is the convolution padding; stride-2 convolutions use four parity maps),
+//     which is the convolution padding; stride-2 convolutions use four parity maps; the 3x3x3 convolution is the
+//     same with a 5-D {C, Z, Y, X, B} map, the rank limit of the TMA unit, and a PZ x PY x PX box of output voxels),
 //   * gathered sources (index / batch-relative index / shadow rows) by 16-byte cp.async into the same
 //     128-byte-swizzled layout,
 //   * the weight slices (hi and lo image) by two more tensor copies.
@@ -26,6 +27,7 @@
 // Every GT_FLUSH slices the wgmma accumulator is folded into a second fp32 register set with
 // round-to-nearest adds, so that long products do not rely on the tensor core's internal accumulation.
 #include "../../include/o3dml_b200.h"
+#include "../../include/o3dml_b200_pvcnn.h"
 #include "dense.cuh"
 #include "tc.cuh"
 #include <cuda.h>
@@ -46,12 +48,13 @@ struct alignas(64) GemmTcParams {
     CUtensorMap mapB;      // {Kpad, 2*Npad}: hi rows [0, Npad), lo rows [Npad, 2*Npad)
     int64_t N;
     int K, Kpad, Cout, Npad;
-    int mode;  // 0 rows, 1 conv3x3
+    int mode;  // 0 rows, 1 conv3x3, 2 conv3x3x3
     int nsrc;
     o3dml_src_t src[GT_MAX_SRC];
     int koff[GT_MAX_SRC + 1];
     int H, W, OH, OW, stride, C;
     int lpw, PH, tiles_x, tiles_y;   // conv: patch = (1 << lpw) x PH output pixels per CTA
+    int X, Y, Z, lpz, lpy, tiles_z;  // conv3x3x3: box = (1 << lpz) x (1 << lpy) x (128 >> (lpz + lpy)) output voxels, z fastest
     DenseEpilogue ep;
 };
 
@@ -85,6 +88,14 @@ __device__ __forceinline__ void tma_load_4d(uint32_t smem_dst, const CUtensorMap
         "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], "
         "[%2];" ::"r"(smem_dst),
         "l"(map), "r"(tc::smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+        : "memory");
+}
+__device__ __forceinline__ void tma_load_5d(uint32_t smem_dst, const CUtensorMap* map, int c0, int c1, int c2, int c3, int c4,
+                                            uint64_t* bar) {
+    asm volatile(
+        "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], "
+        "[%2];" ::"r"(smem_dst),
+        "l"(map), "r"(tc::smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
         : "memory");
 }
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
@@ -141,15 +152,23 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
     const int tid = threadIdx.x;
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // warp-uniform for the compiler
     const int col0 = blockIdx.y * BN;
-    // rows mode: 128 consecutive output rows; conv mode: a PW x PH patch of output pixels of one image
+    // rows mode: 128 consecutive output rows; conv mode: a PW x PH patch of output pixels of one image; conv3x3x3:
+    // a PZ x PY x PX box of output voxels of one grid
     int64_t row0 = (int64_t)blockIdx.x * GT_ROWS;
-    int cb = 0, oy0 = 0, ox0 = 0;
+    int cb = 0, oy0 = 0, ox0 = 0, oz0 = 0;
     if (p.mode == 1) {
         const int per = p.tiles_x * p.tiles_y;
         cb = blockIdx.x / per;
         const int t = blockIdx.x - cb * per;
         oy0 = (t / p.tiles_x) * p.PH;
         ox0 = (t % p.tiles_x) << p.lpw;
+    } else if (p.mode == 2) {
+        const int per = p.tiles_x * p.tiles_y * p.tiles_z;
+        cb = blockIdx.x / per;
+        const int t = blockIdx.x - cb * per, txy = t / p.tiles_z;
+        oz0 = (t - txy * p.tiles_z) << p.lpz;
+        oy0 = (txy % p.tiles_y) << p.lpy;
+        ox0 = (txy / p.tiles_y) * (GT_ROWS >> (p.lpz + p.lpy));
     }
 
     // ---- per-row bookkeeping
@@ -158,9 +177,13 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
         if (p.mode == 0) {
             n = row0 + m;
             if (n >= p.N) n = -1;
-        } else {
+        } else if (p.mode == 1) {
             const int oy = oy0 + (m >> p.lpw), ox = ox0 + (m & ((1 << p.lpw) - 1));
             n = (oy < p.OH && ox < p.OW) ? ((int64_t)cb * p.OH + oy) * p.OW + ox : -1;
+        } else {
+            const int oz = oz0 + (m & ((1 << p.lpz) - 1)), oy = oy0 + ((m >> p.lpz) & ((1 << p.lpy) - 1));
+            const int ox = ox0 + (m >> (p.lpz + p.lpy));
+            n = (ox < p.X && oy < p.Y && oz < p.Z) ? (((int64_t)cb * p.X + ox) * p.Y + oy) * p.Z + oz : -1;
         }
         rown[m] = n;
     }
@@ -194,7 +217,7 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
         const int rt = tid - GT_CONV_THREADS;                   // loader index; 0 is also the producer
         if (GATHER || rt == 0) {
             if (rt == 0) tma_prefetch_desc(&p.mapB);
-            const int spt = p.mode == 1 ? p.C / GT_KS : 1;      // slices per convolution tap
+            const int spt = p.mode != 0 ? p.C / GT_KS : 1;      // slices per convolution tap
             int sidx = 0;
             for (int sl = 0; sl < nsl; ++sl) {
                 const int stage = sl % S, use = sl / S;
@@ -214,6 +237,10 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
                     if (a_tma) {
                         if (p.mode == 0) {
                             tma_load_2d(ah, &p.mapA[sidx], k0 - p.koff[sidx], (int)row0, &full_bar[stage]);
+                        } else if (p.mode == 2) {   // tap (kx * 3 + ky) * 3 + kz, as the weight rows
+                            const int tap = sl / spt, cc = (sl - tap * spt) * GT_KS;
+                            const int dx = tap / 9, dy = (tap - dx * 9) / 3, dz = tap - dx * 9 - dy * 3;
+                            tma_load_5d(ah, &p.mapA[0], cc, oz0 - 1 + dz, oy0 - 1 + dy, ox0 - 1 + dx, cb, &full_bar[stage]);
                         } else {
                             const int tap = sl / spt, cc = (sl - tap * spt) * GT_KS;
                             const int dy = tap / 3, dx = tap - dy * 3;
@@ -442,9 +469,11 @@ static int gemm_tc_launch(GemmTcParams& p, const void* wimg, int k_pad, int n_pa
         int best_tiles = 1 << 30;
         for (int l = 0; l <= 7; ++l) best_tiles = std::min(best_tiles, ceil_div(p.OW, 1 << l) * ceil_div(p.OH, GT_ROWS >> l));
         row_tiles = (p.N / ((int64_t)p.OH * p.OW)) * best_tiles;
+    } else if (p.mode == 2) {
+        row_tiles = (p.N / ((int64_t)p.X * p.Y * p.Z)) * p.tiles_x * p.tiles_y * p.tiles_z;
     }
     // products of plain row sources, at most 16 k-slices long, that fill the SMs more than once as 64-column tiles run on
-    // the LITE kernels, two CTAs per SM (GtCfg); the convolutions (K = 9 C) stay on the one-CTA-per-SM kernels
+    // the LITE kernels, two CTAs per SM (GtCfg); the convolutions (K = 9 C, 27 C) stay on the one-CTA-per-SM kernels
     const bool lite = p.mode == 0 && !any_gather && p.Kpad / GT_KS <= GT_LITE_MAX_SLICES &&
                       row_tiles * (p.Npad / (bn == 32 ? 32 : 64)) > sms;
     if (lite && bn == 128) bn = 64;
@@ -471,6 +500,15 @@ static int gemm_tc_launch(GemmTcParams& p, const void* wimg, int k_pad, int n_pa
             int rc = make_map(&p.mapA[s], p.src[s].data, 2, dims, str, box);
             if (rc) return rc;
         }
+    } else if (p.mode == 2) {   // the box of output voxels per CTA was chosen by set_conv3x3x3
+        const int64_t batch = p.N / ((int64_t)p.X * p.Y * p.Z);
+        grid_x = (unsigned)row_tiles;
+        const uint32_t box[5] = {GT_KS, 1u << p.lpz, 1u << p.lpy, (uint32_t)(GT_ROWS >> (p.lpz + p.lpy)), 1};
+        const uint64_t dims[5] = {(uint64_t)p.C, (uint64_t)p.Z, (uint64_t)p.Y, (uint64_t)p.X, (uint64_t)batch};
+        const uint64_t str[4] = {(uint64_t)p.C * 4, (uint64_t)p.Z * p.C * 4, (uint64_t)p.Y * p.Z * p.C * 4,
+                                 (uint64_t)p.X * p.Y * p.Z * p.C * 4};
+        int rc = make_map(&p.mapA[0], p.src[0].data, 5, dims, str, box);
+        if (rc) return rc;
     } else {
         // patch of output pixels per CTA: PW x PH = 128, the shape with the fewest tiles
         int best = -1, best_tiles = 0;
@@ -581,5 +619,16 @@ extern "C" int o3dml_deconv_nhwc_tc(const float* in, int batch, int H, int W, in
                         out_channels);
     if (rc) return rc;
     O3DML_CHECK((C % 4) == 0 && (reinterpret_cast<uintptr_t>(in) & 15) == 0, "deconv_tc: C % 4, aligned input");
+    return gemm_tc_launch(p, weight_image, k_pad, n_pad, (cudaStream_t)stream);
+}
+
+extern "C" int o3dml_conv3x3x3_ndhwc_tc(const float* in, int batch, int X, int Y, int Z, int C, const void* weight_image,
+                                        int k_pad, int n_pad, const float* scale, const float* shift, int act,
+                                        float slope, float* out, int out_channels, void* stream) {
+    GemmTcParams p = {};
+    int rc = set_conv3x3x3("conv3x3x3_tc", p, in, batch, X, Y, Z, C, GT_KS, GT_ROWS);
+    if (!rc) rc = set_epilogue("conv3x3x3_tc", p, weight_image, scale, shift, nullptr, 0, act, slope, out, out_channels,
+                               out_channels, 0);
+    if (rc) return rc;
     return gemm_tc_launch(p, weight_image, k_pad, n_pad, (cudaStream_t)stream);
 }

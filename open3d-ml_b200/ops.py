@@ -620,6 +620,31 @@ def invert_neighbors_list(num_points, inp_neighbors_index, inp_neighbors_row_spl
     return _back(InvertNeighborsListResult(out_idx, out_rs, out_attrs), inp_neighbors_index.device)
 
 
+def trilinear_devoxelize_forward(resolution, is_training, coords, features):
+    """open3d.ml.torch.ops.trilinear_devoxelize_forward (pvcnn.py:37): coords [B, 3, N] voxel coordinates in
+    [0, r - 1], features [B, C, r, r, r] -> (outs [B, C, N], inds int32 [B, 8, N], wgts [B, 8, N]); the rule is in
+    DESIGN.md section 2.  The kernel works on point rows and a channels-last grid, so the reference layout is
+    permuted on the way in and out; the fused PVCNN forward keeps its own layout and skips that.  inds and wgts are
+    written whether or not is_training is set.  No host read."""
+    r = int(resolution)
+    c, f = _dev(coords), _dev(features)
+    if c.dim() != 3 or c.shape[1] != 3 or f.dim() != 5 or tuple(f.shape[2:]) != (r, r, r) or f.shape[0] != c.shape[0]:
+        raise RuntimeError("trilinear_devoxelize_forward: coords [B, 3, N] and features [B, C, r, r, r] expected")
+    if c.dtype != torch.float32 or f.dtype != torch.float32:
+        raise RuntimeError("trilinear_devoxelize_forward: float32 inputs expected")
+    B, _, N = c.shape
+    C = f.shape[1]
+    rows = c.permute(0, 2, 1).contiguous()
+    grid = f.permute(0, 2, 3, 4, 1).contiguous()
+    out = torch.empty((B, N, C), dtype=torch.float32, device=c.device)
+    inds = torch.empty((B, 8, N), dtype=torch.int32, device=c.device)
+    wgts = torch.empty((B, 8, N), dtype=torch.float32, device=c.device)
+    L.check(L.lib().o3dml_trilinear_devoxelize(L.ptr(rows), B, N, r, L.ptr(grid), C, C, 0, L.ptr(out), C, L.ptr(inds),
+                                               L.ptr(wgts), L.stream()))
+    dev = coords.device
+    return tuple(_back(t, dev) for t in (out.permute(0, 2, 1).contiguous(), inds, wgts))
+
+
 def continuous_conv_transpose(filters, out_positions, out_importance, extents, offset, inp_positions, inp_features,
                               inp_neighbors_index, inp_neighbors_importance_sum, inp_neighbors_row_splits,
                               neighbors_index, neighbors_importance, neighbors_row_splits, align_corners=False,

@@ -117,7 +117,10 @@ def _library_bindings():
             reduce_subarrays_sum=O.reduce_subarrays_sum,
             voxel_pooling=O.voxel_pooling,
             continuous_conv=O.continuous_conv, continuous_conv_transpose=O.continuous_conv_transpose,
-            invert_neighbors_list=O.invert_neighbors_list, sparse_conv=O.sparse_conv),
+            invert_neighbors_list=O.invert_neighbors_list, sparse_conv=O.sparse_conv,
+            trilinear_devoxelize_forward=O.trilinear_devoxelize_forward,
+            # inference only: the backward resolves for the reference's import line and raises when called
+            trilinear_devoxelize_backward=_not_on_hot_path("open3d.ml.torch.ops.trilinear_devoxelize_backward")),
         "open3d.ml.torch.layers": dict(
             FixedRadiusSearch=O.FixedRadiusSearch, RadiusSearch=O.RadiusSearch,
             KNNSearch=O.KNNSearch,
@@ -161,8 +164,9 @@ def install(ml3d_root=None, bindings=None):
     mlt = _module("open3d.ml.torch")
     for name in library:
         _module(name, **attrs(name))
-    # device_count() = 0 keeps the reference from importing the CUDA-only PointNet++/PVCNN ops
-    # (pointnet2_utils.py:35-36, roipool3d_utils.py:3-4, pvcnn.py:13-14), which are off the path
+    # device_count() = 0 keeps the reference from importing the CUDA-only PointNet++ ops
+    # (pointnet2_utils.py:35-36, roipool3d_utils.py:3-4), which are off the path; PVCNN's import line
+    # (pvcnn.py:13-14) is skipped with them, and pvcnn.patch_reference_model replaces the forward that needs it
     _module("open3d.core.cuda", device_count=lambda: 0)
     for n in ("open3d.visualization", "open3d.visualization.tensorboard_plugin",
               "open3d.visualization.tensorboard_plugin.summary", "open3d.geometry", "open3d.utility", "open3d.io",

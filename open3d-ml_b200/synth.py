@@ -119,6 +119,15 @@ def room_cloud(n, seed, dl=0.04, room=(6.0, 5.0, 2.7), feat_dim=5):
     return pts, feats
 
 
+def pvcnn_s3dis_input(n, seed):
+    """PVCNN's S3DIS input by the arithmetic of PVCNN.preprocess (pvcnn.py:203-223) on a room_cloud: min-shifted xyz,
+    colour in [0, 1], xyz over its per-axis maximum.  -> (point [n, 3], feat [n, 9]) float32 rows."""
+    pts, f = room_cloud(n, seed)
+    pts = pts - pts.min(0)
+    feat = np.concatenate([pts, f[:, 1:4], pts / pts.max(0)], 1)
+    return pts.astype(np.float32), feat.astype(np.float32)
+
+
 def grid_subsample(points, dl):
     """Barycentre grid subsampling (stand-in for `open3d.ml.contrib.subsample`,
     kpconv.py:2037-2164; a "next" row of SURVEY.md 8f).  Deterministic."""
