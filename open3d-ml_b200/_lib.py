@@ -89,6 +89,11 @@ _PVCNN_SIGNATURES = {
     "o3dml_trilinear_devoxelize": (I, [P, I, I, I, P, I, I, I, P, I, P, P, P]),
 }
 PVCNN_EXPORTS = tuple(_PVCNN_SIGNATURES)
+# the sparse-convolution contraction of the product ABI: exactly what include/o3dml_b200_sparseconvunet.h declares
+_SPARSECONVUNET_SIGNATURES = {
+    "o3dml_sparse_conv_tc": (I, [L, P, L, I, I, P, I, I, P, P, P, I, I, P, P, P, I, I, F, P, I, I, P]),
+}
+SPARSECONVUNET_EXPORTS = tuple(_SPARSECONVUNET_SIGNATURES)
 # bring-up / profiling hooks (include/o3dml_b200_bringup.h): exported by the library, not part of the product ABI
 _BRINGUP_SIGNATURES = {
     "o3dml_tc_gemm_test": (I, [P, P, P, I, I, I, P]),
@@ -115,7 +120,7 @@ def lib():
                 raise
         h = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in (list(_SIGNATURES.items()) + list(_PVCNN_SIGNATURES.items()) +
-                                  list(_BRINGUP_SIGNATURES.items())):
+                                  list(_SPARSECONVUNET_SIGNATURES.items()) + list(_BRINGUP_SIGNATURES.items())):
             fn = getattr(h, name)
             fn.restype, fn.argtypes = res, args
         if h.o3dml_abi_version() != ABI_VERSION:

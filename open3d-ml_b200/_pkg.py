@@ -2,7 +2,7 @@
 
 Hopper (sm_90a) operators behind the `open3d.ml.torch.ops` surface used by
 Open3D-ML's PyTorch models, plus fused forwards for PointPillars, RandLA-Net,
-KPFCNN and PVCNN.  Importing the package does not touch CUDA; calling any operator without the
+KPFCNN, PVCNN and SparseConvUnet.  Importing the package does not touch CUDA; calling any operator without the
 CUDA library or a CUDA device raises RuntimeError (there is no CPU fallback).
 """
 __version__ = "0.1.0"
@@ -27,6 +27,9 @@ def __getattr__(name):
     if name in ("PVCNNB200",):
         from .pvcnn import PVCNNB200
         return PVCNNB200
+    if name in ("SparseConvUnetB200",):
+        from .sparseconvunet import SparseConvUnetB200
+        return SparseConvUnetB200
     if name in ("PipelinedRunner",):
         from .pipeline import PipelinedRunner
         return PipelinedRunner

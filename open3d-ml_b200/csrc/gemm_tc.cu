@@ -24,10 +24,17 @@
 // Shared-memory layout: K-major, SWIZZLE_128B (row r, 16-byte chunk c at r*128 + ((c ^ (r & 7)) << 4)),
 // descriptors with SBO = 1024, K advanced by +32 B per wgmma (K = 8 TF32).
 //
+// Table mode (the sparse convolutions): out[m] = sum over the kernel cells c of W_c^T act(x[table[m, c]]), K = cells x
+// Cin padded to 32.  The loaders gather each 32-channel slice of a cell from the row the table names (a shadow id
+// reads zeros); the (tile, cell) pairs whose 128 rows are all shadow are skipped.  The optional prologue act(x) =
+// relu(pre_scale * x + pre_shift) is applied by the consumers in registers before the split, and keeps shadow rows at
+// zero: an empty cell contributes nothing, not act(0).
+//
 // Every GT_FLUSH slices the wgmma accumulator is folded into a second fp32 register set with
 // round-to-nearest adds, so that long products do not rely on the tensor core's internal accumulation.
 #include "../../include/o3dml_b200.h"
 #include "../../include/o3dml_b200_pvcnn.h"
+#include "../../include/o3dml_b200_sparseconvunet.h"
 #include "dense.cuh"
 #include "tc.cuh"
 #include <cuda.h>
@@ -39,6 +46,7 @@ constexpr int GT_ROWS = 128;
 constexpr int GT_KS = 32;        // fp32 channels per k-slice (= one 128-byte swizzle row)
 constexpr int GT_FLUSH = 4;      // k-slices (128 channels = 48 accumulating MMAs) per register accumulation chunk
 constexpr int GT_MAX_SRC = 3;
+constexpr int GT_TABLE_MAX_CELLS = 512;   // table mode: kernel cells of one contraction (the list fits the rowptr slots)
 constexpr int GT_CONV_THREADS = 256;   // warps 0-7: the two consumer warpgroups
 constexpr int GT_LOADERS = 128;        // warps 8-11 (GATHER kernels only)
 constexpr int GT_A_BYTES = GT_ROWS * 128;
@@ -48,7 +56,7 @@ struct alignas(64) GemmTcParams {
     CUtensorMap mapB;      // {Kpad, 2*Npad}: hi rows [0, Npad), lo rows [Npad, 2*Npad)
     int64_t N;
     int K, Kpad, Cout, Npad;
-    int mode;  // 0 rows, 1 conv3x3, 2 conv3x3x3
+    int mode;  // 0 rows, 1 conv3x3, 2 conv3x3x3, 3 table
     int nsrc;
     o3dml_src_t src[GT_MAX_SRC];
     int koff[GT_MAX_SRC + 1];
@@ -56,6 +64,9 @@ struct alignas(64) GemmTcParams {
     int lpw, PH, tiles_x, tiles_y;   // conv: patch = (1 << lpw) x PH output pixels per CTA
     int X, Y, Z, lpz, lpy, tiles_z;  // conv3x3x3: box = (1 << lpz) x (1 << lpy) x (128 >> (lpz + lpy)) output voxels, z fastest
     DenseEpilogue ep;
+    int cells;                              // table mode: src[0] = features + table (index, index_ld), C = Cin padded to 32
+    const float* pre_scale;                 // table mode prologue (both or neither)
+    const float* pre_shift;
 };
 
 // ---- async-copy primitives ---------------------------------------------------------------------
@@ -102,6 +113,14 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
+// table mode: the feature row that row n of the output reads in kernel cell `cell`, nullptr for a shadow id
+__device__ __forceinline__ const float* table_row(const GemmTcParams& p, int64_t n, int cell) {
+    if (n >= p.N) return nullptr;
+    const o3dml_src_t& S = p.src[0];
+    const int64_t r = ((const int32_t*)S.index)[n * S.index_ld + cell];
+    return (r < 0 || r >= S.rows) ? nullptr : S.data + (size_t)r * S.ld;
+}
+
 // LITE: two stages instead of 4 - 6, so that TWO CTAs share an SM.  A short product (K <= 512) is mostly
 // prologue and epilogue around a few 32-channel slices: with one CTA per SM the tensor pipe and the TMA unit
 // idle through both; a sibling CTA fills them.
@@ -132,7 +151,7 @@ constexpr int GT_PRODUCER_WARP = 8;
 template <bool GATHER>
 __host__ __device__ constexpr int gt_threads() { return GT_CONV_THREADS + (GATHER ? GT_LOADERS : 32); }
 
-template <int BN, bool GATHER, bool LITE>
+template <int BN, bool GATHER, bool LITE, bool TABLE = false>
 __global__ void __launch_bounds__(gt_threads<GATHER>(), LITE ? 2 : 1)
 gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
     using C = GtCfg<BN, LITE>;
@@ -174,7 +193,7 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
     // ---- per-row bookkeeping
     for (int m = tid; m < GT_ROWS; m += blockDim.x) {
         int64_t n;
-        if (p.mode == 0) {
+        if (TABLE || p.mode == 0) {
             n = row0 + m;
             if (n >= p.N) n = -1;
         } else if (p.mode == 1) {
@@ -192,7 +211,23 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
         s_scale[i] = (ep.scale && c < p.Cout) ? ep.scale[c] : 1.f;
         s_shift[i] = (ep.shift && c < p.Cout) ? ep.shift[c] : 0.f;
     }
-    if (GATHER) {
+    // table mode: act[] lists the kernel cells that some row of this tile reads, act[GT_TABLE_MAX_CELLS] counts them
+    int* act = reinterpret_cast<int*>(rowptr);
+    if (TABLE) {
+        for (int c = tid; c < p.cells; c += blockDim.x) act[c] = 0;
+        __syncthreads();
+        for (int i = tid; i < p.cells * GT_ROWS; i += blockDim.x) {
+            const int m = i / p.cells, c = i - m * p.cells;
+            if (table_row(p, row0 + m, c)) act[c] = 1;
+        }
+        __syncthreads();
+        if (tid == 0) {
+            int k = 0;
+            for (int c = 0; c < p.cells; ++c)
+                if (act[c]) act[k++] = c;
+            act[GT_TABLE_MAX_CELLS] = k;
+        }
+    } else if (GATHER) {
         for (int i = tid; i < p.nsrc * GT_ROWS; i += blockDim.x) {
             const int s = i / GT_ROWS, m = i % GT_ROWS;
             const int64_t n = row0 + m;
@@ -209,13 +244,43 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
     }
     __syncthreads();
 
-    const int nsl = p.Kpad / GT_KS;
+    const int spc = p.C / GT_KS;                      // table mode: slices per kernel cell
+    const int nsl = TABLE ? act[GT_TABLE_MAX_CELLS] * spc : p.Kpad / GT_KS;
     const uint32_t stage0 = tc::smem_u32(stages);
 
     if (warp >= GT_PRODUCER_WARP) {
         // ================================================================= TMA producer (+ gather loaders)
         const int rt = tid - GT_CONV_THREADS;                   // loader index; 0 is also the producer
-        if (GATHER || rt == 0) {
+        if (TABLE) {
+            // loader rt fills 16-byte chunk rt & 7 of rows (rt >> 3) + 16 j; their feature rows change with the cell
+            const float* base[(GT_ROWS * 8) / GT_LOADERS] = {};
+            if (rt == 0) tma_prefetch_desc(&p.mapB);
+            const int cin = p.src[0].channels;
+            for (int sl = 0; sl < nsl; ++sl) {
+                const int stage = sl % S, use = sl / S;
+                if (use >= 1) tc::mbar_wait(&empty_bar[stage], (use - 1) & 1);
+                const int ci = sl / spc, j = sl - ci * spc, cell = act[ci];
+                const uint32_t ah = stage0 + (uint32_t)stage * C::STAGE;
+                if (rt == 0) {
+                    const uint32_t bh = ah + GT_A_BYTES;
+                    const int k0 = cell * p.C + j * GT_KS;
+                    mbar_arrive_expect_tx(&full_bar[stage], 2 * C::B_BYTES);
+                    tma_load_2d(bh, &p.mapB, k0, col0, &full_bar[stage]);
+                    tma_load_2d(bh + C::B_BYTES, &p.mapB, k0, p.Npad + col0, &full_bar[stage]);
+                }
+#pragma unroll
+                for (int jj = 0; jj < (GT_ROWS * 8) / GT_LOADERS; ++jj) {
+                    const int item = rt + jj * GT_LOADERS;
+                    const int m = item >> 3, c = item & 7;
+                    if (j == 0) base[jj] = table_row(p, row0 + m, cell);
+                    const int kk = j * GT_KS + c * 4;
+                    const int bytes = base[jj] != nullptr ? 4 * max(0, min(4, cin - kk)) : 0;   // zero past Cin
+                    cp_async16(ah + (uint32_t)m * 128u + (uint32_t)((c ^ (m & 7)) << 4),
+                               bytes ? (const void*)(base[jj] + kk) : (const void*)p.src[0].data, bytes);
+                }
+                cp_async_arrive(&full_bar[stage]);
+            }
+        } else if (GATHER || rt == 0) {
             if (rt == 0) tma_prefetch_desc(&p.mapB);
             const int spt = p.mode != 0 ? p.C / GT_KS : 1;      // slices per convolution tap
             int sidx = 0;
@@ -286,8 +351,18 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
         float acc[ND], racc[ND];
 #pragma unroll
         for (int i = 0; i < ND; ++i) { acc[i] = 0.f; racc[i] = 0.f; }
+        bool live[2] = {true, true};       // table prologue: rows r0 and r0 + 8 read a feature row in this cell
         for (int s = 0; s < nsl; ++s) {
             const int stage = s % S, use = s / S;
+            int ch0 = 0;                   // table prologue: first input channel of this slice
+            if (TABLE && p.pre_scale) {
+                const int ci = s / spc, j = s - ci * spc;
+                ch0 = j * GT_KS;
+                if (j == 0) {
+                    live[0] = table_row(p, row0 + r0, act[ci]) != nullptr;
+                    live[1] = table_row(p, row0 + r0 + 8, act[ci]) != nullptr;
+                }
+            }
             tc::mbar_wait(&full_bar[stage], use & 1);
             // A fragments of this thread (m16n8k8 TF32: (r0, t), (r0+8, t), (r0, t+4), (r0+8, t+4) per k-step),
             // read from the swizzled tile: the 32 lanes of a warp hit 32 different banks
@@ -298,8 +373,15 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
                     const int r = r0 + (e & 1) * 8, k = ks * 8 + t + (e >> 1) * 4;
-                    const uint32_t x = *reinterpret_cast<const uint32_t*>(
+                    uint32_t x = *reinterpret_cast<const uint32_t*>(
                         a_tile + r * 128 + (((k >> 2) ^ (r & 7)) << 4) + (k & 3) * 4);
+                    if (TABLE && p.pre_scale) {
+                        const int ch = ch0 + k;
+                        x = __float_as_uint(live[e & 1] && ch < p.src[0].channels
+                                                ? fmaxf(fmaf(__uint_as_float(x), __ldg(p.pre_scale + ch),
+                                                             __ldg(p.pre_shift + ch)), 0.f)
+                                                : 0.f);
+                    }
                     tc::split_tf32(x, ah[ks][e], al[ks][e]);
                 }
             const uint32_t bh = stage0 + (uint32_t)stage * C::STAGE + GT_A_BYTES, bl = bh + C::B_BYTES;
@@ -441,11 +523,11 @@ static int make_map(CUtensorMap* map, const void* base, int rank, const uint64_t
     return O3DML_OK;
 }
 
-template <int BN, bool GATHER, bool LITE = false>
+template <int BN, bool GATHER, bool LITE = false, bool TABLE = false>
 static int gemm_tc_launch_bn(const GemmTcParams& p, unsigned grid_x, cudaStream_t st) {
     using C = GtCfg<BN, LITE>;
     dim3 grid(grid_x, (unsigned)(p.Npad / BN));
-    O3DML_CUDA(launch<gemm_tc_kernel<BN, GATHER, LITE>>(grid, gt_threads<GATHER>(), C::SMEM, st, p));
+    O3DML_CUDA(launch<gemm_tc_kernel<BN, GATHER, LITE, TABLE>>(grid, gt_threads<GATHER>(), C::SMEM, st, p));
     return O3DML_OK;
 }
 
@@ -460,7 +542,7 @@ static int gemm_tc_launch(GemmTcParams& p, const void* wimg, int k_pad, int n_pa
     O3DML_CHECK(p.Npad == 32 || p.Npad == 64 || p.Npad % 128 == 0,
                 "linear_tc: weight image rows must be padded to 32, 64 or a multiple of 128");
     int bn = p.Npad == 32 ? 32 : (p.Npad == 64 ? 64 : 128);
-    bool any_gather = false;
+    bool any_gather = p.mode == 3;
     if (p.mode == 0)
         for (int s = 0; s < p.nsrc; ++s) any_gather = any_gather || p.src[s].index != nullptr;
     const int sms = device_sm_count();
@@ -489,7 +571,12 @@ static int gemm_tc_launch(GemmTcParams& p, const void* wimg, int k_pad, int n_pa
     }
     bool gather = false;
     unsigned grid_x;
-    if (p.mode == 0) {
+    if (p.mode == 3) {
+        grid_x = (unsigned)ceil_div<int64_t>(p.N, GT_ROWS);
+        if (bn == 32) return gemm_tc_launch_bn<32, true, false, true>(p, grid_x, st);
+        if (bn == 64) return gemm_tc_launch_bn<64, true, false, true>(p, grid_x, st);
+        return gemm_tc_launch_bn<128, true, false, true>(p, grid_x, st);
+    } else if (p.mode == 0) {
         grid_x = (unsigned)ceil_div<int64_t>(p.N, GT_ROWS);
         for (int s = 0; s < p.nsrc; ++s) {
             if (p.src[s].index) { gather = true; continue; }
@@ -629,6 +716,42 @@ extern "C" int o3dml_conv3x3x3_ndhwc_tc(const float* in, int batch, int X, int Y
     int rc = set_conv3x3x3("conv3x3x3_tc", p, in, batch, X, Y, Z, C, GT_KS, GT_ROWS);
     if (!rc) rc = set_epilogue("conv3x3x3_tc", p, weight_image, scale, shift, nullptr, 0, act, slope, out, out_channels,
                                out_channels, 0);
+    if (rc) return rc;
+    return gemm_tc_launch(p, weight_image, k_pad, n_pad, (cudaStream_t)stream);
+}
+
+extern "C" int o3dml_sparse_conv_tc(int64_t num_out, const float* features, int64_t num_in, int channels,
+                                    int features_ld, const int32_t* table, int cells, int table_ld,
+                                    const float* pre_scale, const float* pre_shift, const void* weight_image,
+                                    int k_pad, int n_pad, const float* scale, const float* shift,
+                                    const float* residual, int residual_ld, int act, float slope, float* out,
+                                    int out_ld, int out_channels, void* stream) {
+    GemmTcParams p = {};
+    O3DML_CHECK(num_out >= 0 && num_in >= 0 && num_in < ((int64_t)1 << 31), "sparse_conv_tc: bad sizes");
+    O3DML_CHECK(cells >= 1 && cells <= GT_TABLE_MAX_CELLS, "sparse_conv_tc: 1..%d kernel cells", GT_TABLE_MAX_CELLS);
+    if (num_out == 0) return O3DML_OK;
+    O3DML_CHECK(features && table && table_ld >= cells, "sparse_conv_tc: null features / table or table_ld < cells");
+    O3DML_CHECK(channels > 0 && features_ld >= channels && (features_ld & 3) == 0 &&
+                    (reinterpret_cast<uintptr_t>(features) & 15) == 0,
+                "sparse_conv_tc: feature rows need a stride that is a multiple of 4 floats and 16-byte alignment");
+    O3DML_CHECK((pre_scale == nullptr) == (pre_shift == nullptr), "sparse_conv_tc: pre_scale and pre_shift go together");
+    p.mode = 3;
+    p.N = num_out;
+    p.nsrc = 1;
+    p.cells = cells;
+    p.C = (channels + GT_KS - 1) / GT_KS * GT_KS;
+    p.K = cells * p.C;
+    O3DML_CHECK(k_pad == p.K, "sparse_conv_tc: the weight image must have cells * pad32(channels) = %d rows", p.K);
+    p.src[0].data = features;
+    p.src[0].index = table;
+    p.src[0].rows = num_in;
+    p.src[0].channels = channels;
+    p.src[0].ld = features_ld;
+    p.src[0].index_ld = table_ld;
+    p.pre_scale = pre_scale;
+    p.pre_shift = pre_shift;
+    int rc = set_epilogue("sparse_conv_tc", p, weight_image, scale, shift, residual, residual_ld, act, slope, out, out_ld,
+                          out_channels, 0);
     if (rc) return rc;
     return gemm_tc_launch(p, weight_image, k_pad, n_pad, (cudaStream_t)stream);
 }

@@ -4,8 +4,8 @@ SparseConvUnet).  Same constructor arguments and parameter names (``kernel`` [kx
 the upstream layers, so reference checkpoints load; inference only (no autograd through the CUDA path).
 
 forward = one neighbour-table kernel (o3dml_sparse_conv_neighbors: radix sort of the input voxels + one binary
-search per (output, kernel cell)) followed by the gathered tensor-core GEMM with up to three kernel cells per
-launch as index operands -- the [M, 27 * Cin] im2col tensor never exists.
+search per (output, kernel cell)) followed by one table-mode tensor-core launch over all kernel cells
+(o3dml_sparse_conv_tc) -- the [M, 27 * Cin] im2col tensor never exists.
 """
 import numpy as np
 import torch
@@ -33,21 +33,41 @@ def sparse_conv_neighbors(inp_positions, out_positions, voxel_size, offset, kern
     return nbr, cnt
 
 
-def pack_cell_groups(w):
-    """Kernel weights [cells, Cin, Cout] -> [(first cell, end cell, PackedWeight [cells * Cin, Cout])]: the cells
-    grouped three at a time, one gathered GEMM each."""
-    kc, cout = w.shape[0], w.shape[2]
-    return [(a, min(a + 3, kc),L.pack_linear(w[a:a + 3].reshape(-1, cout))) for a in range(0, kc, 3)]
+def pack_cells(w):
+    """Kernel weights [cells, Cin, Cout] -> the PackedWeight of [cells * Cp, Cout], Cp = Cin rounded up to 32 (rows
+    past Cin zero): the weight operand of contract_cells."""
+    kc, cin, cout = w.shape
+    cp = (cin + 31) // 32 * 32
+    wp = torch.zeros((kc, cp, cout), dtype=torch.float32)
+    wp[:, :cin] = w.detach().float().cpu()
+    return L.pack_linear(wp.reshape(kc * cp, cout))
 
 
-def contract_cells(feat, table, groups, out, bias=None):
-    """out [M, Cout] = sum over the cells c of feat[table[:, c]] @ W_c, + bias: one gathered GEMM per group of
-    pack_cell_groups, the first writing out (with the bias), the others adding onto it through their residual.
-    table int32 [M, cells]; an empty cell holds the shadow id feat.shape[0]."""
-    kc = table.shape[1]
-    for gi, (a, b, pw) in enumerate(groups):
-        srcs = [L.make_src(feat, index=table[:, c:], index_ld=kc) for c in range(a, b)]
-        L.linear(srcs, pw, out, None, None if gi else bias, residual=out if gi else None, act=None)
+def aligned_rows(feat):
+    """feat [N, C] float32 CUDA, or a copy whose row stride is a multiple of 4 floats (what contract_cells reads)."""
+    if feat.stride(1) == 1 and feat.stride(0) % 4 == 0 and feat.data_ptr() % 16 == 0:
+        return feat
+    n, c = feat.shape
+    out = torch.zeros((n, (c + 3) // 4 * 4), dtype=torch.float32, device=feat.device)
+    out[:, :c] = feat
+    return out[:, :c]
+
+
+def contract_cells(feat, table, weight, out, shift=None, pre=None, scale=None, residual=None, act=None):
+    """out [M, Cout] = act(scale * sum over the cells c of W_c^T pre(feat[table[:, c]]) + shift + residual): one
+    tensor-core launch (o3dml_sparse_conv_tc).  table int32 [M, cells] (row stride >= cells); an id outside
+    [0, N) -- the shadow id N of sparse_conv_neighbors -- reads as a zero row.  weight: pack_cells of [cells, Cin,
+    Cout].  pre: None or (scale, shift) [Cin], pre(x) = relu(scale * x + shift), zero rows staying zero.  feat rows
+    need a stride that is a multiple of 4 floats (aligned_rows)."""
+    m, kc = table.shape
+    assert table.dtype == torch.int32 and table.stride(1) == 1
+    ps, pt = pre if pre is not None else (None, None)
+    L.check(L.lib().o3dml_sparse_conv_tc(
+        m, L.ptr(feat), feat.shape[0], feat.shape[1], feat.stride(0), L.ptr(table), kc, table.stride(0), L.ptr(ps),
+        L.ptr(pt), L.ptr(weight.img), weight.k_pad, weight.n_pad, L.ptr(scale), L.ptr(shift), L.ptr(residual),
+        residual.stride(0) if residual is not None else 0, L.act_code(act), 0.0, L.ptr(out), out.stride(0),
+        out.shape[1], L.stream()))
+    return out
 
 
 def _kernel_and_bias(layer, kernel_initializer, bias_initializer):
@@ -88,11 +108,11 @@ class _SparseConvBase(torch.nn.Module):
         self._packed = None
 
     def _weights(self, dev):
-        """pack_cell_groups of the kernel, cached per version."""
+        """pack_cells of the kernel, cached per version."""
         key = (self.kernel._version, self.kernel.data_ptr(), str(dev))
         if self._packed is None or self._packed[0] != key:
             w = self.kernel.detach().reshape(-1, self.in_channels, self.filters).float().cpu()
-            self._packed = (key, pack_cell_groups(w))
+            self._packed = (key, pack_cells(w))
         return self._packed[1]
 
     def forward(self, inp_features, inp_positions, out_positions, voxel_size, inp_importance=None, **kwargs):
@@ -111,7 +131,7 @@ class _SparseConvBase(torch.nn.Module):
         fused_bias = bool(m and n and self.use_bias and not self.normalize)     # added by the GEMM's epilogue
         if m and n:
             bias = self.bias.detach().to(feat.device, torch.float32) if fused_bias else None
-            contract_cells(feat, nbr, self._weights(feat.device), out, bias)
+            contract_cells(aligned_rows(feat), nbr, self._weights(feat.device), out, bias)
         if self.normalize:
             out = out / cnt.clamp_min(1).to(torch.float32).unsqueeze(1)
         return ops._back(_bias_activation(self, out, bias=not fused_bias), inp_features.device)

@@ -693,7 +693,8 @@ def sparse_conv(filters, inp_features, inp_importance, neighbors_index, neighbor
                 neighbors_row_splits, normalize=False, max_temp_mem_MB=64):
     """open3d.ml.torch.ops.sparse_conv (raw op): out[o] = sum_j filters[kernel_index[j]]^T f[neighbors_index[j]] over
     the ragged rows of `neighbors_row_splits`; filters [.., Cin, Cout] with the leading dims flattened into the kernel
-    index.  Runs as gathered tensor-core GEMMs over a dense [num_out, kernel_cells] table (one neighbour per cell)."""
+    index.  Runs as one table-mode tensor-core launch over a dense [num_out, kernel_cells] table (one neighbour per
+    cell)."""
     if (inp_importance is not None and inp_importance.numel()) or \
             (neighbors_importance is not None and neighbors_importance.numel()):
         raise RuntimeError("sparse_conv: importance is not implemented")
@@ -701,7 +702,7 @@ def sparse_conv(filters, inp_features, inp_importance, neighbors_index, neighbor
     cin, cout = w.shape[-2], w.shape[-1]
     w = w.reshape(-1, cin, cout)
     kc = w.shape[0]
-    feat = _dev(inp_features).to(torch.float32).contiguous()
+    feat = layers.aligned_rows(_dev(inp_features).to(torch.float32).contiguous())
     rs = _dev(neighbors_row_splits).to(torch.int64)
     m = rs.numel() - 1
     lens = rs[1:] - rs[:-1]
@@ -709,7 +710,7 @@ def sparse_conv(filters, inp_features, inp_importance, neighbors_index, neighbor
     table = torch.full((m, kc), feat.shape[0], dtype=torch.int32, device=feat.device)
     table[rows, _dev(neighbors_kernel_index).long()] = _dev(neighbors_index).to(torch.int32)
     out = torch.zeros((m, cout), dtype=torch.float32, device=feat.device)
-    layers.contract_cells(feat, table, layers.pack_cell_groups(w), out)
+    layers.contract_cells(feat, table, layers.pack_cells(w), out)
     if normalize:
         out = out / lens.clamp_min(1).to(torch.float32).unsqueeze(1)
     return _back(out, inp_features.device)

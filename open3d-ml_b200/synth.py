@@ -128,6 +128,17 @@ def pvcnn_s3dis_input(n, seed):
     return pts.astype(np.float32), feat.astype(np.float32)
 
 
+def sparseconvunet_scannet_input(n, seed, voxel_size=0.02, grid_size=4096):
+    """SparseConvUnet's test-split input by the arithmetic of SparseConvUnet.preprocess (sparseconvnet.py:106-145) on a
+    room_cloud sampled at 1 cm: xyz over voxel_size, shifted to a random place inside the grid and moved to the voxel
+    centre k + 0.5; colour in [0, 1].  -> (point [n, 3], feat [n, 3]) float32 rows."""
+    pts, f = room_cloud(n, seed, dl=0.01)
+    rng = np.random.default_rng(seed + 1)
+    p = pts / np.float32(voxel_size)
+    p = p - p.min(0) + np.clip(grid_size - (p.max(0) - p.min(0)) - 0.001, 0, None) * rng.random(3)
+    return (p.astype(np.int32) + 0.5).astype(np.float32), f[:, 1:4].copy()
+
+
 def grid_subsample(points, dl):
     """Barycentre grid subsampling (stand-in for `open3d.ml.contrib.subsample`,
     kpconv.py:2037-2164; a "next" row of SURVEY.md 8f).  Deterministic."""
