@@ -3,9 +3,9 @@
 SparseConvUnet).  Same constructor arguments and parameter names (``kernel`` [kx, ky, kz, Cin, Cout], ``bias``) as
 the upstream layers, so reference checkpoints load; inference only (no autograd through the CUDA path).
 
-forward = one neighbour-table kernel (o3dml_sparse_conv_neighbors: radix sort of the input voxels + one binary
-search per (output, kernel cell)) followed by one table-mode tensor-core launch over all kernel cells
-(o3dml_sparse_conv_tc) -- the [M, 27 * Cin] im2col tensor never exists.
+forward = one neighbour-table kernel (o3dml_sparse_conv_neighbors: radix sort of the input voxels + a binary
+search per (output, kernel cell) and input voxel that the cell can reach) followed by one table-mode tensor-core
+launch over all kernel cells (o3dml_sparse_conv_tc) -- the [M, 27 * Cin] im2col tensor never exists.
 """
 import numpy as np
 import torch

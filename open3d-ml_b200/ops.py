@@ -693,8 +693,10 @@ def sparse_conv(filters, inp_features, inp_importance, neighbors_index, neighbor
                 neighbors_row_splits, normalize=False, max_temp_mem_MB=64):
     """open3d.ml.torch.ops.sparse_conv (raw op): out[o] = sum_j filters[kernel_index[j]]^T f[neighbors_index[j]] over
     the ragged rows of `neighbors_row_splits`; filters [.., Cin, Cout] with the leading dims flattened into the kernel
-    index.  Runs as one table-mode tensor-core launch over a dense [num_out, kernel_cells] table (one neighbour per
-    cell)."""
+    index.  A row may name one kernel cell several times (a radius search over points that are not voxel-unique):
+    entry j goes to column rank_j * cells + kernel_index[j] of a dense [num_out, R * cells] table, rank_j counting the
+    earlier entries of its (row, cell), R the largest such count, against the filters repeated R times.  One
+    table-mode tensor-core launch; one host read (R)."""
     if (inp_importance is not None and inp_importance.numel()) or \
             (neighbors_importance is not None and neighbors_importance.numel()):
         raise RuntimeError("sparse_conv: importance is not implemented")
@@ -703,14 +705,27 @@ def sparse_conv(filters, inp_features, inp_importance, neighbors_index, neighbor
     w = w.reshape(-1, cin, cout)
     kc = w.shape[0]
     feat = layers.aligned_rows(_dev(inp_features).to(torch.float32).contiguous())
+    dev = feat.device
     rs = _dev(neighbors_row_splits).to(torch.int64)
     m = rs.numel() - 1
     lens = rs[1:] - rs[:-1]
-    rows = torch.repeat_interleave(torch.arange(m, device=feat.device), lens)
-    table = torch.full((m, kc), feat.shape[0], dtype=torch.int32, device=feat.device)
-    table[rows, _dev(neighbors_kernel_index).long()] = _dev(neighbors_index).to(torch.int32)
-    out = torch.zeros((m, cout), dtype=torch.float32, device=feat.device)
-    layers.contract_cells(feat, table, layers.pack_cells(w), out)
+    idx = _dev(neighbors_index).reshape(-1)
+    e = idx.numel()
+    pos = torch.arange(e, device=dev)
+    rows = torch.searchsorted(rs[1:], pos, right=True)
+    group = rows * kc + _dev(neighbors_kernel_index).reshape(-1).long()
+    order = torch.argsort(group, stable=True)
+    g = group[order]
+    first = torch.ones(e, dtype=torch.bool, device=dev)
+    first[1:] = g[1:] != g[:-1]
+    start = torch.cummax(torch.where(first, pos, 0), 0).values
+    rank = torch.empty_like(pos)
+    rank[order] = pos - start
+    reps = int(rank.max()) + 1 if e else 1                                   # the one host read
+    table = torch.full((m, reps * kc), feat.shape[0], dtype=torch.int32, device=dev)
+    table[rows, rank * kc + group - rows * kc] = idx.to(torch.int32)
+    out = torch.zeros((m, cout), dtype=torch.float32, device=dev)
+    layers.contract_cells(feat, table, layers.pack_cells(w.repeat(reps, 1, 1)), out)
     if normalize:
         out = out / lens.clamp_min(1).to(torch.float32).unsqueeze(1)
     return _back(out, inp_features.device)

@@ -121,3 +121,72 @@ def test_matches_recorded_reference_class(tag):
         got = SparseConvUnetB200(sd, cfg)(batch)
     assert tuple(got.shape) == tuple(want.shape)
     assert SS.rel_err(got, want) < 1e-4
+
+
+def grid_edge_items():
+    """Items whose voxels touch 0 and grid_size - 1 on every axis; along x, item b's last cell and item b + 1's first
+    sit on the faces that meet across ITEM_SPACING."""
+    rng = np.random.default_rng(5)
+    g = CFG["grid_size"]
+    items = []
+    for i in range(3):
+        corners = np.array([[x, y, z] for x in (0, 1, g - 2, g - 1) for y in (0, g - 1) for z in (0, 1, g - 1)])
+        inner = rng.integers(0, 6, (300, 3)) + rng.choice([0, g - 6], (300, 3))
+        k = np.concatenate([corners, inner])
+        pts = (k + rng.random(k.shape) * 0.999).astype(np.float32)
+        items.append((pts, rng.random((len(pts), 3)).astype(np.float32)))
+    return items
+
+
+def test_tables_at_grid_edges_match_the_lattice_rules():
+    """tables(): the 3^3 tables against np_sub_table and the up / down links against np_parent_cell, per item, on every
+    level, for items at the edges of the grid."""
+    import torch
+    from open3d_ml_b200.sparseconvunet import ITEM_SPACING, LEVELS, SparseConvUnetB200
+    from oracle import sparseconvunet as SP
+    cfg = dict(CFG, multiplier=16)
+    net = SparseConvUnetB200(SP.seeded_state_dict(cfg, 0), cfg)
+    items = grid_edge_items()
+    pts = torch.cat([torch.from_numpy(p) for p, _ in items]).cuda()
+    splits = torch.tensor([0] + list(np.cumsum([len(p) for p, _ in items]))).cuda()
+    with torch.no_grad():
+        lv, sizes, outside = net.pyramid(pts, splits)
+        sub, down, up = net.tables(lv, sizes)
+    assert outside == 0
+    for l in range(LEVELS):
+        k = lv[l][0][:sizes[l]].long().cpu().numpy()
+        bid = lv[l][4][:sizes[l]].long().cpu().numpy()
+        shifted = k + np.stack([bid * ITEM_SPACING, 0 * bid, 0 * bid], 1)
+        assert np.array_equal(sub[l].cpu().numpy(), SP.np_sub_table(shifted)), l
+        if l == 0:
+            continue
+        kf = lv[l - 1][0][:sizes[l - 1]].long().cpu().numpy()
+        bf = lv[l - 1][4][:sizes[l - 1]].long().cpu().numpy()
+        u = up[l].long().cpu().numpy()
+        parent, cell = u // 8, u % 8
+        _, _, want_cell = SP.np_parent_cell(kf)
+        assert np.array_equal(cell, want_cell)
+        assert np.array_equal(k[parent], kf // 2) and np.array_equal(bid[parent], bf)
+        d = down[l].cpu().numpy()
+        assert np.array_equal(d[parent, cell], np.arange(len(kf)))
+        assert (d < len(kf)).sum() == len(kf)
+    assert sizes[-1] >= 2 * len(items)          # the corners stay apart up to the coarsest level
+
+
+def test_grid_edges_and_the_largest_batch_against_float64():
+    from open3d_ml_b200.sparseconvunet import ITEM_SPACING, MAX_KEY
+    cfg = dict(CFG, multiplier=16)
+    assert run_both(cfg, grid_edge_items()) < 1e-4
+    most = (MAX_KEY - cfg["grid_size"]) // ITEM_SPACING + 1
+    assert most == 255
+    rng = np.random.default_rng(6)
+    one = [(rng.integers(0, cfg["grid_size"], (1, 3)).astype(np.float32) + 0.5, rng.random((1, 3)).astype(np.float32))
+           for _ in range(most)]
+    one[0] = (np.zeros((1, 3), np.float32), one[0][1])
+    one[-1] = (np.full((1, 3), cfg["grid_size"] - 0.5, np.float32), one[-1][1])
+    assert run_both(cfg, one) < 1e-4
+    from open3d_ml_b200.sparseconvunet import SparseConvUnetB200
+    from oracle import sparseconvunet as SP
+    with pytest.raises(RuntimeError, match="items per batch"):
+        with torch.no_grad():
+            SparseConvUnetB200(SP.seeded_state_dict(cfg, 0), cfg)(batch_of(one + one[:1]))

@@ -220,6 +220,29 @@ def test_sparse_conv_oracle_equals_dense_conv3d_on_a_full_lattice():
     assert np.abs(up - ref).max() < 1e-4
 
 
+@pytest.mark.parametrize("v,fi,fo,transpose", [(1.0, 0.9, 0.1, False), (0.3, 0.0, 0.0, True), (0.05, 0.1, 0.8, False)])
+def test_brute_force_table_contracts_to_the_sparse_conv_oracle(v, fi, fo, transpose):
+    """The float32 brute-force table of the GPU table tests (tests/sparse_tables_support.py), contracted in float64,
+    equals c_sparse_conv on voxel-unique inputs off the grid and at voxel corners, with bias and normalize."""
+    from sparse_tables_support import brute_table, contract64
+    rng = np.random.default_rng(3)
+    inp = ((np.unique(rng.integers(0, 12, (900, 3)), axis=0) + 5000 + fi) * np.float32(v)).astype(np.float32)
+    out = ((np.unique(rng.integers(0, 12, (400, 3)), axis=0) + 5000 + fo) * np.float32(v)).astype(np.float32)
+    cin, cout = 5, 7
+    feat = rng.standard_normal((len(inp), cin)).astype(np.float32)
+    for ks, off in (((3, 3, 3), [0.0, 0.25, -0.25]), ((2, 3, 4), [-0.5, 0.0, -0.5])):
+        kernel = rng.standard_normal(ks + (cin, cout)).astype(np.float32)
+        bias = rng.standard_normal(cout).astype(np.float32)
+        table, cnt = brute_table(inp, out, v, off, ks, transpose)
+        assert (table < len(inp)).sum() > 1000
+        for normalize in (False, True):
+            want = O.c_sparse_conv(feat, inp, out, v, off, kernel, bias, normalize, transpose)
+            got = contract64(feat, table, kernel)
+            if normalize:
+                got = got / np.maximum(cnt, 1)[:, None]
+            assert np.abs(got + bias - want).max() < 1e-5 * np.abs(want).max()
+
+
 def test_continuous_conv_oracle_known_answers():
     """A spatially constant filter makes the convolution a plain sum: out = (sum_n imp_n f_n) W; nearest-neighbour
     interpolation with the identity mapping on lattice offsets reproduces the sparse 3x3x3 convolution."""
