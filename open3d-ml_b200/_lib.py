@@ -94,6 +94,12 @@ _SPARSECONVUNET_SIGNATURES = {
     "o3dml_sparse_conv_tc": (I, [L, P, L, I, I, P, I, I, P, P, P, I, I, P, P, P, I, I, F, P, I, I, P]),
 }
 SPARSECONVUNET_EXPORTS = tuple(_SPARSECONVUNET_SIGNATURES)
+# the weighted sparse-convolution contraction of the product ABI: exactly what include/o3dml_b200_sparse_weighted.h
+# declares
+_SPARSE_WEIGHTED_SIGNATURES = {
+    "o3dml_sparse_conv_weighted_tc": (I, [L, P, L, I, I, P, I, I, P, P, P, I, I, P, P, P, I, I, F, P, I, I, P, I, P]),
+}
+SPARSE_WEIGHTED_EXPORTS = tuple(_SPARSE_WEIGHTED_SIGNATURES)
 # bring-up / profiling hooks (include/o3dml_b200_bringup.h): exported by the library, not part of the product ABI
 _BRINGUP_SIGNATURES = {
     "o3dml_tc_gemm_test": (I, [P, P, P, I, I, I, P]),
@@ -120,7 +126,8 @@ def lib():
                 raise
         h = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in (list(_SIGNATURES.items()) + list(_PVCNN_SIGNATURES.items()) +
-                                  list(_SPARSECONVUNET_SIGNATURES.items()) + list(_BRINGUP_SIGNATURES.items())):
+                                  list(_SPARSECONVUNET_SIGNATURES.items()) +
+                                  list(_SPARSE_WEIGHTED_SIGNATURES.items()) + list(_BRINGUP_SIGNATURES.items())):
             fn = getattr(h, name)
             fn.restype, fn.argtypes = res, args
         if h.o3dml_abi_version() != ABI_VERSION:

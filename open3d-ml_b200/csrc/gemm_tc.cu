@@ -28,13 +28,16 @@
 // Cin padded to 32.  The loaders gather each 32-channel slice of a cell from the row the table names (a shadow id
 // reads zeros); the (tile, cell) pairs whose 128 rows are all shadow are skipped.  The optional prologue act(x) =
 // relu(pre_scale * x + pre_shift) is applied by the consumers in registers before the split, and keeps shadow rows at
-// zero: an empty cell contributes nothing, not act(0).
+// zero: an empty cell contributes nothing, not act(0).  The weighted instances (o3dml_sparse_conv_weighted_tc) also
+// scale every entry by a float table parallel to the neighbour table, x' = w[m, c] * act(x), read once per (row, cell)
+// where the consumers test the entry for a shadow id; a shadow entry stays zero whatever its weight.
 //
 // Every GT_FLUSH slices the wgmma accumulator is folded into a second fp32 register set with
 // round-to-nearest adds, so that long products do not rely on the tensor core's internal accumulation.
 #include "../../include/o3dml_b200.h"
 #include "../../include/o3dml_b200_pvcnn.h"
 #include "../../include/o3dml_b200_sparseconvunet.h"
+#include "../../include/o3dml_b200_sparse_weighted.h"
 #include "dense.cuh"
 #include "tc.cuh"
 #include <cuda.h>
@@ -67,6 +70,8 @@ struct alignas(64) GemmTcParams {
     int cells;                              // table mode: src[0] = features + table (index, index_ld), C = Cin padded to 32
     const float* pre_scale;                 // table mode prologue (both or neither)
     const float* pre_shift;
+    const float* entry_weight;              // table mode, weighted instances: float [N, weight_ld], parallel to the table
+    int weight_ld;
 };
 
 // ---- async-copy primitives ---------------------------------------------------------------------
@@ -121,6 +126,11 @@ __device__ __forceinline__ const float* table_row(const GemmTcParams& p, int64_t
     return (r < 0 || r >= S.rows) ? nullptr : S.data + (size_t)r * S.ld;
 }
 
+// weighted table mode: the weight of the entry that row n reads in kernel cell `cell` (0 past the last row)
+__device__ __forceinline__ float table_weight(const GemmTcParams& p, int64_t n, int cell) {
+    return n < p.N ? __ldg(p.entry_weight + n * p.weight_ld + cell) : 0.f;
+}
+
 // LITE: two stages instead of 4 - 6, so that TWO CTAs share an SM.  A short product (K <= 512) is mostly
 // prologue and epilogue around a few 32-channel slices: with one CTA per SM the tensor pipe and the TMA unit
 // idle through both; a sibling CTA fills them.
@@ -151,9 +161,10 @@ constexpr int GT_PRODUCER_WARP = 8;
 template <bool GATHER>
 __host__ __device__ constexpr int gt_threads() { return GT_CONV_THREADS + (GATHER ? GT_LOADERS : 32); }
 
-template <int BN, bool GATHER, bool LITE, bool TABLE = false>
+template <int BN, bool GATHER, bool LITE, bool TABLE = false, bool WEIGHTED = false>
 __global__ void __launch_bounds__(gt_threads<GATHER>(), LITE ? 2 : 1)
 gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
+    static_assert(TABLE || !WEIGHTED, "entry weights belong to table mode");
     using C = GtCfg<BN, LITE>;
     constexpr int S = C::STAGES;
     extern __shared__ uint8_t smem_raw[];
@@ -352,15 +363,20 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
 #pragma unroll
         for (int i = 0; i < ND; ++i) { acc[i] = 0.f; racc[i] = 0.f; }
         bool live[2] = {true, true};       // table prologue: rows r0 and r0 + 8 read a feature row in this cell
+        float wt[2] = {1.f, 1.f};          // weighted table mode: the entry weights of rows r0 and r0 + 8 in this cell
         for (int s = 0; s < nsl; ++s) {
             const int stage = s % S, use = s / S;
             int ch0 = 0;                   // table prologue: first input channel of this slice
-            if (TABLE && p.pre_scale) {
+            if (TABLE && (WEIGHTED || p.pre_scale)) {
                 const int ci = s / spc, j = s - ci * spc;
                 ch0 = j * GT_KS;
                 if (j == 0) {
                     live[0] = table_row(p, row0 + r0, act[ci]) != nullptr;
                     live[1] = table_row(p, row0 + r0 + 8, act[ci]) != nullptr;
+                    if (WEIGHTED) {      // a shadow entry weighs zero
+                        wt[0] = live[0] ? table_weight(p, row0 + r0, act[ci]) : 0.f;
+                        wt[1] = live[1] ? table_weight(p, row0 + r0 + 8, act[ci]) : 0.f;
+                    }
                 }
             }
             tc::mbar_wait(&full_bar[stage], use & 1);
@@ -375,7 +391,15 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
                     const int r = r0 + (e & 1) * 8, k = ks * 8 + t + (e >> 1) * 4;
                     uint32_t x = *reinterpret_cast<const uint32_t*>(
                         a_tile + r * 128 + (((k >> 2) ^ (r & 7)) << 4) + (k & 3) * 4);
-                    if (TABLE && p.pre_scale) {
+                    if (WEIGHTED) {
+                        const int ch = ch0 + k;
+                        const float v = __uint_as_float(x);
+                        x = __float_as_uint(ch < p.src[0].channels
+                                                ? wt[e & 1] * (p.pre_scale ? fmaxf(fmaf(v, __ldg(p.pre_scale + ch),
+                                                                                        __ldg(p.pre_shift + ch)), 0.f)
+                                                                           : v)
+                                                : 0.f);
+                    } else if (TABLE && p.pre_scale) {
                         const int ch = ch0 + k;
                         x = __float_as_uint(live[e & 1] && ch < p.src[0].channels
                                                 ? fmaxf(fmaf(__uint_as_float(x), __ldg(p.pre_scale + ch),
@@ -523,12 +547,19 @@ static int make_map(CUtensorMap* map, const void* base, int rank, const uint64_t
     return O3DML_OK;
 }
 
-template <int BN, bool GATHER, bool LITE = false, bool TABLE = false>
+template <int BN, bool GATHER, bool LITE = false, bool TABLE = false, bool WEIGHTED = false>
 static int gemm_tc_launch_bn(const GemmTcParams& p, unsigned grid_x, cudaStream_t st) {
     using C = GtCfg<BN, LITE>;
     dim3 grid(grid_x, (unsigned)(p.Npad / BN));
-    O3DML_CUDA(launch<gemm_tc_kernel<BN, GATHER, LITE, TABLE>>(grid, gt_threads<GATHER>(), C::SMEM, st, p));
+    O3DML_CUDA(launch<gemm_tc_kernel<BN, GATHER, LITE, TABLE, WEIGHTED>>(grid, gt_threads<GATHER>(), C::SMEM, st, p));
     return O3DML_OK;
+}
+
+template <bool WEIGHTED>
+static int gemm_tc_launch_table(const GemmTcParams& p, int bn, unsigned grid_x, cudaStream_t st) {
+    if (bn == 32) return gemm_tc_launch_bn<32, true, false, true, WEIGHTED>(p, grid_x, st);
+    if (bn == 64) return gemm_tc_launch_bn<64, true, false, true, WEIGHTED>(p, grid_x, st);
+    return gemm_tc_launch_bn<128, true, false, true, WEIGHTED>(p, grid_x, st);
 }
 
 constexpr int GT_LITE_MAX_SLICES = 16;   // longest product, in 32-channel k-slices, that runs on the LITE kernels
@@ -573,9 +604,8 @@ static int gemm_tc_launch(GemmTcParams& p, const void* wimg, int k_pad, int n_pa
     unsigned grid_x;
     if (p.mode == 3) {
         grid_x = (unsigned)ceil_div<int64_t>(p.N, GT_ROWS);
-        if (bn == 32) return gemm_tc_launch_bn<32, true, false, true>(p, grid_x, st);
-        if (bn == 64) return gemm_tc_launch_bn<64, true, false, true>(p, grid_x, st);
-        return gemm_tc_launch_bn<128, true, false, true>(p, grid_x, st);
+        return p.entry_weight ? gemm_tc_launch_table<true>(p, bn, grid_x, st)
+                              : gemm_tc_launch_table<false>(p, bn, grid_x, st);
     } else if (p.mode == 0) {
         grid_x = (unsigned)ceil_div<int64_t>(p.N, GT_ROWS);
         for (int s = 0; s < p.nsrc; ++s) {
@@ -720,28 +750,28 @@ extern "C" int o3dml_conv3x3x3_ndhwc_tc(const float* in, int batch, int X, int Y
     return gemm_tc_launch(p, weight_image, k_pad, n_pad, (cudaStream_t)stream);
 }
 
-extern "C" int o3dml_sparse_conv_tc(int64_t num_out, const float* features, int64_t num_in, int channels,
-                                    int features_ld, const int32_t* table, int cells, int table_ld,
-                                    const float* pre_scale, const float* pre_shift, const void* weight_image,
-                                    int k_pad, int n_pad, const float* scale, const float* shift,
-                                    const float* residual, int residual_ld, int act, float slope, float* out,
-                                    int out_ld, int out_channels, void* stream) {
-    GemmTcParams p = {};
-    O3DML_CHECK(num_out >= 0 && num_in >= 0 && num_in < ((int64_t)1 << 31), "sparse_conv_tc: bad sizes");
-    O3DML_CHECK(cells >= 1 && cells <= GT_TABLE_MAX_CELLS, "sparse_conv_tc: 1..%d kernel cells", GT_TABLE_MAX_CELLS);
+// The argument checks and table-mode parameters of both sparse-convolution entries.  Returns O3DML_OK with p.N == 0
+// when there is nothing to launch.
+static int set_sparse_table(const char* op, GemmTcParams& p, int64_t num_out, const float* features, int64_t num_in,
+                            int channels, int features_ld, const int32_t* table, int cells, int table_ld,
+                            const float* pre_scale, const float* pre_shift, const void* weight_image, int k_pad,
+                            const float* scale, const float* shift, const float* residual, int residual_ld, int act,
+                            float slope, float* out, int out_ld, int out_channels) {
+    O3DML_CHECK(num_out >= 0 && num_in >= 0 && num_in < ((int64_t)1 << 31), "%s: bad sizes", op);
+    O3DML_CHECK(cells >= 1 && cells <= GT_TABLE_MAX_CELLS, "%s: 1..%d kernel cells", op, GT_TABLE_MAX_CELLS);
     if (num_out == 0) return O3DML_OK;
-    O3DML_CHECK(features && table && table_ld >= cells, "sparse_conv_tc: null features / table or table_ld < cells");
+    O3DML_CHECK(features && table && table_ld >= cells, "%s: null features / table or table_ld < cells", op);
     O3DML_CHECK(channels > 0 && features_ld >= channels && (features_ld & 3) == 0 &&
                     (reinterpret_cast<uintptr_t>(features) & 15) == 0,
-                "sparse_conv_tc: feature rows need a stride that is a multiple of 4 floats and 16-byte alignment");
-    O3DML_CHECK((pre_scale == nullptr) == (pre_shift == nullptr), "sparse_conv_tc: pre_scale and pre_shift go together");
+                "%s: feature rows need a stride that is a multiple of 4 floats and 16-byte alignment", op);
+    O3DML_CHECK((pre_scale == nullptr) == (pre_shift == nullptr), "%s: pre_scale and pre_shift go together", op);
     p.mode = 3;
     p.N = num_out;
     p.nsrc = 1;
     p.cells = cells;
     p.C = (channels + GT_KS - 1) / GT_KS * GT_KS;
     p.K = cells * p.C;
-    O3DML_CHECK(k_pad == p.K, "sparse_conv_tc: the weight image must have cells * pad32(channels) = %d rows", p.K);
+    O3DML_CHECK(k_pad == p.K, "%s: the weight image must have cells * pad32(channels) = %d rows", op, p.K);
     p.src[0].data = features;
     p.src[0].index = table;
     p.src[0].rows = num_in;
@@ -750,8 +780,38 @@ extern "C" int o3dml_sparse_conv_tc(int64_t num_out, const float* features, int6
     p.src[0].index_ld = table_ld;
     p.pre_scale = pre_scale;
     p.pre_shift = pre_shift;
-    int rc = set_epilogue("sparse_conv_tc", p, weight_image, scale, shift, residual, residual_ld, act, slope, out, out_ld,
-                          out_channels, 0);
-    if (rc) return rc;
+    return set_epilogue(op, p, weight_image, scale, shift, residual, residual_ld, act, slope, out, out_ld, out_channels,
+                        0);
+}
+
+extern "C" int o3dml_sparse_conv_tc(int64_t num_out, const float* features, int64_t num_in, int channels,
+                                    int features_ld, const int32_t* table, int cells, int table_ld,
+                                    const float* pre_scale, const float* pre_shift, const void* weight_image,
+                                    int k_pad, int n_pad, const float* scale, const float* shift,
+                                    const float* residual, int residual_ld, int act, float slope, float* out,
+                                    int out_ld, int out_channels, void* stream) {
+    GemmTcParams p = {};
+    const int rc = set_sparse_table("sparse_conv_tc", p, num_out, features, num_in, channels, features_ld, table, cells,
+                                    table_ld, pre_scale, pre_shift, weight_image, k_pad, scale, shift, residual,
+                                    residual_ld, act, slope, out, out_ld, out_channels);
+    if (rc || p.N == 0) return rc;
+    return gemm_tc_launch(p, weight_image, k_pad, n_pad, (cudaStream_t)stream);
+}
+
+extern "C" int o3dml_sparse_conv_weighted_tc(int64_t num_out, const float* features, int64_t num_in, int channels,
+                                             int features_ld, const int32_t* table, int cells, int table_ld,
+                                             const float* pre_scale, const float* pre_shift, const void* weight_image,
+                                             int k_pad, int n_pad, const float* scale, const float* shift,
+                                             const float* residual, int residual_ld, int act, float slope, float* out,
+                                             int out_ld, int out_channels, const float* entry_weight, int weight_ld,
+                                             void* stream) {
+    GemmTcParams p = {};
+    const int rc = set_sparse_table("sparse_conv_weighted_tc", p, num_out, features, num_in, channels, features_ld,
+                                    table, cells, table_ld, pre_scale, pre_shift, weight_image, k_pad, scale, shift,
+                                    residual, residual_ld, act, slope, out, out_ld, out_channels);
+    if (rc || p.N == 0) return rc;
+    O3DML_CHECK(entry_weight && weight_ld >= cells, "sparse_conv_weighted_tc: null entry_weight or weight_ld < cells");
+    p.entry_weight = entry_weight;
+    p.weight_ld = weight_ld;
     return gemm_tc_launch(p, weight_image, k_pad, n_pad, (cudaStream_t)stream);
 }

@@ -53,20 +53,28 @@ def aligned_rows(feat):
     return out[:, :c]
 
 
-def contract_cells(feat, table, weight, out, shift=None, pre=None, scale=None, residual=None, act=None):
-    """out [M, Cout] = act(scale * sum over the cells c of W_c^T pre(feat[table[:, c]]) + shift + residual): one
-    tensor-core launch (o3dml_sparse_conv_tc).  table int32 [M, cells] (row stride >= cells); an id outside
-    [0, N) -- the shadow id N of sparse_conv_neighbors -- reads as a zero row.  weight: pack_cells of [cells, Cin,
-    Cout].  pre: None or (scale, shift) [Cin], pre(x) = relu(scale * x + shift), zero rows staying zero.  feat rows
-    need a stride that is a multiple of 4 floats (aligned_rows)."""
+def contract_cells(feat, table, weight, out, shift=None, pre=None, scale=None, residual=None, act=None,
+                   entry_weight=None):
+    """out [M, Cout] = act(scale * sum over the cells c of W_c^T (w[:, c] * pre(feat[table[:, c]])) + shift +
+    residual): one tensor-core launch.  table int32 [M, cells] (row stride >= cells); an id outside [0, N) -- the
+    shadow id N of sparse_conv_neighbors -- reads as a zero row.  weight: pack_cells of [cells, Cin, Cout].  pre: None
+    or (scale, shift) [Cin], pre(x) = relu(scale * x + shift), zero rows staying zero.  entry_weight: None (all ones:
+    o3dml_sparse_conv_tc) or float32 [M, cells] parallel to the table (row stride >= cells:
+    o3dml_sparse_conv_weighted_tc); a shadow entry stays zero whatever its weight.  feat rows need a stride that is a
+    multiple of 4 floats (aligned_rows)."""
     m, kc = table.shape
     assert table.dtype == torch.int32 and table.stride(1) == 1
     ps, pt = pre if pre is not None else (None, None)
-    L.check(L.lib().o3dml_sparse_conv_tc(
-        m, L.ptr(feat), feat.shape[0], feat.shape[1], feat.stride(0), L.ptr(table), kc, table.stride(0), L.ptr(ps),
-        L.ptr(pt), L.ptr(weight.img), weight.k_pad, weight.n_pad, L.ptr(scale), L.ptr(shift), L.ptr(residual),
-        residual.stride(0) if residual is not None else 0, L.act_code(act), 0.0, L.ptr(out), out.stride(0),
-        out.shape[1], L.stream()))
+    args = (m, L.ptr(feat), feat.shape[0], feat.shape[1], feat.stride(0), L.ptr(table), kc, table.stride(0), L.ptr(ps),
+            L.ptr(pt), L.ptr(weight.img), weight.k_pad, weight.n_pad, L.ptr(scale), L.ptr(shift), L.ptr(residual),
+            residual.stride(0) if residual is not None else 0, L.act_code(act), 0.0, L.ptr(out), out.stride(0),
+            out.shape[1])
+    if entry_weight is None:
+        L.check(L.lib().o3dml_sparse_conv_tc(*args, L.stream()))
+    else:
+        assert (entry_weight.dtype == torch.float32 and tuple(entry_weight.shape) == (m, kc) and
+                entry_weight.stride(1) == 1)
+        L.check(L.lib().o3dml_sparse_conv_weighted_tc(*args, L.ptr(entry_weight), entry_weight.stride(0), L.stream()))
     return out
 
 
@@ -115,15 +123,25 @@ class _SparseConvBase(torch.nn.Module):
             self._packed = (key, pack_cells(w))
         return self._packed[1]
 
-    def forward(self, inp_features, inp_positions, out_positions, voxel_size, inp_importance=None, **kwargs):
-        if inp_importance is not None or kwargs.get("user_neighbors_index") is not None:
-            raise RuntimeError("SparseConv: importance / user neighbours are not implemented")
+    def _forward(self, inp_features, inp_positions, out_positions, voxel_size, importance, kwargs):
+        """importance: the layer's importance argument (inp_importance of SparseConv, out_importance of
+        SparseConvTranspose) or None; it weights the table entries of the one contraction."""
+        other = "out_importance" if not self.TRANSPOSE else "inp_importance"
+        if kwargs.get(other) is not None or kwargs.get("user_neighbors_index") is not None:
+            raise RuntimeError("%s: %s / user neighbours are not implemented" % (type(self).__name__, other))
         if torch.is_grad_enabled() and (inp_features.requires_grad or self.kernel.requires_grad and self.training):
             raise RuntimeError("open3d_ml_b200: SparseConv is inference-only (call under torch.no_grad() / eval())")
         from . import ops
         L.require_cuda()
         feat = inp_features.detach().to("cuda", torch.float32).contiguous()
         n, m = feat.shape[0], out_positions.shape[0]
+        imp = None
+        if importance is not None:
+            imp = importance.detach().to(feat.device, torch.float32).reshape(-1)
+            want = m if self.TRANSPOSE else n
+            if imp.numel() != want:
+                raise RuntimeError("%s: %s must have %d elements" % (
+                    type(self).__name__, "out_importance" if self.TRANSPOSE else "inp_importance", want))
         vs = float(torch.as_tensor(voxel_size).reshape(-1)[0]) if not isinstance(voxel_size, (int, float)) else float(voxel_size)
         nbr, cnt = sparse_conv_neighbors(inp_positions, out_positions, vs, self.offset, self.kernel_size,
                                          self.TRANSPOSE, want_count=self.normalize)
@@ -131,20 +149,33 @@ class _SparseConvBase(torch.nn.Module):
         fused_bias = bool(m and n and self.use_bias and not self.normalize)     # added by the GEMM's epilogue
         if m and n:
             bias = self.bias.detach().to(feat.device, torch.float32) if fused_bias else None
-            contract_cells(aligned_rows(feat), nbr, self._weights(feat.device), out, bias)
+            w = None
+            if imp is not None and self.TRANSPOSE:          # oimp[m] on every cell of row m
+                w = imp.unsqueeze(1).expand(m, nbr.shape[1]).contiguous()
+            elif imp is not None:                           # iimp of the input each entry reads; shadow ids read 0
+                w = torch.cat([imp, imp.new_zeros(1)])[nbr.long()]
+            contract_cells(aligned_rows(feat), nbr, self._weights(feat.device), out, bias, entry_weight=w)
         if self.normalize:
             out = out / cnt.clamp_min(1).to(torch.float32).unsqueeze(1)
         return ops._back(_bias_activation(self, out, bias=not fused_bias), inp_features.device)
 
 
 class SparseConv(_SparseConvBase):
-    """open3d.ml.torch.layers.SparseConv: cell = floor((in - out) / voxel_size + offset + kernel_size / 2)."""
+    """open3d.ml.torch.layers.SparseConv: cell = floor((in - out) / voxel_size + offset + kernel_size / 2).
+    inp_importance [N] (optional) scales each input feature row before the contraction."""
     TRANSPOSE = False
+
+    def forward(self, inp_features, inp_positions, out_positions, voxel_size, inp_importance=None, **kwargs):
+        return self._forward(inp_features, inp_positions, out_positions, voxel_size, inp_importance, kwargs)
 
 
 class SparseConvTranspose(_SparseConvBase):
-    """open3d.ml.torch.layers.SparseConvTranspose: cell = floor((out - in) / voxel_size + offset + kernel_size / 2)."""
+    """open3d.ml.torch.layers.SparseConvTranspose: cell = floor((out - in) / voxel_size + offset + kernel_size / 2).
+    out_importance [M] (optional) scales each output row's sum, before the normalisation, bias and activation."""
     TRANSPOSE = True
+
+    def forward(self, inp_features, inp_positions, out_positions, voxel_size, out_importance=None, **kwargs):
+        return self._forward(inp_features, inp_positions, out_positions, voxel_size, out_importance, kwargs)
 
 
 class ContinuousConv(torch.nn.Module):

@@ -689,31 +689,47 @@ def continuous_conv_transpose(filters, out_positions, out_importance, extents, o
     return _back(out, inp_features.device)
 
 
-def sparse_conv(filters, inp_features, inp_importance, neighbors_index, neighbors_kernel_index, neighbors_importance,
-                neighbors_row_splits, normalize=False, max_temp_mem_MB=64):
-    """open3d.ml.torch.ops.sparse_conv (raw op): out[o] = sum_j filters[kernel_index[j]]^T f[neighbors_index[j]] over
-    the ragged rows of `neighbors_row_splits`; filters [.., Cin, Cout] with the leading dims flattened into the kernel
-    index.  A row may name one kernel cell several times (a radius search over points that are not voxel-unique):
-    entry j goes to column rank_j * cells + kernel_index[j] of a dense [num_out, R * cells] table, rank_j counting the
-    earlier entries of its (row, cell), R the largest such count, against the filters repeated R times.  One
-    table-mode tensor-core launch; one host read (R)."""
-    if (inp_importance is not None and inp_importance.numel()) or \
-            (neighbors_importance is not None and neighbors_importance.numel()):
-        raise RuntimeError("sparse_conv: importance is not implemented")
+def _sparse_filters(name, filters, feat):
+    """filters [.., Cin, Cout] -> float32 CPU [cells, Cin, Cout], the leading dims flattened into the kernel index."""
     w = filters.detach().float().cpu()
     cin, cout = w.shape[-2], w.shape[-1]
-    w = w.reshape(-1, cin, cout)
-    kc = w.shape[0]
-    feat = layers.aligned_rows(_dev(inp_features).to(torch.float32).contiguous())
-    dev = feat.device
-    rs = _dev(neighbors_row_splits).to(torch.int64)
+    if feat.dim() != 2 or feat.shape[1] != cin:
+        raise RuntimeError("%s: feature channels do not match the filter" % name)
+    return w.reshape(-1, cin, cout)
+
+
+def _sparse_importance(name, what, t, n, dev):
+    """An importance argument: None for an empty tensor (all ones), else float32 [n] on `dev`."""
+    if t is None or t.numel() == 0:
+        return None
+    t = _dev(t).to(dev, torch.float32).reshape(-1)
+    if t.numel() != n:
+        raise RuntimeError("%s: %s must be empty or have %d elements" % (name, what, n))
+    return t
+
+
+def _sparse_table(name, neighbors_index, neighbors_kernel_index, neighbors_row_splits, kc, num_in, dev,
+                  entry_weight=None):
+    """Ragged (index, kernel cell) lists -> the dense table of the contraction: entry e goes to column
+    rank_e * cells + kernel_index[e] of an int32 [num_out, R * cells] table, rank_e counting the earlier entries of its
+    (row, cell), R the largest such count (the filters are repeated R times).  entry_weight: None, or rows -> float
+    [E], the entries' weights, scattered into a parallel float table (zero where the table holds the shadow id num_in).
+    One host read (none without entries), which also returns the smallest and largest kernel index and the end of the
+    row splits: a kernel index outside [0, cells), or splits that do not end at E, raise before anything is scattered
+    or weighed.  -> (table, weight table or None, R, rows of the entries, row lengths)."""
+    rs = _dev(neighbors_row_splits).to(dev, torch.int64).reshape(-1)
+    if rs.numel() < 1:
+        raise RuntimeError("%s: neighbors_row_splits must have num_out + 1 elements" % name)
     m = rs.numel() - 1
     lens = rs[1:] - rs[:-1]
-    idx = _dev(neighbors_index).reshape(-1)
+    idx = _dev(neighbors_index).to(dev).reshape(-1)
+    kidx = _dev(neighbors_kernel_index).to(dev).reshape(-1).long()
     e = idx.numel()
+    if kidx.numel() != e:
+        raise RuntimeError("%s: neighbors_kernel_index must have one entry per neighbour" % name)
     pos = torch.arange(e, device=dev)
     rows = torch.searchsorted(rs[1:], pos, right=True)
-    group = rows * kc + _dev(neighbors_kernel_index).reshape(-1).long()
+    group = rows * kc + kidx
     order = torch.argsort(group, stable=True)
     g = group[order]
     first = torch.ones(e, dtype=torch.bool, device=dev)
@@ -721,11 +737,105 @@ def sparse_conv(filters, inp_features, inp_importance, neighbors_index, neighbor
     start = torch.cummax(torch.where(first, pos, 0), 0).values
     rank = torch.empty_like(pos)
     rank[order] = pos - start
-    reps = int(rank.max()) + 1 if e else 1                                   # the one host read
-    table = torch.full((m, reps * kc), feat.shape[0], dtype=torch.int32, device=dev)
-    table[rows, rank * kc + group - rows * kc] = idx.to(torch.int32)
+    reps = 1
+    if e:
+        top, kmin, kmax, last = (int(v) for v in torch.stack([rank.max(), kidx.min(), kidx.max(), rs[-1]]).cpu())
+        if kmin < 0 or kmax >= kc:
+            raise RuntimeError("%s: neighbors_kernel_index holds %d, outside [0, %d)" % (name, kmin if kmin < 0 else kmax,
+                                                                                      kc))
+        if last != e:
+            raise RuntimeError("%s: neighbors_row_splits ends at %d, not at the %d neighbour entries" % (name, last, e))
+        reps = top + 1
+    col = rank * kc + kidx
+    table = torch.full((m, reps * kc), num_in, dtype=torch.int32, device=dev)
+    table[rows, col] = idx.to(torch.int32)
+    wt = None
+    if entry_weight is not None:
+        wt = torch.zeros((m, reps * kc), dtype=torch.float32, device=dev)
+        wt[rows, col] = entry_weight(rows)
+    return table, wt, reps, rows, lens
+
+
+def sparse_conv(filters, inp_features, inp_importance, neighbors_index, neighbors_kernel_index, neighbors_importance,
+                neighbors_row_splits, normalize=False, max_temp_mem_MB=64):
+    """open3d.ml.torch.ops.sparse_conv (raw op):
+        out[o] = (1 / n_o) sum_e nimp_e * iimp_i * filters[kernel_index[e]]^T f[i],   i = neighbors_index[e],
+    over the ragged rows of `neighbors_row_splits`; filters [.., Cin, Cout] with the leading dims flattened into the
+    kernel index.  Empty importance tensors mean all ones.  Under normalize n_o = sum_e nimp_e * iimp_i (the row length
+    without importances; a zero divisor gives 1), otherwise 1.  A row may name one kernel cell several times (a
+    radius search over points that are not voxel-unique): see _sparse_table.  One table-mode tensor-core launch, the
+    weighted one when an importance is given; one host read (R and the kernel index range)."""
+    name = "sparse_conv"
+    feat = layers.aligned_rows(_dev(inp_features).to(torch.float32).contiguous())
+    w = _sparse_filters(name, filters, feat)
+    kc, cout = w.shape[0], w.shape[2]
+    dev, num_in = feat.device, feat.shape[0]
+    e = neighbors_index.numel()
+    iimp = _sparse_importance(name, "inp_importance", inp_importance, num_in, dev)
+    nimp = _sparse_importance(name, "neighbors_importance", neighbors_importance, e, dev)
+    weighted = iimp is not None or nimp is not None
+
+    def entry_weight(_rows):
+        wt = torch.ones(e, dtype=torch.float32, device=dev) if nimp is None else nimp
+        if iimp is not None:     # an index outside [0, num_in) is a shadow entry: any weight does
+            idx = _dev(neighbors_index).to(dev).reshape(-1).long()
+            wt = wt * torch.cat([iimp, iimp.new_zeros(1)])[torch.where((idx >= 0) & (idx < num_in), idx, num_in)]
+        return wt
+    table, wt, reps, _, lens = _sparse_table(name, neighbors_index, neighbors_kernel_index, neighbors_row_splits,
+                                             kc, num_in, dev, entry_weight if weighted else None)
+    m = lens.numel()
     out = torch.zeros((m, cout), dtype=torch.float32, device=dev)
-    layers.contract_cells(feat, table, layers.pack_cells(w.repeat(reps, 1, 1)), out)
-    if normalize:
+    layers.contract_cells(feat, table, layers.pack_cells(w.repeat(reps, 1, 1)), out, entry_weight=wt)
+    if normalize and not weighted:
         out = out / lens.clamp_min(1).to(torch.float32).unsqueeze(1)
+    elif normalize:
+        n_o = wt.sum(1)                       # the weight table holds every entry's weight once, zeros elsewhere
+        out = out / torch.where(n_o != 0, n_o, torch.ones_like(n_o)).unsqueeze(1)
+    return _back(out, inp_features.device)
+
+
+def sparse_conv_transpose(filters, out_importance, inp_features, inp_neighbors_index, inp_neighbors_importance_sum,
+                          inp_neighbors_row_splits, neighbors_index, neighbors_kernel_index, neighbors_importance,
+                          neighbors_row_splits, normalize=False, max_temp_mem_MB=64):
+    """open3d.ml.torch.ops.sparse_conv_transpose (raw op), the adjoint of sparse_conv: for output j and the entries e
+    of its ragged row (input i = neighbors_index[e]),
+        out[j] = oimp_j * sum_e nimp_e * s_i * filters[kernel_index[e]]^T f[i],
+    filters [.., Cin, Cout] with the leading dims flattened into the kernel index, inp_features [num_inp, Cin] ->
+    [num_out, Cout].  The neighbors_* lists are those of sparse_conv inverted (invert_neighbors_list, with the kernel
+    index and importance carried as attributes).  Empty importance tensors mean all ones.  Under normalize
+    s_i = 1 / inp_neighbors_importance_sum[i], or 1 / the length of row i of inp_neighbors_row_splits when that sum is
+    empty (one of the two is required), 1 for a zero divisor; s_i = 1 without normalize.  inp_neighbors_index is taken
+    for signature parity and not read.  One table-mode launch, the weighted one unless every weight is one; one host
+    read, as sparse_conv."""
+    name = "sparse_conv_transpose"
+    feat = layers.aligned_rows(_dev(inp_features).to(torch.float32).contiguous())
+    w = _sparse_filters(name, filters, feat)
+    kc, cout = w.shape[0], w.shape[2]
+    dev, num_in = feat.device, feat.shape[0]
+    e, num_out = neighbors_index.numel(), neighbors_row_splits.numel() - 1
+    oimp = _sparse_importance(name, "out_importance", out_importance, num_out, dev)
+    nimp = _sparse_importance(name, "neighbors_importance", neighbors_importance, e, dev)
+    s = None
+    if normalize:
+        s = _sparse_importance(name, "inp_neighbors_importance_sum", inp_neighbors_importance_sum, num_in, dev)
+        if s is None:
+            if inp_neighbors_row_splits is None or inp_neighbors_row_splits.numel() == 0:
+                raise RuntimeError("%s: normalize needs inp_neighbors_importance_sum or inp_neighbors_row_splits" % name)
+            irs = _dev(inp_neighbors_row_splits).to(dev, torch.int64).reshape(-1)
+            if irs.numel() != num_in + 1:
+                raise RuntimeError("%s: inp_neighbors_row_splits must have num_inp + 1 elements" % name)
+            s = (irs[1:] - irs[:-1]).to(torch.float32)
+        s = torch.where(s != 0, 1.0 / s, torch.ones_like(s))
+
+    def entry_weight(rows):
+        wt = torch.ones(e, dtype=torch.float32, device=dev) if nimp is None else nimp
+        if s is not None:        # an index outside [0, num_inp) is a shadow entry: any weight does
+            idx = _dev(neighbors_index).to(dev).reshape(-1).long()
+            wt = wt * torch.cat([s, s.new_ones(1)])[torch.where((idx >= 0) & (idx < num_in), idx, num_in)]
+        return wt if oimp is None else wt * oimp[rows]
+    weighted = oimp is not None or nimp is not None or s is not None
+    table, wt, reps, _, _ = _sparse_table(name, neighbors_index, neighbors_kernel_index, neighbors_row_splits, kc,
+                                          num_in, dev, entry_weight if weighted else None)
+    out = torch.zeros((num_out, cout), dtype=torch.float32, device=dev)
+    layers.contract_cells(feat, table, layers.pack_cells(w.repeat(reps, 1, 1)), out, entry_weight=wt)
     return _back(out, inp_features.device)

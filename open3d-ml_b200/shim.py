@@ -118,6 +118,7 @@ def _library_bindings():
             voxel_pooling=O.voxel_pooling,
             continuous_conv=O.continuous_conv, continuous_conv_transpose=O.continuous_conv_transpose,
             invert_neighbors_list=O.invert_neighbors_list, sparse_conv=O.sparse_conv,
+            sparse_conv_transpose=O.sparse_conv_transpose,
             trilinear_devoxelize_forward=O.trilinear_devoxelize_forward,
             # inference only: the backward resolves for the reference's import line and raises when called
             trilinear_devoxelize_backward=_not_on_hot_path("open3d.ml.torch.ops.trilinear_devoxelize_backward")),
