@@ -203,14 +203,49 @@ O3DML_API int o3dml_pp_pfn2_scatter(const float* points, int point_stride, int p
  *   in kernel cell (x, y, z) (row-major, the layout of the layer's `kernel` parameter [kx, ky, kz, Cin, Cout])
  *   of each output, or num_in when the cell is empty; neighbor_count int32 [num_out] (may be NULL) = non-empty
  *   cells (the `normalize` divisor).  cell_a = floor((in_a - out_a) / voxel_size + offset_a + ks_a / 2), with
- *   in / out swapped for the transposed convolution.  The contraction is o3dml_linear(_tc) with the table
- *   columns as index operands. */
+ *   in / out swapped for the transposed convolution.  The contraction is o3dml_sparse_conv_tc (or
+ *   o3dml_sparse_conv_weighted_tc) below, over the table. */
 O3DML_API size_t o3dml_sparse_conv_workspace_bytes(int64_t num_in);
 O3DML_API int o3dml_sparse_conv_neighbors(const float* in_positions, int64_t num_in,
                                           const float* out_positions, int64_t num_out, float voxel_size,
                                           const float* h_offset, const int* h_kernel_size, int transpose,
                                           int32_t* neighbors, int32_t* neighbor_count, void* workspace,
                                           size_t workspace_bytes, void* stream);
+
+/* The contraction of open3d.ml.torch.layers.SparseConv / SparseConvTranspose, ops.sparse_conv and the fused
+ * SparseConvUnet forward.  One tensor-core launch (3xTF32, as o3dml_linear_tc) of
+ *   out[m, :] = act(scale * sum_c W_c^T pre(features[table[m, c], :]) + shift + residual[m, :]),   m < num_out,
+ * over the cells c < cells of an int32 neighbour table [num_out, table_ld] such as o3dml_sparse_conv_neighbors
+ * writes.  An id outside [0, num_in) is a shadow id: its row is zero and stays zero through the prologue.
+ * pre(x) = relu(pre_scale * x + pre_shift) per input channel when pre_scale / pre_shift are given (both or neither),
+ * x otherwise.  features [num_in, features_ld]: channels used, features_ld a multiple of 4 and rows 16-byte aligned.
+ * weight_image: the TF32 hi / lo image (as o3dml_linear_tc takes it) of the [cells * Cp, out_channels] matrix whose
+ * row c * Cp + i is W_c[i], Cp = channels rounded up to 32 (rows past channels zero); k_pad = cells * Cp.  cells <=
+ * 512.  scale / shift / residual may be NULL; act 0 none, 1 relu, 2 leaky relu (slope).  num_out == 0 returns without
+ * a launch. */
+O3DML_API int o3dml_sparse_conv_tc(int64_t num_out, const float* features, int64_t num_in, int channels,
+                                   int features_ld, const int32_t* table, int cells, int table_ld,
+                                   const float* pre_scale, const float* pre_shift, const void* weight_image,
+                                   int k_pad, int n_pad, const float* scale, const float* shift,
+                                   const float* residual, int residual_ld, int act, float slope, float* out,
+                                   int out_ld, int out_channels, void* stream);
+
+/* o3dml_sparse_conv_tc above with a weight per table entry (the importances of open3d.ml.torch.ops.sparse_conv /
+ * sparse_conv_transpose and the `inp_importance` / `out_importance` arguments of layers.SparseConv /
+ * SparseConvTranspose), in one tensor-core launch:
+ *   out[m, :] = act(scale * sum_c W_c^T (w[m, c] * pre(features[table[m, c], :])) + shift + residual[m, :]),
+ * m < num_out, c < cells, with entry_weight w float [num_out, weight_ld], weight_ld >= cells, parallel to the table.
+ * The weight multiplies after the prologue pre(x) and before the 3xTF32 split, so a power-of-two weight scales the
+ * product exactly (away from the subnormal range) and a weight of one gives o3dml_sparse_conv_tc's result bit for
+ * bit.  A shadow entry contributes zero whatever its weight (also Inf or NaN).  Every other argument, limit and
+ * refusal is that of o3dml_sparse_conv_tc; num_out == 0 returns without a launch. */
+O3DML_API int o3dml_sparse_conv_weighted_tc(int64_t num_out, const float* features, int64_t num_in, int channels,
+                                            int features_ld, const int32_t* table, int cells, int table_ld,
+                                            const float* pre_scale, const float* pre_shift, const void* weight_image,
+                                            int k_pad, int n_pad, const float* scale, const float* shift,
+                                            const float* residual, int residual_ld, int act, float slope, float* out,
+                                            int out_ld, int out_channels, const float* entry_weight, int weight_ld,
+                                            void* stream);
 
 /* open3d.ml.torch.ops.continuous_conv (op surface named by the north star; no call site in the reference):
  *   out[o] = sum_n imp_n * W(map((inp_pos[n] - out_pos[o]) * 2 / extent + offset))^T f[n] over the neighbour list
@@ -464,6 +499,47 @@ O3DML_API int o3dml_kpconv_gather_deformable(const float* query_points, int64_t 
                         const float* features, int in_channels, const float* kernel_points,
                         int num_kernel_points, float kp_extent, const float* offsets, int offset_ld,
                         float* weighted_features, void* stream);
+
+/* --------------------------------------------------------------- PVCNN ---- */
+
+/* None of these entries takes a workspace: scratch comes as typed output arguments whose size follows from the
+ * shapes.
+ *
+ * Grids of PVConv (pvcnn.py:559-664) are channels-last: [batch, X, Y, Z, C] with z fastest among the spatial axes, so
+ * cell (x, y, z) of cloud b is row b * r^3 + (x * r + y) * r + z.
+ *
+ * Voxelization coordinates (pvcnn.py:642-664, normalize = True).  coords [batch * num_points, 3] point rows.  Per
+ * cloud, the mean of its points and denom = 2 * max_n |c_n - mean| + eps are reduced in a fixed order and written to
+ * stats [batch, 4]; per point voxel_coords [batch * num_points, 3] = clamp(((c - mean) / denom + 0.5) * r, 0, r - 1),
+ * the coordinates trilinear devoxelization interpolates at, and cell_ids int32 [batch * num_points] = the row of the
+ * cell (round half to even per axis) the point is averaged into.  batch * r^3 < 2^31.  Two kernels, no host read. */
+O3DML_API int o3dml_pv_voxel_cells(const float* coords, int batch, int num_points, int resolution, float eps,
+                                   float* stats, float* voxel_coords, int32_t* cell_ids, void* stream);
+
+/* avg_voxelize (pvcnn.py:579-619) from the points grouped by cell: cell_row_splits int64 [num_cells + 1] and point_ids
+ * int32, as o3dml_invert_neighbors_list gives them for one cell id per point.  grid [num_cells, channels_pad]: the mean
+ * of features [., features_ld] over the points of the cell, added in list order; zeros for an empty cell and in
+ * channels [channels, channels_pad).  Every element of grid is written. */
+O3DML_API int o3dml_pv_cell_mean(const int64_t* cell_row_splits, const int32_t* point_ids, int64_t num_cells,
+                                 const float* features, int features_ld, int channels, int channels_pad, float* grid,
+                                 void* stream);
+
+/* Conv3d(kernel 3, padding 1, stride 1) over a channels-last grid on the tensor cores (3xTF32, as o3dml_conv3x3_nhwc_tc):
+ * in [batch, X, Y, Z, C], C % 32 == 0, out [batch, X, Y, Z, out_channels]; weight image of the [27 C, out_channels]
+ * matrix whose row is ((kx * 3 + ky) * 3 + kz) * C + c. */
+O3DML_API int o3dml_conv3x3x3_ndhwc_tc(const float* in, int batch, int X, int Y, int Z, int C, const void* weight_image,
+                                       int k_pad, int n_pad, const float* scale, const float* shift, int act,
+                                       float slope, float* out, int out_channels, void* stream);
+
+/* open3d.ml.torch.ops.trilinear_devoxelize_forward on a channels-last grid [batch * r^3, grid_ld] at voxel_coords
+ * [batch * num_points, 3] in [0, r - 1].  Per axis lo = floor(v), d = v - lo, hi = lo + (d > 0 ? 1 : 0); corner k =
+ * 0..7 takes hi on x / y / z where bit 2 / 1 / 0 of k is set, its weight is the product of d (hi) or 1 - d (lo) and its
+ * cell is (x * r + y) * r + z.  out [batch * num_points, out_ld] gets (accumulate = 0) or is increased by
+ * (accumulate = 1) the weighted sum of the eight rows, added in corner order.  inds int32 / wgts float
+ * [batch, 8, num_points] are written when not null. */
+O3DML_API int o3dml_trilinear_devoxelize(const float* voxel_coords, int batch, int num_points, int resolution,
+                                         const float* grid, int channels, int grid_ld, int accumulate, float* out,
+                                         int out_ld, int32_t* inds, float* wgts, void* stream);
 
 #ifdef __cplusplus
 }

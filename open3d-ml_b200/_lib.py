@@ -48,6 +48,8 @@ _SIGNATURES = {
     "o3dml_reduce_subarrays_sum": (I, [P, P, L, P, P]),
     "o3dml_sparse_conv_workspace_bytes": (Z, [L]),
     "o3dml_sparse_conv_neighbors": (I, [P, L, P, L, F, P, P, I, P, P, P, Z, P]),
+    "o3dml_sparse_conv_tc": (I, [L, P, L, I, I, P, I, I, P, P, P, I, I, P, P, P, I, I, F, P, I, I, P]),
+    "o3dml_sparse_conv_weighted_tc": (I, [L, P, L, I, I, P, I, I, P, P, P, I, I, P, P, P, I, I, F, P, I, I, P, I, P]),
     "o3dml_continuous_conv": (I, [P, I, I, I, I, I, P, L, P, I, P, P, P, L, P, P, I, P, P, I, I, I, I, P, P]),
     "o3dml_continuous_conv_transpose": (I, [P, I, I, I, I, I, P, L, P, P, I, P, P, P, L, P, P, P, I, P, P, I, I, I, I,
                                             P, P]),
@@ -79,27 +81,12 @@ _SIGNATURES = {
     "o3dml_gather_max": (I, [P, L, I, I, P, I, L, I, L, L, I, P, I, P]),
     "o3dml_kpconv_gather": (I, [P, L, P, L, P, I, I, P, I, P, I, F, P, P]),
     "o3dml_kpconv_gather_deformable": (I, [P, L, P, L, P, I, I, P, I, P, I, F, P, I, P, P]),
-}
-EXPORTS = tuple(_SIGNATURES)           # the product ABI: exactly what include/o3dml_b200.h declares
-# the PVCNN entries of the product ABI: exactly what include/o3dml_b200_pvcnn.h declares
-_PVCNN_SIGNATURES = {
     "o3dml_pv_voxel_cells": (I, [P, I, I, I, F, P, P, P, P]),
     "o3dml_pv_cell_mean": (I, [P, P, L, P, I, I, I, P, P]),
     "o3dml_conv3x3x3_ndhwc_tc": (I, [P, I, I, I, I, I, P, I, I, P, P, I, F, P, I, P]),
     "o3dml_trilinear_devoxelize": (I, [P, I, I, I, P, I, I, I, P, I, P, P, P]),
 }
-PVCNN_EXPORTS = tuple(_PVCNN_SIGNATURES)
-# the sparse-convolution contraction of the product ABI: exactly what include/o3dml_b200_sparseconvunet.h declares
-_SPARSECONVUNET_SIGNATURES = {
-    "o3dml_sparse_conv_tc": (I, [L, P, L, I, I, P, I, I, P, P, P, I, I, P, P, P, I, I, F, P, I, I, P]),
-}
-SPARSECONVUNET_EXPORTS = tuple(_SPARSECONVUNET_SIGNATURES)
-# the weighted sparse-convolution contraction of the product ABI: exactly what include/o3dml_b200_sparse_weighted.h
-# declares
-_SPARSE_WEIGHTED_SIGNATURES = {
-    "o3dml_sparse_conv_weighted_tc": (I, [L, P, L, I, I, P, I, I, P, P, P, I, I, P, P, P, I, I, F, P, I, I, P, I, P]),
-}
-SPARSE_WEIGHTED_EXPORTS = tuple(_SPARSE_WEIGHTED_SIGNATURES)
+EXPORTS = tuple(_SIGNATURES)           # the product ABI: exactly what include/o3dml_b200.h declares
 # bring-up / profiling hooks (include/o3dml_b200_bringup.h): exported by the library, not part of the product ABI
 _BRINGUP_SIGNATURES = {
     "o3dml_tc_gemm_test": (I, [P, P, P, I, I, I, P]),
@@ -125,9 +112,7 @@ def lib():
                         "There is no CPU fallback." % (LIB_PATH, e)) from e
                 raise
         h = ctypes.CDLL(LIB_PATH)
-        for name, (res, args) in (list(_SIGNATURES.items()) + list(_PVCNN_SIGNATURES.items()) +
-                                  list(_SPARSECONVUNET_SIGNATURES.items()) +
-                                  list(_SPARSE_WEIGHTED_SIGNATURES.items()) + list(_BRINGUP_SIGNATURES.items())):
+        for name, (res, args) in list(_SIGNATURES.items()) + list(_BRINGUP_SIGNATURES.items()):
             fn = getattr(h, name)
             fn.restype, fn.argtypes = res, args
         if h.o3dml_abi_version() != ABI_VERSION:

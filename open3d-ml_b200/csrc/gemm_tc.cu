@@ -35,9 +35,6 @@
 // Every GT_FLUSH slices the wgmma accumulator is folded into a second fp32 register set with
 // round-to-nearest adds, so that long products do not rely on the tensor core's internal accumulation.
 #include "../../include/o3dml_b200.h"
-#include "../../include/o3dml_b200_pvcnn.h"
-#include "../../include/o3dml_b200_sparseconvunet.h"
-#include "../../include/o3dml_b200_sparse_weighted.h"
 #include "dense.cuh"
 #include "tc.cuh"
 #include <cuda.h>

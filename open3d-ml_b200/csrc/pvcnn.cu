@@ -2,7 +2,7 @@
 // voxel coordinates and cell ids of every point, the mean of the points of every cell, trilinear devoxelization.
 // Grids are [B, X, Y, Z, C] with z fastest among the spatial axes, i.e. cell (x * r + y) * r + z of cloud b is row
 // b * r^3 + (x * r + y) * r + z.  Nothing here adds floats atomically: two runs agree bit for bit.
-#include "../../include/o3dml_b200_pvcnn.h"
+#include "../../include/o3dml_b200.h"
 #include "common.cuh"
 
 namespace o3dml {

@@ -1,7 +1,7 @@
-"""Seeded calls of the C-ABI entries and the case tables of the ABI contract tests: LAUNCH_CASES and EXPECTED_KERNEL
-(tests/test_gpu_launch_count.py), WORKSPACE_CASES (tests/test_gpu_workspace.py) and REFUSAL_ROWS
-(tests/test_workspace.py).  tests/test_abi.py checks that these tables cover every entry the library exports, so a
-new entry is added here.  Each builder allocates everything its call needs on the GPU; an entry that takes a workspace
+"""Seeded calls of the C-ABI entries (include/o3dml_b200.h) and the case tables of the ABI contract tests: LAUNCH_CASES,
+EXPECTED_LAUNCHES and EXPECTED_KERNEL (tests/test_gpu_launch_count.py), WORKSPACE_CASES (tests/test_gpu_workspace.py)
+and REFUSAL_ROWS (tests/test_workspace.py).  tests/test_abi.py checks that these tables cover every entry the library
+exports, so a new entry is added here.  Each builder allocates everything its call needs on the GPU; an entry that takes a workspace
 is built as a WsCase whose `run` takes the workspace as an argument, so that a test can choose where the workspace lies
 and how large it is said to be.  Importing this module needs no GPU."""
 import json
@@ -11,7 +11,7 @@ import tempfile
 import numpy as np
 import torch
 
-from open3d_ml_b200 import _lib as L
+from open3d_ml_b200 import _lib as L, layers as LY
 from oracle import ops as O, search as S
 import cconv_transpose_oracle as R
 
@@ -461,6 +461,58 @@ def case_kpconv_gather_deformable():
                                                           L.ptr(off), off.stride(0), L.ptr(out), L.stream())
 
 
+def case_sparse_conv(cells, pre, weighted):
+    """One contraction over a seeded table with shadow entries, with or without the BN-ReLU prologue, and with or
+    without a weight per table entry."""
+    m, n, cin, cout = 300, 250, 48, 40
+    seed = 70 if weighted else 60
+    g = torch.Generator().manual_seed(seed)
+    table = torch.randint(0, n + n // 3, (m, cells), generator=g, dtype=torch.int32).cuda()
+    weight = torch.randn(m, cells, generator=g).cuda() if weighted else None
+    feat, w = rnd(n, cin, seed=seed + 1), rnd(cells, cin, cout, seed=seed + 2)
+    prologue = (rnd(cin, seed=seed + 3), rnd(cin, seed=seed + 4)) if pre else None
+    packed, out = LY.pack_cells(w.cpu()), torch.empty(m, cout).cuda()
+    return lambda: LY.contract_cells(feat, table, packed, out, pre=prologue, entry_weight=weight)
+
+
+def pv_inputs(B=2, N=500, r=6, seed=50):
+    """Point rows of B clouds and their voxel coordinates and cell ids at resolution r, from o3dml_pv_voxel_cells."""
+    pts = (torch.rand(B * N, 3, generator=torch.Generator().manual_seed(seed)) * 4).cuda()
+    stats, vox = torch.empty(B, 4).cuda(), torch.empty(B * N, 3).cuda()
+    cell = torch.empty(B * N, dtype=torch.int32).cuda()
+
+    def call():
+        return L.lib().o3dml_pv_voxel_cells(L.ptr(pts), B, N, r, 1e-6, L.ptr(stats), L.ptr(vox), L.ptr(cell),
+                                            L.stream())
+    return pts, vox, cell, call
+
+
+def case_pv_cell_mean(B=2, N=500, r=6, C=9):
+    _, _, cell, call = pv_inputs(B, N, r)
+    L.check(call())
+    order = torch.argsort(cell.long(), stable=True)
+    ids = order.to(torch.int32)
+    splits = torch.searchsorted(cell.long()[order].contiguous(), torch.arange(B * r ** 3 + 1).cuda()).contiguous()
+    feat, grid = rnd(B * N, C, seed=51), torch.empty(B * r ** 3, 32).cuda()
+    return lambda: L.lib().o3dml_pv_cell_mean(L.ptr(splits), L.ptr(ids), B * r ** 3, L.ptr(feat), C, C, 32,
+                                              L.ptr(grid), L.stream())
+
+
+def case_conv3x3x3():
+    x, w = rnd(2, 5, 6, 7, 32, seed=52), rnd(27 * 32, 16, seed=53)
+    weight, out = L.pack_linear(w), torch.empty(2, 5, 6, 7, 16).cuda()
+    return lambda: L.conv3x3x3(x, weight, out, act="leaky", slope=0.1)
+
+
+def case_trilinear_devoxelize(B=2, N=500, r=6, C=32):
+    _, vox, _, call = pv_inputs(B, N, r)
+    L.check(call())
+    grid, out = rnd(B * r ** 3, C, seed=54), torch.zeros(B * N, C).cuda()
+    inds, wgts = torch.empty(B, 8, N, dtype=torch.int32).cuda(), torch.empty(B, 8, N).cuda()
+    return lambda: L.lib().o3dml_trilinear_devoxelize(L.ptr(vox), B, N, r, L.ptr(grid), C, C, 1, L.ptr(out), C,
+                                                      L.ptr(inds), L.ptr(wgts), L.stream())
+
+
 # ------------------------------------------------------------------------------------------------------ the tables
 # {case: (the C entry the case is meant to reach, builder of its call)}.  The entries that take a workspace run over a
 # workspace of exactly the size their sizing function gives.
@@ -513,11 +565,33 @@ LAUNCH_CASES = {
     "kpconv_gather_shuffle_4": ("o3dml_kpconv_gather", lambda: case_kpconv_gather(130)),
     "kpconv_gather_shuffle_unaligned": ("o3dml_kpconv_gather", lambda: case_kpconv_gather(64, offset=4)),
     "kpconv_gather_deformable": ("o3dml_kpconv_gather_deformable", case_kpconv_gather_deformable),
+    "sparse_conv_tc_27_pre": ("o3dml_sparse_conv_tc", lambda: case_sparse_conv(27, True, False)),
+    "sparse_conv_tc_27": ("o3dml_sparse_conv_tc", lambda: case_sparse_conv(27, False, False)),
+    "sparse_conv_tc_8_pre": ("o3dml_sparse_conv_tc", lambda: case_sparse_conv(8, True, False)),
+    "sparse_conv_tc_1": ("o3dml_sparse_conv_tc", lambda: case_sparse_conv(1, False, False)),
+    "sparse_conv_weighted_tc_27_pre": ("o3dml_sparse_conv_weighted_tc", lambda: case_sparse_conv(27, True, True)),
+    "sparse_conv_weighted_tc_27": ("o3dml_sparse_conv_weighted_tc", lambda: case_sparse_conv(27, False, True)),
+    "sparse_conv_weighted_tc_8_pre": ("o3dml_sparse_conv_weighted_tc", lambda: case_sparse_conv(8, True, True)),
+    "sparse_conv_weighted_tc_8": ("o3dml_sparse_conv_weighted_tc", lambda: case_sparse_conv(8, False, True)),
+    "sparse_conv_weighted_tc_1_pre": ("o3dml_sparse_conv_weighted_tc", lambda: case_sparse_conv(1, True, True)),
+    "sparse_conv_weighted_tc_1": ("o3dml_sparse_conv_weighted_tc", lambda: case_sparse_conv(1, False, True)),
+    "pv_voxel_cells": ("o3dml_pv_voxel_cells", lambda: pv_inputs()[3]),
+    "pv_cell_mean": ("o3dml_pv_cell_mean", case_pv_cell_mean),
+    "conv3x3x3_tc": ("o3dml_conv3x3x3_ndhwc_tc", case_conv3x3x3),
+    "trilinear_devoxelize": ("o3dml_trilinear_devoxelize", case_trilinear_devoxelize),
 }
 
-# the kernel a case is meant to reach, where the entry chooses among several instances or kernels; with the spaces of
-# the trace's name removed, it is followed by "<" or "("
+# the number of kernels a case must enqueue, where the entry promises one: a sparse contraction is one launch whatever
+# the number of kernel cells
+EXPECTED_LAUNCHES = {case: 1 for case, (entry, _) in LAUNCH_CASES.items()
+                     if entry in ("o3dml_sparse_conv_tc", "o3dml_sparse_conv_weighted_tc")}
+
+# the kernel a case is meant to reach, for the cases that name one; with the spaces of the trace's name removed, it is
+# followed by "<" or "("
 EXPECTED_KERNEL = {
+    **dict.fromkeys(EXPECTED_LAUNCHES, "gemm_tc_kernel"),
+    "pv_voxel_cells": "pv_point_cells_kernel", "pv_cell_mean": "pv_cell_mean_kernel",
+    "conv3x3x3_tc": "gemm_tc_kernel", "trilinear_devoxelize": "pv_devoxelize_kernel",
     "linear_simt": "gemm_gather_kernel", "linear_tc": "gemm_tc_kernel", "linear_rows_small": "rowmlp_kernel",
     "conv3x3_simt": "gemm_gather_kernel", "conv3x3_tc": "gemm_tc_kernel",
     "deconv_simt": "gemm_gather_kernel", "deconv_tc": "gemm_tc_kernel",

@@ -8,16 +8,21 @@ from conftest import ROOT
 
 
 def declared_symbols():
+    """Every declaration of the header in order, a name declared twice listed twice."""
     src = open(os.path.join(ROOT, "include", "o3dml_b200.h")).read()
-    return sorted(set(re.findall(r"O3DML_API[^;(]*?\b(o3dml_\w+)\s*\(", src)))
+    return re.findall(r"O3DML_API[^;(]*?\b(o3dml_\w+)\s*\(", src)
 
 
 def test_header_declares_the_path():
     names = declared_symbols()
     for must in ("o3dml_voxelize", "o3dml_ragged_to_dense", "o3dml_knn_search", "o3dml_radius_count",
                  "o3dml_radius_fill", "o3dml_pp_pfn_scatter", "o3dml_linear", "o3dml_conv3x3_nhwc",
-                 "o3dml_deconv_nhwc", "o3dml_randla_lfa_pool", "o3dml_gather_max", "o3dml_kpconv_gather"):
+                 "o3dml_deconv_nhwc", "o3dml_randla_lfa_pool", "o3dml_gather_max", "o3dml_kpconv_gather",
+                 "o3dml_sparse_conv_tc", "o3dml_sparse_conv_weighted_tc", "o3dml_pv_voxel_cells", "o3dml_pv_cell_mean",
+                 "o3dml_conv3x3x3_ndhwc_tc", "o3dml_trilinear_devoxelize"):
         assert must in names
+    twice = sorted({n for n in names if names.count(n) > 1})
+    assert not twice, "declared more than once: %s" % ", ".join(twice)
 
 
 def test_library_builds_loads_and_exports_everything():
@@ -42,14 +47,16 @@ ENQUEUE_NOTHING = (
 
 
 def test_contract_tables_cover_every_export():
-    """Every export is reached by a launch-count case or enqueues nothing, and every sizing function is checked by an
-    exact-workspace case on the GPU and by a refusal row without one."""
+    """Every export is reached by a launch-count case or enqueues nothing, every expected kernel or launch count belongs
+    to a launch-count case, and every sizing function is checked by an exact-workspace case on the GPU and by a refusal
+    row without one."""
     from open3d_ml_b200 import _lib
-    from abi_cases import LAUNCH_CASES, REFUSAL_ROWS, WORKSPACE_CASES
+    from abi_cases import EXPECTED_KERNEL, EXPECTED_LAUNCHES, LAUNCH_CASES, REFUSAL_ROWS, WORKSPACE_CASES
     exports, quiet = set(_lib.EXPORTS), set(ENQUEUE_NOTHING)
     launched = {entry for entry, _ in LAUNCH_CASES.values()}
     sizing = {name for name in exports if name.endswith("_workspace_bytes")}
-    for what, names in [("not exported", (launched | quiet) - exports),
+    for what, names in [("not a launch case", (set(EXPECTED_KERNEL) | set(EXPECTED_LAUNCHES)) - set(LAUNCH_CASES)),
+                        ("not exported", (launched | quiet) - exports),
                         ("both launched and enqueuing nothing", launched & quiet),
                         ("no launch-count case", exports - launched - quiet),
                         ("no exact-workspace case", sizing - {s for s, _ in WORKSPACE_CASES.values()}),

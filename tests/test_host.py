@@ -1,12 +1,14 @@
 """Host-side logic that needs no GPU: the open3d shim wiring, seeded generators,
 frame sharding + the post-batch collectives over gloo (world_size 2)."""
 import os
+import subprocess
 import sys
 
 import numpy as np
 import pytest
 import torch
 
+from conftest import ROOT
 from oracle import refshim, weights
 from open3d_ml_b200 import synth, shard
 import helpers as H
@@ -72,7 +74,6 @@ def test_frame_shard_collectives_gloo_world2():
 @pytest.mark.skipif(not refshim.available(), reason="/root/reference absent (GPU box)")
 def test_shim_exposes_the_reference_tree_unmodified():
     """run in a subprocess: the shim owns sys.modules['open3d']"""
-    import subprocess
     code = ("import sys; sys.path.insert(0, %r)\n"
             "from open3d_ml_b200 import shim; shim.install('/root/reference')\n"
             "import open3d as o3d, open3d.ml as _ml3d, open3d.ml.torch as ml3d\n"
@@ -90,6 +91,34 @@ def test_shim_exposes_the_reference_tree_unmodified():
     r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=300)
     assert r.returncode == 0, r.stderr[-2000:]
     assert "ok 1242307" in r.stdout
+
+
+def _run(code):
+    env = dict(os.environ, PYTHONPATH=ROOT)
+    r = subprocess.run([sys.executable, "-c", code], cwd=ROOT, env=env, capture_output=True, text=True, timeout=300)
+    assert r.returncode == 0, r.stderr
+
+
+def test_shim_resolves_sparse_conv_transpose_without_cuda():
+    _run("import torch, open3d_ml_b200.shim as shim\n"
+         "shim.install()\n"
+         "from open3d.ml.torch.ops import sparse_conv, sparse_conv_transpose\n"
+         "from open3d_ml_b200 import _lib, ops\n"
+         "assert sparse_conv_transpose is ops.sparse_conv_transpose and sparse_conv is ops.sparse_conv\n"
+         "assert _lib._lib is None and not torch.cuda.is_initialized()\n")
+
+
+def test_shim_under_the_oracle_bindings_raises_when_called():
+    _run("import open3d_ml_b200.shim as shim\n"
+         "from oracle import refshim\n"
+         "shim.install(bindings=refshim.BINDINGS)\n"
+         "from open3d.ml.torch.ops import sparse_conv_transpose\n"
+         "try:\n"
+         "    sparse_conv_transpose()\n"
+         "except NotImplementedError:\n"
+         "    pass\n"
+         "else:\n"
+         "    raise SystemExit('sparse_conv_transpose did not raise')\n")
 
 
 def test_pipelined_runner_tree_helpers_and_cpu_refusal():
