@@ -39,7 +39,8 @@ def rnd(*shape, seed=0):
 @pytest.mark.parametrize("n,cin,cout", [(1000, 8, 8), (4099, 3, 8), (777, 32, 19), (5000, 64, 64),
                                         (300, 768, 256), (2048, 128, 1024), (65, 75, 64), (1, 16, 13),
                                         (129, 40, 72), (70000, 256, 32),
-                                        # short products on many row tiles: the two-CTAs-per-SM LITE kernels (gemm_tc.cu GtCfg)
+                                        # short products on many row tiles: the two-CTAs-per-SM LITE kernels (gemm_tc.cu GtCfg),
+                                        # which test_gpu_gemm_tc_matrix.py::test_linear_plain_lite_rows_run_lite asserts
                                         (30000, 64, 64), (20011, 96, 128), (40000, 128, 32)])
 def test_linear_plain(n, cin, cout, tc):
     """tc=True: PackedWeight -> wgmma kernel (gemm_tc.cu) whenever cin % 8 == 0, SIMT otherwise."""
