@@ -13,7 +13,11 @@
 // Result order (implementation-defined upstream, fixed here): rows ascend by
 // (distance, index); in float32 without FMA, d = q - p per axis, L2 is returned squared,
 // ((dx*dx + dy*dy) + dz*dz), L1 is (|dx| + |dy|) + |dz| and Linf max(max(|dx|, |dy|), |dz|)
-// (oracle/ops_ref.c, oracle/search_ref.c).  HBM/latency-bound: 12 B/query in, 8*k (or 4*L) B/query out.
+// (oracle/ops_ref.c, oracle/search_ref.c).  Non-finite input: a NaN distance (a NaN coordinate, or +inf - +inf) is
+// never ranked nor within a radius; a distance that is +inf (an infinite coordinate, or an overflowing sum) ranks
+// after every finite one; so a k-NN row may be short, padded with -1 / +inf.  An axis whose bounding-box extent is
+// not finite gets one cell (grid_setup_kernel): the search stays exact, at the cost of visiting more points.
+// HBM/latency-bound: 12 B/query in, 8*k (or 4*L) B/query out.
 #include "../../include/o3dml_b200.h"
 #include "prims.cuh"
 #include <float.h>
@@ -102,6 +106,9 @@ __global__ void item_radius_kernel(const float* __restrict__ radii, int64_t nq, 
 // k points at the mean surface / volume density of the bounding box.  The cell size is then raised to 2^-20 of the
 // longest side of the bounding box, so that the growth below (1.26^64 > 2^21) always ends inside grid_cell_cap, and
 // grows until the item's cells fit grid_cell_cap.  The cell size affects speed only: every search is exact.
+// An axis whose extent is not a finite float (a NaN or infinite coordinate, or max - min past FLT_MAX) gets one cell
+// and origin 0: every point and query is clamped into it, which keeps the searches exact, and no NaN or infinity
+// reaches the float -> int conversions of the grid dims.
 __global__ void grid_setup_kernel(const unsigned* __restrict__ bbox,
                                   const int64_t* __restrict__ splits, int batch, float fixed_cs,
                                   int k, GridInfo* __restrict__ info, uint32_t* total_cells,
@@ -118,7 +125,9 @@ __global__ void grid_setup_kernel(const unsigned* __restrict__ bbox,
             for (int d = 0; d < 3; ++d) {
                 mn[d] = ord2f(bbox[b * 6 + d]);
                 mx[d] = ord2f(bbox[b * 6 + 3 + d]);
-                e[d] = fmaxf(mx[d] - mn[d], 1e-6f);
+                const float ext = mx[d] - mn[d];
+                if (ext <= FLT_MAX) e[d] = fmaxf(ext, 1e-6f);
+                else { e[d] = 0.f; mn[d] = 0.f; }  // NaN or infinite: one cell along this axis
             }
             float cs = item_radius ? fmaxf(__uint_as_float(item_radius[b]), 1e-6f) : fixed_cs;
             if (!(cs > 0.f)) {
@@ -241,8 +250,10 @@ __device__ __forceinline__ bool coincident(float qx, float qy, float qz, const f
 }
 
 // ------------------------------------------------------------------- k-NN ----
-// IGNORE: row_len[qi] = the neighbours found (fewer than k when coincident points were skipped); the row is written
-// dense and -1 / +inf padded like a batch item with fewer than k points.
+// A row holds the first k points by (d, id) among those with a distance that is not NaN (+inf ranks after every finite
+// distance), then -1 / +inf padding: it is short when its item holds fewer than k such points.
+// IGNORE: row_len[qi] = the neighbours found (fewer than k when coincident points were skipped or the row is short).
+// Without IGNORE the row stays dense [k], padded in place.
 // The min-blocks hint of 1 lets ptxas give the metric / ignore instances the registers they need without spilling;
 // the L2 instances keep the bare bound (0 = none), which they were tuned under.
 template <int KMAX, int M = L2, bool IGNORE = false>
@@ -260,8 +271,9 @@ knn_kernel(const float* __restrict__ queries, int64_t nq, const int64_t* __restr
     const float qx = queries[3 * qi], qy = queries[3 * qi + 1], qz = queries[3 * qi + 2];
     float bd[KMAX];
     int bi[KMAX];
+    const float inf = __int_as_float(0x7f800000);
 #pragma unroll
-    for (int j = 0; j < KMAX; ++j) { bd[j] = FLT_MAX; bi[j] = 0x7fffffff; }
+    for (int j = 0; j < KMAX; ++j) { bd[j] = inf; bi[j] = 0x7fffffff; }  // empty: ranks after every point
     const int64_t nsup = psplits[b + 1] - psplits[b];
     const int kk = (int)(nsup < k ? nsup : k);  // neighbours that exist
     if (kk > 0) {
@@ -306,19 +318,21 @@ knn_kernel(const float* __restrict__ queries, int64_t nq, const int64_t* __restr
             // everything closer than r*cs has been seen (cells are >= cs wide, the query sits
             // inside its own cell or outside the grid on the far side); 1e-4 relative slack
             // covers the float rounding of the cell assignment.  That bound is in Linf, and L1 >= Linf.
+            // A k-th best at +inf (or an empty slot) never stops the walk: a point further out may tie it at +inf and
+            // rank first by index.
             const float cover = (float)r * g.cs * 0.9999f;
-            float kth = FLT_MAX;  // the k-th best so far sits at slot kk-1 (slots are sorted)
+            float kth = inf;  // the k-th best so far sits at slot kk-1 (slots are sorted)
 #pragma unroll
             for (int j = 0; j < KMAX; ++j)
                 if (j == kk - 1) kth = bd[j];
-            if (kth != FLT_MAX && kth <= (M == L2 ? cover * cover : cover)) break;
+            if (kth < inf && kth <= (M == L2 ? cover * cover : cover)) break;
         }
     }
     uint32_t found = 0;
 #pragma unroll
     for (int j = 0; j < KMAX; ++j) {
         if (j < k) {
-            const bool have = j < kk && (!IGNORE || bi[j] != 0x7fffffff);
+            const bool have = j < kk && bi[j] != 0x7fffffff;  // filled: NaN distances are never ranked
             if (idx_is64) ((int64_t*)out_idx)[qi * k + j] = have ? (int64_t)bi[j] : -1;
             else ((int32_t*)out_idx)[qi * k + j] = have ? bi[j] : -1;
             if (out_d2) out_d2[qi * k + j] = have ? bd[j] : __int_as_float(0x7f800000);

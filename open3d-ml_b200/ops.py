@@ -192,7 +192,9 @@ def knn_search(points, queries, k, points_row_splits=None, queries_row_splits=No
     """open3d.ml.torch.ops.knn_search.  Rows ascend by (distance, index) in `metric` (L1, L2, Linf); L2 distances are
     squared, as upstream returns them.  Dense [Nq * k] rows with row splits 0, k, 2k, ...; with ignore_query_point
     (points equal to the query are skipped) a row may hold fewer than k neighbours, and the rows are ragged (one
-    device->host read of their total)."""
+    device->host read of their total).  NaN distances are never ranked and +inf ones rank last, so a row that finds
+    fewer than k rankable points (NaN coordinates) is padded with index -1 and distance +inf: dense rows in place,
+    ragged rows by their length."""
     m, p, q, ps, qs, batch = _search_args("knn_search", points, queries, points_row_splits, queries_row_splits,
                                           index_dtype, metric)
     dev = p.device

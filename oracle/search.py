@@ -97,6 +97,10 @@ def np_dist(q, p, metric):
     return np.maximum(np.maximum(a[..., 0], a[..., 1]), a[..., 2])       # np.maximum propagates NaN
 
 
+def _finite(P, Q):
+    return bool(np.isfinite(P).all() and np.isfinite(Q).all())
+
+
 def _coincides(q, p):
     return np.all(q[None, :] == p, axis=1)
 
@@ -105,6 +109,13 @@ def np_search_radius(points, queries, radius, radii=None, points_row_splits=None
                      ignore=False, normalize=False):
     """cKDTree.query_ball_point candidates (Minkowski p of the metric, one radius per query, 1e-5 relative slack), then
     the float32 test and ordering of the contract."""
+    with np.errstate(over="ignore", invalid="ignore"):
+        return _np_search_radius(points, queries, radius, radii, points_row_splits, queries_row_splits, metric, ignore,
+                                 normalize)
+
+
+def _np_search_radius(points, queries, radius, radii, points_row_splits, queries_row_splits, metric, ignore,
+                      normalize):
     from scipy.spatial import cKDTree
     points, queries = _f32(points), _f32(queries)
     ps, qs = _splits(points_row_splits, len(points)), _splits(queries_row_splits, len(queries))
@@ -115,7 +126,9 @@ def np_search_radius(points, queries, radius, radii=None, points_row_splits=None
         P, Q, R = points[ps[b]:ps[b + 1]], queries[qs[b]:qs[b + 1]], r_all[qs[b]:qs[b + 1]]
         valid = (R >= 0) & np.isfinite(R)
         cand = [[] for _ in range(len(Q))]
-        if len(P) and valid.any():
+        if len(P) and valid.any() and not _finite(P, Q):        # cKDTree takes finite coordinates only
+            cand = [np.arange(len(P))] * len(Q)
+        elif len(P) and valid.any():
             slack = np.where(valid, R.astype(np.float64) * (1 + 1e-5) + 1e-7, 0.0)
             cand = cKDTree(P).query_ball_point(Q.astype(np.float64), slack, p=_P[metric])
         for qi in range(len(Q)):
@@ -142,6 +155,11 @@ def np_search_knn(points, queries, k, points_row_splits=None, queries_row_splits
                   extra=16):
     """cKDTree.query candidates (Minkowski p of the metric) re-ranked in float32 by (d, idx) after dropping the points
     equal to the query under `ignore`; brute force for a row whose candidate set cannot be proven complete."""
+    with np.errstate(over="ignore", invalid="ignore"):
+        return _np_search_knn(points, queries, k, points_row_splits, queries_row_splits, metric, ignore, extra)
+
+
+def _np_search_knn(points, queries, k, points_row_splits, queries_row_splits, metric, ignore, extra):
     from scipy.spatial import cKDTree
     points, queries = _f32(points), _f32(queries)
     ps, qs = _splits(points_row_splits, len(points)), _splits(queries_row_splits, len(queries))
@@ -152,9 +170,12 @@ def np_search_knn(points, queries, k, points_row_splits=None, queries_row_splits
         P, Q = points[ps[b]:ps[b + 1]], queries[qs[b]:qs[b + 1]]
         if len(P) == 0 or len(Q) == 0:
             continue
-        kk = int(min(len(P), k + extra))
-        _, cand = cKDTree(P).query(Q.astype(np.float64), k=kk, p=_P[metric])
-        cand = np.asarray(cand).reshape(len(Q), kk)
+        kk = int(min(len(P), k + extra)) if _finite(P, Q) else len(P)       # cKDTree takes finite coordinates only
+        if kk < len(P):
+            _, cand = cKDTree(P).query(Q.astype(np.float64), k=kk, p=_P[metric])
+            cand = np.asarray(cand).reshape(len(Q), kk)
+        else:
+            cand = np.broadcast_to(np.arange(len(P)), (len(Q), kk))
         for qi in range(len(Q)):
             c = cand[qi]
             complete = kk == len(P)

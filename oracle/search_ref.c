@@ -113,7 +113,9 @@ EXPORT int oracle_search_radius(const float *points, const int64_t *p_splits, co
 }
 
 /* k nearest: out_idx int64 [Nq,k] (-1 pads), out_d float32 [Nq,k] (+inf pads), out_len int64 [Nq] = the
- * neighbours found (fewer than k when the item is smaller or ignore skipped points). */
+ * neighbours found (fewer than k when the item is smaller, ignore skipped points or distances were NaN).  A NaN d is
+ * never ranked; +inf ranks after every finite d.  The k best are kept in a sorted buffer: a point enters when it sorts
+ * before the buffer's last entry (or the buffer is not full), the order of a full sort by (d, index). */
 EXPORT int oracle_search_knn(const float *points, const int64_t *p_splits, const float *queries,
                              const int64_t *q_splits, int64_t batch, int k, int metric, int ignore,
                              int64_t *out_idx, float *out_d, int64_t *out_len) {
@@ -123,24 +125,26 @@ EXPORT int oracle_search_knn(const float *points, const int64_t *p_splits, const
 #pragma omp parallel for schedule(dynamic, 64)
         for (int64_t qi = q_splits[b]; qi < q_splits[b + 1]; ++qi) {
             const float *q = queries + 3 * qi;
-            nb_t *tmp = (nb_t *)malloc(sizeof(nb_t) * (size_t)(p1 - p0 > 0 ? p1 - p0 : 1));
-            int64_t c = 0;
+            nb_t *best = (nb_t *)malloc(sizeof(nb_t) * (size_t)k);
+            int64_t n = 0;
             for (int64_t pi = p0; pi < p1; ++pi) {
                 if (ignore && coincides(q, points + 3 * pi)) continue;
-                float d = metric_dist(q, points + 3 * pi, metric);
-                if (d != d) continue;
-                tmp[c].d = d;
-                tmp[c].i = (int32_t)pi;
-                ++c;
+                nb_t c = {metric_dist(q, points + 3 * pi, metric), (int32_t)pi};
+                if (c.d != c.d) continue;
+                if (n == k && nb_cmp(&c, &best[k - 1]) >= 0) continue;
+                int64_t j = n < k ? n++ : k - 1;
+                while (j > 0 && nb_cmp(&c, &best[j - 1]) < 0) {
+                    best[j] = best[j - 1];
+                    --j;
+                }
+                best[j] = c;
             }
-            qsort(tmp, (size_t)c, sizeof(nb_t), nb_cmp);
-            int64_t n = c < k ? c : k;
             for (int64_t j = 0; j < k; ++j) {
-                out_idx[qi * k + j] = j < n ? tmp[j].i : -1;
-                out_d[qi * k + j] = j < n ? tmp[j].d : INFINITY;
+                out_idx[qi * k + j] = j < n ? best[j].i : -1;
+                out_d[qi * k + j] = j < n ? best[j].d : INFINITY;
             }
             out_len[qi] = n;
-            free(tmp);
+            free(best);
         }
     }
     return 0;
