@@ -57,6 +57,24 @@ struct DenseEpilogue {
     int ds, dIH, dIW, dC;   // pixel shuffle: stride, input height and width, channels per sub-pixel
 };
 
+// Element offset in e.out of output (n, c) of a product with `cout` output columns.  Pixel shuffle: row n is input pixel
+// (b, iy, ix), and column c = (dy * ds + dx) * dC + co goes to channel co of output pixel (b, iy * ds + dy, ix * ds + dx).
+__device__ __forceinline__ size_t out_offset(const DenseEpilogue& e, int64_t n, int c, int cout) {
+    if (e.mode == 0) return (size_t)n * e.out_ld + c;
+    if (e.mode == 1) {
+        const int64_t b = n / e.plane, pix = n % e.plane;
+        return ((size_t)b * cout + c) * e.plane + pix;
+    }
+    const int64_t per = (int64_t)e.dIH * e.dIW;
+    const int64_t b = n / per;
+    const int rr = (int)(n % per);
+    const int iy = rr / e.dIW, ix = rr % e.dIW;
+    const int sub = c / e.dC, co = c - sub * e.dC;
+    const int dy = sub / e.ds, dx = sub - dy * e.ds;
+    const size_t opix = ((size_t)b * e.dIH * e.ds + (size_t)iy * e.ds + dy) * (e.dIW * e.ds) + (size_t)ix * e.ds + dx;
+    return opix * e.out_ld + co;
+}
+
 // Fills p.ep and p.Cout for a row-major (out_nchw_plane == 0) or NCHW output and checks them together with the weight
 // operand the caller passes to its kernel.
 template <class P>
@@ -100,11 +118,8 @@ inline int set_conv3x3(const char* fn, P& p, const float* in, int batch, int H, 
 
 // A 3x3x3 convolution, padding 1, stride 1, over a channels-last grid [batch, X, Y, Z, C] (z fastest among the
 // spatial axes) as an implicit GEMM: one row per output voxel, K = 27 C, weight row ((kx * 3 + ky) * 3 + kz) * C + c.
-// A CTA owns a PZ x PY x PX = `rows` box of output voxels with power-of-two sides: the shape with the fewest boxes,
-// then the most compact one (its 27 shifted copies overlap most in L2), then the longest run along z.
 template <class P>
-inline int set_conv3x3x3(const char* fn, P& p, const float* in, int batch, int X, int Y, int Z, int C, int c_multiple,
-                         int rows) {
+inline int set_conv3x3x3(const char* fn, P& p, const float* in, int batch, int X, int Y, int Z, int C, int c_multiple) {
     O3DML_CHECK(in && batch > 0 && X > 0 && Y > 0 && Z > 0, "%s: bad input", fn);
     O3DML_CHECK((C % c_multiple) == 0 && C > 0, "%s: input channels must be a multiple of %d", fn, c_multiple);
     O3DML_CHECK((reinterpret_cast<uintptr_t>(in) & 15) == 0, "%s: input must be 16-byte aligned", fn);
@@ -115,26 +130,6 @@ inline int set_conv3x3x3(const char* fn, P& p, const float* in, int batch, int X
     p.X = X; p.Y = Y; p.Z = Z; p.C = C;
     p.N = (int64_t)batch * X * Y * Z;
     p.K = 27 * C;
-    int lr = 0;
-    while ((1 << lr) < rows) ++lr;
-    int64_t best_tiles = -1;
-    int best_sum = 0;
-    for (int lz = 0; lz <= lr; ++lz)
-        for (int ly = 0; lz + ly <= lr; ++ly) {
-            const int pz = 1 << lz, py = 1 << ly, px = rows >> (lz + ly);
-            const int64_t tiles = (int64_t)ceil_div(Z, pz) * ceil_div(Y, py) * ceil_div(X, px);
-            const int sum = pz + py + px;
-            if (best_tiles < 0 || tiles < best_tiles || (tiles == best_tiles && sum < best_sum) ||
-                (tiles == best_tiles && sum == best_sum && lz > p.lpz)) {
-                best_tiles = tiles;
-                best_sum = sum;
-                p.lpz = lz;
-                p.lpy = ly;
-            }
-        }
-    p.tiles_z = ceil_div(Z, 1 << p.lpz);
-    p.tiles_y = ceil_div(Y, 1 << p.lpy);
-    p.tiles_x = ceil_div(X, rows >> (p.lpz + p.lpy));
     return O3DML_OK;
 }
 

@@ -220,39 +220,13 @@ gemm_gather_kernel(const __grid_constant__ GemmParams p) {
             if (ep.residual && c < p.Cout) x += ep.residual[(size_t)n * ep.res_ld + c];
             v[j] = apply_act(x, ep.act, ep.slope);
         }
-        if (ep.mode == 0) {
-            float* o = ep.out + (size_t)n * ep.out_ld + cbase;
-            if (cbase + 3 < p.Cout && (ep.out_ld & 3) == 0 &&
-                ((reinterpret_cast<uintptr_t>(ep.out) & 15) == 0)) {
-                *reinterpret_cast<float4*>(o) = make_float4(v[0], v[1], v[2], v[3]);
-            } else {
-#pragma unroll
-                for (int j = 0; j < GEMM_TN; ++j)
-                    if (cbase + j < p.Cout) o[j] = v[j];
-            }
-        } else if (ep.mode == 1) {
-            const int64_t b = n / ep.plane, pix = n % ep.plane;
+        if (ep.mode == 0 && cbase + 3 < p.Cout && (ep.out_ld & 3) == 0 &&
+            ((reinterpret_cast<uintptr_t>(ep.out) & 15) == 0)) {
+            *reinterpret_cast<float4*>(ep.out + out_offset(ep, n, cbase, p.Cout)) = make_float4(v[0], v[1], v[2], v[3]);
+        } else {
 #pragma unroll
             for (int j = 0; j < GEMM_TN; ++j)
-                if (cbase + j < p.Cout)
-                    ep.out[((size_t)b * p.Cout + cbase + j) * ep.plane + pix] = v[j];
-        } else {
-            const int64_t per = (int64_t)ep.dIH * ep.dIW;
-            const int64_t b = n / per;
-            const int r = (int)(n % per);
-            const int iy = r / ep.dIW, ix = r % ep.dIW;
-            const int OWd = ep.dIW * ep.ds;
-#pragma unroll
-            for (int j = 0; j < GEMM_TN; ++j) {
-                int c = cbase + j;
-                if (c < p.Cout) {
-                    int sub = c / ep.dC, co = c - sub * ep.dC;
-                    int dy = sub / ep.ds, dx = sub - dy * ep.ds;
-                    size_t opix = ((size_t)b * ep.dIH * ep.ds + (size_t)iy * ep.ds + dy) * OWd +
-                                  (size_t)ix * ep.ds + dx;
-                    ep.out[opix * ep.out_ld + co] = v[j];
-                }
-            }
+                if (cbase + j < p.Cout) ep.out[out_offset(ep, n, cbase + j, p.Cout)] = v[j];
         }
     }
 }

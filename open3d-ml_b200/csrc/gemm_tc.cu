@@ -38,7 +38,7 @@
 #include "dense.cuh"
 #include "tc.cuh"
 #include <cuda.h>
-#include <algorithm>
+#include <type_traits>
 
 namespace o3dml {
 
@@ -123,9 +123,96 @@ __device__ __forceinline__ const float* table_row(const GemmTcParams& p, int64_t
     return (r < 0 || r >= S.rows) ? nullptr : S.data + (size_t)r * S.ld;
 }
 
-// weighted table mode: the weight of the entry that row n reads in kernel cell `cell` (0 past the last row)
-__device__ __forceinline__ float table_weight(const GemmTcParams& p, int64_t n, int cell) {
-    return n < p.N ? __ldg(p.entry_weight + n * p.weight_ld + cell) : 0.f;
+// table mode: the factor of an entry, its weight in the WEIGHTED instances and a liveness flag in the others
+template <bool WEIGHTED>
+using TableFactor = typename std::conditional<WEIGHTED, float, bool>::type;
+
+// table mode: the factor of the entry that row n reads in kernel cell `cell`, 0 (false) for a shadow entry or past the
+// last row
+template <bool WEIGHTED>
+__device__ __forceinline__ TableFactor<WEIGHTED> table_entry(const GemmTcParams& p, int64_t n, int cell) {
+    if (!table_row(p, n, cell)) return 0;
+    if constexpr (WEIGHTED) return __ldg(p.entry_weight + n * p.weight_ld + cell);
+    else return true;
+}
+
+// table mode: element x of input channel ch as the consumers multiply it, w * relu(pre_scale * x + pre_shift), or w * x
+// without a prologue, 0 past Cin.  w is table_entry's factor; outside the WEIGHTED instances it is a liveness flag and
+// selects, so that a live entry passes exactly act(x) and a shadow one exactly 0 without reading the prologue.
+template <bool WEIGHTED>
+__device__ __forceinline__ float table_prologue(const GemmTcParams& p, float x, int ch, TableFactor<WEIGHTED> w) {
+    if (ch >= p.src[0].channels || (!WEIGHTED && !w)) return 0.f;
+    const float a = p.pre_scale ? fmaxf(fmaf(x, __ldg(p.pre_scale + ch), __ldg(p.pre_shift + ch)), 0.f) : x;
+    return WEIGHTED ? w * a : a;
+}
+
+// The outputs of one CTA: 128 consecutive rows from row0 (rows and table mode), a (1 << lpw) x PH patch of output pixels
+// of image cb from (oy0, ox0) (conv3x3) or a PZ x PY x PX box of output voxels of grid cb from (ox0, oy0, oz0)
+// (conv3x3x3); set_tiles chooses the patch and box shapes
+struct GtTile {
+    int64_t row0;
+    int cb, oy0, ox0, oz0;
+};
+
+__device__ __forceinline__ GtTile gt_tile(const GemmTcParams& p) {
+    GtTile t = {(int64_t)blockIdx.x * GT_ROWS, 0, 0, 0, 0};
+    if (p.mode == 1) {
+        const int per = p.tiles_x * p.tiles_y;
+        t.cb = blockIdx.x / per;
+        const int i = blockIdx.x - t.cb * per;
+        t.oy0 = (i / p.tiles_x) * p.PH;
+        t.ox0 = (i % p.tiles_x) << p.lpw;
+    } else if (p.mode == 2) {
+        const int per = p.tiles_x * p.tiles_y * p.tiles_z;
+        t.cb = blockIdx.x / per;
+        const int i = blockIdx.x - t.cb * per, ixy = i / p.tiles_z;
+        t.oz0 = (i - ixy * p.tiles_z) << p.lpz;
+        t.oy0 = (ixy % p.tiles_y) << p.lpy;
+        t.ox0 = (ixy / p.tiles_y) * (GT_ROWS >> (p.lpz + p.lpy));
+    }
+    return t;
+}
+
+// the output row of row m of the tile, -1 past the output
+template <bool TABLE>
+__device__ __forceinline__ int64_t gt_out_row(const GemmTcParams& p, const GtTile& t, int m) {
+    if (TABLE || p.mode == 0) return t.row0 + m < p.N ? t.row0 + m : -1;
+    if (p.mode == 1) {
+        const int oy = t.oy0 + (m >> p.lpw), ox = t.ox0 + (m & ((1 << p.lpw) - 1));
+        return (oy < p.OH && ox < p.OW) ? ((int64_t)t.cb * p.OH + oy) * p.OW + ox : -1;
+    }
+    const int oz = t.oz0 + (m & ((1 << p.lpz) - 1)), oy = t.oy0 + ((m >> p.lpz) & ((1 << p.lpy) - 1));
+    const int ox = t.ox0 + (m >> (p.lpz + p.lpy));
+    return (ox < p.X && oy < p.Y && oz < p.Z) ? (((int64_t)t.cb * p.X + ox) * p.Y + oy) * p.Z + oz : -1;
+}
+
+// The tensor copy of A slice `sl` into dst: from identity source sidx (rows mode), else from the convolution tap the
+// slice belongs to, the tile shifted by the tap (taps in the order of the weight rows)
+__device__ __forceinline__ void tma_load_a(const GemmTcParams& p, const GtTile& t, int sl, int sidx, uint32_t dst,
+                                           uint64_t* bar) {
+    if (p.mode == 0) {
+        tma_load_2d(dst, &p.mapA[sidx], sl * GT_KS - p.koff[sidx], (int)t.row0, bar);
+        return;
+    }
+    const int spt = p.C / GT_KS;                      // slices per tap
+    const int tap = sl / spt, cc = (sl - tap * spt) * GT_KS;
+    if (p.mode == 2) {   // tap (kx * 3 + ky) * 3 + kz
+        const int dx = tap / 9, dy = (tap - dx * 9) / 3, dz = tap - dx * 9 - dy * 3;
+        tma_load_5d(dst, &p.mapA[0], cc, t.oz0 - 1 + dz, t.oy0 - 1 + dy, t.ox0 - 1 + dx, t.cb, bar);
+        return;
+    }
+    const int dy = tap / 3, dx = tap - dy * 3;
+    if (p.stride == 1) {
+        tma_load_4d(dst, &p.mapA[0], cc, t.ox0 - 1 + dx, t.oy0 - 1 + dy, t.cb, bar);
+    } else {   // input pixel 2*o - 1 + d: odd parity for d = 0 (coordinate o - 1) and d = 2 (o)
+        // A 1-pixel-wide (-high) image has no odd columns (rows), and its odd map is the even one (make_a_maps).  Its
+        // only output column (row) is 0, and tap d = 2 then reads the padding: coordinate -1, as for d = 0, which the
+        // TMA unit fills with zeros.
+        const int py = dy != 1, px = dx != 1;
+        const int x = t.ox0 - (dx == 0 || (dx == 2 && p.W == 1));
+        const int y = t.oy0 - (dy == 0 || (dy == 2 && p.H == 1));
+        tma_load_4d(dst, &p.mapA[py * 2 + px], cc, x, y, t.cb, bar);
+    }
 }
 
 // LITE: two stages instead of 4 - 6, so that TWO CTAs share an SM.  A short product (K <= 512) is mostly
@@ -158,7 +245,7 @@ constexpr int GT_PRODUCER_WARP = 8;
 template <bool GATHER>
 __host__ __device__ constexpr int gt_threads() { return GT_CONV_THREADS + (GATHER ? GT_LOADERS : 32); }
 
-template <int BN, bool GATHER, bool LITE, bool TABLE = false, bool WEIGHTED = false>
+template <int BN, bool GATHER, bool LITE, bool TABLE, bool WEIGHTED>
 __global__ void __launch_bounds__(gt_threads<GATHER>(), LITE ? 2 : 1)
 gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
     static_assert(TABLE || !WEIGHTED, "entry weights belong to table mode");
@@ -179,41 +266,11 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
     const int tid = threadIdx.x;
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // warp-uniform for the compiler
     const int col0 = blockIdx.y * BN;
-    // rows mode: 128 consecutive output rows; conv mode: a PW x PH patch of output pixels of one image; conv3x3x3:
-    // a PZ x PY x PX box of output voxels of one grid
-    int64_t row0 = (int64_t)blockIdx.x * GT_ROWS;
-    int cb = 0, oy0 = 0, ox0 = 0, oz0 = 0;
-    if (p.mode == 1) {
-        const int per = p.tiles_x * p.tiles_y;
-        cb = blockIdx.x / per;
-        const int t = blockIdx.x - cb * per;
-        oy0 = (t / p.tiles_x) * p.PH;
-        ox0 = (t % p.tiles_x) << p.lpw;
-    } else if (p.mode == 2) {
-        const int per = p.tiles_x * p.tiles_y * p.tiles_z;
-        cb = blockIdx.x / per;
-        const int t = blockIdx.x - cb * per, txy = t / p.tiles_z;
-        oz0 = (t - txy * p.tiles_z) << p.lpz;
-        oy0 = (txy % p.tiles_y) << p.lpy;
-        ox0 = (txy / p.tiles_y) * (GT_ROWS >> (p.lpz + p.lpy));
-    }
+    const GtTile tile = gt_tile(p);
+    const int64_t row0 = tile.row0;
 
     // ---- per-row bookkeeping
-    for (int m = tid; m < GT_ROWS; m += blockDim.x) {
-        int64_t n;
-        if (TABLE || p.mode == 0) {
-            n = row0 + m;
-            if (n >= p.N) n = -1;
-        } else if (p.mode == 1) {
-            const int oy = oy0 + (m >> p.lpw), ox = ox0 + (m & ((1 << p.lpw) - 1));
-            n = (oy < p.OH && ox < p.OW) ? ((int64_t)cb * p.OH + oy) * p.OW + ox : -1;
-        } else {
-            const int oz = oz0 + (m & ((1 << p.lpz) - 1)), oy = oy0 + ((m >> p.lpz) & ((1 << p.lpy) - 1));
-            const int ox = ox0 + (m >> (p.lpz + p.lpy));
-            n = (ox < p.X && oy < p.Y && oz < p.Z) ? (((int64_t)cb * p.X + ox) * p.Y + oy) * p.Z + oz : -1;
-        }
-        rown[m] = n;
-    }
+    for (int m = tid; m < GT_ROWS; m += blockDim.x) rown[m] = gt_out_row<TABLE>(p, tile, m);
     for (int i = tid; i < BN; i += blockDim.x) {      // per-column epilogue constants: read once, not per element
         const int c = col0 + i;
         s_scale[i] = (ep.scale && c < p.Cout) ? ep.scale[c] : 1.f;
@@ -259,45 +316,23 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
     if (warp >= GT_PRODUCER_WARP) {
         // ================================================================= TMA producer (+ gather loaders)
         const int rt = tid - GT_CONV_THREADS;                   // loader index; 0 is also the producer
-        if (TABLE) {
-            // loader rt fills 16-byte chunk rt & 7 of rows (rt >> 3) + 16 j; their feature rows change with the cell
-            const float* base[(GT_ROWS * 8) / GT_LOADERS] = {};
+        if (GATHER || rt == 0) {
             if (rt == 0) tma_prefetch_desc(&p.mapB);
-            const int cin = p.src[0].channels;
+            // loader rt fills 16-byte chunk rt & 7 of rows (rt >> 3) + 16 jj; table mode reads the rows of a cell's
+            // table entries at its first slice and keeps them here for the others
+            const float* cell_row[(GT_ROWS * 8) / GT_LOADERS] = {};
+            int sidx = 0;                                       // the source of the slice (rows mode; table mode: 0)
             for (int sl = 0; sl < nsl; ++sl) {
                 const int stage = sl % S, use = sl / S;
                 if (use >= 1) tc::mbar_wait(&empty_bar[stage], (use - 1) & 1);
-                const int ci = sl / spc, j = sl - ci * spc, cell = act[ci];
-                const uint32_t ah = stage0 + (uint32_t)stage * C::STAGE;
-                if (rt == 0) {
-                    const uint32_t bh = ah + GT_A_BYTES;
-                    const int k0 = cell * p.C + j * GT_KS;
-                    mbar_arrive_expect_tx(&full_bar[stage], 2 * C::B_BYTES);
-                    tma_load_2d(bh, &p.mapB, k0, col0, &full_bar[stage]);
-                    tma_load_2d(bh + C::B_BYTES, &p.mapB, k0, p.Npad + col0, &full_bar[stage]);
-                }
-#pragma unroll
-                for (int jj = 0; jj < (GT_ROWS * 8) / GT_LOADERS; ++jj) {
-                    const int item = rt + jj * GT_LOADERS;
-                    const int m = item >> 3, c = item & 7;
-                    if (j == 0) base[jj] = table_row(p, row0 + m, cell);
-                    const int kk = j * GT_KS + c * 4;
-                    const int bytes = base[jj] != nullptr ? 4 * max(0, min(4, cin - kk)) : 0;   // zero past Cin
-                    cp_async16(ah + (uint32_t)m * 128u + (uint32_t)((c ^ (m & 7)) << 4),
-                               bytes ? (const void*)(base[jj] + kk) : (const void*)p.src[0].data, bytes);
-                }
-                cp_async_arrive(&full_bar[stage]);
-            }
-        } else if (GATHER || rt == 0) {
-            if (rt == 0) tma_prefetch_desc(&p.mapB);
-            const int spt = p.mode != 0 ? p.C / GT_KS : 1;      // slices per convolution tap
-            int sidx = 0;
-            for (int sl = 0; sl < nsl; ++sl) {
-                const int stage = sl % S, use = sl / S;
-                if (use >= 1) tc::mbar_wait(&empty_bar[stage], (use - 1) & 1);
-                const int k0 = sl * GT_KS;
-                bool a_tma = true;
-                if (p.mode == 0) {
+                int k0 = sl * GT_KS, j = 0, cell = 0;          // weight row; table mode: slice j of kernel cell `cell`
+                bool a_tma = !TABLE;                            // an identity source or convolution tap
+                if (TABLE) {
+                    const int ci = sl / spc;
+                    j = sl - ci * spc;
+                    cell = act[ci];
+                    k0 = cell * p.C + j * GT_KS;
+                } else if (p.mode == 0) {
                     while (sidx + 1 < p.nsrc && k0 >= p.koff[sidx + 1]) ++sidx;
                     a_tma = p.src[sidx].index == nullptr;
                 }
@@ -307,48 +342,28 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
                     mbar_arrive_expect_tx(&full_bar[stage], 2 * C::B_BYTES + (a_tma ? GT_A_BYTES : 0));
                     tma_load_2d(bh, &p.mapB, k0, col0, &full_bar[stage]);
                     tma_load_2d(bh + C::B_BYTES, &p.mapB, k0, p.Npad + col0, &full_bar[stage]);
-                    if (a_tma) {
-                        if (p.mode == 0) {
-                            tma_load_2d(ah, &p.mapA[sidx], k0 - p.koff[sidx], (int)row0, &full_bar[stage]);
-                        } else if (p.mode == 2) {   // tap (kx * 3 + ky) * 3 + kz, as the weight rows
-                            const int tap = sl / spt, cc = (sl - tap * spt) * GT_KS;
-                            const int dx = tap / 9, dy = (tap - dx * 9) / 3, dz = tap - dx * 9 - dy * 3;
-                            tma_load_5d(ah, &p.mapA[0], cc, oz0 - 1 + dz, oy0 - 1 + dy, ox0 - 1 + dx, cb, &full_bar[stage]);
-                        } else {
-                            const int tap = sl / spt, cc = (sl - tap * spt) * GT_KS;
-                            const int dy = tap / 3, dx = tap - dy * 3;
-                            if (p.stride == 1) {
-                                tma_load_4d(ah, &p.mapA[0], cc, ox0 - 1 + dx, oy0 - 1 + dy, cb, &full_bar[stage]);
-                            } else {   // input pixel 2*o - 1 + d: odd parity for d = 0 (coordinate o - 1) and d = 2 (o)
-                                // A 1-pixel-wide (-high) image has no odd columns (rows), and its odd map is the even
-                                // one (host side).  Its only output column (row) is 0, and tap d = 2 then reads the
-                                // padding: coordinate -1, as for d = 0, which the TMA unit fills with zeros.
-                                const int py = dy != 1, px = dx != 1;
-                                const int x = ox0 - (dx == 0 || (dx == 2 && p.W == 1));
-                                const int y = oy0 - (dy == 0 || (dy == 2 && p.H == 1));
-                                tma_load_4d(ah, &p.mapA[py * 2 + px], cc, x, y, cb, &full_bar[stage]);
-                            }
-                        }
-                    }
+                    if (a_tma) tma_load_a(p, tile, sl, sidx, ah, &full_bar[stage]);
                 }
                 if (!GATHER) continue;
-                if (!a_tma) {
-                    const int kloc = k0 - p.koff[sidx];
-                    const int cs = p.src[sidx].channels;
-#pragma unroll
-                    for (int j = 0; j < (GT_ROWS * 8) / GT_LOADERS; ++j) {     // 8 consecutive lanes = one row's 128 B
-                        const int item = rt + j * GT_LOADERS;
-                        const int m = item >> 3, c = item & 7;
-                        const float* base = rowptr[sidx * GT_ROWS + m];
-                        const int kk = kloc + c * 4;
-                        const bool ok = base != nullptr && kk < cs;
-                        cp_async16(ah + (uint32_t)m * 128u + (uint32_t)((c ^ (m & 7)) << 4),
-                                   ok ? (const void*)(base + kk) : (const void*)p.src[0].data, ok ? 16 : 0);
-                    }
-                    cp_async_arrive(&full_bar[stage]);
-                } else {
+                if (a_tma) {
                     mbar_arrive(&full_bar[stage]);
+                    continue;
                 }
+                const int kloc = TABLE ? j * GT_KS : k0 - p.koff[sidx];   // first channel of the slice in its rows
+                const int cs = p.src[sidx].channels;
+#pragma unroll
+                for (int jj = 0; jj < (GT_ROWS * 8) / GT_LOADERS; ++jj) {     // 8 consecutive lanes = one row's 128 B
+                    const int item = rt + jj * GT_LOADERS;
+                    const int m = item >> 3, c = item & 7;
+                    if (TABLE && j == 0) cell_row[jj] = table_row(p, row0 + m, cell);
+                    const float* base = TABLE ? cell_row[jj] : rowptr[sidx * GT_ROWS + m];
+                    const int kk = kloc + c * 4;
+                    // zero past the channels; a gathered source has a multiple of 4 (o3dml_linear_tc_supported)
+                    const int bytes = base == nullptr || kk >= cs ? 0 : TABLE ? 4 * min(4, cs - kk) : 16;
+                    cp_async16(ah + (uint32_t)m * 128u + (uint32_t)((c ^ (m & 7)) << 4),
+                               bytes ? (const void*)(base + kk) : (const void*)p.src[0].data, bytes);
+                }
+                cp_async_arrive(&full_bar[stage]);
             }
         }
     } else if (warp < GT_PRODUCER_WARP) {
@@ -359,21 +374,17 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
         float acc[ND], racc[ND];
 #pragma unroll
         for (int i = 0; i < ND; ++i) { acc[i] = 0.f; racc[i] = 0.f; }
-        bool live[2] = {true, true};       // table prologue: rows r0 and r0 + 8 read a feature row in this cell
-        float wt[2] = {1.f, 1.f};          // weighted table mode: the entry weights of rows r0 and r0 + 8 in this cell
+        const bool prologue = TABLE && (WEIGHTED || p.pre_scale);
+        TableFactor<WEIGHTED> w[2] = {1, 1};   // table prologue: table_entry of rows r0 and r0 + 8 in this cell
         for (int s = 0; s < nsl; ++s) {
             const int stage = s % S, use = s / S;
             int ch0 = 0;                   // table prologue: first input channel of this slice
-            if (TABLE && (WEIGHTED || p.pre_scale)) {
+            if (prologue) {
                 const int ci = s / spc, j = s - ci * spc;
                 ch0 = j * GT_KS;
                 if (j == 0) {
-                    live[0] = table_row(p, row0 + r0, act[ci]) != nullptr;
-                    live[1] = table_row(p, row0 + r0 + 8, act[ci]) != nullptr;
-                    if (WEIGHTED) {      // a shadow entry weighs zero
-                        wt[0] = live[0] ? table_weight(p, row0 + r0, act[ci]) : 0.f;
-                        wt[1] = live[1] ? table_weight(p, row0 + r0 + 8, act[ci]) : 0.f;
-                    }
+                    w[0] = table_entry<WEIGHTED>(p, row0 + r0, act[ci]);
+                    w[1] = table_entry<WEIGHTED>(p, row0 + r0 + 8, act[ci]);
                 }
             }
             tc::mbar_wait(&full_bar[stage], use & 1);
@@ -388,21 +399,7 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
                     const int r = r0 + (e & 1) * 8, k = ks * 8 + t + (e >> 1) * 4;
                     uint32_t x = *reinterpret_cast<const uint32_t*>(
                         a_tile + r * 128 + (((k >> 2) ^ (r & 7)) << 4) + (k & 3) * 4);
-                    if (WEIGHTED) {
-                        const int ch = ch0 + k;
-                        const float v = __uint_as_float(x);
-                        x = __float_as_uint(ch < p.src[0].channels
-                                                ? wt[e & 1] * (p.pre_scale ? fmaxf(fmaf(v, __ldg(p.pre_scale + ch),
-                                                                                        __ldg(p.pre_shift + ch)), 0.f)
-                                                                           : v)
-                                                : 0.f);
-                    } else if (TABLE && p.pre_scale) {
-                        const int ch = ch0 + k;
-                        x = __float_as_uint(live[e & 1] && ch < p.src[0].channels
-                                                ? fmaxf(fmaf(__uint_as_float(x), __ldg(p.pre_scale + ch),
-                                                             __ldg(p.pre_shift + ch)), 0.f)
-                                                : 0.f);
-                    }
+                    if (prologue) x = __float_as_uint(table_prologue<WEIGHTED>(p, __uint_as_float(x), ch0 + k, w[e & 1]));
                     tc::split_tf32(x, ah[ks][e], al[ks][e]);
                 }
             const uint32_t bh = stage0 + (uint32_t)stage * C::STAGE + GT_A_BYTES, bl = bh + C::B_BYTES;
@@ -458,20 +455,8 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
                     }
                     v.x = apply_act(v.x, ep.act, ep.slope); v.y = apply_act(v.y, ep.act, ep.slope);
                     v.z = apply_act(v.z, ep.act, ep.slope); v.w = apply_act(v.w, ep.act, ep.slope);
-                    float* o;
-                    if (ep.mode == 0) {
-                        o = ep.out + (size_t)nr * ep.out_ld + cg;
-                    } else {
-                        const int64_t per = (int64_t)ep.dIH * ep.dIW;
-                        const int64_t b = nr / per;
-                        const int rr = (int)(nr % per);
-                        const int iy = rr / ep.dIW, ix = rr % ep.dIW;
-                        const int sub = cg / ep.dC, co = cg - sub * ep.dC;
-                        const int dy = sub / ep.ds, dx = sub - dy * ep.ds;
-                        const size_t opix = ((size_t)b * ep.dIH * ep.ds + (size_t)iy * ep.ds + dy) * (ep.dIW * ep.ds) +
-                                            (size_t)ix * ep.ds + dx;
-                        o = ep.out + opix * ep.out_ld + co;
-                    }
+                    __builtin_assume(ep.mode != 1);
+                    float* o = ep.out + out_offset(ep, nr, cg, p.Cout);
                     if (vec && cg + 3 < p.Cout) {
                         *reinterpret_cast<float4*>(o) = v;
                     } else {
@@ -491,21 +476,8 @@ gemm_tc_kernel(const __grid_constant__ GemmTcParams p) {
                 if (n < 0 || c >= p.Cout) continue;
                 float x = stg[r * SLD + cl];
                 if (ep.residual) x += ep.residual[(size_t)n * ep.res_ld + c];
-                x = apply_act(x, ep.act, ep.slope);
-                if (ep.mode == 1) {
-                    const int64_t b = n / ep.plane, pix = n % ep.plane;
-                    ep.out[((size_t)b * p.Cout + c) * ep.plane + pix] = x;
-                } else {
-                    const int64_t per = (int64_t)ep.dIH * ep.dIW;
-                    const int64_t b = n / per;
-                    const int rr = (int)(n % per);
-                    const int iy = rr / ep.dIW, ix = rr % ep.dIW;
-                    const int sub = c / ep.dC, co = c - sub * ep.dC;
-                    const int dy = sub / ep.ds, dx = sub - dy * ep.ds;
-                    const size_t opix = ((size_t)b * ep.dIH * ep.ds + (size_t)iy * ep.ds + dy) * (ep.dIW * ep.ds) +
-                                        (size_t)ix * ep.ds + dx;
-                    ep.out[opix * ep.out_ld + co] = x;
-                }
+                __builtin_assume(ep.mode != 0);
+                ep.out[out_offset(ep, n, c, p.Cout)] = apply_act(x, ep.act, ep.slope);
             }
         }
     }
@@ -544,69 +516,22 @@ static int make_map(CUtensorMap* map, const void* base, int rank, const uint64_t
     return O3DML_OK;
 }
 
-template <int BN, bool GATHER, bool LITE = false, bool TABLE = false, bool WEIGHTED = false>
-static int gemm_tc_launch_bn(const GemmTcParams& p, unsigned grid_x, cudaStream_t st) {
-    using C = GtCfg<BN, LITE>;
-    dim3 grid(grid_x, (unsigned)(p.Npad / BN));
-    O3DML_CUDA(launch<gemm_tc_kernel<BN, GATHER, LITE, TABLE, WEIGHTED>>(grid, gt_threads<GATHER>(), C::SMEM, st, p));
-    return O3DML_OK;
+// The weight image's map: fp32 [2 * Npad][Kpad] (TF32 hi rows, then lo rows), a box of 32 channels x BN columns
+static int make_b_map(GemmTcParams& p, const void* wimg, int bn) {
+    const uint64_t dims[2] = {(uint64_t)p.Kpad, (uint64_t)2 * p.Npad};
+    const uint64_t str[1] = {(uint64_t)p.Kpad * 4};
+    const uint32_t box[2] = {GT_KS, (uint32_t)bn};
+    return make_map(&p.mapB, wimg, 2, dims, str, box);
 }
 
-template <bool WEIGHTED>
-static int gemm_tc_launch_table(const GemmTcParams& p, int bn, unsigned grid_x, cudaStream_t st) {
-    if (bn == 32) return gemm_tc_launch_bn<32, true, false, true, WEIGHTED>(p, grid_x, st);
-    if (bn == 64) return gemm_tc_launch_bn<64, true, false, true, WEIGHTED>(p, grid_x, st);
-    return gemm_tc_launch_bn<128, true, false, true, WEIGHTED>(p, grid_x, st);
-}
-
-constexpr int GT_LITE_MAX_SLICES = 16;   // longest product, in 32-channel k-slices, that runs on the LITE kernels
-
-static int gemm_tc_launch(GemmTcParams& p, const void* wimg, int k_pad, int n_pad, cudaStream_t st) {
-    p.Kpad = k_pad;
-    p.Npad = n_pad;
-    O3DML_CHECK(n_pad >= p.Cout, "linear_tc: weight image has fewer rows than out_channels");
-    if (p.N <= 0 || p.Cout <= 0) return O3DML_OK;
-    O3DML_CHECK(p.Kpad % GT_KS == 0 && p.Kpad >= p.K, "linear_tc: weight image K padding must be a multiple of 32");
-    O3DML_CHECK(p.Npad == 32 || p.Npad == 64 || p.Npad % 128 == 0,
-                "linear_tc: weight image rows must be padded to 32, 64 or a multiple of 128");
-    int bn = p.Npad == 32 ? 32 : (p.Npad == 64 ? 64 : 128);
-    bool any_gather = p.mode == 3;
-    if (p.mode == 0)
-        for (int s = 0; s < p.nsrc; ++s) any_gather = any_gather || p.src[s].index != nullptr;
-    const int sms = device_sm_count();
-    int64_t row_tiles = ceil_div<int64_t>(p.N, GT_ROWS);
-    if (p.mode == 1) {
-        int best_tiles = 1 << 30;
-        for (int l = 0; l <= 7; ++l) best_tiles = std::min(best_tiles, ceil_div(p.OW, 1 << l) * ceil_div(p.OH, GT_ROWS >> l));
-        row_tiles = (p.N / ((int64_t)p.OH * p.OW)) * best_tiles;
-    } else if (p.mode == 2) {
-        row_tiles = (p.N / ((int64_t)p.X * p.Y * p.Z)) * p.tiles_x * p.tiles_y * p.tiles_z;
-    }
-    // products of plain row sources, at most 16 k-slices long, that fill the SMs more than once as 64-column tiles run on
-    // the LITE kernels, two CTAs per SM (GtCfg); the convolutions (K = 9 C, 27 C) stay on the one-CTA-per-SM kernels
-    const bool lite = p.mode == 0 && !any_gather && p.Kpad / GT_KS <= GT_LITE_MAX_SLICES &&
-                      row_tiles * (p.Npad / (bn == 32 ? 32 : 64)) > sms;
-    if (lite && bn == 128) bn = 64;
-    // a grid that fills less than half of the SMs (PointPillars block 3: 27 x 2 CTAs; one cloud per GPU: 6 - 88)
-    // runs as 64-column tiles instead: twice the CTAs, each with half the tensor-core work per slice
-    if (bn == 128 && 2 * row_tiles * (p.Npad / 128) <= sms) bn = 64;
-    {   // weight image: fp32 [2 * Npad][Kpad] (TF32 hi rows, then lo rows)
-        const uint64_t dims[2] = {(uint64_t)p.Kpad, (uint64_t)2 * p.Npad};
-        const uint64_t str[1] = {(uint64_t)p.Kpad * 4};
-        const uint32_t box[2] = {GT_KS, (uint32_t)bn};
-        int rc = make_map(&p.mapB, wimg, 2, dims, str, box);
-        if (rc) return rc;
-    }
-    bool gather = false;
-    unsigned grid_x;
-    if (p.mode == 3) {
-        grid_x = (unsigned)ceil_div<int64_t>(p.N, GT_ROWS);
-        return p.entry_weight ? gemm_tc_launch_table<true>(p, bn, grid_x, st)
-                              : gemm_tc_launch_table<false>(p, bn, grid_x, st);
-    } else if (p.mode == 0) {
-        grid_x = (unsigned)ceil_div<int64_t>(p.N, GT_ROWS);
+// The A operand's maps, whose box is one slice of the CTA's tile: rows mode a 2-D {channels, rows} map per identity
+// source; conv3x3 a 4-D {C, W, H, B} map (stride 1) or one per (row, column) parity of the input (stride 2); conv3x3x3 a
+// 5-D {C, Z, Y, X, B} map.  Gathered sources and table mode have none.
+static int make_a_maps(GemmTcParams& p) {
+    const float* in = p.src[0].data;
+    if (p.mode == 0) {
         for (int s = 0; s < p.nsrc; ++s) {
-            if (p.src[s].index) { gather = true; continue; }
+            if (p.src[s].index) continue;
             const uint64_t rows = (uint64_t)(p.src[s].rows > 0 ? p.src[s].rows : p.N);
             const uint64_t dims[2] = {(uint64_t)p.src[s].channels, rows};
             const uint64_t str[1] = {(uint64_t)p.src[s].ld * 4};
@@ -614,19 +539,45 @@ static int gemm_tc_launch(GemmTcParams& p, const void* wimg, int k_pad, int n_pa
             int rc = make_map(&p.mapA[s], p.src[s].data, 2, dims, str, box);
             if (rc) return rc;
         }
-    } else if (p.mode == 2) {   // the box of output voxels per CTA was chosen by set_conv3x3x3
+    } else if (p.mode == 1) {
+        const int64_t batch = p.N / ((int64_t)p.OH * p.OW);
+        const uint32_t box[4] = {GT_KS, (uint32_t)(1 << p.lpw), (uint32_t)p.PH, 1};
+        if (p.stride == 1) {
+            const uint64_t dims[4] = {(uint64_t)p.C, (uint64_t)p.W, (uint64_t)p.H, (uint64_t)batch};
+            const uint64_t str[3] = {(uint64_t)p.C * 4, (uint64_t)p.W * p.C * 4, (uint64_t)p.H * p.W * p.C * 4};
+            return make_map(&p.mapA[0], in, 4, dims, str, box);
+        }
+        for (int py = 0; py < 2; ++py)
+            for (int px = 0; px < 2; ++px) {
+                const uint64_t wp = (uint64_t)(p.W - px + 1) / 2, hp = (uint64_t)(p.H - py + 1) / 2;
+                if (wp == 0 || hp == 0) {      // no odd columns (rows): the producer reads it at -1 only
+                    p.mapA[py * 2 + px] = p.mapA[0];
+                    continue;
+                }
+                const uint64_t dims[4] = {(uint64_t)p.C, wp, hp, (uint64_t)batch};
+                const uint64_t str[3] = {(uint64_t)2 * p.C * 4, (uint64_t)2 * p.W * p.C * 4, (uint64_t)p.H * p.W * p.C * 4};
+                int rc = make_map(&p.mapA[py * 2 + px], in + ((size_t)py * p.W + px) * p.C, 4, dims, str, box);
+                if (rc) return rc;
+            }
+    } else if (p.mode == 2) {
         const int64_t batch = p.N / ((int64_t)p.X * p.Y * p.Z);
-        grid_x = (unsigned)row_tiles;
         const uint32_t box[5] = {GT_KS, 1u << p.lpz, 1u << p.lpy, (uint32_t)(GT_ROWS >> (p.lpz + p.lpy)), 1};
         const uint64_t dims[5] = {(uint64_t)p.C, (uint64_t)p.Z, (uint64_t)p.Y, (uint64_t)p.X, (uint64_t)batch};
         const uint64_t str[4] = {(uint64_t)p.C * 4, (uint64_t)p.Z * p.C * 4, (uint64_t)p.Y * p.Z * p.C * 4,
                                  (uint64_t)p.X * p.Y * p.Z * p.C * 4};
-        int rc = make_map(&p.mapA[0], p.src[0].data, 5, dims, str, box);
-        if (rc) return rc;
-    } else {
-        // patch of output pixels per CTA: PW x PH = 128, the shape with the fewest tiles
+        return make_map(&p.mapA[0], in, 5, dims, str, box);
+    }
+    return O3DML_OK;
+}
+
+// Chooses the outputs one CTA owns (GtTile) and returns how many CTAs cover the output, batch x tiles per image or grid
+// in the convolutions.  conv3x3: a PW x PH = 128 patch of output pixels, the shape with the fewest patches, on a tie the
+// first with PW >= 8.  conv3x3x3: a PZ x PY x PX = 128 box of output voxels with power-of-two sides, the shape with the
+// fewest boxes, then the most compact one (its 27 shifted copies overlap most in L2), then the longest run along z.
+static int64_t set_tiles(GemmTcParams& p) {
+    if (p.mode == 1) {
         int best = -1, best_tiles = 0;
-        for (int l = 0; l <= 7; ++l) {
+        for (int l = 0; (1 << l) <= GT_ROWS; ++l) {
             const int pw = 1 << l, ph = GT_ROWS >> l;
             const int tiles = ceil_div(p.OW, pw) * ceil_div(p.OH, ph);
             if (best < 0 || tiles < best_tiles || (tiles == best_tiles && pw >= 8 && (1 << best) < 8)) {
@@ -638,43 +589,104 @@ static int gemm_tc_launch(GemmTcParams& p, const void* wimg, int k_pad, int n_pa
         p.PH = GT_ROWS >> best;
         p.tiles_x = ceil_div(p.OW, 1 << best);
         p.tiles_y = ceil_div(p.OH, p.PH);
-        const int64_t batch = p.N / ((int64_t)p.OH * p.OW);
-        grid_x = (unsigned)(batch * p.tiles_x * p.tiles_y);
-        const uint32_t box[4] = {GT_KS, (uint32_t)(1 << best), (uint32_t)p.PH, 1};
-        const float* in = p.src[0].data;
-        if (p.stride == 1) {
-            const uint64_t dims[4] = {(uint64_t)p.C, (uint64_t)p.W, (uint64_t)p.H, (uint64_t)batch};
-            const uint64_t str[3] = {(uint64_t)p.C * 4, (uint64_t)p.W * p.C * 4, (uint64_t)p.H * p.W * p.C * 4};
-            int rc = make_map(&p.mapA[0], in, 4, dims, str, box);
-            if (rc) return rc;
-        } else {
-            for (int py = 0; py < 2; ++py)
-                for (int px = 0; px < 2; ++px) {
-                    const uint64_t wp = (uint64_t)(p.W - px + 1) / 2, hp = (uint64_t)(p.H - py + 1) / 2;
-                    if (wp == 0 || hp == 0) {      // no odd columns (rows): the producer reads it at -1 only
-                        p.mapA[py * 2 + px] = p.mapA[0];
-                        continue;
-                    }
-                    const uint64_t dims[4] = {(uint64_t)p.C, wp, hp, (uint64_t)batch};
-                    const uint64_t str[3] = {(uint64_t)2 * p.C * 4, (uint64_t)2 * p.W * p.C * 4,
-                                             (uint64_t)p.H * p.W * p.C * 4};
-                    int rc = make_map(&p.mapA[py * 2 + px], in + ((size_t)py * p.W + px) * p.C, 4, dims, str, box);
-                    if (rc) return rc;
+        return p.N / ((int64_t)p.OH * p.OW) * p.tiles_x * p.tiles_y;
+    }
+    if (p.mode == 2) {
+        int64_t best_tiles = -1;
+        int best_sum = 0;
+        for (int lz = 0; (1 << lz) <= GT_ROWS; ++lz)
+            for (int ly = 0; (1 << (lz + ly)) <= GT_ROWS; ++ly) {
+                const int pz = 1 << lz, py = 1 << ly, px = GT_ROWS >> (lz + ly);
+                const int64_t tiles = (int64_t)ceil_div(p.Z, pz) * ceil_div(p.Y, py) * ceil_div(p.X, px);
+                const int sum = pz + py + px;
+                if (best_tiles < 0 || tiles < best_tiles || (tiles == best_tiles && sum < best_sum) ||
+                    (tiles == best_tiles && sum == best_sum && lz > p.lpz)) {
+                    best_tiles = tiles;
+                    best_sum = sum;
+                    p.lpz = lz;
+                    p.lpy = ly;
                 }
-        }
+            }
+        p.tiles_z = ceil_div(p.Z, 1 << p.lpz);
+        p.tiles_y = ceil_div(p.Y, 1 << p.lpy);
+        p.tiles_x = ceil_div(p.X, GT_ROWS >> (p.lpz + p.lpy));
+        return p.N / ((int64_t)p.X * p.Y * p.Z) * p.tiles_x * p.tiles_y * p.tiles_z;
     }
-    if (gather) {
-        if (bn == 32) return gemm_tc_launch_bn<32, true>(p, grid_x, st);
-        if (bn == 64) return gemm_tc_launch_bn<64, true>(p, grid_x, st);
-        return gemm_tc_launch_bn<128, true>(p, grid_x, st);
+    return ceil_div<int64_t>(p.N, GT_ROWS);
+}
+
+// An instance of gemm_tc_kernel by its template arguments
+struct GtInstance {
+    int bn;
+    bool gather, lite, table, weighted;
+    bool operator==(const GtInstance& o) const {
+        return bn == o.bn && gather == o.gather && lite == o.lite && table == o.table && weighted == o.weighted;
     }
-    if (lite) {
-        if (bn == 32) return gemm_tc_launch_bn<32, false, true>(p, grid_x, st);
-        return gemm_tc_launch_bn<64, false, true>(p, grid_x, st);
-    }
-    if (bn == 32) return gemm_tc_launch_bn<32, false>(p, grid_x, st);
-    if (bn == 64) return gemm_tc_launch_bn<64, false>(p, grid_x, st);
-    return gemm_tc_launch_bn<128, false>(p, grid_x, st);
+};
+
+constexpr int GT_LITE_MAX_SLICES = 16;   // longest product, in 32-channel k-slices, that runs on the LITE kernels
+
+// The instance for `row_tiles` CTAs per column tile on `sms` SMs.  BN is the weight image's padded width up to 64 and
+// 128 beyond.  Products of plain row sources, at most 16 k-slices long, that fill the SMs more than once as 64-column
+// tiles run on the LITE kernels, two CTAs per SM (GtCfg); the convolutions (K = 9 C, 27 C) stay on the one-CTA-per-SM
+// kernels.  A 128-column grid that fills at most half of the SMs (PointPillars block 3: 27 x 2 CTAs; one cloud per GPU:
+// 6 - 88) runs as 64-column tiles instead: twice the CTAs, each with half the tensor-core work per slice.
+static GtInstance choose_instance(const GemmTcParams& p, int64_t row_tiles, int sms) {
+    GtInstance i = {p.Npad == 32 ? 32 : (p.Npad == 64 ? 64 : 128), p.mode == 3, false, p.mode == 3,
+                    p.entry_weight != nullptr};
+    if (p.mode == 0)
+        for (int s = 0; s < p.nsrc; ++s) i.gather = i.gather || p.src[s].index != nullptr;
+    i.lite = p.mode == 0 && !i.gather && p.Kpad / GT_KS <= GT_LITE_MAX_SLICES &&
+             row_tiles * (p.Npad / (i.bn == 32 ? 32 : 64)) > sms;
+    if (i.lite && i.bn == 128) i.bn = 64;
+    if (i.bn == 128 && 2 * row_tiles * (p.Npad / 128) <= sms) i.bn = 64;
+    return i;
+}
+
+template <int BN, bool GATHER, bool LITE, bool TABLE, bool WEIGHTED>
+static int gemm_tc_launch_bn(const GemmTcParams& p, unsigned grid_x, cudaStream_t st) {
+    using C = GtCfg<BN, LITE>;
+    dim3 grid(grid_x, (unsigned)(p.Npad / BN));
+    O3DML_CUDA(launch<gemm_tc_kernel<BN, GATHER, LITE, TABLE, WEIGHTED>>(grid, gt_threads<GATHER>(), C::SMEM, st, p));
+    return O3DML_OK;
+}
+
+struct GtEntry {
+    GtInstance inst;
+    int (*launch)(const GemmTcParams&, unsigned, cudaStream_t);
+};
+
+template <int BN, bool GATHER, bool LITE, bool TABLE, bool WEIGHTED>
+constexpr GtEntry gt_entry = {{BN, GATHER, LITE, TABLE, WEIGHTED}, gemm_tc_launch_bn<BN, GATHER, LITE, TABLE, WEIGHTED>};
+
+// Every instance that choose_instance can name (tests/gemm_tc_support.py reads this list)
+static const GtEntry GT_INSTANCES[] = {
+    gt_entry<128, false, false, false, false>, gt_entry<64, false, false, false, false>,
+    gt_entry<32, false, false, false, false>,  gt_entry<64, false, true, false, false>,
+    gt_entry<32, false, true, false, false>,   gt_entry<128, true, false, false, false>,
+    gt_entry<64, true, false, false, false>,   gt_entry<32, true, false, false, false>,
+    gt_entry<128, true, false, true, false>,   gt_entry<64, true, false, true, false>,
+    gt_entry<32, true, false, true, false>,    gt_entry<128, true, false, true, true>,
+    gt_entry<64, true, false, true, true>,     gt_entry<32, true, false, true, true>,
+};
+
+static int gemm_tc_launch(GemmTcParams& p, const void* wimg, int k_pad, int n_pad, cudaStream_t st) {
+    p.Kpad = k_pad;
+    p.Npad = n_pad;
+    O3DML_CHECK(n_pad >= p.Cout, "linear_tc: weight image has fewer rows than out_channels");
+    if (p.N <= 0 || p.Cout <= 0) return O3DML_OK;
+    O3DML_CHECK(p.Kpad % GT_KS == 0 && p.Kpad >= p.K, "linear_tc: weight image K padding must be a multiple of 32");
+    O3DML_CHECK(p.Npad == 32 || p.Npad == 64 || p.Npad % 128 == 0,
+                "linear_tc: weight image rows must be padded to 32, 64 or a multiple of 128");
+    const int64_t row_tiles = set_tiles(p);
+    const GtInstance inst = choose_instance(p, row_tiles, device_sm_count());
+    int rc = make_b_map(p, wimg, inst.bn);
+    if (!rc) rc = make_a_maps(p);
+    if (rc) return rc;
+    for (const GtEntry& e : GT_INSTANCES)
+        if (e.inst == inst) return e.launch(p, (unsigned)row_tiles, st);
+    O3DML_FAIL(O3DML_ERR_UNSUPPORTED, "linear_tc: no gemm_tc_kernel instance <%d, %d, %d, %d, %d>", inst.bn,
+               (int)inst.gather, (int)inst.lite, (int)inst.table, (int)inst.weighted);
 }
 
 }  // namespace o3dml
@@ -740,7 +752,7 @@ extern "C" int o3dml_conv3x3x3_ndhwc_tc(const float* in, int batch, int X, int Y
                                         int k_pad, int n_pad, const float* scale, const float* shift, int act,
                                         float slope, float* out, int out_channels, void* stream) {
     GemmTcParams p = {};
-    int rc = set_conv3x3x3("conv3x3x3_tc", p, in, batch, X, Y, Z, C, GT_KS, GT_ROWS);
+    int rc = set_conv3x3x3("conv3x3x3_tc", p, in, batch, X, Y, Z, C, GT_KS);
     if (!rc) rc = set_epilogue("conv3x3x3_tc", p, weight_image, scale, shift, nullptr, 0, act, slope, out, out_channels,
                                out_channels, 0);
     if (rc) return rc;

@@ -1,4 +1,4 @@
-"""The instances of gemm_tc_kernel (open3d-ml_b200/csrc/gemm_tc.cu) and a Python copy of the rule in gemm_tc_launch that
+"""The instances of gemm_tc_kernel (open3d-ml_b200/csrc/gemm_tc.cu) and a Python copy of the rule in choose_instance that
 picks one, so that tests/test_gpu_gemm_tc_matrix.py can derive from the SM count a shape that reaches each instance and
 check from the profiler trace that it did.  Importing this module needs no GPU."""
 import os
@@ -32,20 +32,17 @@ def _arg(tok):
 
 
 def launched_instances(path=os.path.join(CSRC, "gemm_tc.cu")):
-    """Every gemm_tc_launch_bn<...> call in gemm_tc.cu, template defaults filled in, as a sorted list with one entry per
-    call.  A `WEIGHTED` argument is the parameter of gemm_tc_launch_table, which is instantiated for both values."""
+    """The entries of GT_INSTANCES in gemm_tc.cu, the instances gemm_tc_launch dispatches to, as a sorted list with one
+    entry per gt_entry<...>."""
     with open(path) as f:
         src = f.read()
+    table = re.search(r"GT_INSTANCES\[\] = \{(.*?)\};", src, re.S)
+    assert table, "no GT_INSTANCES list in " + path
     found = []
-    for m in re.finditer(r"gemm_tc_launch_bn<([^<>]*)>\s*\(", src):
-        toks = [t.strip() for t in m.group(1).split(",")]
-        choices = [[False, True] if t == "WEIGHTED" else [_arg(t)] for t in toks]
-        assert all(c != [None] for c in choices), "unparsed template arguments: " + m.group(0)
-        combos = [[]]
-        for c in choices:
-            combos = [a + [v] for a in combos for v in c]
-        for a in combos:
-            found.append(inst(*a))
+    for m in re.finditer(r"gt_entry<([^<>]*)>", table.group(1)):
+        args = [_arg(t) for t in m.group(1).split(",")]
+        assert len(args) == 5 and None not in args, "unparsed template arguments: " + m.group(0)
+        found.append(inst(*args))
     return sorted(found)
 
 
@@ -82,19 +79,19 @@ def ceil_div(a, b):
 
 
 def conv3x3_tiles(H, W, stride):
-    """128-pixel patches per image of a 3x3 convolution: the fewest over the patch shapes gemm_tc_launch tries."""
+    """128-pixel patches per image of a 3x3 convolution: the fewest over the patch shapes set_tiles tries."""
     OH, OW = (H - 1) // stride + 1, (W - 1) // stride + 1
     return min(ceil_div(OW, 1 << l) * ceil_div(OH, ROWS >> l) for l in range(8))
 
 
 def conv3x3x3_tiles(X, Y, Z):
-    """128-voxel boxes per grid of a 3x3x3 convolution: the fewest over the box shapes set_conv3x3x3 tries."""
+    """128-voxel boxes per grid of a 3x3x3 convolution: the fewest over the box shapes set_tiles tries."""
     return min(ceil_div(Z, 1 << lz) * ceil_div(Y, 1 << ly) * ceil_div(X, ROWS >> (lz + ly))
                for lz in range(8) for ly in range(8 - lz))
 
 
 def route(row_tiles, cout, k, sms, rows_mode=True, gather=False):
-    """gemm_tc_launch's choice for a product of `row_tiles` 128-row tiles, K = k, `cout` output columns, on `sms` SMs:
+    """choose_instance's choice for a product of `row_tiles` 128-row tiles, K = k, `cout` output columns, on `sms` SMs:
     the padded width is the tile width up to 64 and 128 beyond; short products of plain row sources that fill the SMs
     more than once run on the LITE kernels (64 columns at most); 128-column grids that fill at most half the SMs run as
     64-column tiles."""

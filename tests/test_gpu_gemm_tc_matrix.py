@@ -400,8 +400,8 @@ CASES = {
 
 
 def test_every_instance_has_cases():
-    """The instances gemm_tc.cu launches are the matrix's and the table mode's, one launch site each: adding or removing
-    an instance without its cases fails here."""
+    """The instances gemm_tc.cu launches are the matrix's and the table mode's, one GT_INSTANCES entry each: adding or
+    removing an instance without its cases fails here."""
     assert launched_instances() == sorted(MATRIX_INSTANCES + TABLE_INSTANCES)
     assert sorted({tgt for tgt, _ in CASES.values()}) == MATRIX_INSTANCES
 
