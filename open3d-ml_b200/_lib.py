@@ -1,97 +1,91 @@
 """ctypes binding of libo3dml_b200.so (the C ABI declared in include/o3dml_b200.h).
 
+The argument and result types of every entry are read from the headers, which state them once for nvcc and for this
+binding alike.
+
 There is NO CPU fallback: every entry point needs the CUDA library and a CUDA
 device, and fails loudly otherwise.
 """
 import ctypes
 import math
 import os
+import re
 
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libo3dml_b200.so")
+INCLUDE = os.path.join(os.path.dirname(_HERE), "include")
 _lib = None
-ABI_VERSION = 2
-
-c_void_p, c_int, c_int64, c_float, c_size_t = (ctypes.c_void_p, ctypes.c_int, ctypes.c_int64,
-                                               ctypes.c_float, ctypes.c_size_t)
 
 
 class Src(ctypes.Structure):
     """o3dml_src_t"""
-    _fields_ = [("data", c_void_p), ("index", c_void_p), ("rows", c_int64),
-                ("out_rows_per_batch", c_int64), ("src_rows_per_batch", c_int64),
+    _fields_ = [("data", ctypes.c_void_p), ("index", ctypes.c_void_p), ("rows", ctypes.c_int64),
+                ("out_rows_per_batch", ctypes.c_int64), ("src_rows_per_batch", ctypes.c_int64),
                 ("channels", ctypes.c_int32), ("ld", ctypes.c_int32),
                 ("index_is64", ctypes.c_int32), ("index_ld", ctypes.c_int32)]
 
 
-P, I, L, F, Z = c_void_p, c_int, c_int64, c_float, c_size_t
-_SIGNATURES = {
-    "o3dml_abi_version": (c_int, []),
-    "o3dml_last_error": (ctypes.c_char_p, []),
-    "o3dml_launch_count": (ctypes.c_ulonglong, []),
-    "o3dml_launch_count_add": (None, [ctypes.c_ulonglong]),
-    "o3dml_voxelize_workspace_bytes": (Z, [L, L]),
-    "o3dml_voxelize": (I, [P, L, I, P, L, P, P, P, L, L, P, P, P, P, P, P, P, Z, P]),
-    "o3dml_ragged_to_dense": (I, [P, I, L, P, L, L, L, L, P, P]),
-    "o3dml_knn_workspace_bytes": (Z, [L, L, L]),
-    "o3dml_knn_search": (I, [P, L, P, P, L, P, L, I, P, I, P, P, Z, P]),
-    "o3dml_radius_workspace_bytes": (Z, [L, L, L]),
-    "o3dml_radius_count": (I, [P, L, P, P, L, P, L, F, P, P, P, Z, P]),
-    "o3dml_radius_fill": (I, [P, L, L, P, L, F, P, P, P, P, Z, P]),
-    "o3dml_radius_search_count": (I, [P, L, P, P, L, P, L, F, P, I, I, P, P, P, Z, P]),
-    "o3dml_radius_search_fill": (I, [P, L, L, P, L, F, P, I, I, I, P, P, I, P, P, Z, P]),
-    "o3dml_knn_search_metric_workspace_bytes": (Z, [L, L, L, I, I]),
-    "o3dml_knn_search_metric": (I, [P, L, P, P, L, P, L, I, I, I, P, I, P, P, P, P, Z, P]),
-    "o3dml_voxel_reduce": (I, [P, I, P, I, I, P, P, P, P, L, I, I, P, P, P, P]),
-    "o3dml_reduce_subarrays_sum": (I, [P, P, L, P, P]),
-    "o3dml_sparse_conv_workspace_bytes": (Z, [L]),
-    "o3dml_sparse_conv_neighbors": (I, [P, L, P, L, F, P, P, I, P, P, P, Z, P]),
-    "o3dml_sparse_conv_tc": (I, [L, P, L, I, I, P, I, I, P, P, P, I, I, P, P, P, I, I, F, P, I, I, P]),
-    "o3dml_sparse_conv_weighted_tc": (I, [L, P, L, I, I, P, I, I, P, P, P, I, I, P, P, P, I, I, F, P, I, I, P, I, P]),
-    "o3dml_continuous_conv": (I, [P, I, I, I, I, I, P, L, P, I, P, P, P, L, P, P, I, P, P, I, I, I, I, P, P]),
-    "o3dml_continuous_conv_transpose": (I, [P, I, I, I, I, I, P, L, P, P, I, P, P, P, L, P, P, P, I, P, P, I, I, I, I,
-                                            P, P]),
-    "o3dml_invert_neighbors_list_workspace_bytes": (Z, [L]),
-    "o3dml_invert_neighbors_list": (I, [L, P, I, P, L, L, P, P, P, P, Z, P]),
-    "o3dml_nms_workspace_bytes": (Z, [L]),
-    "o3dml_nms": (I, [P, P, L, F, P, P, P, Z, P]),
-    "o3dml_iou_matrix": (I, [P, L, P, L, I, P, P]),
-    "o3dml_pp_detect_workspace_bytes": (Z, [L, L, L, I, I, L]),
-    "o3dml_pp_detect": (I, [P, L, P, L, P, L, L, L, L, I, I, P, L, F, F, P, P, P, P, P, Z, P]),
-    "o3dml_pp_pfn_scatter": (I, [P, I, I, P, P, P, P, P, L, P, P, P, I, F, F, F, F, I, I, I, P, P,
-                                 I, P]),
-    "o3dml_pp_pfn2_scatter": (I, [P, I, I, P, P, P, P, P, L, P, P, P, P, P, P, I, F, F, F, F, I, I, I, P, P,
-                                  I, P]),
-    "o3dml_linear": (I, [L, ctypes.POINTER(Src), I, P, P, P, P, I, I, F, P, I, I, I, P]),
-    "o3dml_conv3x3_nhwc": (I, [P, I, I, I, I, I, P, P, P, I, F, P, I, P]),
-    "o3dml_deconv_nhwc": (I, [P, I, I, I, I, I, P, P, P, I, F, P, I, I, P]),
-    "o3dml_linear_tc_supported": (I, [ctypes.POINTER(Src), I]),
-    "o3dml_linear_tc": (I, [L, ctypes.POINTER(Src), I, P, I, I, P, P, P, I, I, F, P, I, I, I, P]),
-    "o3dml_conv3x3_nhwc_tc": (I, [P, I, I, I, I, I, P, I, I, P, P, I, F, P, I, P]),
-    "o3dml_deconv_nhwc_tc": (I, [P, I, I, I, I, I, P, I, I, P, P, I, F, P, I, I, P]),
-    "o3dml_randla_lfa_pool": (I, [I, I, P, P, I, I, P, L, L, P, P, P, P, P, P, P, P, P, P]),
-    "o3dml_linear_rows_small_supported": (I, [I, I, I]),
-    "o3dml_linear_rows_small": (I, [L, P, I, P, P, P, I, F, P, I, I, P]),
-    "o3dml_randla_lfa16_pool": (I, [I, P, P, I, I, P, L, L, P, P, P]),
-    "o3dml_randla_lfa_pool_tc": (I, [I, I, P, P, I, I, P, L, L, P, P, P, P, P, P, P, P, P, P]),
-    "o3dml_randla_tail_supported": (I, [I, I, I, I, I, I]),
-    "o3dml_randla_tail": (I, [P, I, P, I, L, P, I, L, L, L, P, P, P, F, I, P, P]),
-    "o3dml_gather_max": (I, [P, L, I, I, P, I, L, I, L, L, I, P, I, P]),
-    "o3dml_kpconv_gather": (I, [P, L, P, L, P, I, I, P, I, P, I, F, P, P]),
-    "o3dml_kpconv_gather_deformable": (I, [P, L, P, L, P, I, I, P, I, P, I, F, P, I, P, P]),
-    "o3dml_pv_voxel_cells": (I, [P, I, I, I, F, P, P, P, P]),
-    "o3dml_pv_cell_mean": (I, [P, P, L, P, I, I, I, P, P]),
-    "o3dml_conv3x3x3_ndhwc_tc": (I, [P, I, I, I, I, I, P, I, I, P, P, I, F, P, I, P]),
-    "o3dml_trilinear_devoxelize": (I, [P, I, I, I, P, I, I, I, P, I, P, P, P]),
-}
-EXPORTS = tuple(_SIGNATURES)           # the product ABI: exactly what include/o3dml_b200.h declares
-# bring-up / profiling hooks (include/o3dml_b200_bringup.h): exported by the library, not part of the product ABI
-_BRINGUP_SIGNATURES = {
-    "o3dml_tc_gemm_test": (I, [P, P, P, I, I, I, P]),
-    "o3dml_tc_mma_rate": (I, [I, I, P, P]),
-}
+_VALUE_TYPES = {"int": ctypes.c_int, "int64_t": ctypes.c_int64, "float": ctypes.c_float, "size_t": ctypes.c_size_t,
+                "unsigned long long": ctypes.c_ulonglong}
+# pointers passed as plain addresses (tensor data_ptr(), host buffers, the stream)
+_ADDRESS_POINTEES = {"float", "void", "int32_t", "int64_t", "int", "long long"}
+_DECLARATION = re.compile(r"O3DML_API\s+([\w\s*]+?)\s*\b(\w+)\s*\(([^()]*)\)\s*;")
+_PARAMETER = re.compile(r"([\w\s*]+?[\s*])(\w+)")
+
+
+def _ctype(c_type, result):
+    """The ctypes type of a C parameter (result=False) or return type; `const` does not matter."""
+    t = re.sub(r"\s*\*", "*", " ".join(re.sub(r"\bconst\b", " ", c_type).split()))
+    if t in _VALUE_TYPES:
+        return _VALUE_TYPES[t]
+    if t == "o3dml_src_t*":
+        return ctypes.POINTER(Src)
+    if t.endswith("*") and t[:-1] in _ADDRESS_POINTEES:
+        return ctypes.c_void_p
+    if result and t == "char*":
+        return ctypes.c_char_p
+    if result and t == "void":
+        return None
+    raise ValueError("open3d_ml_b200: no ctypes type for C %s type %r"
+                     % ("return" if result else "parameter", c_type.strip()))
+
+
+def declarations(header):
+    """[(name, restype, argtypes)] of every `O3DML_API` prototype in a header's text, in declaration order; a name
+    declared twice is listed twice.  A declaration this cannot read, or a type it has no ctypes type for, raises
+    ValueError: nothing is skipped or bound to a guessed type."""
+    code = re.sub(r"/\*.*?\*/|//[^\n]*", " ", header, flags=re.S)
+    code = re.sub(r"^[ \t]*#.*$", "", code, flags=re.M)      # preprocessor lines, `#define O3DML_API` among them
+    out = []
+    for token in re.finditer(r"\bO3DML_API\b", code):
+        m = _DECLARATION.match(code, token.start())
+        if m is None:
+            raise ValueError("open3d_ml_b200: cannot read the declaration %r" % code[token.start():].split(";")[0])
+        ret, name, params = m.groups()
+        args = []
+        if params.strip() != "void":
+            for p in params.split(","):
+                pm = _PARAMETER.fullmatch(p.strip())
+                if pm is None:
+                    raise ValueError("open3d_ml_b200: cannot read parameter %r of %s" % (p.strip(), name))
+                args.append(_ctype(pm.group(1), False))
+        out.append((name, _ctype(ret, True), args))
+    return out
+
+
+def read_header(name):
+    with open(os.path.join(INCLUDE, name)) as f:
+        return f.read()
+
+
+_PRODUCT_HEADER = read_header("o3dml_b200.h")
+ABI_VERSION = int(re.search(r"^#define O3DML_ABI_VERSION (\d+)\s*$", _PRODUCT_HEADER, re.M).group(1))
+_PRODUCT = declarations(_PRODUCT_HEADER)
+EXPORTS = tuple(name for name, _, _ in _PRODUCT)           # the product ABI, in declaration order
+# bring-up / profiling hooks: exported by the library and bound here, not part of the product ABI
+_BRINGUP = declarations(read_header("o3dml_b200_bringup.h"))
 
 
 def lib():
@@ -112,7 +106,7 @@ def lib():
                         "There is no CPU fallback." % (LIB_PATH, e)) from e
                 raise
         h = ctypes.CDLL(LIB_PATH)
-        for name, (res, args) in list(_SIGNATURES.items()) + list(_BRINGUP_SIGNATURES.items()):
+        for name, res, args in _PRODUCT + _BRINGUP:
             fn = getattr(h, name)
             fn.restype, fn.argtypes = res, args
         if h.o3dml_abi_version() != ABI_VERSION:
