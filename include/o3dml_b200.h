@@ -251,7 +251,8 @@ O3DML_API int o3dml_sparse_conv_weighted_tc(int64_t num_out, const float* featur
  *   out[o] = sum_n imp_n * W(map((inp_pos[n] - out_pos[o]) * 2 / extent + offset))^T f[n] over the neighbour list
  *   [neighbors_row_splits[o], neighbors_row_splits[o+1]) of neighbors_index; filters [size_z, size_y, size_x, Cin, Cout];
  *   coordinate_mapping 0 identity / 1 ball_to_cube_radial; interpolation 0 nearest / 1 linear (clamped) /
- *   2 linear_border (zero outside); normalize divides by the sum of the importances (or the neighbour count). */
+ *   2 linear_border (zero outside); normalize divides by the sum of the importances (or the neighbour count).
+ *   out_positions / out may be NULL when num_out == 0, inp_positions / inp_features when num_inp == 0. */
 O3DML_API int o3dml_continuous_conv(const float* filters, int size_x, int size_y, int size_z, int in_channels,
                                     int out_channels, const float* out_positions, int64_t num_out,
                                     const float* extents, int extents_per_point, const float* h_offset,

@@ -46,6 +46,7 @@ struct CConvParams {
     const float* out_importance;      // [num_out] or NULL
     const float* inp_imp_sum;         // [num_inp] or NULL: the normaliser of input n
     const int64_t* inp_row_splits;    // [num_inp + 1] or NULL: the forward lists, whose lengths normalise otherwise
+    float Sf[3];                      // S as floats: the bounds of cconv_corners' clamps, read from the parameters
 };
 
 // s_n of the transposed op: the forward's normaliser of input n, inverted (1 for a zero divisor or without normalize)
@@ -67,10 +68,14 @@ __device__ __forceinline__ int cconv_corners(const CConvParams& p, const float* 
 #pragma unroll
     for (int a = 0; a < 3; ++a)
         u[a] = p.align_corners ? (q[a] + 1.f) * 0.5f * (float)(p.S[a] - 1) : (q[a] + 1.f) * 0.5f * (float)p.S[a] - 0.5f;
+    // A far neighbour's floor(u) can be past the int range, so it is clamped in float before it becomes an int: to
+    // the filter for nearest, to [-2, S] for the linear kinds (both corners outside on either side stay outside).
+    // fmaxf takes a NaN floor to the low end: cell 0 for nearest; both corners outside for the linear kinds, which
+    // linear_border weighs 0 and linear with the NaN weight of the unclamped floor, as the oracle does.
     if (p.interpolation == 0) {
         int c[3];
 #pragma unroll
-        for (int a = 0; a < 3; ++a) c[a] = min(max((int)floorf(u[a] + 0.5f), 0), p.S[a] - 1);
+        for (int a = 0; a < 3; ++a) c[a] = (int)fminf(fmaxf(floorf(u[a] + 0.5f), 0.f), p.Sf[a] - 1.f);
         idx[0] = (c[2] * p.S[1] + c[1]) * p.S[0] + c[0];
         wgt[0] = 1.f;
         return 1;
@@ -80,7 +85,7 @@ __device__ __forceinline__ int cconv_corners(const CConvParams& p, const float* 
 #pragma unroll
     for (int a = 0; a < 3; ++a) {
         const float fl = floorf(u[a]);
-        i0[a] = (int)fl;
+        i0[a] = (int)fminf(fmaxf(fl, -2.f), p.Sf[a]);
         f[a] = u[a] - fl;
     }
     int n = 0;
@@ -193,6 +198,7 @@ static int cconv_run(const char* op, const float* filters, int size_x, int size_
     CConvParams p;
     p.filters = filters;
     p.S[0] = size_x; p.S[1] = size_y; p.S[2] = size_z;
+    for (int a = 0; a < 3; ++a) p.Sf[a] = (float)p.S[a];
     p.cin = in_channels; p.cout = out_channels;
     p.out_pos = out_positions; p.inp_pos = inp_positions; p.inp_feat = inp_features;
     p.inp_importance = TRANSPOSE ? nullptr : importance;
@@ -265,7 +271,9 @@ extern "C" int o3dml_continuous_conv(const float* filters, int size_x, int size_
                                      const float* neighbors_importance, const int64_t* neighbors_row_splits,
                                      int align_corners, int coordinate_mapping, int normalize, int interpolation,
                                      float* out, void* stream) {
-    O3DML_CHECK(filters && out_positions && extents && inp_positions && inp_features && neighbors_row_splits && out,
+    O3DML_CHECK(num_out >= 0 && num_inp >= 0, "continuous_conv: negative size");
+    O3DML_CHECK(filters && extents && neighbors_row_splits && (num_out == 0 || (out_positions && out)) &&
+                    (num_inp == 0 || (inp_positions && inp_features)),
                 "continuous_conv: null input");
     return cconv_run<false>("continuous_conv", filters, size_x, size_y, size_z, in_channels, out_channels, out_positions,
                             num_out, extents, extents_per_point, h_offset, inp_positions, inp_features, num_inp,

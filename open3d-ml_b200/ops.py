@@ -541,8 +541,9 @@ _CCONV_INTERP = {"nearest_neighbor": 0, "linear": 1, "linear_border": 2}
 def _cconv_args(name, filters, out_positions, extents, offset, inp_positions, inp_features, neighbors_index,
                 neighbors_row_splits, coordinate_mapping, interpolation, extents_per_inp):
     """The arguments continuous_conv and its transpose share, checked and on the device: (filters, out_positions,
-    inp_positions, inp_features, extents, host offset, neighbors_index, neighbors_row_splits).  Per-point extents
-    count the outputs, or the inputs when `extents_per_inp` (the transpose, which also refuses them with no input)."""
+    inp_positions, inp_features, extents, host offset, neighbors_index, neighbors_row_splits).  Positions are
+    [N, 3] and inp_features [num_inp, Cin].  Per-point extents count the outputs, or the inputs when
+    `extents_per_inp` (the transpose, which also refuses them with no input)."""
     if coordinate_mapping not in _CCONV_MAPPING:
         raise RuntimeError("%s: coordinate_mapping '%s' is not implemented (identity, ball_to_cube_radial)"
                            % (name, coordinate_mapping))
@@ -550,6 +551,13 @@ def _cconv_args(name, filters, out_positions, extents, offset, inp_positions, in
         raise RuntimeError("%s: unknown interpolation '%s'" % (name, interpolation))
     if filters.dim() != 5:
         raise RuntimeError("%s: filters must have shape [Sz, Sy, Sx, Cin, Cout]" % name)
+    for what, t in (("out_positions", out_positions), ("inp_positions", inp_positions)):
+        if t.dim() != 2 or t.shape[1] != 3:
+            raise RuntimeError("%s: %s must have shape [N, 3], got %s" % (name, what, tuple(t.shape)))
+    if inp_features.dim() != 2 or inp_features.shape[0] != inp_positions.shape[0] or \
+            inp_features.shape[1] != filters.shape[3]:
+        raise RuntimeError("%s: feature channels do not match the filter (inp_features must be [num_inp, Cin])"
+                           % name)
     f = _dev(filters).to(torch.float32).contiguous()
     op, ip = _dev(out_positions).to(torch.float32).contiguous(), _dev(inp_positions).to(torch.float32).contiguous()
     feat = _dev(inp_features).to(torch.float32).contiguous()
@@ -567,21 +575,31 @@ def _cconv_args(name, filters, out_positions, extents, offset, inp_positions, in
     return f, op, ip, feat, ext, off, idx, rs
 
 
+def _cconv_opt(name, t, n, what):
+    """An optional per-point or per-entry float argument of the continuous convolutions: None for None or an empty
+    tensor ("all ones"), else float32 [n] on the device.  The kernels read it by index, so a short one is refused."""
+    if t is None or t.numel() == 0:
+        return None
+    t = _dev(t).float().reshape(-1).contiguous()
+    if t.numel() != n:
+        raise RuntimeError("%s: %s must be empty or have %d elements" % (name, what, n))
+    return t
+
+
 def continuous_conv(filters, out_positions, extents, offset, inp_positions, inp_features, inp_importance,
                     neighbors_index, neighbors_importance, neighbors_row_splits, align_corners=False,
                     coordinate_mapping="ball_to_cube_radial", normalize=False, interpolation="linear",
                     max_temp_mem_MB=64):
     """open3d.ml.torch.ops.continuous_conv (raw op; contract in csrc/cconv.cu).  filters [Sz, Sy, Sx, Cin, Cout];
-    empty importance tensors mean "all ones"; extents [1] or [num_out]."""
+    empty importance tensors mean "all ones", others have num_inp (inp_importance) or one per neighbour entry
+    (neighbors_importance) elements; extents [1] or [num_out]."""
+    name = "continuous_conv"
     f, op, ip, feat, ext, off, idx, rs = _cconv_args(
-        "continuous_conv", filters, out_positions, extents, offset, inp_positions, inp_features, neighbors_index,
+        name, filters, out_positions, extents, offset, inp_positions, inp_features, neighbors_index,
         neighbors_row_splits, coordinate_mapping, interpolation, extents_per_inp=False)
-    imp = None if inp_importance is None or inp_importance.numel() == 0 else _dev(inp_importance).float().contiguous()
-    nimp = (None if neighbors_importance is None or neighbors_importance.numel() == 0
-            else _dev(neighbors_importance).float().contiguous())
+    imp = _cconv_opt(name, inp_importance, ip.shape[0], "inp_importance")
+    nimp = _cconv_opt(name, neighbors_importance, idx.numel(), "neighbors_importance")
     sz, sy, sx, cin, cout = f.shape
-    if feat.shape[1] != cin:
-        raise RuntimeError("continuous_conv: feature channels do not match the filter")
     out = torch.empty((op.shape[0], cout), dtype=torch.float32, device=f.device)
     L.check(L.lib().o3dml_continuous_conv(
         L.ptr(f), sx, sy, sz, cin, cout, L.ptr(op), op.shape[0], L.ptr(ext), 1 if ext.numel() > 1 else 0,
@@ -663,25 +681,15 @@ def continuous_conv_transpose(filters, out_positions, out_importance, extents, o
         name, filters, out_positions, extents, offset, inp_positions, inp_features, neighbors_index,
         neighbors_row_splits, coordinate_mapping, interpolation, extents_per_inp=True)
     num_out, num_inp = op.shape[0], ip.shape[0]
-
-    def opt(t, n, what):
-        if t is None or t.numel() == 0:
-            return None
-        t = _dev(t).float().reshape(-1).contiguous()
-        if t.numel() != n:
-            raise RuntimeError("%s: %s must be empty or have %d elements" % (name, what, n))
-        return t
-    oimp = opt(out_importance, num_out, "out_importance")
-    isum = opt(inp_neighbors_importance_sum, num_inp, "inp_neighbors_importance_sum")
-    nimp = opt(neighbors_importance, neighbors_index.numel(), "neighbors_importance")
+    oimp = _cconv_opt(name, out_importance, num_out, "out_importance")
+    isum = _cconv_opt(name, inp_neighbors_importance_sum, num_inp, "inp_neighbors_importance_sum")
+    nimp = _cconv_opt(name, neighbors_importance, idx.numel(), "neighbors_importance")
     irs = None
     if inp_neighbors_row_splits is not None and inp_neighbors_row_splits.numel():
         irs = _dev(inp_neighbors_row_splits).to(torch.int64).contiguous()
         if irs.numel() != num_inp + 1:
             raise RuntimeError("%s: inp_neighbors_row_splits must have num_inp + 1 elements" % name)
     sz, sy, sx, cin, cout = f.shape
-    if feat.dim() != 2 or feat.shape[0] != num_inp or feat.shape[1] != cin:
-        raise RuntimeError("%s: feature channels do not match the filter" % name)
     out = torch.empty((num_out, cout), dtype=torch.float32, device=f.device)
     L.check(L.lib().o3dml_continuous_conv_transpose(
         L.ptr(f), sx, sy, sz, cin, cout, L.ptr(op), num_out, L.ptr(oimp), L.ptr(ext), 1 if ext.numel() > 1 else 0,

@@ -491,17 +491,24 @@ EXPORT int oracle_continuous_conv(const float *filters, int sx, int sy, int sz, 
                 double w = 1;
                 int inside = 1;
                 for (int a = 0; a < 3; ++a) {
-                    int i;
+                    /* the cell is clamped in double before it becomes an int: a far neighbour's floor(u) can be past
+                     * the int range.  A NaN u fails both comparisons: cell 0, outside the filter (linear_border
+                     * weighs it 0, linear keeps its NaN weight). */
+                    double cell;
                     if (interp == 0) {
-                        i = (int)floor(u[a] + 0.5);
+                        cell = floor(u[a] + 0.5);
                     } else {
                         int bit = (c >> a) & 1;
                         double fl = floor(u[a]);
-                        i = (int)fl + bit;
+                        cell = fl + bit;
                         w *= bit ? (u[a] - fl) : 1 - (u[a] - fl);
                     }
-                    if (i < 0 || i >= S[a]) { inside = 0; i = i < 0 ? 0 : S[a] - 1; }
-                    ii[a] = i;
+                    if (cell >= 0 && cell <= S[a] - 1) {
+                        ii[a] = (int)cell;
+                    } else {
+                        inside = 0;
+                        ii[a] = cell > 0 ? S[a] - 1 : 0;
+                    }
                 }
                 if (interp == 2 && !inside) w = 0;
                 if (w == 0) continue;

@@ -52,11 +52,14 @@ def ref_op(filt, op, oimp, ext, off, ip, feat, isum, fsplits, tidx, nimp, tsplit
 
 
 # ------------------------------------------------------------------------------------------------------ the op
+@pytest.mark.parametrize("cin,cout,n,m", [(6, 10, 200, 600), (129, 640, 40, 60)])
 @pytest.mark.parametrize("index_dtype", [torch.int32, torch.int64])
 @pytest.mark.parametrize("mapping,interp,align,normalize", GRID)
-def test_op_vs_oracle(mapping, interp, align, normalize, index_dtype):
+def test_op_vs_oracle(mapping, interp, align, normalize, index_dtype, cin, cout, n, m):
+    """Cin 129 stages each input row in two passes of the 128-thread CTA and Cout 640 gives each thread 5
+    accumulators; the smaller graph keeps the oracle's [entries, Cin, Cout] gathers small."""
     rng = np.random.default_rng(41)
-    n, m, cin, cout, ext = 200, 600, 6, 10, 0.5
+    ext = 0.5
     ip, op, fidx, fsplits, tidx, tsplits, perm = graph(rng, n, m, ext)
     filt = rng.standard_normal((3, 4, 5, cin, cout)).astype(np.float32)
     feat = rng.standard_normal((n, cin)).astype(np.float32)
@@ -177,6 +180,9 @@ def test_op_refusals():
         call(idx_dtype=torch.int16)
     with pytest.raises(RuntimeError, match="row_splits"):
         call(ts=tsplits[:-1])
+    with pytest.raises(RuntimeError, match=r"inp_positions must have shape \[N, 3\]"):
+        run_op(np.zeros((2, 2, 2, 3, 4), np.float32), op, None, [0.6], [0, 0, 0], np.ascontiguousarray(ip[:, :2]),
+               feat, None, fsplits, tidx, None, tsplits, "identity", "linear", False, False)
 
 
 # ------------------------------------------------------------------------------------------- invert_neighbors_list

@@ -369,46 +369,6 @@ def test_reduce_subarrays_sum_and_voxel_pooling():
     assert np.array_equal(c.pooled_features.numpy(), feats[nn])
 
 
-@pytest.mark.parametrize("mapping,interp,align,normalize", [("identity", "nearest_neighbor", True, False),
-                                                             ("ball_to_cube_radial", "linear", True, True),
-                                                             ("ball_to_cube_radial", "linear_border", False, False),
-                                                             ("identity", "linear", False, True)])
-def test_continuous_conv_op_and_layer_vs_oracle(mapping, interp, align, normalize):
-    import open3d_ml_b200 as M
-    from open3d_ml_b200 import layers as LY
-    from oracle import ops as O
-    rng = np.random.default_rng(21)
-    n, m, cin, cout = 600, 200, 6, 10
-    ip = rng.random((n, 3)).astype(np.float32)
-    op = rng.random((m, 3)).astype(np.float32)
-    feat = rng.standard_normal((n, cin)).astype(np.float32)
-    filt = rng.standard_normal((3, 4, 5, cin, cout)).astype(np.float32)
-    ext = 0.5
-    idx, rs, _ = O.c_radius(ip, op, ext / 2)
-    imp = rng.random(n).astype(np.float32)
-    ref = O.c_continuous_conv(filt, op, [ext], [0.1, 0, -0.1], ip, feat, imp, idx, None, rs, align,
-                              {"identity": 0, "ball_to_cube_radial": 1}[mapping], normalize,
-                              {"nearest_neighbor": 0, "linear": 1, "linear_border": 2}[interp])
-    got = M.ops.continuous_conv(torch.from_numpy(filt).cuda(), torch.from_numpy(op).cuda(), torch.tensor([ext]),
-                                torch.tensor([0.1, 0, -0.1]), torch.from_numpy(ip).cuda(), torch.from_numpy(feat).cuda(),
-                                torch.from_numpy(imp).cuda(), torch.from_numpy(idx).cuda(), torch.empty(0),
-                                torch.from_numpy(rs).cuda(), align, mapping, normalize, interp)
-    assert rel_err(got, ref) < 1e-4
-    with torch.no_grad():
-        layer = LY.ContinuousConv(cin, cout, [3, 3, 3], align_corners=align, coordinate_mapping=mapping,
-                                  interpolation=interp, normalize=normalize, use_bias=True).eval()
-        layer.bias.normal_()
-        out = layer(torch.from_numpy(feat), torch.from_numpy(ip), torch.from_numpy(op), ext)
-        ref2 = O.c_continuous_conv(layer.kernel.numpy(), op, [ext], [0, 0, 0], ip, feat, None, idx, None, rs, align,
-                                   {"identity": 0, "ball_to_cube_radial": 1}[mapping], normalize,
-                                   {"nearest_neighbor": 0, "linear": 1, "linear_border": 2}[interp]) + layer.bias.numpy()
-    assert rel_err(out, ref2) < 1e-4
-    with pytest.raises(RuntimeError):
-        M.ops.continuous_conv(torch.from_numpy(filt), torch.from_numpy(op), torch.tensor([ext]), torch.zeros(3),
-                              torch.from_numpy(ip), torch.from_numpy(feat), None, torch.from_numpy(idx), None,
-                              torch.from_numpy(rs), coordinate_mapping="ball_to_cube_volume_preserving")
-
-
 def test_raw_sparse_conv_op_vs_dense_table():
     import open3d_ml_b200 as M
     from oracle import ops as O

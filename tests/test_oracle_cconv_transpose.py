@@ -1,6 +1,7 @@
 """The float64 oracle of continuous_conv_transpose and invert_neighbors_list, pinned without a GPU: the transposed op
 is the exact adjoint of continuous_conv's oracle, known answers on a lattice and for a constant filter, and the
 inversion against a numpy stable-argsort restatement.  The shim resolves the new names without touching CUDA."""
+import itertools
 import os
 import subprocess
 import sys
@@ -10,6 +11,7 @@ import pytest
 
 from oracle import ops as O
 import cconv_transpose_oracle as R
+from cconv_cases import FAR
 from conftest import ROOT
 
 
@@ -34,11 +36,15 @@ def random_lists(rng, rows, num_points, max_len, bad=0.0):
     return idx, splits
 
 
-def adjoint_gap(rng, mapping, interp, align, normalize, importances, per_point, by_count=False):
-    """(|<z, x> - <y, T(x)>|, sum of |terms|) for one random mirrored pair of graphs."""
+def adjoint_gap(rng, mapping, interp, align, normalize, importances, per_point, by_count=False, far=False):
+    """(|<z, x> - <y, T(x)>|, sum of |terms|) for one random mirrored pair of graphs.  far: the first 18 outputs are
+    moved 1e3, 1e9 and 1e12 out on either side of each axis, so their entries take a border cell or weigh 0."""
     num_inp, num_out, cin, cout = 30, 50, 3, 4
     inp_pos = rng.random((num_inp, 3)).astype(np.float32)
     out_pos = rng.random((num_out, 3)).astype(np.float32)
+    if far:
+        for k, (a, side, mag) in enumerate(itertools.product(range(3), (-1, 1), FAR)):
+            out_pos[k, a] += np.float32(side * mag)
     W = rng.standard_normal((3, 4, 2, cin, cout)).astype(np.float32)
     G = np.ascontiguousarray(W.transpose(0, 1, 2, 4, 3))
     x = rng.standard_normal((num_inp, cin)).astype(np.float32)
@@ -70,9 +76,10 @@ def adjoint_gap(rng, mapping, interp, align, normalize, importances, per_point, 
 @pytest.mark.parametrize("normalize", [False, True])
 def test_transpose_oracle_is_the_adjoint_of_the_forward(interp, mapping, align, normalize):
     rng = np.random.default_rng(100 + 12 * interp + 4 * mapping + 2 * align + normalize)
-    for importances, per_point in ((False, False), (True, False), (True, True)):
-        gap, terms = adjoint_gap(rng, mapping, interp, align, normalize, importances, per_point)
-        assert terms > 0 and gap <= 1e-5 * terms, (importances, per_point, gap, terms)
+    for importances, per_point, far in ((False, False, False), (True, False, False), (True, True, False),
+                                        (True, True, True)):
+        gap, terms = adjoint_gap(rng, mapping, interp, align, normalize, importances, per_point, far=far)
+        assert terms > 0 and gap <= 1e-5 * terms, (importances, per_point, far, gap, terms)
 
 
 def test_adjoint_with_the_neighbour_count_as_normaliser():

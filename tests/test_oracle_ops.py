@@ -6,6 +6,7 @@ import pytest
 
 from oracle import ops as O
 from open3d_ml_b200 import synth
+from cconv_cases import far_neighbours
 
 KITTI = dict(voxel_size=[0.16, 0.16, 4], range_min=[0, -39.68, -3], range_max=[69.12, 39.68, 1])
 
@@ -273,3 +274,17 @@ def test_continuous_conv_oracle_known_answers():
     got = O.c_continuous_conv(np.ascontiguousarray(k.transpose(2, 1, 0, 3, 4)), lp, [2.0], [0, 0, 0], lp, lf, None, idx, None,
                               rs, True, 0, False, 0)
     assert np.abs(got - ref).max() < 1e-4
+
+
+@pytest.mark.parametrize("interp", [0, 1, 2])
+@pytest.mark.parametrize("align", [False, True])
+def test_continuous_conv_oracle_far_neighbours_take_the_border_cell(interp, align):
+    """Neighbours 1e3, 1e9 and 1e12 extents out on either side of each axis: nearest and linear take the border cell
+    on that side and linear_border weighs them 0, however far out they are (a filter coordinate past 2^31 is clamped
+    before it becomes an int)."""
+    for sizes in ((3, 4, 5), (5, 1, 2)):
+        c = far_neighbours(sizes, align, interp)
+        for mapping in (0, 1):
+            got = O.c_continuous_conv(c.filters, c.out_pos, [1.0], [0, 0, 0], c.inp_pos, c.feat, None, c.index, None,
+                                      c.splits, align, mapping, False, interp)
+            assert np.array_equal(got, c.want), (sizes, mapping, got.ravel(), c.want.ravel())
