@@ -3,26 +3,26 @@
 //   3xFP16 split (tc.cuh) -> softmax over the 16 neighbours -> weighted sum  ==> agg [N, d]
 // Same contract as lfa_pool_kernel (lfa.cu); replaces randlanet.py:521-639 as used at :667-692.
 //
-// One tile = 128 neighbour rows = 8 points x 16 neighbours, 256 threads = two warpgroups of 64 rows:
-//   A  [128 x d]  : X = [feat[nbr] | r1 or r2], built by the CTA in shared memory directly in the
-//                   chunk-major layout (one conflict-free 16-byte store per (row, 8 channels)),
-//                   as fp16 hi/lo pairs.  In stage 2 the first half of A first holds r1 (the A
-//                   operand of the lse2 GEMM) and is then overwritten by the gathered features.
-//   B  [d x d]    : score weight, host-packed hi/lo operand image; resident in shared memory for
-//                   d <= 128, streamed for d = 256 through a ring of two 32-row column blocks filled by bulk
-//                   copies (mbarrier completion), one tile's blocks after the other's
-//   D             : CB score columns per block (64 for d = 64 / 128, 32 for d = 256, d below), each warpgroup's
-//                   [64 x CB] block in registers; block j + 1 is issued into a second accumulator set before the
-//                   epilogue of block j runs (wait_group 1)
-// Epilogue on the accumulator registers: warp w of a warpgroup holds rows [16w, 16w + 16) = the 16 neighbours of one
-// point, a thread rows g and g + 8 of its column pairs.  Column max and the sums of e and e.x over the 16 rows: the two
-// rows in registers, then the 8 lanes sharing lane % 4 (max: butterfly; sums: reduce-scatter, so that the lanes store
-// distinct columns of the point's agg row).  x = hi + lo is read from A at (row, column pair), one conflict-free 4-byte
-// load per operand.
-// Stage 2 chains a second GEMM (r2 = lrelu(BN(Wl2 . r1)), N = d/2) whose epilogue writes r2 from the registers into
-// A (d = 16: that 8x8 product stays in registers).  The score bias is not applied: it is constant over the neighbours of
-// a point and cancels in the softmax.  CTAs are persistent over tiles.  Two tiles are in flight per SM at d = 64 (two
-// CTAs) and d = 128 (two A tiles in one CTA: tile t+1 is built while tile t's score MMAs run).
+// One tile = 128 neighbour rows = 8 points x 16 neighbours, 256 threads = two warpgroups of 64 rows (4 points each).
+//   X  [128 x d]  : [feat[nbr] | r1 or r2], built by the CTA in shared memory directly in the chunk-major layout (one
+//                   conflict-free 16-byte store per (row, 8 channels)), as fp16 hi/lo pairs.  In stage 2 the first
+//                   half of X first holds r1 (the A operand of the lse2 GEMM) and is then overwritten by the gathered
+//                   features.
+//   Ws [d x d]    : score weight, host-packed hi/lo operand image [d/8][d][8]; resident in shared memory for d <= 128
+//                   (d = 16, 32: zero rows up to 64), streamed for d = 256 through a ring of four 64-row x 64-k chunks
+//                   filled by bulk copies (mbarrier completion), one slab's chunks after the other's
+// The score product is computed channel-major, S^T = Ws . X^T: warpgroup w multiplies each 64-row slab s of Ws (the A
+// operand) by its 64 rows of X (the B operand) into a [64 channels x 64 neighbour rows] accumulator (m64n64k16);
+// slab s + 1 is issued into a second accumulator set before the epilogue of slab s runs.
+// Epilogue on the accumulator registers: a thread holds channels g and g + 8 of the warp's 16 and, for each of the
+// warpgroup's 4 points, neighbours 8q + 2t + {0, 1} (q = 0, 1): a point's 16 neighbours are 4 registers x the 4 lanes of
+// a quad.  Max and the sums of e and e.x over them: the 4 registers, then lane bits 0 and 1 (max: butterfly; sums:
+// reduce-scatter, after which lane t holds point t).  x = hi + lo comes from X by ldmatrix.trans, whose fragment
+// (channel g, neighbours 2t, 2t + 1) is the accumulator's.
+// Stage 2 chains a second GEMM (r2 = lrelu(BN(Wl2 . r1)), N = d/2) in the row-major orientation, whose epilogue writes r2
+// from the registers into X (d = 16: that 8x8 product stays in registers).  The score bias is not applied: it is
+// constant over the neighbours of a point and cancels in the softmax.  CTAs are persistent over tiles.  Two tiles are in
+// flight per SM at d = 64 (two CTAs).
 #include "../../include/o3dml_b200.h"
 #include "common.cuh"
 #include "tc.cuh"
@@ -57,50 +57,56 @@ struct LtcCfg {
     static constexpr bool MMA2 = STAGE == 2 && H >= 16;  // lse2 on the tensor core
     static constexpr int NTH = 256;                  // threads per CTA: two warpgroups
     static constexpr int NPART = NTH / LTC_ROWS;     // threads sharing one row
-    // score columns per block: 64 where the weight is resident, 32 where it streams through the ring (two 64-column
-    // slots would not fit next to the 128 KB A tile)
-    static constexpr int CB = D < 64 ? D : (STREAM ? 32 : 64);
-    static constexpr int NBLK = D / CB;
+    static constexpr int NS = D < 64 ? 1 : D / 64;   // score-channel slabs of 64 weight rows
+    static constexpr int WROWS = NS * 64;            // rows of the weight in shared memory (d < 64: zero rows up to 64)
+    // streamed weight: a slab in chunks of 64 k, one ring slot each (hi, then lo); the ring holds one slab
+    static constexpr int KCH = 64;
+    static constexpr int NKC = STREAM ? D / KCH : 1;
+    static constexpr int CHUNK_HALF = KCH / 8 * 64 * 16;
     static constexpr int CB2 = STREAM ? 32 : (H < 64 ? H : 64);  // lse2 columns per block
     static constexpr int A_BYTES = D / 8 * LTC_ROWS * 16;  // one of hi / lo
-    static constexpr int SLOT_BYTES = D / 8 * CB * 16;     // one of hi / lo of one streamed column block
-    static constexpr int B_BYTES = STREAM ? 2 * SLOT_BYTES : D / 8 * D * 16;  // per hi / lo; streamed: two ring slots
+    static constexpr int W_HALF = STREAM ? CHUNK_HALF : D / 8 * WROWS * 16;  // lo behind hi (resident image, ring slot)
+    static constexpr int W_BYTES = NKC * 2 * W_HALF;
     static constexpr int B2_BYTES = MMA2 ? (STREAM ? H / 8 * CB2 * 16 : H / 8 * H * 16) : 0;
     static constexpr int W10_BYTES = 12 * H * 4;
     static constexpr int ST2_BYTES = STAGE == 2 ? (2 * H + (H < 16 ? H * H : 0)) * 4 : 0;
-    // Two tiles in flight per SM, so that the SIMT build of one tile overlaps the score MMAs of the other: d = 64 as two
-    // CTAs per SM (<= 128 registers), d = 128 as two A tiles in one CTA (the CTA builds tile t+1 into one while the
-    // tensor core works on tile t in the other).  d = 256 has room for neither.
+    // Two tiles in flight per SM at d = 64, as two CTAs (<= 128 registers), so that the SIMT build of one tile overlaps
+    // the score MMAs of the other.  d = 128 and 256 have room for one.
     static constexpr int MIN_CTAS = D == 64 ? 2 : 1;
-    static constexpr bool DBUF = D == 128;
-    static constexpr int NBUF = DBUF ? 2 : 1;
-    static constexpr size_t SMEM = NBUF * 2 * A_BYTES + 2 * B_BYTES + 2 * B2_BYTES + W10_BYTES + ST2_BYTES + 16 + 128;
+    static constexpr size_t SMEM = 2 * A_BYTES + W_BYTES + 2 * B2_BYTES + W10_BYTES + ST2_BYTES + 8 * NKC + 128;
 };
 
-// Issues (does not wait for) the warpgroup's 64 rows of A[128 x K] times a block of CBN rows of B (both hi / lo,
-// chunk-major) -> d[CBN / 2], as one committed wgmma group
-template <int CBN, int K>
-__device__ __forceinline__ void ltc_issue(float* d, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
-                                          uint32_t b_lbo, int wg) {
-    constexpr uint32_t A_LBO = LTC_ROWS * 16;
-    a_hi += (uint32_t)wg * 64 * 16;
-    a_lo += (uint32_t)wg * 64 * 16;
+// Issues (does not wait for) D[64 x N] (+)= A[64 x K] . B[N x K]^T -> d[N / 2] as one committed wgmma group.  Each
+// operand is a hi / lo pair of chunk-major images addressed at its first row (rows 16 bytes apart, 8-k chunks lbo
+// apart); the three products of the split run in the order hi.hi, hi.lo, lo.hi.  With `acc` the group adds to d.  SET
+// overwrites d without reading it: its old values need not be live (the score accumulators, two sets of 32 registers,
+// would otherwise stay live across the tile build).
+template <int N, int K, bool SET = false>
+__device__ __forceinline__ void ltc_issue(float* d, uint32_t a_hi, uint32_t a_lo, uint32_t a_lbo, uint32_t b_hi,
+                                          uint32_t b_lo, uint32_t b_lbo, bool acc) {
+    if (!SET) {
 #pragma unroll
-    for (int i = 0; i < CBN / 2; ++i) tc::fence_operand(d[i]);
+        for (int i = 0; i < N / 2; ++i) tc::fence_operand(d[i]);
+    }
     tc::wgmma_fence();
 #pragma unroll
     for (int ks = 0; ks < K / 16; ++ks) {
-        const uint64_t ah = tc::smem_desc(a_hi + ks * 2 * A_LBO, A_LBO, 128);
-        const uint64_t al = tc::smem_desc(a_lo + ks * 2 * A_LBO, A_LBO, 128);
+        const uint64_t ah = tc::smem_desc(a_hi + ks * 2 * a_lbo, a_lbo, 128);
+        const uint64_t al = tc::smem_desc(a_lo + ks * 2 * a_lbo, a_lbo, 128);
         const uint64_t bh = tc::smem_desc(b_hi + ks * 2 * b_lbo, b_lbo, 128);
         const uint64_t bl = tc::smem_desc(b_lo + ks * 2 * b_lbo, b_lbo, 128);
-        tc::wgmma_f16_ss<CBN>(d, ah, bh, ks > 0);
-        tc::wgmma_f16_ss<CBN>(d, ah, bl, 1u);
-        tc::wgmma_f16_ss<CBN>(d, al, bh, 1u);
+        if constexpr (SET) {
+            if (ks == 0) tc::wgmma_f16_ss_set<N>(d, ah, bh);
+            else tc::wgmma_f16_ss<N>(d, ah, bh, 1u);
+        } else {
+            tc::wgmma_f16_ss<N>(d, ah, bh, acc || ks > 0);
+        }
+        tc::wgmma_f16_ss<N>(d, ah, bl, 1u);
+        tc::wgmma_f16_ss<N>(d, al, bh, 1u);
     }
     tc::wgmma_commit();
 #pragma unroll
-    for (int i = 0; i < CBN / 2; ++i) tc::fence_operand(d[i]);
+    for (int i = 0; i < N / 2; ++i) tc::fence_operand(d[i]);
 }
 
 // Waits until at most N of this warpgroup's wgmma groups are pending; d (the oldest group's accumulators) is then final
@@ -111,54 +117,60 @@ __device__ __forceinline__ void ltc_wait(float* d) {
     for (int i = 0; i < CNT; ++i) tc::fence_operand(d[i]);
 }
 
-// One bulk copy (TMA) per (hi / lo, 8-row k chunk) of column block nb of a weight image [K/8][NIMG][8] (hi, then lo)
-// into a ring slot [hi | lo] of [K/8][CBN][8] each, completing on bar.  Every thread of the CTA runs it and the lanes of
-// the warp with `issuer` set issue the copies: the instructions are predicated rather than branched around, because a
-// divergent branch while a wgmma group is in flight makes ptxas serialize the wgmma instructions.
-template <int CBN, int K, int NIMG>
-__device__ __forceinline__ void ltc_fill(uint8_t* slot, uint64_t* bar, const uint4* __restrict__ img, int nb, int lane,
-                                         bool issuer) {
-    constexpr uint32_t ROW = CBN * 16, HALF = K / 8 * ROW;
+// One bulk copy (TMA) per (hi / lo, 8-k chunk) of chunk kc (k in [KCH kc, KCH kc + KCH)) of the 64 rows of slab s of
+// the score weight image [D/8][D][8] (hi, then lo) into a ring slot [hi | lo] of [KCH/8][64][8] each, completing on
+// bar.  Every thread of the CTA runs it and the lanes of the warp with `issuer` set issue the copies: the instructions
+// are predicated rather than branched around, because a divergent branch while a wgmma group is in flight makes ptxas
+// serialize the wgmma instructions.
+template <int D, int KCH>
+__device__ __forceinline__ void ltc_fill(uint8_t* slot, uint64_t* bar, const uint4* __restrict__ img, int s, int kc,
+                                         int lane, bool issuer) {
+    constexpr uint32_t ROW = 64 * 16, HALF = KCH / 8 * ROW;
+    constexpr int NCP = 2 * (KCH / 8);
+    static_assert(NCP <= 32, "one copy per lane");
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t"
                  "@p mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n\t}" ::"r"(tc::smem_u32(bar)),
                  "r"(2 * HALF), "r"((int)(issuer && lane == 0))
                  : "memory");
-#pragma unroll
-    for (int i0 = 0; i0 < 2 * (K / 8); i0 += 32) {
-        const int i = i0 + lane, im = i / (K / 8), kc = i % (K / 8);
-        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                     "@p cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n\t}"
-                     ::"r"(tc::smem_u32(slot + im * HALF + kc * ROW)),
-                     "l"(img + ((size_t)im * (K / 8) + kc) * NIMG + nb * CBN), "r"(ROW), "r"(tc::smem_u32(bar)),
-                     "r"((int)(issuer && i < 2 * (K / 8)))
-                     : "memory");
+    const int im = lane / (KCH / 8), k8 = lane % (KCH / 8);
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
+                 "@p cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n\t}"
+                 ::"r"(tc::smem_u32(slot + (im & 1) * HALF + k8 * ROW)),
+                 "l"(img + ((size_t)(im & 1) * (D / 8) + kc * (KCH / 8) + k8) * D + s * 64), "r"(ROW),
+                 "r"(tc::smem_u32(bar)), "r"((int)(issuer && lane < NCP))
+                 : "memory");
+}
+
+// With NKC wgmma groups pending, runs f(kc) for kc = KC .. NKC - 1, each as soon as group kc has completed
+// (wait_group NKC - 1 - kc)
+template <int KC, int NKC, class F>
+__device__ __forceinline__ void ltc_release(F&& f) {
+    if constexpr (KC < NKC) {
+        tc::wgmma_wait<NKC - 1 - KC>();
+        f(KC);
+        ltc_release<KC + 1, NKC>(f);
     }
 }
 
-// Column sums of one score block over the 16 rows (neighbours) of the warp's point, reduce-scattered over the 8 lanes
-// that share lane % 4 (lane bits 4, 3, 2).  a[i], b[i] hold column 8 (i / 2) + 2 (lane % 4) + i % 2 of the block;
-// afterwards a[0 .. CNT), b[0 .. CNT) hold columns i = base + k (same mapping) summed over all 16 rows, with
-// CNT = max(CNT0 / 8, 1).  Trip counts are template parameters so that a and b stay in registers.
+// Sums over the 4 lanes of a quad (lane bits 1, 0; call with BIT = 2) as a reduce-scatter: a[i], b[i] hold this lane's
+// partial of pair i; afterwards a[0 .. CNT), b[0 .. CNT) hold pairs base + k summed over the quad, with
+// CNT = CNT0 / 4 (CNT0 >= 4).  Each pair's sum is (v0 + v2) + (v1 + v3) of the lanes' partials, whichever lane ends up
+// with it.  Trip counts are template parameters so that a and b stay in registers.
 template <int CNT, int BIT>
 __device__ __forceinline__ void ltc_reduce_scatter(float* a, float* b, int lane, int& base) {
-    if constexpr (BIT >= 4) {
-        if constexpr (CNT > 1) {
-            constexpr int h = CNT / 2;
-            const bool up = (lane & BIT) != 0;
+    if constexpr (BIT >= 1) {
+        static_assert(CNT > 1, "one pair per lane and bit at least");
+        constexpr int h = CNT / 2;
+        const bool up = (lane & BIT) != 0;
 #pragma unroll
-            for (int i = 0; i < h; ++i) {
-                const float ra = __shfl_xor_sync(0xffffffffu, up ? a[i] : a[i + h], BIT);
-                const float rb = __shfl_xor_sync(0xffffffffu, up ? b[i] : b[i + h], BIT);
-                a[i] = (up ? a[i + h] : a[i]) + ra;
-                b[i] = (up ? b[i + h] : b[i]) + rb;
-            }
-            base += up ? h : 0;
-            ltc_reduce_scatter<h, BIT / 2>(a, b, lane, base);
-        } else {
-            a[0] += __shfl_xor_sync(0xffffffffu, a[0], BIT);
-            b[0] += __shfl_xor_sync(0xffffffffu, b[0], BIT);
-            ltc_reduce_scatter<1, BIT / 2>(a, b, lane, base);
+        for (int i = 0; i < h; ++i) {
+            const float ra = __shfl_xor_sync(0xffffffffu, up ? a[i] : a[i + h], BIT);
+            const float rb = __shfl_xor_sync(0xffffffffu, up ? b[i] : b[i + h], BIT);
+            a[i] = (up ? a[i + h] : a[i]) + ra;
+            b[i] = (up ? b[i + h] : b[i]) + rb;
         }
+        base += up ? h : 0;
+        ltc_reduce_scatter<h, BIT / 2>(a, b, lane, base);
     }
 }
 
@@ -166,11 +178,11 @@ template <int D, int STAGE>
 __global__ void __launch_bounds__(LtcCfg<D, STAGE>::NTH, LtcCfg<D, STAGE>::MIN_CTAS)
 lfa_pool_tc_kernel(const __grid_constant__ LfaTcParams p) {
     using C = LtcCfg<D, STAGE>;
-    constexpr int H = C::H, NTH = C::NTH, NPART = C::NPART, CB = C::CB, CB2 = C::CB2;
+    constexpr int H = C::H, NTH = C::NTH, NPART = C::NPART, NS = C::NS, NKC = C::NKC, CB2 = C::CB2;
     extern __shared__ __align__(128) uint8_t smem[];
-    // A buffer i: hi at smem + 2 i A_BYTES, lo right behind it
-    uint8_t* b_sm = smem + C::NBUF * 2 * C::A_BYTES;  // [hi | lo] resident score weight, or two ring slots [hi | lo] each
-    uint8_t* b2_sm = b_sm + 2 * C::B_BYTES;                           // [hi | lo] lse2 weight (or one column block)
+    // X tile: hi at smem, lo right behind it
+    uint8_t* w_sm = smem + 2 * C::A_BYTES;  // [hi | lo] resident score weight, or NKC ring slots [hi | lo] each
+    uint8_t* b2_sm = w_sm + C::W_BYTES;                               // [hi | lo] lse2 weight (or one column block)
     float* W10 = reinterpret_cast<float*>(b2_sm + 2 * C::B2_BYTES);  // [12][H]
     float* ST2 = W10 + 12 * H;                                       // [2][H] (+ Wl2^T [H][H] for H < 16)
     uint64_t* ring_full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(W10) + C::W10_BYTES + C::ST2_BYTES);
@@ -178,16 +190,17 @@ lfa_pool_tc_kernel(const __grid_constant__ LfaTcParams p) {
     const int tid = threadIdx.x, lane = tid & 31;
     const int row = tid & (LTC_ROWS - 1);   // neighbour row of the tile this thread works on
     const int half = tid >> 7;              // which part of the channels / columns (0 .. NPART-1)
-    // accumulator fragment of this thread (tc.cuh): rows r0 and r0 + 8 of the tile, i.e. neighbours g and g + 8 of point
-    // wg * 4 + warp of the tile
+    // accumulator fragment of this thread in the lse2 product (tc.cuh): rows r0 and r0 + 8 of the tile
     const int wg = tid >> 7, g = lane >> 2, t = lane & 3;
     const int r0 = wg * 64 + ((tid >> 5) & 3) * 16 + g;
-    const int pt = r0 >> 4;
 
     // ---- once per CTA: resident weights and the small per-channel constants
     if (!C::STREAM) {
-        for (int i = tid; i < 2 * C::B_BYTES / 16; i += NTH)
-            reinterpret_cast<uint4*>(b_sm)[i] = p.ws_img[i];
+        // [hi | lo][D/8][WROWS][8] from the image [hi | lo][D/8][D][8]; rows past d (d < 64) are zero
+        for (int i = tid; i < C::W_BYTES / 16; i += NTH) {
+            const int r = i % C::WROWS, kc = i / C::WROWS;
+            reinterpret_cast<uint4*>(w_sm)[i] = r < D ? p.ws_img[kc * D + r] : make_uint4(0u, 0u, 0u, 0u);
+        }
         if (C::MMA2)
             for (int i = tid; i < 2 * C::B2_BYTES / 16; i += NTH)
                 reinterpret_cast<uint4*>(b2_sm)[i] = p.wl2_img[i];
@@ -205,26 +218,28 @@ lfa_pool_tc_kernel(const __grid_constant__ LfaTcParams p) {
         W10[10 * H + i] = p.s10[i];
         W10[11 * H + i] = p.t10[i];
     }
-    // streamed score weight: a ring of two column blocks, filled by bulk copies.  The ring runs over the block sequence
-    // 0 .. NBLK-1 of every tile in turn, so blocks 0 and 1 of the next tile are in flight during this tile's last blocks.
-    uint32_t ring_phase = 0;                // bit s: parity of the next completion of slot s
+    // streamed score weight: slot kc of the ring holds chunk kc of a slab.  The ring runs over the slabs 0 .. NS-1 of
+    // every tile in turn, all slots completing once per slab, so one parity serves them all; slab 0 of the next tile
+    // arrives while this tile's last slab is worked on.
+    uint32_t ring_phase = 0;
     if (C::STREAM && tid == 0) {
-        tc::mbar_init(&ring_full[0], 1);
-        tc::mbar_init(&ring_full[1], 1);
+        for (int kc = 0; kc < NKC; ++kc) tc::mbar_init(&ring_full[kc], 1);
         tc::fence_mbar_init();
     }
     tc::fence_async_smem();
     __syncthreads();
     if (C::STREAM) {
-        ltc_fill<CB, D, D>(b_sm, &ring_full[0], p.ws_img, 0, lane, tid < 32);
-        ltc_fill<CB, D, D>(b_sm + 2 * C::SLOT_BYTES, &ring_full[1], p.ws_img, 1, lane, tid < 32);
+#pragma unroll
+        for (int kc = 0; kc < NKC; ++kc)
+            ltc_fill<D, C::KCH>(w_sm + kc * 2 * C::W_HALF, &ring_full[kc], p.ws_img, 0, kc, lane, tid < 32);
     }
 
     // The gathers are software-pipelined over tiles (d >= 64): the neighbour index of tile t+2 and the
     // coordinates / feature rows of tile t+1 are requested while tile t is worked on and land behind its
     // MMAs and epilogue (two dependent global round trips leave the per-tile critical path).  d = 256 holds 64
-    // feature registers per tile: there the requests for tile t+1 go out after the rows of tile t have been stored
-    // (LATE) and the index stays a raw loaded word until its tile comes up (RAW_INDEX, common.cuh RawIndex).  The
+    // feature registers per tile, which do not fit next to the two 32-register score accumulator sets: there the
+    // requests for tile t+1 go out once the last score slab's MMAs are done, behind its softmax (LATE), and the index
+    // stays a raw loaded word until its tile comes up (RAW_INDEX, common.cuh RawIndex).  The
     // resident-weight kernels resolve the index of tile t+2 right behind its load.
     constexpr bool PREF = D >= 64;
     constexpr bool LATE = C::STREAM;
@@ -425,8 +440,8 @@ lfa_pool_tc_kernel(const __grid_constant__ LfaTcParams p) {
                 }
                 const uint32_t bh = tc::smem_u32(b2_sm) + (C::STREAM ? 0u : (uint32_t)blk * CB2 * 16);
                 float d2[CB2 / 2];
-                ltc_issue<CB2, H>(d2, tc::smem_u32(a_hi), tc::smem_u32(a_lo), bh, bh + C::B2_BYTES,
-                                  (C::STREAM ? CB2 : H) * 16, wg);
+                ltc_issue<CB2, H>(d2, tc::smem_u32(a_hi) + wg * 64 * 16, tc::smem_u32(a_lo) + wg * 64 * 16,
+                                  LTC_ROWS * 16, bh, bh + C::B2_BYTES, (C::STREAM ? CB2 : H) * 16, false);
                 ltc_wait<0, CB2 / 2>(d2);
                 // r2 = lrelu(BN(.)) of the fragment, split, straight from the registers into channels [H, D) of A
 #pragma unroll
@@ -450,83 +465,80 @@ lfa_pool_tc_kernel(const __grid_constant__ LfaTcParams p) {
             __syncthreads();   // every lse2 MMA has read r1
         }
         store_features();      // (overwrites r1 in stage 2)
-        if (PREF && LATE) advance(tile);     // lands behind the score GEMM and the epilogue
         tc::fence_async_smem();
     };
 
-    // ---------------- scores = X . Ws^T on the tensor core, CB columns per block; block j + 1 is issued before the
-    // softmax over the 16 rows of the point + weighted sum of block j runs on the accumulator registers.
+    // ---------------- scores S^T = Ws . X^T on the tensor core, one 64-channel slab at a time; slab j + 1 is issued
+    // before the softmax over the 16 neighbours of each point + weighted sum of slab j runs on the accumulator registers.
+    // Accumulator register 8p + 4q + 2h + u of a thread is channel 64 slab + 16 warp + 8h + g, neighbour 8q + 2t + u
+    // of the warpgroup's point p (tc.cuh).
     // A NaN score still yields NaN: fmaxf skips it in the max, but its own exponential is NaN and enters both sums.
-    auto softmax = [&](int64_t tile, const float* s, int c0, const uint8_t* a_hi, const uint8_t* a_lo) {
-            const int64_t gp = tile * (LTC_ROWS / LTC_K) + pt;   // this warp's point
-            constexpr int M = CB / 4;   // columns of the block in this thread's fragment
-            float den[M], num[M];
+    auto softmax = [&](int64_t tile, const float* s, int slab, uint32_t x_hi, uint32_t x_lo) {
+            const int c0 = slab * 64 + ((tid >> 5) & 3) * 16;   // channel of this warp's accumulator row 0
+            const bool live = c0 < D;                           // d < 64: the warps past d hold zero rows of the slab
+            // ldmatrix rows: lanes 8j .. 8j + 7 address matrix j = neighbour rows 32pp + 8j .. + 7 of the warpgroup
+            const uint32_t x0 = (uint32_t)(live ? c0 / 8 : 0) * LTC_ROWS * 16 + (uint32_t)(wg * 64 + lane) * 16;
 #pragma unroll
-            for (int q = 0; q < CB / 8; ++q) {
-                // x = hi + lo of this thread's (row, column pair), rows r0 and r0 + 8
-                const uint32_t off = tc::op_off(LTC_ROWS, r0, c0 / 8 + q) + 4 * t;
-                const float2 h0 = __half22float2(*reinterpret_cast<const __half2*>(a_hi + off));
-                const float2 l0 = __half22float2(*reinterpret_cast<const __half2*>(a_lo + off));
-                const float2 h1 = __half22float2(*reinterpret_cast<const __half2*>(a_hi + off + 8 * 16));
-                const float2 l1 = __half22float2(*reinterpret_cast<const __half2*>(a_lo + off + 8 * 16));
-                const float x0[2] = {h0.x + l0.x, h0.y + l0.y}, x1[2] = {h1.x + l1.x, h1.y + l1.y};
+            for (int h = 0; h < 2; ++h) {   // channel 8h + g
+                float den[4], num[4];       // point p
 #pragma unroll
-                for (int u = 0; u < 2; ++u) {
-                    const float v0 = s[4 * q + u], v1 = s[4 * q + 2 + u];
-                    float m = fmaxf(v0, v1);
-                    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
-                    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 8));
-                    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 16));
-                    const float ml = -m * kLog2e;
-                    const float e0 = ex2_ftz(fmaf(v0, kLog2e, ml)), e1 = ex2_ftz(fmaf(v1, kLog2e, ml));
-                    den[2 * q + u] = e0 + e1;
-                    num[2 * q + u] = e0 * x0[u] + e1 * x1[u];
+                for (int pp = 0; pp < 2; ++pp) {
+                    // x = hi + lo at neighbours 8q + 2t, 8q + 2t + 1 of points 2pp, 2pp + 1, q = 0, 1
+                    uint32_t xh[4], xl[4];
+                    const uint32_t off = x0 + (uint32_t)h * LTC_ROWS * 16 + (uint32_t)pp * 32 * 16;
+                    tc::ldsm_x4_trans(xh, x_hi + off);
+                    tc::ldsm_x4_trans(xl, x_lo + off);
+#pragma unroll
+                    for (int pl = 0; pl < 2; ++pl) {
+                        const int pq = 2 * pp + pl;
+                        float v[4], x[4];
+#pragma unroll
+                        for (int q = 0; q < 2; ++q) {
+                            const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(&xh[2 * pl + q]));
+                            const float2 fl = __half22float2(*reinterpret_cast<const __half2*>(&xl[2 * pl + q]));
+                            v[2 * q] = s[8 * pq + 4 * q + 2 * h];
+                            v[2 * q + 1] = s[8 * pq + 4 * q + 2 * h + 1];
+                            x[2 * q] = fh.x + fl.x;
+                            x[2 * q + 1] = fh.y + fl.y;
+                        }
+                        float m = fmaxf(fmaxf(v[0], v[1]), fmaxf(v[2], v[3]));
+                        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+                        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+                        const float ml = -m * kLog2e;
+                        float e[4];
+#pragma unroll
+                        for (int k = 0; k < 4; ++k) e[k] = ex2_ftz(fmaf(v[k], kLog2e, ml));
+                        den[pq] = (e[0] + e[1]) + (e[2] + e[3]);
+                        num[pq] = fmaf(e[1], x[1], e[0] * x[0]) + fmaf(e[3], x[3], e[2] * x[2]);
+                    }
                 }
-            }
-            int base = 0;
-            ltc_reduce_scatter<M, 16>(den, num, lane, base);
-            if (gp < p.total) {
-                float* dst = p.agg + (size_t)gp * D + c0 + 8 * (base >> 1) + 2 * t;
-                if (M == 16) *reinterpret_cast<float2*>(dst) = make_float2(num[0] / den[0], num[1] / den[1]);
-                else if (M > 4 || !(lane & 4)) dst[base & 1] = num[0] / den[0];   // M = 4: lane bit 2 holds a copy
+                int base = 0;
+                ltc_reduce_scatter<4, 2>(den, num, lane, base);   // lane t: point t
+                const int64_t gp = tile * (LTC_ROWS / LTC_K) + wg * 4 + base;
+                if (live && gp < p.total) p.agg[(size_t)gp * D + c0 + 8 * h + g] = num[0] / den[0];
             }
         };
-    auto issue = [&](float* d, int j, uint32_t ah, uint32_t al) {   // block j: resident weight in place, streamed weight from ring slot j % 2
+    // slab j against X (hi at x_hi, lo at x_lo): the resident weight in place, or the streamed one from the ring, one
+    // wgmma group per chunk as soon as the chunk has landed (the last chunk's copy starts as the previous slab ends)
+    auto issue = [&](float* d, int j, uint32_t x_hi, uint32_t x_lo) {
+            const uint32_t bh = x_hi + wg * 64 * 16, bl = x_lo + wg * 64 * 16;
+            const uint32_t w = tc::smem_u32(w_sm);
             if (C::STREAM) {
-                const int s = j & 1;
-                tc::mbar_wait(&ring_full[s], (ring_phase >> s) & 1u);
-                ring_phase ^= 1u << s;
-                const uint32_t bh = tc::smem_u32(b_sm) + (uint32_t)s * 2 * C::SLOT_BYTES;
-                ltc_issue<CB, D>(d, ah, al, bh, bh + C::SLOT_BYTES, CB * 16, wg);
+                tc::mbar_wait(&ring_full[0], ring_phase);
+                ltc_issue<64, C::KCH, true>(d, w, w + C::W_HALF, 64 * 16, bh, bl, LTC_ROWS * 16, false);
+#pragma unroll
+                for (int kc = 1; kc < NKC; ++kc) {
+                    const uint32_t a = w + kc * 2 * C::W_HALF, xo = kc * (C::KCH / 8) * LTC_ROWS * 16;
+                    tc::mbar_wait(&ring_full[kc], ring_phase);
+                    ltc_issue<64, C::KCH>(d, a, a + C::W_HALF, 64 * 16, bh + xo, bl + xo, LTC_ROWS * 16, true);
+                }
+                ring_phase ^= 1u;
             } else {
-                const uint32_t bh = tc::smem_u32(b_sm) + (uint32_t)j * CB * 16;
-                ltc_issue<CB, D>(d, ah, al, bh, bh + C::B_BYTES, D * 16, wg);
+                const uint32_t a = w + j * 64 * 16;
+                ltc_issue<64, D, true>(d, a, a + C::W_HALF, C::WROWS * 16, bh, bl, LTC_ROWS * 16, false);
             }
         };
-    float acc0[CB / 2], acc1[CB / 2];
-    if (C::DBUF) {
-        // tile t's two score blocks are issued, then tile t+1 is built in the other A buffer, then tile t's softmax runs
-        static_assert(!C::DBUF || (C::NBLK == 2 && !C::STREAM), "double-buffered A: two resident score blocks");
-        build(blockIdx.x, smem, smem + C::A_BYTES);
-        __syncthreads();
-        int buf = 0;
-#pragma unroll 1
-        for (int64_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-            uint8_t* a_hi = smem + buf * 2 * C::A_BYTES;
-            uint8_t* nx_hi = smem + (buf ^ 1) * 2 * C::A_BYTES;
-            const uint32_t ah = tc::smem_u32(a_hi), al = ah + C::A_BYTES;
-            issue(acc0, 0, ah, al);
-            issue(acc1, 1, ah, al);
-            build(tile + gridDim.x, nx_hi, nx_hi + C::A_BYTES);
-            ltc_wait<1, CB / 2>(acc0);
-            softmax(tile, acc0, 0, a_hi, a_hi + C::A_BYTES);
-            ltc_wait<0, CB / 2>(acc1);
-            softmax(tile, acc1, CB, a_hi, a_hi + C::A_BYTES);
-            __syncthreads();   // tile t's buffer is read, tile t+1's is built
-            buf ^= 1;
-        }
-        return;
-    }
+    float acc0[32], acc1[32];
     uint8_t* a_hi = smem;
     uint8_t* a_lo = smem + C::A_BYTES;
     const uint32_t ah = tc::smem_u32(a_hi), al = tc::smem_u32(a_lo);
@@ -534,31 +546,38 @@ lfa_pool_tc_kernel(const __grid_constant__ LfaTcParams p) {
         build(tile, a_hi, a_lo);
         __syncthreads();
         const bool more = tile + gridDim.x < p.num_tiles;
-        auto step = [&](int j, float* cur, float* nxt) {   // block j lands in cur; block j + 1 goes to nxt
-            if (j + 1 < C::NBLK) {
-                issue(nxt, j + 1, ah, al);
-                ltc_wait<1, CB / 2>(cur);
-            } else {
-                ltc_wait<0, CB / 2>(cur);
-            }
+        auto step = [&](int j, float* cur, float* nxt) {   // slab j lands in cur; slab j + 1 goes to nxt
             if (C::STREAM) {
-                __syncthreads();      // both warpgroups are done with slot j % 2: refill it with the block two ahead
-                ltc_fill<CB, D, D>(b_sm + (j & 1) * 2 * C::SLOT_BYTES, &ring_full[j & 1], p.ws_img,
-                                   j + 2 < C::NBLK ? j + 2 : j + 2 - C::NBLK, lane, tid < 32 && (j + 2 < C::NBLK || more));
+                // as each chunk group of slab j completes, both warpgroups are done with its slot: refill it with the
+                // same chunk of the next slab (slab 0 of the next tile after the last)
+                ltc_release<0, NKC>([&](int kc) {
+                    __syncthreads();
+                    ltc_fill<D, C::KCH>(w_sm + kc * 2 * C::W_HALF, &ring_full[kc], p.ws_img, j + 1 < NS ? j + 1 : 0,
+                                        kc, lane, tid < 32 && (j + 1 < NS || more));
+                });
+#pragma unroll
+                for (int i = 0; i < 32; ++i) tc::fence_operand(cur[i]);
+                if (j + 1 < NS) issue(nxt, j + 1, ah, al);
+                else if (PREF && LATE) advance(tile);   // lands behind the last softmax
+            } else if (j + 1 < NS) {
+                issue(nxt, j + 1, ah, al);
+                ltc_wait<1, 32>(cur);
+            } else {
+                ltc_wait<0, 32>(cur);
             }
-            softmax(tile, cur, j * CB, a_hi, a_lo);
+            softmax(tile, cur, j, ah, al);
         };
         issue(acc0, 0, ah, al);
-        if (C::NBLK == 1) {
+        if (NS == 1) {
             step(0, acc0, acc1);
         } else {
-#pragma unroll 1
-            for (int j = 0; j < C::NBLK; j += 2) {
+#pragma unroll   // unrolled: no wgmma group is in flight across a back-edge, which ptxas would serialize
+            for (int j = 0; j < NS; j += 2) {
                 step(j, acc0, acc1);
                 step(j + 1, acc1, acc0);
             }
         }
-        __syncthreads();   // MMAs and softmax have read the A tile: free for the next tile
+        __syncthreads();   // MMAs and softmax have read the X tile: free for the next tile
     }
 }
 

@@ -144,6 +144,17 @@ template <> __device__ __forceinline__ void wgmma_f16_ss<64>(float* d, uint64_t 
         : "l"(adesc), "l"(bdesc), "r"(scale_d)
         : "memory");
 }
+// wgmma_f16_ss_set<N>: D[64 x N] = A[smem] * B[smem]^T, fp16 operands; the old values of d are not read, so that they
+// need not stay live up to the instruction
+template <int N> __device__ void wgmma_f16_ss_set(float* d, uint64_t adesc, uint64_t bdesc);
+template <> __device__ __forceinline__ void wgmma_f16_ss_set<64>(float* d, uint64_t adesc, uint64_t bdesc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+        : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3]), "=f"(d[4]), "=f"(d[5]), "=f"(d[6]), "=f"(d[7]), "=f"(d[8]), "=f"(d[9]), "=f"(d[10]), "=f"(d[11]), "=f"(d[12]), "=f"(d[13]), "=f"(d[14]), "=f"(d[15]), "=f"(d[16]), "=f"(d[17]), "=f"(d[18]), "=f"(d[19]), "=f"(d[20]), "=f"(d[21]), "=f"(d[22]), "=f"(d[23]), "=f"(d[24]), "=f"(d[25]), "=f"(d[26]), "=f"(d[27]), "=f"(d[28]), "=f"(d[29]), "=f"(d[30]), "=f"(d[31])
+        : "l"(adesc), "l"(bdesc), "r"(0)
+        : "memory");
+}
 // wait until at most N committed wgmma groups of this warpgroup are pending
 template <int N> __device__ __forceinline__ void wgmma_wait() {
     asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
@@ -177,6 +188,16 @@ __device__ __forceinline__ void split8(const float* x, uint4& hi, uint4& lo) {
     }
     hi = make_uint4(h[0], h[1], h[2], h[3]);
     lo = make_uint4(l[0], l[1], l[2], l[3]);
+}
+
+// ldmatrix.x4.trans: four 8x8 fp16 matrices, lanes 8j .. 8j + 7 addressing the 16-byte rows of matrix j; r[j] holds
+// matrix j transposed in the mma fragment layout: lane (g = lane / 4, t = lane % 4) gets elements (row 2t, column g)
+// in the low half and (row 2t + 1, column g) in the high half
+__device__ __forceinline__ void ldsm_x4_trans(uint32_t* r, uint32_t saddr) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+                 : "r"(saddr)
+                 : "memory");
 }
 
 // byte offset of (row, k-chunk) in the chunk-major canonical layout
