@@ -16,7 +16,8 @@ included (SURVEY.md A11).
 
 Built from a reference ``state_dict`` (kernel points travel in it, SURVEY.md A8) plus the
 architecture list; the batch object is the reference's (points / neighbors / pools /
-upsamples / features), CPU or CUDA, int64 or int32 indices.
+upsamples / features), CPU or CUDA, int64 or int32 indices.  ``patch_reference_model`` puts it
+behind a reference ``KPFCNN`` instance's forward.
 """
 import torch
 
@@ -241,6 +242,25 @@ class KPFCNNB200:
         return self._lin("head_softmax", [L.make_src(x)], x.shape[0], None if self.reduce_fc else "leaky")
 
     __call__ = forward
+
+
+def patch_reference_model(model):
+    """Drop-in: make an (unmodified) reference ``KPFCNN`` instance run its forward on the fused CUDA path (keeps
+    preprocess / transform / losses, ``inference_*`` and ``update_probs``).  Built from ``model.state_dict()`` and
+    ``model.cfg``, so ``reduce_fc``, ``l_relu``, ``use_batch_norm`` and the architecture are the ones the model was
+    built with; BN must be in eval mode.  The fused weights are a snapshot taken here: patch again after loading new
+    ones.  The batch is the reference ``KPConvBatch`` (its geometry still comes from the reference batcher), on the
+    CPU or the device; the result is ``[sum N_i, num_classes]`` float32 on the device.  A config the fused path does
+    not build (``modulated`` deformable KPConv, another ``KP_influence`` or ``aggregation_mode``) raises here and
+    leaves ``model.forward`` as it was."""
+    fused = KPFCNNB200(model.state_dict(), dict(model.cfg))
+
+    def forward(batch):
+        if model.training:
+            raise RuntimeError("open3d_ml_b200: the fused KPFCNN path is inference-only")
+        return fused.forward(batch)
+    model.forward = forward
+    return model
 
 
 def layer_radii(cfg):
