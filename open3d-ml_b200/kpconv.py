@@ -244,6 +244,11 @@ class KPFCNNB200:
     __call__ = forward
 
 
+def fused_from_reference(model):
+    """The fused model of a reference ``KPFCNN`` instance, from its current ``state_dict()`` and ``cfg``."""
+    return KPFCNNB200(model.state_dict(), dict(model.cfg))
+
+
 def patch_reference_model(model):
     """Drop-in: make an (unmodified) reference ``KPFCNN`` instance run its forward on the fused CUDA path (keeps
     preprocess / transform / losses, ``inference_*`` and ``update_probs``).  Built from ``model.state_dict()`` and
@@ -253,7 +258,7 @@ def patch_reference_model(model):
     CPU or the device; the result is ``[sum N_i, num_classes]`` float32 on the device.  A config the fused path does
     not build (``modulated`` deformable KPConv, another ``KP_influence`` or ``aggregation_mode``) raises here and
     leaves ``model.forward`` as it was."""
-    fused = KPFCNNB200(model.state_dict(), dict(model.cfg))
+    fused = fused_from_reference(model)
 
     def forward(batch):
         if model.training:

@@ -306,11 +306,9 @@ def cfg_from_reference(model_cfg):
                 head=head, num_classes=num_classes)
 
 
-def patch_reference_model(model):
-    """Drop-in: make an (unmodified) reference ``PointPillars`` instance run its forward and its
-    ``bbox_head.get_bboxes`` on the fused CUDA path, so that its own ``inference_end`` and
-    ``ObjectDetection.run_inference`` return the fused boxes.  Built from ``model.state_dict()`` and the
-    modules' own attributes; BN must be in eval mode."""
+def fused_from_reference(model):
+    """The fused model of a reference ``PointPillars`` instance, from its current ``state_dict()`` and the
+    modules' own attributes."""
     vl, hd = model.voxel_layer, model.bbox_head
     gen = hd.anchor_generator
     cfg = dict(point_cloud_range=list(model.point_cloud_range), voxel_size=[float(v) for v in vl.voxel_size],
@@ -324,7 +322,15 @@ def patch_reference_model(model):
                          sizes=[[float(v) for v in s] for s in gen.sizes],
                          rotations=[float(r) for r in gen.rotations]),
                num_classes=int(hd.num_classes))
-    fused = PointPillarsB200(model.state_dict(), cfg)
+    return PointPillarsB200(model.state_dict(), cfg)
+
+
+def patch_reference_model(model):
+    """Drop-in: make an (unmodified) reference ``PointPillars`` instance run its forward and its
+    ``bbox_head.get_bboxes`` on the fused CUDA path, so that its own ``inference_end`` and
+    ``ObjectDetection.run_inference`` return the fused boxes.  Built from ``model.state_dict()`` and the
+    modules' own attributes; BN must be in eval mode."""
+    fused = fused_from_reference(model)
 
     def forward(inputs):
         if model.training:

@@ -236,10 +236,15 @@ class PVCNNB200:
         return graph_replay(self._graphs, "forward", flat, lambda: self.forward(inputs), self.device)
 
 
+def fused_from_reference(model):
+    """The fused model of a reference ``PVCNN`` instance, from its current ``state_dict()`` and ``cfg``."""
+    return PVCNNB200(model.state_dict(), cfg_from_reference(model.cfg))
+
+
 def patch_reference_model(model):
     """Drop-in: make an (unmodified) reference ``PVCNN`` instance run its forward on the fused CUDA path (keeps
     preprocess / transform / losses).  BN must be in eval mode."""
-    fused = PVCNNB200(model.state_dict(), cfg_from_reference(model.cfg))
+    fused = fused_from_reference(model)
 
     def forward(inputs):
         if model.training:

@@ -316,11 +316,16 @@ class RandLANetB200:
                             self.device)
 
 
+def fused_from_reference(model):
+    """The fused model of a reference ``RandLANet`` instance, from its current ``state_dict()`` and ``cfg``."""
+    return RandLANetB200(model.state_dict(), model.cfg.num_layers, model.cfg.num_neighbors,
+                         sub_sampling_ratio=list(model.cfg.sub_sampling_ratio))
+
+
 def patch_reference_model(model):
     """Drop-in: make an (unmodified) reference ``RandLANet`` instance run its forward on the
     fused CUDA path (keeps preprocess/transform/losses).  BN must be in eval mode."""
-    fused = RandLANetB200(model.state_dict(), model.cfg.num_layers, model.cfg.num_neighbors,
-                          sub_sampling_ratio=list(model.cfg.sub_sampling_ratio))
+    fused = fused_from_reference(model)
 
     def forward(inputs):
         if model.training:

@@ -280,10 +280,15 @@ class SparseConvUnetB200:
         return x
 
 
+def fused_from_reference(model):
+    """The fused model of a reference ``SparseConvUnet`` instance, from its current ``state_dict()`` and ``cfg``."""
+    return SparseConvUnetB200(model.state_dict(), cfg_from_reference(model.cfg))
+
+
 def patch_reference_model(model):
     """Drop-in: make an (unmodified) reference ``SparseConvUnet`` instance run its forward on the fused CUDA path
     (keeps preprocess / transform / losses).  BN must be in eval mode."""
-    fused = SparseConvUnetB200(model.state_dict(), cfg_from_reference(model.cfg))
+    fused = fused_from_reference(model)
 
     def forward(inputs):
         if model.training:
