@@ -10,6 +10,9 @@ the reference pipelines, which call ``model.eval()`` before they load a checkpoi
 PointPillars' ``bbox_head.get_bboxes`` decodes on the device after a fused forward.  Train mode runs the reference
 forward and ``get_bboxes`` untouched.  A config the fused path refuses logs one warning and keeps the
 reference forward.
+
+``patch`` is the other way in, behind each model module's ``patch_reference_model``: it switches one instance to a
+fused model built once, a snapshot of the weights it holds then.
 """
 import importlib
 import logging
@@ -24,11 +27,27 @@ _DECODER = weakref.WeakKeyDictionary()    # PointPillars bbox_head -> the fused 
 
 
 def _builders():
-    """Reference class name -> the builder its ``patch_reference_model`` uses."""
+    """Reference class name -> the builder of its fused model (``fused_from_reference`` of its model module)."""
     from . import kpconv, pointpillars, pvcnn, randlanet, sparseconvunet
     return dict(RandLANet=randlanet.fused_from_reference, PointPillars=pointpillars.fused_from_reference,
                 KPFCNN=kpconv.fused_from_reference, PVCNN=pvcnn.fused_from_reference,
                 SparseConvUnet=sparseconvunet.fused_from_reference)
+
+
+def patch(model, build):
+    """Makes the reference instance `model` run its forward on ``build(model)``, a fused model of the weights it holds
+    now, and, when that model decodes boxes (PointPillars), its ``bbox_head.get_bboxes`` too.  The forward raises in
+    train mode.  A `build` that raises leaves `model` as it was.  Returns `model`."""
+    fused = build(model)
+
+    def forward(inputs):
+        if model.training:
+            raise RuntimeError("open3d_ml_b200: the fused %s path is inference-only" % type(model).__name__)
+        return fused.forward(inputs)
+    model.forward = forward
+    if hasattr(fused, "get_bboxes"):
+        model.bbox_head.get_bboxes = fused.get_bboxes
+    return model
 
 
 def _weights_key(model):

@@ -22,6 +22,7 @@ behind a reference ``KPFCNN`` instance's forward.
 import torch
 
 from . import _lib as L
+from .fuse import patch
 
 BN_EPS = 1e-5  # nn.BatchNorm1d default, kpconv.py:1231
 
@@ -250,22 +251,8 @@ def fused_from_reference(model):
 
 
 def patch_reference_model(model):
-    """Drop-in: make an (unmodified) reference ``KPFCNN`` instance run its forward on the fused CUDA path (keeps
-    preprocess / transform / losses, ``inference_*`` and ``update_probs``).  Built from ``model.state_dict()`` and
-    ``model.cfg``, so ``reduce_fc``, ``l_relu``, ``use_batch_norm`` and the architecture are the ones the model was
-    built with; BN must be in eval mode.  The fused weights are a snapshot taken here: patch again after loading new
-    ones.  The batch is the reference ``KPConvBatch`` (its geometry still comes from the reference batcher), on the
-    CPU or the device; the result is ``[sum N_i, num_classes]`` float32 on the device.  A config the fused path does
-    not build (``modulated`` deformable KPConv, another ``KP_influence`` or ``aggregation_mode``) raises here and
-    leaves ``model.forward`` as it was."""
-    fused = fused_from_reference(model)
-
-    def forward(batch):
-        if model.training:
-            raise RuntimeError("open3d_ml_b200: the fused KPFCNN path is inference-only")
-        return fused.forward(batch)
-    model.forward = forward
-    return model
+    """Makes a reference ``KPFCNN`` instance run its forward on the fused path (see ``fuse.patch``)."""
+    return patch(model, fused_from_reference)
 
 
 def layer_radii(cfg):

@@ -24,6 +24,7 @@ import torch
 
 from . import _lib as L
 from . import ops
+from .fuse import patch
 from .pipeline import BufferCache, graph_replay
 
 BN_EPS = 1e-3  # point_pillars.py:409,648,724
@@ -326,16 +327,5 @@ def fused_from_reference(model):
 
 
 def patch_reference_model(model):
-    """Drop-in: make an (unmodified) reference ``PointPillars`` instance run its forward and its
-    ``bbox_head.get_bboxes`` on the fused CUDA path, so that its own ``inference_end`` and
-    ``ObjectDetection.run_inference`` return the fused boxes.  Built from ``model.state_dict()`` and the
-    modules' own attributes; BN must be in eval mode."""
-    fused = fused_from_reference(model)
-
-    def forward(inputs):
-        if model.training:
-            raise RuntimeError("open3d_ml_b200: the fused PointPillars path is inference-only")
-        return fused.forward(inputs)
-    model.forward = forward
-    model.bbox_head.get_bboxes = fused.get_bboxes
-    return model
+    """Makes a reference ``PointPillars`` instance forward and decode boxes on the fused path (see ``fuse.patch``)."""
+    return patch(model, fused_from_reference)

@@ -18,6 +18,7 @@ Inference only; no host read anywhere in the forward.
 import torch
 
 from . import _lib as L
+from .fuse import patch
 from .pipeline import BufferCache, graph_replay
 
 BN3D_EPS = 1e-4      # pvcnn.py:544,551
@@ -242,13 +243,5 @@ def fused_from_reference(model):
 
 
 def patch_reference_model(model):
-    """Drop-in: make an (unmodified) reference ``PVCNN`` instance run its forward on the fused CUDA path (keeps
-    preprocess / transform / losses).  BN must be in eval mode."""
-    fused = fused_from_reference(model)
-
-    def forward(inputs):
-        if model.training:
-            raise RuntimeError("open3d_ml_b200: the fused PVCNN path is inference-only")
-        return fused.forward(inputs)
-    model.forward = forward
-    return model
+    """Makes a reference ``PVCNN`` instance run its forward on the fused path (see ``fuse.patch``)."""
+    return patch(model, fused_from_reference)

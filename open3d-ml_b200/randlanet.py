@@ -19,6 +19,7 @@ import torch
 
 from . import _lib as L
 from . import ops
+from .fuse import patch
 from .pipeline import BufferCache, graph_replay
 
 BN_EPS = 1e-6  # randlanet.py:77,499
@@ -323,13 +324,5 @@ def fused_from_reference(model):
 
 
 def patch_reference_model(model):
-    """Drop-in: make an (unmodified) reference ``RandLANet`` instance run its forward on the
-    fused CUDA path (keeps preprocess/transform/losses).  BN must be in eval mode."""
-    fused = fused_from_reference(model)
-
-    def forward(inputs):
-        if model.training:
-            raise RuntimeError("open3d_ml_b200: the fused RandLA-Net path is inference-only")
-        return fused.forward(inputs)
-    model.forward = forward
-    return model
+    """Makes a reference ``RandLANet`` instance run its forward on the fused path (see ``fuse.patch``)."""
+    return patch(model, fused_from_reference)

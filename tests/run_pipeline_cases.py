@@ -9,7 +9,8 @@ runs it in a fresh process (the shim owns sys.modules['open3d']).
         seeds the global RNGs, then runs the script in this process:
           launch   as ``python -m open3d_ml_b200.run_pipeline`` does (shim + fused dispatch)
           shim     with the shim alone: the reference forwards
-          patched  the shim, and pointpillars/.../patch_reference_model right after the pipeline loaded the checkpoint
+          patched  the shim, and the patch every model module's patch_reference_model makes (fuse.patch) right after
+                   the pipeline loaded the checkpoint
           stale    the same patch right before the checkpoint is loaded (after ``model.eval()``), on the init weights
         and stores every result the dataset's save_test_result receives under <out> (labels and scores of each
         cloud, the boxes of each frame).
@@ -178,14 +179,11 @@ def _record_results(out):
 
 def _patch_at_load(after):
     """Patches the model explicitly when the pipeline loads its checkpoint: after loading it or (stale) before."""
-    import importlib
     import ml3d.torch.pipelines as P
+    from open3d_ml_b200 import fuse
 
     def patch(model):
-        name = type(model).__name__
-        mod = dict(RandLANet="randlanet", PointPillars="pointpillars", KPFCNN="kpconv", PVCNN="pvcnn",
-                   SparseConvUnet="sparseconvunet")[name]
-        importlib.import_module("open3d_ml_b200." + mod).patch_reference_model(model)
+        fuse.patch(model, fuse._builders()[type(model).__name__])
 
     for cls in (P.SemanticSegmentation, P.ObjectDetection):
         load = cls.load_ckpt

@@ -3,6 +3,7 @@ frame sharding + the post-batch collectives over gloo (world_size 2)."""
 import os
 import subprocess
 import sys
+import types
 
 import numpy as np
 import pytest
@@ -137,6 +138,31 @@ def test_pipelined_runner_tree_helpers_and_cpu_refusal():
     if not torch.cuda.is_available():
         with pytest.raises(RuntimeError):
             P.PipelinedRunner(lambda x: x)
+
+
+@pytest.mark.parametrize("module", ["randlanet", "pointpillars", "kpconv", "pvcnn", "sparseconvunet"])
+def test_patch_reference_model_builds_before_it_touches_the_model(module):
+    """A fused build that fails (here: an instance without weights or config) reaches the caller and leaves the
+    instance without a patched forward."""
+    import importlib
+    model = types.SimpleNamespace(training=False)
+    with pytest.raises(AttributeError):
+        importlib.import_module("open3d_ml_b200." + module).patch_reference_model(model)
+    assert not hasattr(model, "forward")
+
+
+def test_patch_refuses_train_mode_and_redirects_box_decoding():
+    from open3d_ml_b200 import fuse
+    model = types.SimpleNamespace(training=False)
+    assert fuse.patch(model, lambda m: types.SimpleNamespace(forward=lambda x: x + 1)) is model
+    assert model.forward(1) == 2
+    model.training = True
+    with pytest.raises(RuntimeError, match="^open3d_ml_b200: .*inference-only"):
+        model.forward(1)
+    decoder = types.SimpleNamespace(forward=lambda x: x, get_bboxes=lambda *a: "boxes")
+    model = types.SimpleNamespace(training=False, bbox_head=types.SimpleNamespace(get_bboxes=None))
+    fuse.patch(model, lambda m: decoder)
+    assert model.bbox_head.get_bboxes is decoder.get_bboxes
 
 
 @pytest.mark.skipif(not refshim.available(), reason="/root/reference absent (GPU box)")
