@@ -80,7 +80,8 @@ O3DML_API int o3dml_ragged_to_dense(const void* values, int elem_bytes, int64_t 
  *   return_distances) (ml3d/torch/models/point_transformer.py:724-734).
  * out_index [num_queries, k] int32 or int64 GLOBAL row ids (-1 when a batch item has fewer than
  * k points), out_distance2 [num_queries, k] float32 squared distances (may be NULL).
- * Rows ascend by (distance, index). */
+ * Rows ascend by (distance, index).  k is 1..64: the sizing function has no k, and RandLA-Net's graphed k-NN
+ * pyramid sizes its workspace from it once; o3dml_knn_search_metric takes any k. */
 O3DML_API size_t o3dml_knn_workspace_bytes(int64_t num_points, int64_t num_queries, int64_t batch);
 O3DML_API int o3dml_knn_search(const float* points, int64_t num_points, const int64_t* points_row_splits,
                      const float* queries, int64_t num_queries,
@@ -137,7 +138,12 @@ O3DML_API int o3dml_radius_search_fill(const float* queries, int64_t num_points,
  * L2 case without ignore_query_point.  Without ignore_query_point: out_index [num_queries, k] and out_distance
  * [num_queries, k] (may be NULL) as there, out_row_splits and d_total unused.  With it a row may hold fewer than k
  * neighbours: out_index / out_distance hold the rows back to back (room for num_queries * k entries),
- * out_row_splits int64 [num_queries + 1] places them and d_total (int64 [1], may be NULL) is their total. */
+ * out_row_splits int64 [num_queries + 1] places them and d_total (int64 [1], may be NULL) is their total.
+ * Any k >= 1.  Up to 64 each query's row is kept in registers; beyond, one CTA per query selects and sorts it (rows of
+ * more than 4096 keys are sorted in the workspace).  For k > 64 a call is refused (status 1) before anything is
+ * enqueued when num_queries >= 2^31, when num_queries * k > 2^32 - 1 with ignore_query_point (the ragged rows are
+ * placed by a uint32 scan), or when the workspace size would overflow; the sizing function returns SIZE_MAX for
+ * those. */
 O3DML_API size_t o3dml_knn_search_metric_workspace_bytes(int64_t num_points, int64_t num_queries, int64_t batch,
                                                          int k, int ignore_query_point);
 O3DML_API int o3dml_knn_search_metric(const float* points, int64_t num_points, const int64_t* points_row_splits,

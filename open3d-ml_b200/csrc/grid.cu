@@ -358,6 +358,303 @@ __global__ void knn_compact_kernel(const int32_t* __restrict__ idx, const float*
     if (out_dist) out_dist[o] = dist[t];
 }
 
+// ------------------------------------------------------------ k-NN, k > 64 ----
+// knn_kernel keeps a row in registers, which ends at KMAX = 64.  Beyond it one CTA of KSEL_T threads serves one query
+// (in the cell order of grid_build) with the same row contract, selecting instead of inserting:
+//   bound  -- the smallest Chebyshev box of cells around the query's cell that holds at least min(k, item size)
+//             points, from the cell counts alone;
+//   select -- a CTA-wide radix select of the k-th smallest key (ordered bits of d, then id) over the rankable points
+//             of the box, 8 bits per pass over 256 shared-memory bins, re-reading the cell-sorted float4s and
+//             recomputing d on each pass (no candidate buffer).  With D the k-th distance, every point within D lies
+//             in the cells of reach_box(D) (the slack of radius_kernel): when those lie inside the box the box's k
+//             smallest keys are the item's, otherwise the select runs again over reach_box(D).  A box that holds too
+//             few rankable points (NaN distances, ignore_query_point) or whose k-th distance is +inf (a point further
+//             out may tie it and rank first by index) is widened to the whole batch item, which is exact by itself;
+//   emit   -- every rankable point whose key is at most the k-th key goes to the row, which is then sorted by key: in
+//             shared memory up to KSEL_SMEM_K keys, in the workspace (`rows`, [nq, k] keys) beyond.
+// Keys are unique (the id is part of the key), so the row holds exactly min(k, rankable points) entries.
+constexpr int KSEL_T = 128;
+constexpr int KSEL_SMEM_K = 4096;  // 8-byte keys: 32 KB of shared memory
+constexpr int KNN_REG_KMAX = 64;   // largest k of knn_kernel
+
+struct CellBox {
+    int x0, x1, y0, y1, z0, z1;
+};
+
+__device__ __forceinline__ CellBox whole_box(const GridInfo& g) { return {0, g.dx - 1, 0, g.dy - 1, 0, g.dz - 1}; }
+__device__ __forceinline__ bool box_is_whole(const GridInfo& g, const CellBox& b) {
+    return b.x0 == 0 && b.y0 == 0 && b.z0 == 0 && b.x1 == g.dx - 1 && b.y1 == g.dy - 1 && b.z1 == g.dz - 1;
+}
+__device__ __forceinline__ bool box_within(const CellBox& a, const CellBox& b) {
+    return a.x0 >= b.x0 && a.x1 <= b.x1 && a.y0 >= b.y0 && a.y1 <= b.y1 && a.z0 >= b.z0 && a.z1 <= b.z1;
+}
+__device__ __forceinline__ int clamp_cell(int64_t c, int n) { return (int)min(max(c, (int64_t)0), (int64_t)n - 1); }
+__device__ __forceinline__ CellBox chebyshev_box(const GridInfo& g, int cx, int cy, int cz, int64_t r) {
+    return {clamp_cell(cx - r, g.dx), clamp_cell(cx + r, g.dx), clamp_cell(cy - r, g.dy),
+            clamp_cell(cy + r, g.dy), clamp_cell(cz - r, g.dz), clamp_cell(cz + r, g.dz)};
+}
+// the cells of every point within metric distance D of the query, with radius_kernel's slack and clamping
+template <int M>
+__device__ __forceinline__ CellBox reach_box(const GridInfo& g, float qx, float qy, float qz, float D) {
+    const float rr = (M == L2 ? sqrtf(D) : D) * 1.0001f + 1e-7f;
+    return {clamp_cell((int)floorf((qx - rr - g.ox) * g.inv_cs), g.dx), clamp_cell((int)floorf((qx + rr - g.ox) * g.inv_cs), g.dx),
+            clamp_cell((int)floorf((qy - rr - g.oy) * g.inv_cs), g.dy), clamp_cell((int)floorf((qy + rr - g.oy) * g.inv_cs), g.dy),
+            clamp_cell((int)floorf((qz - rr - g.oz) * g.inv_cs), g.dz), clamp_cell((int)floorf((qz + rr - g.oz) * g.inv_cs), g.dz)};
+}
+
+// A box is a set of runs of the cell-sorted points: one per (y, z) row of cells, one per z slab when its rows span the
+// grid in x, a single one when its slabs span it in x and y.
+__device__ __forceinline__ int box_runs(const GridInfo& g, const CellBox& b) {
+    const bool fx = b.x0 == 0 && b.x1 == g.dx - 1, fy = b.y0 == 0 && b.y1 == g.dy - 1;
+    if (fx && fy) return 1;
+    if (fx) return b.z1 - b.z0 + 1;
+    return (b.y1 - b.y0 + 1) * (b.z1 - b.z0 + 1);
+}
+__device__ __forceinline__ void box_run(const GridInfo& g, const CellBox& b, const uint32_t* __restrict__ cell_start,
+                                        int i, uint32_t& s, uint32_t& e) {
+    const bool fx = b.x0 == 0 && b.x1 == g.dx - 1, fy = b.y0 == 0 && b.y1 == g.dy - 1;
+    int y0, y1, z0, z1;
+    if (fx && fy) { y0 = b.y0; y1 = b.y1; z0 = b.z0; z1 = b.z1; }
+    else if (fx) { y0 = b.y0; y1 = b.y1; z0 = z1 = b.z0 + i; }
+    else {
+        const int ny = b.y1 - b.y0 + 1;
+        y0 = y1 = b.y0 + i % ny;
+        z0 = z1 = b.z0 + i / ny;
+    }
+    s = cell_start[cell_id(g, b.x0, y0, z0)];
+    e = cell_start[cell_id(g, b.x1, y1, z1) + 1];
+}
+
+__device__ __forceinline__ uint32_t block_sum(uint32_t v, uint32_t* red) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    uint32_t t = 0;
+#pragma unroll
+    for (int w = 0; w < KSEL_T / 32; ++w) t += red[w];
+    __syncthreads();
+    return t;
+}
+
+// points of the box, from the cell counts
+__device__ __forceinline__ uint32_t box_count(const GridInfo& g, const CellBox& b, const uint32_t* __restrict__ cell_start,
+                                              uint32_t* red) {
+    const int n = box_runs(g, b);
+    uint32_t c = 0;
+    for (int i = threadIdx.x; i < n; i += KSEL_T) {
+        uint32_t s, e;
+        box_run(g, b, cell_start, i, s, e);
+        c += e - s;
+    }
+    return block_sum(c, red);
+}
+
+// f(key) for every rankable point of the box, the points spread over the CTA's threads
+template <int M, bool IGNORE, class F>
+__device__ __forceinline__ void box_visit(const GridInfo& g, const CellBox& b, const uint32_t* __restrict__ cell_start,
+                                          const float4* __restrict__ sorted, float qx, float qy, float qz, F f) {
+    const int n = box_runs(g, b);
+    for (int i = 0; i < n; ++i) {
+        uint32_t s, e;
+        box_run(g, b, cell_start, i, s, e);
+        for (uint32_t pi = s + threadIdx.x; pi < e; pi += KSEL_T) {
+            const float4 pt = sorted[pi];
+            if (IGNORE && coincident(qx, qy, qz, pt)) continue;
+            const float d = metric_dist<M>(qx, qy, qz, pt.x, pt.y, pt.z);
+            if (isnan(d)) continue;  // never ranked
+            f(((uint64_t)f2ord(d) << 32) | (uint32_t)__float_as_int(pt.w));
+        }
+    }
+}
+
+// The need-th smallest key (need >= 1) of the box's rankable points, whose number goes to total; all ones when there
+// are fewer.  From the d bytes on, a pass whose bucket holds exactly the keys still needed ends the select early with
+// the largest key of that bucket, which selects the same points (the d bytes are always resolved, so the k-th distance
+// is exact).
+template <int M, bool IGNORE>
+__device__ uint64_t box_select(const GridInfo& g, const CellBox& b, const uint32_t* __restrict__ cell_start,
+                               const float4* __restrict__ sorted, float qx, float qy, float qz, uint32_t need,
+                               uint32_t& total, uint32_t* hist, uint32_t* pick) {
+    uint64_t prefix = 0, mask = 0;
+    for (int shift = 56; shift >= 0; shift -= 8) {
+        for (int i = threadIdx.x; i < 256; i += KSEL_T) hist[i] = 0;
+        __syncthreads();
+        box_visit<M, IGNORE>(g, b, cell_start, sorted, qx, qy, qz, [&](uint64_t key) {
+            if ((key & mask) == prefix) atomicAdd(&hist[(uint32_t)(key >> shift) & 255u], 1u);
+        });
+        __syncthreads();
+        if (threadIdx.x < 32) {  // warp 0: the bucket of the need-th key, each lane scanning 8 bins
+            const int lane = threadIdx.x;
+            uint32_t c[8], s = 0;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) { c[j] = hist[lane * 8 + j]; s += c[j]; }
+            uint32_t incl = s;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const uint32_t v = __shfl_up_sync(0xffffffffu, incl, o);
+                if (lane >= o) incl += v;
+            }
+            const uint32_t all = __shfl_sync(0xffffffffu, incl, 31);
+            uint32_t below = incl - s;
+            if (lane == 0) { pick[0] = all; pick[1] = 256; }
+            __syncwarp();
+            if (need <= all && below < need && need <= incl) {  // exactly one lane
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    if (need <= below + c[j]) { pick[1] = lane * 8 + j; pick[2] = below; pick[3] = c[j]; break; }
+                    below += c[j];
+                }
+            }
+        }
+        __syncthreads();
+        const uint32_t bucket = pick[1];
+        if (shift == 56) total = pick[0];
+        if (bucket == 256) return ~0ull;  // fewer than need rankable points (first pass only)
+        need -= pick[2];
+        prefix |= (uint64_t)bucket << shift;
+        mask |= 0xffull << shift;
+        if (shift <= 32 && pick[3] == need) return prefix | ~mask;
+    }
+    return prefix;
+}
+
+__device__ __forceinline__ void key_swap(uint64_t* a, int64_t i, int64_t j) {
+    const uint64_t x = a[i], y = a[j];
+    if (y < x) { a[i] = y; a[j] = x; }
+}
+
+// One step of a bitonic sorting network in its all-ascending form over keys [0, n), pairs t0 .. t0 + npairs - 1 of the
+// network over the next power of two: at stride = size / 2 each position of a size-block meets its mirror, below that
+// a position meets the one `stride` above.  Pairs reaching past n are skipped (the positions past n act as +infinity,
+// which never move), so n needs no padding.  a holds the keys from position `base` on.
+__device__ __forceinline__ void sort_step(uint64_t* a, int64_t base, uint32_t n, uint32_t t0, uint32_t npairs,
+                                          uint32_t size, uint32_t stride) {
+    for (uint32_t t = t0 + threadIdx.x; t < t0 + npairs; t += KSEL_T) {
+        int64_t i, j;
+        if (stride == size / 2) {
+            const uint32_t o = t % stride;
+            i = (int64_t)(t / stride) * size + o;
+            j = (int64_t)(t / stride) * size + size - 1 - o;
+        } else {
+            i = (int64_t)(t / stride) * 2 * stride + t % stride;
+            j = i + stride;
+        }
+        if (j < n) key_swap(a, i - base, j - base);
+    }
+}
+
+// Sorts the n keys of row ascending.  n <= KSEL_SMEM_K: row is sh and the network runs there.  Beyond, row is in global
+// memory: the steps of stride >= KSEL_SMEM_K run on it, and the rest chunk by chunk in sh.
+__device__ void sort_keys(uint64_t* row, uint32_t n, uint64_t* sh) {
+    uint32_t P = 2;
+    while (P < n) P <<= 1;
+    if (n <= (uint32_t)KSEL_SMEM_K) {
+        for (uint32_t size = 2; size <= P; size <<= 1)
+            for (uint32_t stride = size / 2; stride > 0; stride >>= 1) {
+                sort_step(row, 0, n, 0, P / 2, size, stride);
+                __syncthreads();
+            }
+        return;
+    }
+    constexpr uint32_t CH = KSEL_SMEM_K;
+    // sizes size_lo..size_hi of the network, from `first` stride on, on each chunk of CH positions in shared memory
+    auto chunked = [&](uint32_t size_lo, uint32_t size_hi, uint32_t first) {
+        for (uint32_t c0 = 0; c0 < n; c0 += CH) {
+            const uint32_t len = min(CH, n - c0);
+            for (uint32_t i = threadIdx.x; i < len; i += KSEL_T) sh[i] = row[c0 + i];
+            __syncthreads();
+            for (uint32_t size = size_lo; size <= size_hi; size <<= 1)
+                for (uint32_t stride = size == size_lo ? first : size / 2; stride > 0; stride >>= 1) {
+                    sort_step(sh, c0, n, c0 / 2, CH / 2, size, stride);
+                    __syncthreads();
+                }
+            for (uint32_t i = threadIdx.x; i < len; i += KSEL_T) row[c0 + i] = sh[i];
+            __syncthreads();
+        }
+    };
+    chunked(2, CH, 1);
+    for (uint32_t size = 2 * CH; size <= P; size <<= 1) {
+        for (uint32_t stride = size / 2; stride >= CH; stride >>= 1) {
+            sort_step(row, 0, n, 0, P / 2, size, stride);
+            __syncthreads();
+        }
+        chunked(size, size, CH / 2);
+    }
+}
+
+template <int M = L2, bool IGNORE = false>
+__global__ void __launch_bounds__(KSEL_T, 1)
+knn_select_kernel(const float* __restrict__ queries, int64_t nq, const int64_t* __restrict__ qsplits,
+                  const int64_t* __restrict__ psplits, int batch, const uint32_t* __restrict__ order,
+                  const GridInfo* __restrict__ info, const uint32_t* __restrict__ cell_start,
+                  const float4* __restrict__ sorted, int k, void* __restrict__ out_idx, int idx_is64,
+                  float* __restrict__ out_d2, uint32_t* __restrict__ row_len, uint64_t* __restrict__ rows) {
+    extern __shared__ uint64_t sh_keys[];  // min(k, KSEL_SMEM_K)
+    __shared__ uint32_t hist[256], red[KSEL_T / 32], pick[4], emitted;
+    const int64_t qi = order[blockIdx.x];
+    const int b = batch_of(qi, qsplits, batch);
+    const GridInfo g = info[b];
+    const float qx = queries[3 * qi], qy = queries[3 * qi + 1], qz = queries[3 * qi + 2];
+    const int64_t nsup = psplits[b + 1] - psplits[b];
+    const uint32_t kk = (uint32_t)(nsup < k ? nsup : k);  // neighbours that exist
+    CellBox box = whole_box(g);
+    uint64_t kth = 0;
+    uint32_t nsel = 0;
+    if (kk > 0) {
+        int cx, cy, cz;
+        cell_coords(g, qx, qy, qz, cx, cy, cz);
+        // bound: grow r = 0, 1, 3, 7, ... until box(r) holds kk points (the whole item does), then bisect
+        int64_t lo = -1, r = 0;
+        while (box_count(g, chebyshev_box(g, cx, cy, cz, r), cell_start, red) < kk) { lo = r; r = 2 * r + 1; }
+        while (r - lo > 1) {
+            const int64_t mid = (lo + r) / 2;
+            if (box_count(g, chebyshev_box(g, cx, cy, cz, mid), cell_start, red) >= kk) r = mid; else lo = mid;
+        }
+        box = chebyshev_box(g, cx, cy, cz, r);
+        for (int tries = 0;; ++tries) {
+            uint32_t total = 0;
+            kth = box_select<M, IGNORE>(g, box, cell_start, sorted, qx, qy, qz, kk, total, hist, pick);
+            if (box_is_whole(g, box)) {
+                nsel = min(kk, total);
+                break;
+            }
+            const float D = ord2f((uint32_t)(kth >> 32));
+            if (total < kk || !(D < __int_as_float(0x7f800000)) || tries == 2) {
+                box = whole_box(g);
+                continue;
+            }
+            const CellBox reach = reach_box<M>(g, qx, qy, qz, D);
+            if (box_within(reach, box)) {
+                nsel = kk;
+                break;
+            }
+            box = reach;
+        }
+    }
+    uint64_t* row = nsel <= (uint32_t)KSEL_SMEM_K ? sh_keys : rows + qi * k;
+    if (threadIdx.x == 0) emitted = 0;
+    __syncthreads();
+    if (nsel > 0)
+        box_visit<M, IGNORE>(g, box, cell_start, sorted, qx, qy, qz, [&](uint64_t key) {
+            if (key <= kth) {
+                const uint32_t slot = atomicAdd(&emitted, 1u);
+                if (slot < nsel) row[slot] = key;
+            }
+        });
+    __syncthreads();
+    sort_keys(row, nsel, sh_keys);
+    for (int j = threadIdx.x; j < k; j += KSEL_T) {
+        const bool have = (uint32_t)j < nsel;
+        const uint64_t key = have ? row[j] : 0;
+        const int id = have ? (int)(uint32_t)key : -1;
+        if (idx_is64) ((int64_t*)out_idx)[qi * k + j] = id;
+        else ((int32_t*)out_idx)[qi * k + j] = id;
+        if (out_d2) out_d2[qi * k + j] = have ? ord2f((uint32_t)(key >> 32)) : __int_as_float(0x7f800000);
+    }
+    if (IGNORE && threadIdx.x == 0) row_len[qi] = nsel;
+}
+
 // ----------------------------------------------------------- fixed radius ----
 // inserts (d, id) into the sorted row [row, j) and keeps it sorted by (d, id)
 template <typename I>
@@ -498,6 +795,7 @@ struct KnnBuf : GridBuf {
     float* dist;
     uint32_t *len, *start, *total;
     void* len_scan_tmp;
+    uint64_t* rows;  // k > KSEL_SMEM_K: the keys of each row while knn_select_kernel sorts them
 };
 
 static KnnBuf knn_carve(Workspace& ws, int64_t np, int64_t nq, int64_t batch, int k, int ragged) {
@@ -510,7 +808,18 @@ static KnnBuf knn_carve(Workspace& ws, int64_t np, int64_t nq, int64_t batch, in
         b.total = ws.take<uint32_t>(16);
         b.len_scan_tmp = scan_carve(ws, nq);
     }
+    b.rows = k > KSEL_SMEM_K ? ws.take<uint64_t>(nq * k) : nullptr;
     return b;
+}
+
+// The limits of a search with k > 64, or nullptr within them: one CTA per query, the ragged rows placed by a uint32
+// scan, and workspace bytes (about 16 per row entry) that size_t holds with room to spare.
+static const char* knn_any_k_limit(int64_t num_points, int64_t num_queries, int k, int ragged) {
+    if (num_queries > INT32_MAX) return "num_queries must be below 2^31 for k > 64";
+    if (ragged && num_queries * k > (int64_t)UINT32_MAX)
+        return "num_queries * k must be at most 2^32 - 1 with ignore_query_point (the ragged row scan is uint32)";
+    if (num_queries > (((int64_t)1 << 58) - 64 * num_points) / 16 / k) return "the workspace size would overflow";
+    return nullptr;
 }
 
 // builds the support grid and the cell-ordered query permutation
@@ -555,14 +864,18 @@ static cudaError_t radius_launch(bool general, int metric, int ignore, unsigned 
     return cudaErrorInvalidValue;  // unreachable: the entries check the metric
 }
 
-// one knn_kernel<KMAX, M, IG> launch, KMAX the smallest instance that holds k
+// one knn_kernel<KMAX, M, IG> launch, KMAX the smallest instance that holds k; beyond 64 one knn_select_kernel<M, IG>
+// launch, a CTA per query
 template <int M, bool IG, class... Args>
-static cudaError_t knn_launch(int k, unsigned nb, cudaStream_t st, Args... args) {
+static cudaError_t knn_launch(int k, int64_t nq, uint64_t* rows, cudaStream_t st, Args... args) {
+    const unsigned nb = (unsigned)ceil_div<int64_t>(nq, 128);
     if (k == 1) return launch<knn_kernel<1, M, IG>>(nb, 128, 0, st, args...);
     if (k <= 8) return launch<knn_kernel<8, M, IG>>(nb, 128, 0, st, args...);
     if (k <= 16) return launch<knn_kernel<16, M, IG>>(nb, 128, 0, st, args...);
     if (k <= 32) return launch<knn_kernel<32, M, IG>>(nb, 128, 0, st, args...);
-    return launch<knn_kernel<64, M, IG>>(nb, 128, 0, st, args...);
+    if (k <= KNN_REG_KMAX) return launch<knn_kernel<KNN_REG_KMAX, M, IG>>(nb, 128, 0, st, args...);
+    return launch<knn_select_kernel<M, IG>>((unsigned)nq, KSEL_T, (size_t)min(k, KSEL_SMEM_K) * sizeof(uint64_t), st,
+                                            args..., rows);
 }
 
 // The k-NN search of every entry.  Without ignore_query_point the rows go straight to out_index / out_distance2
@@ -572,10 +885,14 @@ static int knn_impl(const char* name, const float* points, int64_t num_points, c
                     int metric, int ignore, void* out_index, int index_is64, float* out_distance2,
                     int64_t* out_row_splits, int64_t* d_total, void* workspace, size_t workspace_bytes, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
-    O3DML_CHECK(k >= 1 && k <= 64, "%s: k must be in 1..64 (got %d)", name, k);
+    O3DML_CHECK(k >= 1, "%s: k must be at least 1 (got %d)", name, k);
     O3DML_CHECK(batch >= 1 && num_points >= 0 && num_queries >= 0, "%s: bad sizes", name);
     O3DML_CHECK(num_points < ((int64_t)1 << 30), "%s: too many points", name);
     O3DML_CHECK(metric == L2 || metric == L1 || metric == LINF, "%s: unknown metric %d", name, metric);
+    if (k > KNN_REG_KMAX) {
+        const char* limit = knn_any_k_limit(num_points, num_queries, k, ignore);
+        O3DML_CHECK(!limit, "%s: %s (num_queries %lld, k %d)", name, limit, (long long)num_queries, k);
+    }
     if (num_queries == 0) {
         if (ignore) {
             O3DML_CUDA(cudaMemsetAsync(out_row_splits, 0, sizeof(int64_t), st));
@@ -589,10 +906,9 @@ static int knn_impl(const char* name, const float* points, int64_t num_points, c
     int rc = grid_build(points, num_points, points_row_splits, queries, num_queries, queries_row_splits, (int)batch,
                         0.f, k, nullptr, g, st);
     if (rc) return rc;
-    const unsigned nb = (unsigned)ceil_div<int64_t>(num_queries, 128);
-#define KNN_ARGS(IDX, IS64, DIST, LEN)                                                                              \
-    nb, st, queries, num_queries, queries_row_splits, points_row_splits, (int)batch, g.order, g.info, g.cell_start, \
-        g.sorted, k, IDX, IS64, DIST, LEN
+#define KNN_ARGS(IDX, IS64, DIST, LEN)                                                                           \
+    num_queries, g.rows, st, queries, num_queries, queries_row_splits, points_row_splits, (int)batch, g.order,      \
+        g.info, g.cell_start, g.sorted, k, IDX, IS64, DIST, LEN
     if (!ignore) {
         uint32_t* no_len = nullptr;
         if (metric == L2) O3DML_CUDA(knn_launch<L2, false>(k, KNN_ARGS(out_index, index_is64, out_distance2, no_len)));
@@ -688,6 +1004,7 @@ extern "C" int o3dml_knn_search(const float* points, int64_t num_points,
                                 int64_t batch, int k, void* out_index, int index_is64,
                                 float* out_distance2, void* workspace, size_t workspace_bytes,
                                 void* stream) {
+    O3DML_CHECK(k >= 1 && k <= KNN_REG_KMAX, "knn_search: k must be in 1..64 (got %d)", k);
     return knn_impl("knn_search", points, num_points, points_row_splits, queries, num_queries, queries_row_splits,
                     batch, k, L2, 0, out_index, index_is64, out_distance2, nullptr, nullptr, workspace,
                     workspace_bytes, stream);
@@ -695,6 +1012,7 @@ extern "C" int o3dml_knn_search(const float* points, int64_t num_points,
 
 extern "C" size_t o3dml_knn_search_metric_workspace_bytes(int64_t num_points, int64_t num_queries, int64_t batch,
                                                           int k, int ignore_query_point) {
+    if (k > KNN_REG_KMAX && knn_any_k_limit(num_points, num_queries, k, ignore_query_point ? 1 : 0)) return SIZE_MAX;
     return Workspace::measure(knn_carve, num_points, num_queries, batch, k, ignore_query_point ? 1 : 0);
 }
 

@@ -192,7 +192,8 @@ def knn_search(points, queries, k, points_row_splits=None, queries_row_splits=No
     """open3d.ml.torch.ops.knn_search.  Rows ascend by (distance, index) in `metric` (L1, L2, Linf); L2 distances are
     squared, as upstream returns them.  Dense [Nq * k] rows with row splits 0, k, 2k, ...; with ignore_query_point
     (points equal to the query are skipped) a row may hold fewer than k neighbours, and the rows are ragged (one
-    device->host read of their total).  NaN distances are never ranked and +inf ones rank last, so a row that finds
+    device->host read of their total).  Any k >= 1: up to 64 a row is kept in registers, beyond it one CTA per query
+    selects it.  NaN distances are never ranked and +inf ones rank last, so a row that finds
     fewer than k rankable points (NaN coordinates) is padded with index -1 and distance +inf: dense rows in place,
     ragged rows by their length."""
     m, p, q, ps, qs, batch = _search_args("knn_search", points, queries, points_row_splits, queries_row_splits,
@@ -206,7 +207,7 @@ def knn_search(points, queries, k, points_row_splits=None, queries_row_splits=No
         raise RuntimeError("knn_search: a batch item has %d points, fewer than k = %d (ragged results are not "
                            "implemented)" % (short, k))
     nq = q.shape[0]
-    if m == 0 and not ignore_query_point:
+    if m == 0 and not ignore_query_point and k <= 64:       # o3dml_knn_search takes k in 1..64
         idx = torch.empty((nq, k), dtype=index_dtype, device=dev)
         d2 = torch.empty((nq, k), dtype=torch.float32, device=dev) if return_distances else None
         knn_search_raw(p, ps, q, qs, k, idx, d2)
